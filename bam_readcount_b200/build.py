@@ -1,4 +1,4 @@
-"""In-tree build of libbrc_engine.so for sm_100a (explicit nvcc; no JIT cache, no torch)."""
+"""In-tree build of libbrc_engine.so for sm_90a (H100) (explicit nvcc; no JIT cache, no torch)."""
 from __future__ import annotations
 
 import os
@@ -13,7 +13,7 @@ SOURCES = ["brc_kernels.cu", "brc_engine.cu", "brc_bgzf.cu", "brc_format.cpp"]
 HEADERS = ["brc_device.cuh", "brc_engine_internal.h", "brc_fmt_num.h", "brc_bgzf.cuh", os.path.join("..", "..", "include", "brc_engine.h")]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "--fmad=false",            # bit-exact float parity with the CPU reference: never contract a*b+c
     "-Xcompiler", "-fPIC,-O2,-Wall,-fvisibility=hidden",

@@ -1143,7 +1143,7 @@ int main(int argc, char **argv) {
     if (timing) std::fprintf(stderr, "[brc timing] startup (CUDA context, header, index, first window) %.3fs\n", t_loop0 - t_main0);
     if (!std::getenv("BRC_CLI_CLEAN_EXIT")) {
         // everything is printed: leave without tearing down the CUDA context, the page-locked buffers and the thread pools one by
-        // one (0.3-0.9 s on a B200 box, r02t) — the kernel reclaims them
+        // one (a teardown that takes a noticeable part of a second) — the kernel reclaims them
         std::fflush(nullptr);
         _exit(decode_error ? 1 : 0);
     }

@@ -327,9 +327,9 @@ int brc_push_reads(brc_engine *e, const brc_read_batch *b) {
     // keep a VIEW of the caller's arrays — brc_compute DMAs straight out of them (pin them for full PCIe speed).
     if (e->regions.size() == 1 && e->reads.n() == 0 && b->n_reads > 0 && b->n_reads < (int64_t)e->cfg.max_cnt &&
         b->n_reads < 0x7fffffffLL && e->adm.max_pos < 0) {
-        // Optional (BRC_EARLY_H2D=1): start the copies before the admission scan.  Measured on B200/PCIe Gen5 it is SLOWER end to end
-        // (28.9 vs 23.2 ms): the uploads run ahead alone and the result download then has the link to itself at the end, instead of
-        // both directions streaming concurrently for the whole step — so the default issues H2D from brc_compute.
+        // Optional (BRC_EARLY_H2D=1): start the copies before the admission scan.  The uploads then run ahead alone and the result
+        // download has the link to itself at the end, instead of both directions streaming concurrently for the whole step — so the
+        // default issues H2D from brc_compute.
         e->borrowed = *b; e->h2d_chunks = 0; e->skip_h2d = 0;
         cudaSetDevice(e->cfg.device);
         const bool early = std::getenv("BRC_EARLY_H2D") && issue_h2d_chunks(e) == BRC_OK;
@@ -613,9 +613,8 @@ static int issue_h2d_chunks(brc_engine *e) {
     const bool tm = std::getenv("BRC_PIPE_TIMING") != nullptr;
     if (tm) { for (auto &ev : e->tm_ev) if (!ev) CU(cudaEventCreate(&ev), "event"); CU(cudaEventRecord(e->tm_ev[0], e->s_in), "event"); }
     if (!B.lib) CU(cudaMemsetAsync(e->d_in[3].p, 0, (size_t)n * 2, two_streams ? e->s_in2 : e->s_in), "memset lib");
-    // Copy order (r02e, B200 / PCIe Gen5): a cudaMemcpyAsync of a megabyte or less costs ~50 us of link time whatever its size, so
-    // the eleven small arrays are sent WHOLE, once (<= 11 copies), and only the two big byte pools are cut into chunks that the
-    // kernels and the result copies follow; 13 arrays x 8 chunks ran the link at 35 GB/s, this order at > 45 GB/s.
+    // Copy order: a small cudaMemcpyAsync costs a fixed slice of link time whatever its size, so the eleven small arrays are sent
+    // WHOLE, once (<= 11 copies), and only the two big byte pools are cut into chunks that the kernels and the result copies follow.
     e->h2d_bytes_last = 0;
     #define H2D(st, k, host, off, cnt, esz) if ((cnt) > 0) { e->h2d_bytes_last += (int64_t)(cnt) * (int64_t)(esz); CU(cudaMemcpyAsync((char *)e->d_in[k].p + (size_t)(off) * (esz), (const char *)(host) + (size_t)(off) * (esz), (size_t)(cnt) * (esz), cudaMemcpyHostToDevice, st), "H2D"); }
     {

@@ -1,4 +1,4 @@
-// brc_kernels.cu — hand-written sm_100a kernels of the pileup-readcount hot path.
+// brc_kernels.cu — hand-written sm_90a (H100) kernels of the pileup-readcount hot path.
 //
 //   K0  read_precompute_kernel  ≙ fetch_func           R:src/exe/bam-readcount/bamreadcount.cpp:114-253
 //                                 + bam_plp_push admit  V:htslib-1.10/sam.c:4484-4531 (FUNMAP / tid<0)
@@ -1075,7 +1075,7 @@ cudaError_t launch_pileup(const PileupParams &p, cudaStream_t s) {
         cudaError_t e2 = cudaFuncSetAttribute(pileup_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PileupSmem));
         if (e1 != cudaSuccess) return e1;
         if (e2 != cudaSuccess) return e2;
-        if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) { cudaGetLastError(); sms = 148; }
+        if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) { cudaGetLastError(); sms = 132; }
         if (dev < 64) g_sm_count[dev].store(sms, std::memory_order_release);
     }
     const int64_t n_work = p.tile_count * (int64_t)p.res.n_rows;

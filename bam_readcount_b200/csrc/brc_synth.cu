@@ -453,7 +453,7 @@ int brc_synth_checksum_device(const void *buf_dev, int64_t n_bytes, unsigned lon
     if (!buf_dev || !acc_dev || n_bytes < 0 || (n_bytes & 3)) return BRC_E_INVALID;
     if (n_bytes == 0) return BRC_OK;
     const int64_t n = n_bytes / 4;
-    const unsigned grid = (unsigned)std::min<int64_t>(148 * 2, (n / 4 + 255) / 256 + 1);       // 2 CTAs per SM: a reader, not a tenant
+    const unsigned grid = (unsigned)std::min<int64_t>(132 * 2, (n / 4 + 255) / 256 + 1);       // 2 CTAs per SM: a reader, not a tenant
     checksum_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const uint32_t *>(buf_dev), n, ((uintptr_t)buf_dev & 15) == 0 ? 1 : 0, acc_dev);
     return cudaGetLastError() == cudaSuccess ? BRC_OK : BRC_E_CUDA;
 }

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — pileup positions/s of the B200 engine on the BASELINE.json workloads.
+"""bench.py — pileup positions/s of the H100 engine on the BASELINE.json workloads.
 
   --config c4 (default; the configuration the metric is quoted on): synthetic whole genome, 24 contigs x 125 Mb = 3.0 Gb, 30x,
       150 bp reads, --insertion-centric, ONE input split over N GPUs (strong scaling).  The genome is cut into 240 windows of
@@ -19,6 +19,11 @@
           one process per EFFECTIVE host core over disjoint slices.
 After the timed steps (outside the timed region) every rank re-runs 3 of its windows and diffs a sampled range of each against
 the CPU oracle on the host-generated copy of the same reads (`parity`).
+  --dump-outputs DIR : after the timed steps, the packed records (include/brc_engine.h) that the last timed step left in the engine
+          handles — the last windows (c3/c4) or launches (c5) of the step, as a caller of the device path receives them — are written
+          as DIR/<name>.npy in float64 (every uint32 word is exact): a seeded sample of slots of the packed words, with the sampled slot
+          indices, and a seeded sample of the secondary records in a canonical order.  Inputs are fixed by the seed of the
+          workload, so two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -101,11 +106,11 @@ def measured_peak_gbs():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback 6.65 TB/s (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet: 3.35 TB/s HBM3 (not measured)"
 
 
 def profiled_traffic():
-    """DRAM bytes per K1 launch from the newest committed `ncu --set full` capture (profiles/traffic_*.json): a PROFILE
+    """DRAM bytes per K1 launch from a committed profile capture (profiles/traffic_*.json) when one exists: a PROFILE
     constant of the same kernel on the C3 window, not measured in this run."""
     import glob
     fs = sorted(glob.glob(os.path.join(ROOT, "profiles", "traffic_*.json")))
@@ -230,7 +235,7 @@ def reference_arm(args):
         return 0
     m = reference_measure(args.config, args, args.steps, min(args.warmup, 1), size_steps=max(args.steps, 20))
     if m is None:
-        print(json.dumps({"impl": "reference", "unavailable": "oracle/_ref/bam-readcount not built (run oracle/build_ref.sh where /root/reference exists)"}))
+        print(json.dumps({"impl": "reference", "unavailable": "oracle/_ref/bam-readcount not built (run oracle/build_ref.sh with the reference sources)"}))
         return 0
     line = {
         "impl": "reference", "metric": METRIC, "value": m["value"], "unit": UNIT, "n_gpus": args.gpus, "steps": args.steps,
@@ -293,7 +298,7 @@ class ClockSampler:
 
 def bind_to_gpu_numa(local: int):
     """Pin this rank's threads (and so its first-touch pinned allocations) to the NUMA node its GPU hangs off
-    (SCALE_r01.json: GPU0-3 on node 0, GPU4-7 on node 1; unbound ranks made 8-GPU e2e 0.56 efficient)."""
+    (on a two-socket box half of the GPUs hang off each node; unbound ranks lose e2e throughput to cross-node copies)."""
     try:
         bus = subprocess.check_output(["nvidia-smi", f"--id={local}", "--query-gpu=pci.bus_id", "--format=csv,noheader"], text=True).strip().lower()
         if len(bus.split(":")[0]) == 8:      # 00000000:1b:00.0 -> 0000:1b:00.0
@@ -338,6 +343,30 @@ def oracle_dump(spec, flags, contig, pos_lo, pos_hi, lib_names):
     o.region(sub, tid=contig, beg=beg, end=end, contig=f"chr{contig + 1}", chrom_len=spec.contig_len, ref_seq=ref, ref_win_beg=wb,
              site_list_mode=False)
     return o.dump(), hb, blo, (wb, ref)
+
+
+DUMP_WORDS_BYTES = 8 << 20      # per handle: sampled packed words (float64)
+DUMP_SEC_RECORDS = 65536         # per handle: sampled secondary records (17 float64 columns each)
+
+
+def dump_packed(out_dir, name, eng, stream_ptr, seed):
+    """Write what `eng` computed for its last window: a seeded sample of the packed words (N_WORDS x rows x sampled slots) with the
+    slot indices, and a seeded sample of the secondary records.  Pool records come back in allocation order, which depends on thread
+    timing, and their `next` column is a chain link inside the pool: that column is dropped and the records are sorted."""
+    eng.fetch_device_results(stream_ptr)
+    pk = eng.packed()
+    rng = np.random.default_rng(seed)
+    words = pk.words                                             # uint32 [N_WORDS, n_rows, n_slots]
+    k = max(1, min(pk.n_slots, DUMP_WORDS_BYTES // (8 * words.shape[0] * max(pk.n_rows, 1))))
+    slots = np.sort(rng.choice(pk.n_slots, size=k, replace=False)) if k < pk.n_slots else np.arange(pk.n_slots)
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, f"{name}_slots.npy"), slots.astype(np.float64))
+    np.save(os.path.join(out_dir, f"{name}_words.npy"), words[:, :, slots].astype(np.float64))
+    sec = np.delete(pk.sec, 1, axis=1)                           # drop `next`
+    sec = sec[np.lexsort(sec.T[::-1])] if len(sec) else sec
+    if len(sec) > DUMP_SEC_RECORDS:
+        sec = sec[np.sort(rng.choice(len(sec), size=DUMP_SEC_RECORDS, replace=False))]
+    np.save(os.path.join(out_dir, f"{name}_sec.npy"), sec.astype(np.float64))
 
 
 def run_wgs(args, cfg_name):
@@ -500,6 +529,12 @@ def run_wgs(args, cfg_name):
     barrier()
     elapsed_ms = ev0.elapsed_time(ev1)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs:
+        for r_ in runners:
+            if r_.window is not None:
+                wi = shards[rank][0] + my_windows.index(r_.window) if not resident else rank
+                dump_packed(args.dump_outputs, f"window{wi:04d}", r_.eng, r_.stream.cuda_stream, seed=wi)
+        torch.cuda.synchronize()
     gather_overflow = 0
     if world > 1:
         for r_ in runners:
@@ -707,7 +742,7 @@ def run_wgs(args, cfg_name):
                        "windows_resident_rank0": len(resident_dw),
                        "gen_ms_per_window": gen_ms, "window_reads": n_reads_w, "window_sites": w_sites, "window_uncovered_sites": uncovered,
                        "window_events": w_events, "window_keys": w_keys, "window_packed_result_bytes": packed_bytes,
-                       "l2": "every window's inputs (%.0f MB) exceed the 126 MB L2; no flush" % (alg_bytes / 1e6),
+                       "l2": "every window's inputs (%.0f MB) exceed the 50 MB L2; no flush" % (alg_bytes / 1e6),
                        "gather": (None if world == 1 else {"transport": "NCCL send/recv of the packed records to rank 0, one group per round",
                                                            "k1_reserved_cta_slots": int(os.environ.get("BRC_K1_RESERVE_CTAS", "0")),
                                                            "rounds_per_step": rounds, "bytes_to_rank0_per_step": ring.bytes_received / max(args.steps + args.warmup, 1),
@@ -941,6 +976,11 @@ def run_deep(args):
     barrier()
     elapsed_ms = ev0.elapsed_time(ev1)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs:
+        for i in range(max(len(wins) - 2, 0), len(wins)):       # the last launch of each of the two handles
+            h = i % 2
+            dump_packed(args.dump_outputs, f"launch{i:04d}_sites{wins[i][0]}", engs[h], streams[h].cuda_stream, seed=wins[i][0])
+        torch.cuda.synchronize()
     launches = len(wins) * args.steps * (3 + engs[0].launch_count())
 
     # stage times + parity of sampled sites (untimed)
@@ -1036,6 +1076,8 @@ def main():
     ap.add_argument("--reserve-ctas", type=int, default=0, help="N > 1: CTA slots pileup_kernel leaves free for the NCCL kernels of the gather")
     ap.add_argument("--no-resident", action="store_true", help="c4: regenerate every window inside the timed loop instead of keeping windows in HBM")
     ap.add_argument("--hbm-margin-gb", type=float, default=14.0, help="HBM left free when windows are kept resident")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write a seeded sample of the last step's packed records as DIR/<name>.npy (float64)")
     args = ap.parse_args()
     if args.warmup < 3 and args.impl == "ours":
         args.warmup = 3

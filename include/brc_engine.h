@@ -1,5 +1,5 @@
 /*
- * brc_engine.h — C ABI of the B200-native pileup-readcount engine (libbrc_engine.so).
+ * brc_engine.h — C ABI of the H100-native pileup-readcount engine (libbrc_engine.so).
  *
  * Drop-in boundary for ONE path of genome/bam-readcount: the two htslib callbacks its
  * region loops register (SURVEY.md §8b):

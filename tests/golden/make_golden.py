@@ -11,6 +11,8 @@ the UNMODIFIED reference binary oracle/_ref/bam-readcount (oracle/build_ref.sh).
   edge_*.txt.gz                    reference-binary STDOUT on the hand-built edge-case reads
 """
 import gzip
+import hashlib
+import json
 import os
 import shutil
 import subprocess
@@ -72,6 +74,17 @@ def reference_stdout(case, flags, d, site_list):
     return out
 
 
+def fresh_fuzz_jobs():
+    """The fuzz cases of tests/test_differential_fuzz.py, run as site lists."""
+    from test_differential_fuzz import SEEDS, _case
+    jobs = []
+    for seed in SEEDS:
+        fc = _case(seed)
+        for fname, fl in fc["flag_sets"].items():
+            jobs.append((fc, fname, fl, True, f"{seed}_{fname}"))
+    return jobs
+
+
 def main():
     assert os.path.exists(REF_BIN), "run oracle/build_ref.sh first"
     for f in ("expected_all_lib", "expected_per_lib", "expected_insertion_centric_all_lib",
@@ -109,6 +122,16 @@ def main():
         with gzip.open(os.path.join(HERE, outname + ".gz"), "wb", compresslevel=9) as fh:
             fh.write(txt.encode("latin-1"))
         print(outname, len(txt.splitlines()), "lines")
+
+    # the fuzz seeds: only the SHA-256 of the reference's STDOUT is kept
+    sums, dirs = {}, {}
+    for case, fname, fl, sl, key in fresh_fuzz_jobs():
+        if case["name"] not in dirs:
+            dirs[case["name"]] = tempfile.mkdtemp()
+            write_case_files(case, dirs[case["name"]])
+        sums[key] = hashlib.sha256(reference_stdout(case, fl, dirs[case["name"]], sl).encode("latin-1")).hexdigest()
+    with open(os.path.join(HERE, "fresh_fuzz_sha256.json"), "w") as fh:
+        json.dump(sums, fh, indent=1, sort_keys=True)
 
 
 if __name__ == "__main__":

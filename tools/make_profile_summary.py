@@ -31,7 +31,7 @@ def main(tag, session=None):
     (prof_*.ncu-rep, launches_c4.csv); default = the round-1 layout (gpurun_out/prof_k?_<tag>.ncu-rep)."""
     import glob
     out = [f"# ncu summary {tag}", "", "Command: `tools/gpu_session.sh` — `ncu --set full --clock-control none --import-source on -k regex:<kernel> -s 4 -c 1 python bench.py "
-           "--config c3 --steps 2 --warmup 3 ...` (K0/K1 on the resident 10 Mb window; deep: `--config c5`; inflate: the span parity test), 1 B200.", ""]
+           "--config c3 --steps 2 --warmup 3 ...` (K0/K1 on the resident 10 Mb window; deep: `--config c5`; inflate: the span parity test), 1 H100.", ""]
     traffic = {}
     if session:
         reps = sorted(glob.glob(os.path.join(ROOT, "gpurun_out", session, "prof_*.ncu-rep")))
