@@ -571,12 +571,27 @@ __device__ __noinline__ int3 resolve_general(const uint32_t *cig, uint32_t n_cig
 // Rare keys (indel alleles, a third base class at a site): find-or-append a record in the thread's private
 // chain in the L2-resident pool and accumulate there.  Recomputes the event from the global descriptor so
 // the hot loop carries no state for it.  Returns the new chain head.
-__device__ __forceinline__ bool same_insertion(const PileupParams &P, int32_t read_a, int qpos_a, int32_t read_b, int qpos_b, int len) {
+//
+// What the rare path reads, passed BY VALUE: a reference to the kernel's parameter block would make every kernel that
+// calls these out-of-line functions copy the whole block to local memory and read its fields back from there, the hot
+// loop's base-quality threshold included.
+struct RareCtx {
+    const ReadDesc *desc;
+    const uint8_t *seq;
+    const uint64_t *seq_off;
+    SecRec *sec;
+    int32_t *sec_count;
+    int64_t sec_cap;
+};
+__device__ __forceinline__ RareCtx rare_ctx(const PileupParams &P) {
+    return RareCtx{P.desc, P.seq, P.seq_off, P.res.sec, P.res.sec_count, P.res.sec_cap};
+}
+__device__ __forceinline__ bool same_insertion(const RareCtx &C, int32_t read_a, int qpos_a, int32_t read_b, int qpos_b, int len) {
     // same inserted bases?  compare canonicalised read bases (R:bamreadcount.cpp:324-330)
-    const uint64_t oa = P.seq_off[read_a], ob = P.seq_off[read_b];
+    const uint64_t oa = C.seq_off[read_a], ob = C.seq_off[read_b];
     bool same = true;
     for (int k = 1; k <= len && same; ++k)
-        same = canonical16(seq_nib(P.seq, oa, qpos_a + k)) == canonical16(seq_nib(P.seq, ob, qpos_b + k));
+        same = canonical16(seq_nib(C.seq, oa, qpos_a + k)) == canonical16(seq_nib(C.seq, ob, qpos_b + k));
     return same;
 }
 __device__ __forceinline__ void sec_init(SecRec &r, uint32_t slot, int32_t next, uint32_t kind, uint32_t len, int32_t read, int32_t qpos) {
@@ -585,8 +600,8 @@ __device__ __forceinline__ void sec_init(SecRec &r, uint32_t slot, int32_t next,
     for (int k = 0; k < N_STATS; ++k) r.stats[k] = 0u;
 }
 // one event of BasicStat::process_read into a pool record (slow, exact IEEE path)
-__device__ __forceinline__ void sec_accumulate(const PileupParams &P, SecRec &r, int32_t read, int qpos, uint32_t bq, bool is_indel) {
-    const ReadDesc d = P.desc[read];
+__device__ __forceinline__ void sec_accumulate(const ReadDesc *desc, SecRec &r, int32_t read, int qpos, uint32_t bq, bool is_indel) {
+    const ReadDesc d = desc[read];
     const Terms t = event_terms(false, qpos, d.q2, d.tpi, d.lclip, d.clen, d.fl, d.fclen, 0.f, 0.f);
     uint32_t v[N_STATS];
 #pragma unroll
@@ -607,27 +622,26 @@ __device__ __forceinline__ void sec_accumulate(const PileupParams &P, SecRec &r,
 }
 // find-or-append of the allele's record in the chain starting at `head`; returns the record index (>= sec_cap on overflow:
 // the host sees sec_count > cap and retries with a larger pool)
-__device__ __noinline__ int32_t rare_find_or_append(const PileupParams &P, int32_t &head, uint32_t slot, int kind, int len, int32_t read, int qpos) {
-    const ResultsDev &S = P.res;
+__device__ __noinline__ int32_t rare_find_or_append(const RareCtx C, int32_t &head, uint32_t slot, int kind, int len, int32_t read, int qpos) {
     const uint32_t want = (uint32_t)kind | ((uint32_t)len << 8);
     int32_t j = head;
     while (j >= 0) {
-        const SecRec &r = S.sec[j];
-        if (r.kind_len == want && (kind != KIND_INS || same_insertion(P, read, qpos, r.read, r.qpos, len))) break;
+        const SecRec &r = C.sec[j];
+        if (r.kind_len == want && (kind != KIND_INS || same_insertion(C, read, qpos, r.read, r.qpos, len))) break;
         j = r.next;
     }
     if (j < 0) {
-        j = atomicAdd(S.sec_count, 1);
-        if ((int64_t)j >= S.sec_cap) return j;
-        sec_init(S.sec[j], slot, head, (uint32_t)kind, (uint32_t)len, read, qpos);
+        j = atomicAdd(C.sec_count, 1);
+        if ((int64_t)j >= C.sec_cap) return j;
+        sec_init(C.sec[j], slot, head, (uint32_t)kind, (uint32_t)len, read, qpos);
         head = j;
     }
     return j;
 }
-__device__ __noinline__ int32_t rare_event(const PileupParams &P, int32_t head, uint32_t slot, int kind, int len, int32_t read, int qpos,
+__device__ __noinline__ int32_t rare_event(const RareCtx C, int32_t head, uint32_t slot, int kind, int len, int32_t read, int qpos,
                                            uint32_t bq, bool is_indel) {
-    const int32_t j = rare_find_or_append(P, head, slot, kind, len, read, qpos);
-    if ((int64_t)j < P.res.sec_cap) sec_accumulate(P, P.res.sec[j], read, qpos, bq, is_indel);
+    const int32_t j = rare_find_or_append(C, head, slot, kind, len, read, qpos);
+    if ((int64_t)j < C.sec_cap) sec_accumulate(C.desc, C.sec[j], read, qpos, bq, is_indel);
     return head;
 }
 
@@ -642,7 +656,8 @@ struct __align__(16) ChunkInfo {
     uint32_t row, cbase32;
 };
 struct __align__(128) StageBuf {
-    int4 desc[(STAGE_READS + 1) * 5];   // + the sentinel the producer writes behind the chunk's last descriptor
+    int4 desc[(STAGE_READS + 2) * 5];   // + the sentinel the producer writes behind the chunk's last descriptor, + the record the
+                                        // consumers load (and never use) as the sentinel's pair partner
     uint8_t qual[STAGE_QUAL];
     uint8_t seq[STAGE_SEQ];
     uint32_t cigar[STAGE_CIGAR];
@@ -702,14 +717,121 @@ template <bool PER_LIB>
 __device__ __forceinline__ uint32_t slot_index(const PileupParams &P, const ChunkInfo &ci, const SiteState &S) {
     return (uint32_t)((PER_LIB ? (int64_t)S.row * P.res.n_slots : 0) + ci.slot0 + (S.site - ci.pos0));
 }
+constexpr uint32_t DSZ = (uint32_t)sizeof(ReadDesc);
+
+// A passing event whose base is not the site's primary class: the site's second base class accumulates in shared memory,
+// a third one in the record pool.  `da` = the read's staged descriptor, `read` its index.
+template <bool PER_LIB>
+__device__ __forceinline__ void off_primary_event(const PileupParams &P, uint32_t (*sacc)[TILE], const ChunkInfo &ci, SiteState &S, int tid,
+                                                  uint32_t da, int32_t read, bool fast, uint32_t fm, int qpos, uint32_t bq, uint32_t base) {
+    if (S.sbase != NO_BASE && base != S.sbase) {   // third base class at this site: rare
+        S.sec_head = rare_event(rare_ctx(P), S.sec_head, slot_index<PER_LIB>(P, ci, S), (int)base, 0, read, qpos, bq, false);
+        return;
+    }
+    const int4 q1 = lds128(da + 16u);                            // mmq,clen,lclip,tpi
+    const int4 q2 = lds128(da + 32u);                            // q2,nmfrac,se,fl
+    const int4 q4 = lds128(da + 64u);                            // rcp_l, rcp_clen, fclen
+    const Terms t = event_terms(fast, qpos, q2.x, q1.w, q1.z, q1.y, __int_as_float(q2.w), __int_as_float(q4.z),
+                                __int_as_float(q4.x), __int_as_float(q4.y));
+    const uint32_t plus = (fm & 16u) ? 0u : 1u;
+    if (S.sbase == NO_BASE) {
+        S.sbase = base;
+#pragma unroll
+        for (int k = 0; k < N_STATS; ++k) sacc[k][tid] = 0u;
+    }
+    sacc[0][tid] += 1u; sacc[1][tid] += (fm >> 16) & 0xFFu; sacc[2][tid] += bq; sacc[3][tid] += (uint32_t)q2.z;
+    sacc[4][tid] += plus; sacc[5][tid] += 1u - plus;
+    sacc[6][tid] = __float_as_uint(__double2float_rn(__dadd_rn((double)__uint_as_float(sacc[6][tid]), t.posterm)));
+    sacc[7][tid] = __float_as_uint(__fadd_rn(__uint_as_float(sacc[7][tid]), __int_as_float(q2.y)));
+    sacc[8][tid] += (uint32_t)q1.x;
+    if (q2.x > -1) { sacc[9][tid] += 1u; sacc[10][tid] = __float_as_uint(__fadd_rn(__uint_as_float(sacc[10][tid]), t.q2term)); }
+    sacc[11][tid] += (uint32_t)q1.y;
+    sacc[12][tid] = __float_as_uint(__fadd_rn(__uint_as_float(sacc[12][tid]), t.d3pterm));
+}
+
+// Two consecutive staged FM_HOT reads A (descriptor at `da`) and B (at da + DSZ) in one body without branches: every lane
+// computes both events (a lane off a read loads a valid byte of it and drops the result) and applies them as predicated
+// updates, A before B, so each accumulator still sees file order.  Only the rare event that is not the site's primary class
+// (a second or third base class, ~0.5 % of events) branches, again A before B.  -p: neither read is library-less, so the
+// site's library-less flag cannot change here; a lane whose flag is already set takes neither read.
+template <bool PER_LIB>
+__device__ __forceinline__ void hot_pair(const PileupParams &P, uint32_t (*sacc)[TILE], const ChunkInfo &ci, SiteState &S, int tid,
+                                         uint32_t da, uint32_t desc_s, uint32_t qual_s, uint32_t seq_s,
+                                         int2 pe_a, uint32_t fm_a, uint32_t lib_a, int2 pe_b, uint32_t fm_b, uint32_t lib_b,
+                                         uint32_t &pk3, uint32_t &pkmb) {
+    const uint32_t db = da + DSZ;
+    const int4 q3a = lds128(da + 48u), q3b = lds128(db + 48u);    // qual32,seq32,qoff,n_cigar
+    bool cov_a = S.site >= pe_a.x && S.site < pe_a.y;
+    bool cov_b = S.site >= pe_b.x && S.site < pe_b.y;
+    if (PER_LIB) {
+        const bool open = !(S.flags & 1u);
+        cov_a = cov_a && open && (lib_a & 0xFFFFu) == S.row;
+        cov_b = cov_b && open && (lib_b & 0xFFFFu) == S.row;
+    }
+    pk3 += ((uint32_t)cov_a + (uint32_t)cov_b) << 24;
+    const int qpos_a = cov_a ? S.site - pe_a.x + q3a.z : 0;        // FM_HOT reads have l_qseq >= 1: byte 0 exists
+    const int qpos_b = cov_b ? S.site - pe_b.x + q3b.z : 0;
+    const uint32_t bq_a = lds_u8(qual_s + (uint32_t)q3a.x + (uint32_t)qpos_a);
+    const uint32_t bq_b = lds_u8(qual_s + (uint32_t)q3b.x + (uint32_t)qpos_b);
+    const uint32_t byte_a = lds_u8(seq_s + (uint32_t)q3a.y + ((uint32_t)qpos_a >> 1));
+    const uint32_t byte_b = lds_u8(seq_s + (uint32_t)q3b.y + ((uint32_t)qpos_b >> 1));
+    const bool pass_a = cov_a && !(fm_a & FM_DEAD) && (int)bq_a >= P.min_bq;
+    const bool pass_b = cov_b && !(fm_b & FM_DEAD) && (int)bq_b >= P.min_bq;
+    S.npass += (uint32_t)pass_a + (uint32_t)pass_b;
+    const uint32_t base_a = canonical16((byte_a >> ((~qpos_a & 1) << 2)) & 0xFu);
+    const uint32_t base_b = canonical16((byte_b >> ((~qpos_b & 1) << 2)) & 0xFu);
+    if (pass_a && S.pbase == NO_BASE) S.pbase = base_a;
+    const bool prim_a = pass_a && base_a == S.pbase;
+    if (pass_b && S.pbase == NO_BASE) S.pbase = base_b;
+    const bool prim_b = pass_b && base_b == S.pbase;
+
+    const int4 q1a = lds128(da + 16u), q1b = lds128(db + 16u);    // mmq,clen,lclip,tpi
+    const int4 q2a = lds128(da + 32u), q2b = lds128(db + 32u);    // q2,nmfrac,se,fl
+    const int4 q4a = lds128(da + 64u), q4b = lds128(db + 64u);    // rcp_l, rcp_clen, fclen, inc
+    const float fl_a = __int_as_float(q2a.w), rcp_la = __int_as_float(q4a.x);
+    const float fl_b = __int_as_float(q2b.w), rcp_lb = __int_as_float(q4b.x);
+    const float d3_a = div_small((float)abs(qpos_a - q1a.w), fl_a, rcp_la);
+    const float d3_b = div_small((float)abs(qpos_b - q1b.w), fl_b, rcp_lb);
+    const float f_a = div_small((float)abs(2 * (qpos_a - q1a.z) - q1a.y), __int_as_float(q4a.z), __int_as_float(q4a.y));
+    const float f_b = div_small((float)abs(2 * (qpos_b - q1b.z) - q1b.y), __int_as_float(q4b.z), __int_as_float(q4b.y));
+    // the Q2 term only counts when the read has a Q2 position, which for most forward reads IS the effective 3' end
+    const float q2t_a = q2a.x == q1a.w ? d3_a : div_small((float)abs(qpos_a - q2a.x), fl_a, rcp_la);
+    const float q2t_b = q2b.x == q1b.w ? d3_b : div_small((float)abs(qpos_b - q2b.x), fl_b, rcp_lb);
+    const bool q2_a = prim_a && (q4a.w & 0x10000), q2_b = prim_b && (q4b.w & 0x10000);
+
+    // integer sums: adding 0 for a dropped event is exact
+    pk3 += (prim_a ? (uint32_t)q4a.w : 0u) + (prim_b ? (uint32_t)q4b.w : 0u);
+    pkmb += (prim_a ? (fm_a & 0x00FF0000u) + bq_a : 0u) + (prim_b ? (fm_b & 0x00FF0000u) + bq_b : 0u);
+    Acc &a = S.acc;
+    a.mmqs += (prim_a ? (uint32_t)q1a.x : 0u) + (prim_b ? (uint32_t)q1b.x : 0u);
+    a.clip += (prim_a ? (uint32_t)q1a.y : 0u) + (prim_b ? (uint32_t)q1b.y : 0u);
+    a.se += (prim_a ? (uint32_t)q2a.z : 0u) + (prim_b ? (uint32_t)q2b.z : 0u);
+    // float sums: a dropped event keeps the old value (never "+ 0"), A's add before B's
+    a.q2d = q2_a ? __fadd_rn(a.q2d, q2t_a) : a.q2d;
+    a.q2d = q2_b ? __fadd_rn(a.q2d, q2t_b) : a.q2d;
+    a.d3p = prim_a ? __fadd_rn(a.d3p, d3_a) : a.d3p;
+    a.d3p = prim_b ? __fadd_rn(a.d3p, d3_b) : a.d3p;
+    a.posd = prim_a ? round_to_f32_precision(__dadd_rn(a.posd, __dsub_rn(1.0, f32_to_f64_nonneg(f_a)))) : a.posd;
+    a.posd = prim_b ? round_to_f32_precision(__dadd_rn(a.posd, __dsub_rn(1.0, f32_to_f64_nonneg(f_b)))) : a.posd;
+    a.nmf = prim_a ? __fadd_rn(a.nmf, __int_as_float(q2a.y)) : a.nmf;
+    a.nmf = prim_b ? __fadd_rn(a.nmf, __int_as_float(q2b.y)) : a.nmf;
+
+    const bool off_a = pass_a && !prim_a, off_b = pass_b && !prim_b;
+    if (off_a || off_b) {
+        const int32_t read_a = ci.r0 + (int)((da - desc_s) / DSZ);
+        if (off_a) off_primary_event<PER_LIB>(P, sacc, ci, S, tid, da, read_a, true, fm_a, qpos_a, bq_a, base_a);
+        if (off_b) off_primary_event<PER_LIB>(P, sacc, ci, S, tid, db, read_a + 1, true, fm_b, qpos_b, bq_b, base_b);
+    }
+}
 
 // The hot loop: one warp walks the chunk's reads in file order; lane = site.
 //
 // K0 has already classified every read (uniform per iteration): FM_DEAD reads only count as spanning reads; FM_HOT reads
 // (one match-type CIGAR op, lengths <= FASTDIV_MAX, no missing tag) take a straight-line path whose event is the site's
-// primary base class in ~99 % of the cases; everything else takes the general path.  The primary class's small integer
-// sums are kept PACKED for the duration of a chunk (<= STAGE_READS events per lane: three 8-bit counters in one word,
-// two 16-bit sums in another) and flushed into the full-width accumulators at the end of the chunk.
+// primary base class in ~99 % of the cases; everything else takes the general path.  Two consecutive FM_HOT reads of a
+// staged chunk take hot_pair instead.  The primary class's small integer sums and the coverage count are kept PACKED for
+// the duration of a chunk (<= STAGE_READS reads: four 8-bit counters in one word, two 16-bit sums in another) and flushed
+// into the full-width accumulators at the end of the chunk.
 template <bool PER_LIB, bool STAGED>
 __device__ __forceinline__ void process_chunk(const PileupParams &P, const StageBuf &sb, uint32_t (*sacc)[TILE], uint32_t (*warn)[TILE],
                                               const ChunkInfo &ci, SiteState &S, int tid) {
@@ -731,22 +853,30 @@ __device__ __forceinline__ void process_chunk(const PileupParams &P, const Stage
         if (start >= n_in) return;
         da += (uint32_t)start * (uint32_t)sizeof(ReadDesc);
     }
-    uint32_t pk3 = 0u, pkmb = 0u;                                 // count | plus << 8 | nq2 << 16 ;  baseq | mapq << 16
-#ifdef BRC_K1_PREFETCH
-    int2 pe_next = lds64(da);                                     // software prefetch of the next read's (pos,end)
-#endif
-    // no loop bound: the producer wrote a sentinel descriptor (pos = INT_MAX) behind the chunk's last read
-    for (;; da += (uint32_t)sizeof(ReadDesc)) {
-#ifdef BRC_K1_PREFETCH
-        const int2 pe = pe_next;
-        pe_next = lds64(da + (uint32_t)sizeof(ReadDesc));         // may run one record past the chunk: staged garbage, never used
-#else
+    uint32_t pk3 = 0u, pkmb = 0u;                                 // count | plus << 8 | nq2 << 16 | ncover << 24 ;  baseq | mapq << 16
+    // no loop bound: the producer wrote a sentinel descriptor (pos = INT_MAX, fm = 0) behind the chunk's last read
+    for (;; da += DSZ) {
         const int2 pe = lds64(da);                                // pos, end
-#endif
+        const int2 fl2 = lds64(da + 8u);                          // fm, lib_nc
+        // the next read's: when `pe` is the sentinel this is the spare record behind it in desc[], loaded and never used
+        const int2 pe_b = lds64(da + DSZ), fl_b = lds64(da + DSZ + 8u);
         if (pe.x - wfirst > 31) { if (pe.x != 0x7fffffff) S.warp_done = true; break; }   // reads are position-sorted within a region; INT_MAX = end of chunk
+        if (STAGED) {
+            // Two FM_HOT reads (A = this one, B = the next) in one predicated body; the test is uniform across the warp.  -p: a
+            // read without a library (which stops the site's accumulation) is never part of a pair.  B is never the sentinel.
+            bool pair = ((uint32_t)fl2.x & (uint32_t)fl_b.x & FM_HOT) != 0u;
+            if (PER_LIB) pair = pair && ((uint32_t)fl2.y & 0xFFFFu) != LIB_NONE && ((uint32_t)fl_b.y & 0xFFFFu) != LIB_NONE;
+            if (pair) {
+                const bool b_in = pe_b.x - wfirst <= 31;          // B beyond the warp's window: it covers no lane and ends the walk
+                hot_pair<PER_LIB>(P, sacc, ci, S, tid, da, desc_s, qual_s, seq_s, pe, (uint32_t)fl2.x, (uint32_t)fl2.y,
+                                  b_in ? pe_b : make_int2(0x7fffffff, 0), (uint32_t)fl_b.x, (uint32_t)fl_b.y, pk3, pkmb);
+                if (!b_in) { S.warp_done = true; break; }
+                da += DSZ;
+                continue;
+            }
+        }
         if (pe.y <= wfirst) continue;
         const bool cover = S.site >= pe.x && S.site < pe.y;
-        const int2 fl2 = lds64(da + 8u);                          // fm, lib_nc
         if (PER_LIB) {
             const uint32_t lib = (uint32_t)fl2.y & 0xFFFFu;
             if (lib == LIB_NONE) { if (cover) S.flags |= 1u; continue; }
@@ -756,7 +886,7 @@ __device__ __forceinline__ void process_chunk(const PileupParams &P, const Stage
             if (S.flags & 1u) continue;
         }
         if (!cover) continue;
-        S.ncover++;
+        pk3 += 1u << 24;                                          // ncover
         const uint32_t fm = (uint32_t)fl2.x;
         const int4 q3 = lds128(da + 48u);                        // qual32,seq32,cig,n_cigar
         int qpos, indel = 0;
@@ -798,7 +928,10 @@ __device__ __forceinline__ void process_chunk(const PileupParams &P, const Stage
             // ---- general path ----
             if (fm & FM_SIMPLE) qpos = S.site - pe.x + q3.z;
             else {
-                const uint32_t *cig_base = (ci.flags & 16u) ? sb.cigar - ci.cbase32 : P.cigar;   // staged ops are indexed with the reads' pool op indices
+                // staged ops are indexed with the reads' pool op indices; their address derives from desc_s, which the loop
+                // keeps anyway (not from the ring slot's index, which would be reloaded from local memory)
+                const uint32_t *cig_base = (ci.flags & 16u)
+                    ? static_cast<const uint32_t *>(__cvta_shared_to_generic(desc_s + (uint32_t)offsetof(StageBuf, cigar))) - ci.cbase32 : P.cigar;
                 const int3 rr = resolve_general(cig_base + (uint32_t)q3.z, (uint32_t)q3.w, pe.x, S.site);
                 if (rr.z) continue;                              // is_del
                 qpos = rr.x; indel = rr.y;
@@ -811,7 +944,7 @@ __device__ __forceinline__ void process_chunk(const PileupParams &P, const Stage
             const bool warns = (fm & (FM_NM_ABSENT | FM_SM_MISSING)) != 0;   // a tag the reference warns about is missing
             if (indel != 0) {
                 const int32_t r = ci.r0 + (int)((da - desc_s) / (uint32_t)sizeof(ReadDesc));
-                S.sec_head = rare_event(P, S.sec_head, slot_index<PER_LIB>(P, ci, S), indel > 0 ? KIND_INS : KIND_DEL, indel > 0 ? indel : -indel, r, qpos, bq, true);
+                S.sec_head = rare_event(rare_ctx(P), S.sec_head, slot_index<PER_LIB>(P, ci, S), indel > 0 ? KIND_INS : KIND_DEL, indel > 0 ? indel : -indel, r, qpos, bq, true);
                 if (warns) { warn[0][tid] += (fm >> 25) & 1u; warn[1][tid] += (fm >> 26) & 1u; }
                 if (indel > 0 && P.insertion_centric) continue;
             }
@@ -823,8 +956,8 @@ __device__ __forceinline__ void process_chunk(const PileupParams &P, const Stage
             if (S.pbase == NO_BASE) S.pbase = base;
         }
         // ---- an event that is not (hot, primary): full-width accumulation ----
-        if (base != S.pbase && S.sbase != NO_BASE && base != S.sbase) {   // third base class at this site: rare
-            S.sec_head = rare_event(P, S.sec_head, slot_index<PER_LIB>(P, ci, S), (int)base, 0, ci.r0 + (int)((da - desc_s) / (uint32_t)sizeof(ReadDesc)), qpos, bq, false);
+        if (base != S.pbase) {
+            off_primary_event<PER_LIB>(P, sacc, ci, S, tid, da, ci.r0 + (int)((da - desc_s) / DSZ), (fm & FM_FASTDIV) != 0, fm, qpos, bq, base);
             continue;
         }
         const int4 q1 = lds128(da + 16u);                        // mmq,clen,lclip,tpi
@@ -832,38 +965,19 @@ __device__ __forceinline__ void process_chunk(const PileupParams &P, const Stage
         const int4 q4 = lds128(da + 64u);                        // rcp_l, rcp_clen, fclen
         const Terms t = event_terms((fm & FM_FASTDIV) != 0, qpos, q2.x, q1.w, q1.z, q1.y, __int_as_float(q2.w), __int_as_float(q4.z),
                                     __int_as_float(q4.x), __int_as_float(q4.y));
-        const bool has_q2 = q2.x > -1;
-        const uint32_t plus = (fm & 16u) ? 0u : 1u;
-        const uint32_t mapq = (fm >> 16) & 0xFFu;
-        const float nmterm = __int_as_float(q2.y);
-        if (base == S.pbase) {
-            Acc &a = S.acc;
-            a.count++; a.mapq += mapq; a.plus += plus; a.mmqs += (uint32_t)q1.x;
-            if (has_q2) { a.q2d = __fadd_rn(a.q2d, t.q2term); a.nq2++; }
-            a.d3p = __fadd_rn(a.d3p, t.d3pterm);
-            a.clip += (uint32_t)q1.y;
-            a.posd = round_to_f32_precision(__dadd_rn(a.posd, t.posterm));
-            a.se += (uint32_t)q2.z;
-            a.nmf = __fadd_rn(a.nmf, nmterm);
-            a.baseq += bq;
-        } else {   // second base class of the site: accumulators live in shared memory
-            if (S.sbase == NO_BASE) {
-                S.sbase = base;
-#pragma unroll
-                for (int k = 0; k < N_STATS; ++k) sacc[k][tid] = 0u;
-            }
-            sacc[0][tid] += 1u; sacc[1][tid] += mapq; sacc[2][tid] += bq; sacc[3][tid] += (uint32_t)q2.z;
-            sacc[4][tid] += plus; sacc[5][tid] += 1u - plus;
-            sacc[6][tid] = __float_as_uint(__double2float_rn(__dadd_rn((double)__uint_as_float(sacc[6][tid]), t.posterm)));
-            sacc[7][tid] = __float_as_uint(__fadd_rn(__uint_as_float(sacc[7][tid]), nmterm));
-            sacc[8][tid] += (uint32_t)q1.x;
-            if (has_q2) { sacc[9][tid] += 1u; sacc[10][tid] = __float_as_uint(__fadd_rn(__uint_as_float(sacc[10][tid]), t.q2term)); }
-            sacc[11][tid] += (uint32_t)q1.y;
-            sacc[12][tid] = __float_as_uint(__fadd_rn(__uint_as_float(sacc[12][tid]), t.d3pterm));
-        }
+        Acc &a = S.acc;
+        pk3 += (uint32_t)q4.w;                                   // count, plus, nq2: the packed counters, as on the hot path
+        pkmb += (fm & 0x00FF0000u) + bq;
+        a.mmqs += (uint32_t)q1.x;
+        if (q2.x > -1) a.q2d = __fadd_rn(a.q2d, t.q2term);
+        a.d3p = __fadd_rn(a.d3p, t.d3pterm);
+        a.clip += (uint32_t)q1.y;
+        a.posd = round_to_f32_precision(__dadd_rn(a.posd, t.posterm));
+        a.se += (uint32_t)q2.z;
+        a.nmf = __fadd_rn(a.nmf, __int_as_float(q2.y));
     }
     // flush the chunk's packed counters of the primary class
-    S.acc.count += pk3 & 0xFFu; S.acc.plus += (pk3 >> 8) & 0xFFu; S.acc.nq2 += pk3 >> 16;
+    S.acc.count += pk3 & 0xFFu; S.acc.plus += (pk3 >> 8) & 0xFFu; S.acc.nq2 += (pk3 >> 16) & 0xFFu; S.ncover += pk3 >> 24;
     S.acc.baseq += pkmb & 0xFFFFu; S.acc.mapq += pkmb >> 16;
 }
 
@@ -1161,10 +1275,10 @@ __device__ __forceinline__ void deep_indel_event(const PileupParams &P, DeepSmem
     const uint32_t nc = sm.icount[og];
     if (cacheable) for (uint32_t e = 0; e < nc; ++e) if (sm.ikey[og][e] == key) j = sm.irec[og][e];
     if (j < 0) {
-        j = rare_find_or_append(P, sec_head, slot, kind, len, read, qpos);
+        j = rare_find_or_append(rare_ctx(P), sec_head, slot, kind, len, read, qpos);
         if (cacheable && (int64_t)j < P.res.sec_cap && nc < (uint32_t)DEEP_ICACHE) { sm.ikey[og][nc] = key; sm.irec[og][nc] = j; sm.icount[og] = nc + 1u; }
     }
-    if ((int64_t)j < P.res.sec_cap) sec_accumulate(P, P.res.sec[j], read, qpos, bq, true);
+    if ((int64_t)j < P.res.sec_cap) sec_accumulate(P.desc, P.res.sec[j], read, qpos, bq, true);
 }
 
 // this thread's read of the block starting at `blk` -> its own slots of stage st (no other thread touches them)
