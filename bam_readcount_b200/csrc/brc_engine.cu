@@ -7,11 +7,8 @@
 // in the CUDA kernels of brc_kernels.cu; this file only batches, copies and launches.
 #include <algorithm>
 #include <atomic>
-#include <cstdio>
 #include <cstdlib>
 #include <cstring>
-#include <thread>
-#include <chrono>
 
 #include "brc_engine_internal.h"
 
@@ -33,6 +30,56 @@ const HostRef *find_ref(const brc_engine *e, int32_t tid) {
 }  // namespace brc
 
 #define CU(call, what) do { cudaError_t ce_ = (call); if (ce_ != cudaSuccess) return set_cuda_error(e, ce_, what); } while (0)
+
+// bam_cigar2rlen: reference length of a CIGAR; with n_indel, also counts its I and D ops there
+static inline int64_t cigar_rlen(const uint32_t *cig, uint64_t n, int64_t *n_indel = nullptr) {
+    int64_t l = 0;
+    for (uint64_t k = 0; k < n; ++k) {
+        const uint32_t op = cig[k] & 0xF;
+        if (op == 0 || op == 2 || op == 3 || op == 7 || op == 8) l += cig[k] >> 4;
+        if (n_indel && (op == 1 || op == 2)) ++*n_indel;
+    }
+    return l;
+}
+
+// The kernels' view of a batch whose arrays are in device memory.
+static ReadsDev reads_dev(const brc_read_batch &b) {
+    ReadsDev R;
+    R.n_reads = b.n_reads; R.pos = b.pos; R.flag = b.flag; R.mapq = b.mapq; R.lib = b.lib; R.l_qseq = b.l_qseq; R.nm = b.nm; R.sm = b.sm;
+    R.cigar_off = b.cigar_off; R.cigar = b.cigar; R.seq_off = b.seq_off; R.seq = b.seq; R.qual_off = b.qual_off; R.qual = b.qual;
+    return R;
+}
+
+// The read arrays uploaded into d_in[0..12] (brc_read_batch field order) as a device batch of n reads.
+static brc_read_batch d_in_batch(const brc_engine *e, int64_t n) {
+    brc_read_batch b{};
+    b.n_reads = n; b.pos = e->d_in[0].as<int32_t>(); b.flag = e->d_in[1].as<uint16_t>(); b.mapq = e->d_in[2].as<uint8_t>();
+    b.lib = e->d_in[3].as<uint16_t>(); b.l_qseq = e->d_in[4].as<int32_t>(); b.nm = e->d_in[5].as<int32_t>(); b.sm = e->d_in[6].as<int32_t>();
+    b.cigar_off = e->d_in[7].as<uint64_t>(); b.cigar = e->d_in[8].as<uint32_t>(); b.seq_off = e->d_in[9].as<uint64_t>();
+    b.seq = e->d_in[10].as<uint8_t>(); b.qual_off = e->d_in[11].as<uint64_t>(); b.qual = e->d_in[12].as<uint8_t>();
+    return b;
+}
+
+// Installs the reference window of `tid` from win_len FASTA characters in device memory, asynchronously on `s`: finds or adds
+// its HostRef, encodes the characters into the device copy (4-bit codes: K0 compares nibbles) and refreshes the device RefWin
+// table.  `host_seq` is kept as the host copy (the text emitter's deletion alleles and reference column), or null for none.
+static int install_ref(brc_engine *e, int32_t tid, const char *contig_name, int64_t chrom_len, int64_t win_beg, int64_t win_len,
+                       const char *host_seq, const char *dev_ascii, cudaStream_t s) {
+    HostRef *r = nullptr;
+    for (auto &x : e->refs) if (x.tid == tid) r = &x;
+    if (!r) { e->refs.emplace_back(); r = &e->refs.back(); }
+    r->tid = tid; r->name = contig_name ? contig_name : ""; r->chrom_len = chrom_len; r->win_beg = win_beg; r->win_len = win_len;
+    if (host_seq) r->seq.assign(host_seq, (size_t)win_len); else r->seq.clear();
+    CU(r->dev.reserve((size_t)win_len / 2 + 32), "cudaMalloc(reference)");
+    CU(cudaMemsetAsync(r->dev.p, 0xFF, (size_t)win_len / 2 + 32, s), "memset(reference)");
+    CU(launch_ref_encode(dev_ascii, r->dev.as<uint8_t>(), win_len, s), "reference encode");
+    std::vector<RefWin> tab(e->refs.size());
+    for (size_t i = 0; i < e->refs.size(); ++i)
+        tab[i] = RefWin{e->refs[i].dev.as<char>(), e->refs[i].chrom_len, e->refs[i].win_beg, e->refs[i].win_len};
+    CU(e->d_refs.reserve(tab.size() * sizeof(RefWin)), "cudaMalloc(refs)");
+    CU(cudaMemcpyAsync(e->d_refs.p, tab.data(), tab.size() * sizeof(RefWin), cudaMemcpyHostToDevice, s), "H2D refs");   // pageable source: staged before the call returns
+    return BRC_OK;
+}
 
 extern "C" {
 
@@ -91,11 +138,9 @@ void brc_destroy(brc_engine *e) {
     for (auto *b : pins) b->release();
     for (auto &ev : e->ev) if (ev) cudaEventDestroy(ev);
     for (auto &ev : e->pipe_ev) if (ev) cudaEventDestroy(ev);
-    for (auto &ev : e->tm_ev) if (ev) cudaEventDestroy(ev);
     if (e->s_in) cudaStreamDestroy(e->s_in);
     if (e->s_out) cudaStreamDestroy(e->s_out);
     if (e->s_sec) cudaStreamDestroy(e->s_sec);
-    if (e->s_in2) cudaStreamDestroy(e->s_in2);
     if (e->stream) cudaStreamDestroy(e->stream);
     delete e;
 }
@@ -104,29 +149,14 @@ int brc_set_reference(brc_engine *e, int32_t tid, const char *contig_name, int64
                       const char *seq, int64_t win_len) {
     if (!e || !seq || win_len < 0 || win_beg < 0 || chrom_len < 0) return BRC_E_INVALID;
     cudaSetDevice(e->cfg.device);
-    HostRef *r = nullptr;
-    for (auto &x : e->refs) if (x.tid == tid) r = &x;
-    if (!r) { e->refs.emplace_back(); r = &e->refs.back(); }
-    r->tid = tid; r->name = contig_name ? contig_name : ""; r->chrom_len = chrom_len; r->win_beg = win_beg; r->win_len = win_len;
-    r->seq.assign(seq, (size_t)win_len);
-    CU(r->dev.reserve((size_t)win_len / 2 + 32), "cudaMalloc(reference)");
-    CU(cudaMemsetAsync(r->dev.p, 0xFF, (size_t)win_len / 2 + 32, e->stream), "memset(reference)");
-    {   // upload the FASTA characters, keep only their 4-bit codes on the device (K0 compares nibbles)
-        DevBuf ascii;
-        CU(ascii.reserve((size_t)win_len + 16), "cudaMalloc(reference ascii)");
-        cudaError_t ce = cudaMemcpyAsync(ascii.p, r->seq.data(), (size_t)win_len, cudaMemcpyHostToDevice, e->stream);
-        if (ce == cudaSuccess) ce = launch_ref_encode(ascii.as<char>(), r->dev.as<uint8_t>(), win_len, e->stream);
-        if (ce == cudaSuccess) ce = cudaStreamSynchronize(e->stream);
-        ascii.release();
-        if (ce != cudaSuccess) return set_cuda_error(e, ce, "reference upload/encode");
-    }
-    // refresh the device RefWin table
-    std::vector<RefWin> tab(e->refs.size());
-    for (size_t i = 0; i < e->refs.size(); ++i)
-        tab[i] = RefWin{e->refs[i].dev.as<char>(), e->refs[i].chrom_len, e->refs[i].win_beg, e->refs[i].win_len};
-    CU(e->d_refs.reserve(tab.size() * sizeof(RefWin)), "cudaMalloc(refs)");
-    CU(cudaMemcpy(e->d_refs.p, tab.data(), tab.size() * sizeof(RefWin), cudaMemcpyHostToDevice), "H2D refs");
-    return BRC_OK;
+    DevBuf ascii;   // the FASTA characters cross once; the device keeps only their 4-bit codes
+    cudaError_t ce = ascii.reserve((size_t)win_len + 16);
+    if (ce == cudaSuccess) ce = cudaMemcpyAsync(ascii.p, seq, (size_t)win_len, cudaMemcpyHostToDevice, e->stream);
+    int rc = ce != cudaSuccess ? set_cuda_error(e, ce, "reference upload")
+                               : install_ref(e, tid, contig_name, chrom_len, win_beg, win_len, seq, ascii.as<char>(), e->stream);
+    if ((ce = cudaStreamSynchronize(e->stream)) != cudaSuccess && rc == BRC_OK) rc = set_cuda_error(e, ce, "reference upload/encode");
+    ascii.release();
+    return rc;
 }
 
 // Reference window already in DEVICE memory as ASCII (a generator or a device-side FASTA decoder wrote it): encoded on `stream`,
@@ -135,26 +165,11 @@ int brc_set_reference_device(brc_engine *e, int32_t tid, const char *contig_name
                              const char *dev_ascii, int64_t win_len, void *stream) {
     if (!e || !dev_ascii || win_len < 0 || win_beg < 0 || chrom_len < 0) return BRC_E_INVALID;
     cudaSetDevice(e->cfg.device);
-    cudaStream_t s = (cudaStream_t)stream;
-    HostRef *r = nullptr;
-    for (auto &x : e->refs) if (x.tid == tid) r = &x;
-    if (!r) { e->refs.emplace_back(); r = &e->refs.back(); }
-    r->tid = tid; r->name = contig_name ? contig_name : ""; r->chrom_len = chrom_len; r->win_beg = win_beg; r->win_len = win_len;
-    r->seq.clear();
-    CU(r->dev.reserve((size_t)win_len / 2 + 32), "cudaMalloc(reference)");
-    CU(cudaMemsetAsync(r->dev.p, 0xFF, (size_t)win_len / 2 + 32, s), "memset(reference)");
-    CU(launch_ref_encode(dev_ascii, r->dev.as<uint8_t>(), win_len, s), "reference encode");
-    std::vector<RefWin> tab(e->refs.size());
-    for (size_t i = 0; i < e->refs.size(); ++i)
-        tab[i] = RefWin{e->refs[i].dev.as<char>(), e->refs[i].chrom_len, e->refs[i].win_beg, e->refs[i].win_len};
-    CU(e->d_refs.reserve(tab.size() * sizeof(RefWin)), "cudaMalloc(refs)");
-    CU(cudaMemcpyAsync(e->d_refs.p, tab.data(), tab.size() * sizeof(RefWin), cudaMemcpyHostToDevice, s), "H2D refs");   // pageable source: staged before the call returns
-    return BRC_OK;
+    return install_ref(e, tid, contig_name, chrom_len, win_beg, win_len, nullptr, dev_ascii, (cudaStream_t)stream);
 }
 
 int brc_reset(brc_engine *e) {
     if (!e) return BRC_E_INVALID;
-    if (e->h2d_chunks) { cudaSetDevice(e->cfg.device); cudaStreamSynchronize(e->s_in); cudaStreamSynchronize(e->s_in2); e->h2d_chunks = 0; }
     e->reads.clear(); e->is_borrowed = false; e->regions.clear(); e->region_open = false; e->adm.reset(); e->n_indel_ops = 0;
     e->results_valid = false; e->planned = false; e->tiles.clear(); e->regions_dev.clear(); e->n_slots = 0; e->wide.valid = false;
     e->dec.pushed = false; e->dec.ins_reads.clear(); e->dec.ins_off.clear(); e->dec.ins_pool.clear();
@@ -164,7 +179,6 @@ int brc_reset(brc_engine *e) {
 
 // A borrowed batch becomes an owned copy (bulk memcpy) as soon as anything else is pushed after it.
 static void materialize_borrowed(brc_engine *e) {
-    if (e->h2d_chunks) { cudaStreamSynchronize(e->s_in); cudaStreamSynchronize(e->s_in2); e->h2d_chunks = 0; }
     const brc_read_batch &B = e->borrowed;
     HostReads &H = e->reads;
     const size_t n = (size_t)B.n_reads;
@@ -185,12 +199,8 @@ static void materialize_borrowed(brc_engine *e) {
         A.reset();
         A.max_tid = A.it_tid = e->regions.back().tid; A.max_pos = A.it_pos = H.pos[n - 1];
         for (size_t i = 0; i < n; ++i) {
-            int64_t l = 0;
-            for (uint64_t k = H.cigar_off[i]; k < H.cigar_off[i + 1]; ++k) {
-                const uint32_t op = H.cigar[k] & 0xF;
-                if (op == 0 || op == 2 || op == 3 || op == 7 || op == 8) l += H.cigar[k] >> 4;
-            }
-            const int64_t end = H.cigar_off[i + 1] > H.cigar_off[i] ? (int64_t)H.pos[i] + l : (int64_t)H.pos[i] + 1;
+            const uint64_t nc = H.cigar_off[i + 1] - H.cigar_off[i];
+            const int64_t end = nc ? (int64_t)H.pos[i] + cigar_rlen(H.cigar.data() + H.cigar_off[i], nc) : (int64_t)H.pos[i] + 1;
             if (end >= A.it_pos) A.live_ends.push(end);
         }
     }
@@ -209,16 +219,6 @@ int brc_begin_region(brc_engine *e, int32_t tid, int32_t beg, int32_t end, int32
     e->region_open = true; e->adm.reset(); e->open_max_end = r.first_pos;
     e->results_valid = false; e->planned = false;
     return BRC_OK;
-}
-
-static inline int64_t cigar_rlen(const uint32_t *cig, uint32_t n, int64_t *n_indel) {
-    int64_t l = 0;
-    for (uint32_t k = 0; k < n; ++k) {
-        uint32_t op = cig[k] & 0xF;
-        if (op == 0 || op == 2 || op == 3 || op == 7 || op == 8) l += cig[k] >> 4;
-        if (op == 1 || op == 2) ++*n_indel;
-    }
-    return l;
 }
 
 int brc_push_read(brc_engine *e, int32_t tid, int32_t pos, uint16_t flag, uint8_t mapq, uint16_t lib, int32_t l_qseq,
@@ -261,11 +261,8 @@ int brc_push_read(brc_engine *e, int32_t tid, int32_t pos, uint16_t flag, uint8_
     return BRC_OK;
 }
 
-static int issue_h2d_chunks(brc_engine *e);
-
 // Parallel scan of a batch: are all reads admitted by the pileup buffer as they are (so the batch can be used in
 // place), and what is the largest bam_endpos?  The -d rule cannot fire when the whole batch is smaller than max_cnt.
-static double wall_ms_fwd() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
 struct BatchScan {
     bool ok = true; int64_t max_end = 0; int64_t indel_ops = 0;
     // arrays the device can rebuild instead of receiving (fixed-length reads): offsets that are arithmetic, constant columns
@@ -273,10 +270,9 @@ struct BatchScan {
 };
 static BatchScan scan_batch(const brc_read_batch *b, int32_t rtid, int per_lib, int n_rows) {
     const int64_t n = b->n_reads;
-    unsigned hw = std::thread::hardware_concurrency();
-    const int nt = (int)std::max<int64_t>(1, std::min<int64_t>({(int64_t)(hw ? hw : 1), (int64_t)16, n / 65536 + 1}));
+    const int nt = worker_count(n, 65536, 16);
     std::vector<BatchScan> part((size_t)nt);
-    auto work = [&](int t) {
+    fan_out(nt, [&](int t) {
         const int64_t lo = n * t / nt, hi = n * (t + 1) / nt;
         BatchScan r;
         const uint64_t s0 = b->seq_off[0], q0 = b->qual_off[0];
@@ -290,6 +286,8 @@ static BatchScan scan_batch(const brc_read_batch *b, int32_t rtid, int per_lib, 
             if ((b->tid && b->tid[i] != rtid) || (b->flag[i] & 4)) { r.ok = false; break; }
             if (i > 0 && b->pos[i] < b->pos[i - 1]) { r.ok = false; break; }
             if (per_lib && b->lib && b->lib[i] != BRC_LIB_NONE && (int)b->lib[i] >= n_rows) { r.ok = false; break; }
+            // cigar_rlen written out: calling it here made the C3 push path (e2e leg) about 2.5 ms per window slower
+            // (22.7 -> 25.2 ms, H100 80GB HBM3 at 400 W), although its inner loop compiles the same
             const uint64_t c0 = b->cigar_off[i], c1 = b->cigar_off[i + 1];
             int64_t l = 0;
             for (uint64_t k = c0; k < c1; ++k) {
@@ -302,11 +300,7 @@ static BatchScan scan_batch(const brc_read_batch *b, int32_t rtid, int per_lib, 
             if (end > r.max_end) r.max_end = end;
         }
         part[(size_t)t] = r;
-    };
-    std::vector<std::thread> th;
-    for (int t = 1; t < nt; ++t) th.emplace_back(work, t);
-    work(0);
-    for (auto &x : th) x.join();
+    });
     BatchScan out;
     for (auto &r : part) {
         out.ok = out.ok && r.ok; out.max_end = std::max(out.max_end, r.max_end); out.indel_ops += r.indel_ops;
@@ -317,7 +311,6 @@ static BatchScan scan_batch(const brc_read_batch *b, int32_t rtid, int per_lib, 
 
 int brc_push_reads(brc_engine *e, const brc_read_batch *b) {
     if (!e || !b) return BRC_E_INVALID;
-    const double tp0 = wall_ms_fwd();
     if (!e->region_open) return set_error(e, BRC_E_INVALID, "push_reads: no open region");
     if (e->is_borrowed) materialize_borrowed(e);
     brc_region &rg = e->regions.back();
@@ -327,14 +320,7 @@ int brc_push_reads(brc_engine *e, const brc_read_batch *b) {
     // keep a VIEW of the caller's arrays — brc_compute DMAs straight out of them (pin them for full PCIe speed).
     if (e->regions.size() == 1 && e->reads.n() == 0 && b->n_reads > 0 && b->n_reads < (int64_t)e->cfg.max_cnt &&
         b->n_reads < 0x7fffffffLL && e->adm.max_pos < 0) {
-        // Optional (BRC_EARLY_H2D=1): start the copies before the admission scan.  The uploads then run ahead alone and the result
-        // download has the link to itself at the end, instead of both directions streaming concurrently for the whole step — so the
-        // default issues H2D from brc_compute.
-        e->borrowed = *b; e->h2d_chunks = 0; e->skip_h2d = 0;
-        cudaSetDevice(e->cfg.device);
-        const bool early = std::getenv("BRC_EARLY_H2D") && issue_h2d_chunks(e) == BRC_OK;
         const BatchScan sc = scan_batch(b, rtid, e->cfg.per_lib, e->n_rows);
-        if (std::getenv("BRC_PIPE_TIMING")) std::fprintf(stderr, "[brc pipe] scan_batch %.2f ms\n", wall_ms_fwd() - tp0);
         if (sc.ok) {
             e->skip_h2d = (sc.reg_seq ? 1 : 0) | (sc.reg_qual ? 2 : 0) | (sc.const_lq ? 4 : 0) | (sc.const_sm ? 8 : 0);
             if (std::getenv("BRC_NO_H2D_ELISION") || b->n_reads < 2) e->skip_h2d = 0;
@@ -344,8 +330,6 @@ int brc_push_reads(brc_engine *e, const brc_read_batch *b) {
             rg.read_hi = b->n_reads;
             return BRC_OK;
         }
-        if (early) { cudaStreamSynchronize(e->s_in); cudaStreamSynchronize(e->s_in2); }   // not usable as is: drop the speculative upload, take the copying path
-        e->h2d_chunks = 0;
     }
     for (int64_t i = 0; i < b->n_reads; ++i) {
         const uint64_t c0 = b->cigar_off[i], c1 = b->cigar_off[i + 1];
@@ -470,8 +454,7 @@ static void make_params(brc_engine *e, const int32_t *d_region_of_read, Precompu
     P1.tiles = e->d_tiles.as<TileInfo>(); P1.tile_lo = P0.tile_lo; P1.tile_hi = P0.tile_hi; P1.n_tiles = (int64_t)e->tiles.size(); P1.tile_begin = 0; P1.tile_count = P1.n_tiles;
     P1.res = results_dev(e);
     P1.deep_tiles = e->deep_tiles.empty() ? nullptr : e->d_deep_tiles.as<int32_t>(); P1.n_deep = (int32_t)e->deep_tiles.size(); P1.deep_min_reads = e->deep_min_reads;
-    static const bool fixed_stride = std::getenv("BRC_K1_STATIC_TILES") != nullptr;      // A/B switch
-    P1.work_counter = fixed_stride ? nullptr : P1.res.warn + WARN_WORDS;                 // launch k of a run takes dispenser k
+    P1.work_counter = P1.res.warn + WARN_WORDS;                 // launch k of a run takes dispenser k
 }
 
 // K(init) + K0 + K1 on stream s.  Returns BRC_E_OVERFLOW (after syncing) if the secondary pool was too small.
@@ -520,6 +503,22 @@ static int fetch_results(brc_engine *e, cudaStream_t s, bool slots_already_fetch
     return BRC_OK;
 }
 
+// The kernels on the batch e->dev_reads, then the results to the host.  The secondary pool starts at `cap` records and
+// doubles while it overflows, for at most 8 runs.
+static int compute_batch(brc_engine *e, int64_t cap, const int32_t *d_region_of_read, cudaStream_t s) {
+    int rc = upload_geometry(e, s);
+    if (rc != BRC_OK) return rc;
+    for (int attempt = 0; attempt < 8; ++attempt) {
+        rc = alloc_sec(e, cap);
+        if (rc != BRC_OK) return rc;
+        rc = run_kernels(e, d_region_of_read, s, true);
+        if (rc != BRC_E_OVERFLOW) break;
+        cap = std::max<int64_t>(cap * 2, e->h_n_sec + 1024);
+    }
+    if (rc != BRC_OK) return rc == BRC_E_OVERFLOW ? set_error(e, rc, "secondary key pool overflow") : rc;
+    return fetch_results(e, s);
+}
+
 // ---------------------------------------------------------------------------------------------
 // packed host records -> the full-width arrays of brc_results (include/brc_engine.h)
 // ---------------------------------------------------------------------------------------------
@@ -532,9 +531,8 @@ void ensure_wide(brc_engine *e) {
     const SecRec *sec = e->h_sec.as<SecRec>();
     W.ncover.resize((size_t)rs); W.npass.resize((size_t)rs); W.flags.resize((size_t)rs); W.pbase.resize((size_t)rs);
     W.sec_head.resize((size_t)rs); W.pstats.resize((size_t)rs * N_STATS);
-    unsigned hw = std::thread::hardware_concurrency();
-    const int nt = (int)std::max<int64_t>(1, std::min<int64_t>({(int64_t)(hw ? hw : 1), (int64_t)16, rs / 262144 + 1}));
-    auto work = [&](int t) {
+    const int nt = worker_count(rs, 262144, 16);
+    fan_out(nt, [&](int t) {
         const int64_t lo = rs * t / nt, hi = rs * (t + 1) / nt;
         uint32_t *ps = W.pstats.data();
         for (int64_t i = lo; i < hi; ++i) {
@@ -548,11 +546,7 @@ void ensure_wide(brc_engine *e) {
             ps[8 * rs + i] = w3 >> 16; ps[9 * rs + i] = (w1 >> 8) & 0xFFu; ps[10 * rs + i] = words[6 * rs + i]; ps[11 * rs + i] = w3 & 0xFFFFu;
             ps[12 * rs + i] = words[7 * rs + i];
         }
-    };
-    std::vector<std::thread> th;
-    for (int t = 1; t < nt; ++t) th.emplace_back(work, t);
-    work(0);
-    for (auto &x : th) x.join();
+    });
     // secondary records: keys are chained per slot (order is immaterial to every consumer); escaped primaries fill their slot
     const size_t n1 = (size_t)std::max<int64_t>(ns, 1);
     W.sec_next.assign(n1, -1); W.sec_kind.assign(n1, 0); W.sec_len.assign(n1, 0); W.sec_read.assign(n1, 0); W.sec_qpos.assign(n1, 0);
@@ -583,26 +577,25 @@ void ensure_wide(brc_engine *e) {
 // chunk c+1, the kernels of chunk c and the D2H copy of the finished tiles of chunk c-1 overlap (PCIe is full
 // duplex; three streams + events).  Reads are position-sorted, so every tile that ends at or before the first
 // position of chunk c+1 is complete once chunk c is on the device.
-static double wall_ms() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
 
-// Device buffers + chunked H2D of a borrowed batch on s_in; records pipe_ev[2c] after chunk c.  Called speculatively from
-// brc_push_reads (so the copies overlap the admission scan and the caller's remaining host work) or from brc_compute.
-static int issue_h2d_chunks(brc_engine *e) {
+// Device buffers + chunked H2D of the borrowed batch on s_in; records pipe_ev[2c] after chunk c.  The copies are issued here,
+// from brc_compute, and not from brc_push_reads ahead of its admission scan: an upload started that early runs ahead alone and
+// leaves the result download alone on the link at the end, where issued with the kernels both directions stream concurrently
+// for the whole step.
+static int issue_h2d_chunks(brc_engine *e, int &n_chunks) {
     const brc_read_batch &B = e->borrowed;
     const int64_t n = B.n_reads;
     if (!e->s_in) CU(cudaStreamCreateWithFlags(&e->s_in, cudaStreamNonBlocking), "stream");
-    if (!e->s_in2) CU(cudaStreamCreateWithFlags(&e->s_in2, cudaStreamNonBlocking), "stream");
     if (!e->s_out) CU(cudaStreamCreateWithFlags(&e->s_out, cudaStreamNonBlocking), "stream");
     const uint64_t n_cig = B.cigar_off[n], n_seq = B.seq_off[n], n_qual = B.qual_off[n];
     const size_t tot[13] = {(size_t)n * 4, (size_t)n * 2, (size_t)n, (size_t)n * 2, (size_t)n * 4, (size_t)n * 4, (size_t)n * 4,
                             (size_t)(n + 1) * 8, (size_t)n_cig * 4, (size_t)(n + 1) * 8, (size_t)n_seq, (size_t)(n + 1) * 8, (size_t)n_qual};
     for (int k = 0; k < 13; ++k) CU(e->d_in[k].reserve(tot[k] + 16), "cudaMalloc(reads)");
     size_t in_bytes = 0; for (int k = 0; k < 13; ++k) in_bytes += tot[k];
-    int n_chunks = (int)std::min<int64_t>(32, std::max<int64_t>(1, (int64_t)(in_bytes >> 26)));   // ~64 MiB of input per chunk
+    n_chunks = (int)std::min<int64_t>(32, std::max<int64_t>(1, (int64_t)(in_bytes >> 26)));   // ~64 MiB of input per chunk
     n_chunks = (int)std::min<int64_t>(n_chunks, std::max<int64_t>(1, n / 4096));
     if (const char *ov = std::getenv("BRC_PIPE_CHUNKS")) n_chunks = (int)std::max<int64_t>(1, std::min<int64_t>(std::atoi(ov), std::max<int64_t>(1, n)));   // test hook
-    while (e->pipe_ev.size() < (size_t)(4 * n_chunks + 2)) { cudaEvent_t ev; CU(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming), "event"); e->pipe_ev.push_back(ev); }
-    const bool two_streams = std::getenv("BRC_H2D_TWO_STREAMS") != nullptr;
+    while (e->pipe_ev.size() < (size_t)(3 * n_chunks + 2)) { cudaEvent_t ev; CU(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming), "event"); e->pipe_ev.push_back(ev); }
     // fixed-length reads: arithmetic offsets and constant columns are rebuilt on the device instead of crossing PCIe
     // (24 of the 277 bytes a 150 bp read costs: brc_push_reads' admission scan found them regular)
     const int skip = e->skip_h2d;
@@ -610,52 +603,40 @@ static int issue_h2d_chunks(brc_engine *e) {
     if (skip & 2) CU(launch_fill_offsets(e->d_in[11].as<uint64_t>(), n + 1, B.qual_off[0], B.qual_off[1] - B.qual_off[0], e->s_in), "fill qual_off");
     if (skip & 4) CU(launch_fill_i32(e->d_in[4].as<int32_t>(), n, B.l_qseq[0], e->s_in), "fill l_qseq");
     if (skip & 8) CU(launch_fill_i32(e->d_in[6].as<int32_t>(), n, B.sm[0], e->s_in), "fill sm");
-    const bool tm = std::getenv("BRC_PIPE_TIMING") != nullptr;
-    if (tm) { for (auto &ev : e->tm_ev) if (!ev) CU(cudaEventCreate(&ev), "event"); CU(cudaEventRecord(e->tm_ev[0], e->s_in), "event"); }
-    if (!B.lib) CU(cudaMemsetAsync(e->d_in[3].p, 0, (size_t)n * 2, two_streams ? e->s_in2 : e->s_in), "memset lib");
+    if (!B.lib) CU(cudaMemsetAsync(e->d_in[3].p, 0, (size_t)n * 2, e->s_in), "memset lib");
     // Copy order: a small cudaMemcpyAsync costs a fixed slice of link time whatever its size, so the eleven small arrays are sent
     // WHOLE, once (<= 11 copies), and only the two big byte pools are cut into chunks that the kernels and the result copies follow.
+    // All of it goes on s_in, so each chunk's event also follows the small arrays.
     e->h2d_bytes_last = 0;
-    #define H2D(st, k, host, off, cnt, esz) if ((cnt) > 0) { e->h2d_bytes_last += (int64_t)(cnt) * (int64_t)(esz); CU(cudaMemcpyAsync((char *)e->d_in[k].p + (size_t)(off) * (esz), (const char *)(host) + (size_t)(off) * (esz), (size_t)(cnt) * (esz), cudaMemcpyHostToDevice, st), "H2D"); }
-    {
-        cudaStream_t s_small = two_streams ? e->s_in2 : e->s_in;
-        H2D(s_small, 0, B.pos, 0, n, 4); H2D(s_small, 1, B.flag, 0, n, 2); H2D(s_small, 2, B.mapq, 0, n, 1);
-        if (B.lib) H2D(s_small, 3, B.lib, 0, n, 2);
-        if (!(skip & 4)) H2D(s_small, 4, B.l_qseq, 0, n, 4);
-        H2D(s_small, 5, B.nm, 0, n, 4);
-        if (!(skip & 8)) H2D(s_small, 6, B.sm, 0, n, 4);
-        H2D(s_small, 7, B.cigar_off, 0, n + 1, 8); H2D(s_small, 8, B.cigar, B.cigar_off[0], B.cigar_off[n] - B.cigar_off[0], 4);
-        if (!(skip & 1)) H2D(s_small, 9, B.seq_off, 0, n + 1, 8);
-        if (!(skip & 2)) H2D(s_small, 11, B.qual_off, 0, n + 1, 8);
-        for (int c = 0; c < n_chunks; ++c) CU(cudaEventRecord(e->pipe_ev[3 * n_chunks + 2 + c], s_small), "event");   // (two-stream switch: every chunk waits for them)
-    }
+    #define H2D(k, host, off, cnt, esz) if ((cnt) > 0) { e->h2d_bytes_last += (int64_t)(cnt) * (int64_t)(esz); CU(cudaMemcpyAsync((char *)e->d_in[k].p + (size_t)(off) * (esz), (const char *)(host) + (size_t)(off) * (esz), (size_t)(cnt) * (esz), cudaMemcpyHostToDevice, e->s_in), "H2D"); }
+    H2D(0, B.pos, 0, n, 4); H2D(1, B.flag, 0, n, 2); H2D(2, B.mapq, 0, n, 1);
+    if (B.lib) H2D(3, B.lib, 0, n, 2);
+    if (!(skip & 4)) H2D(4, B.l_qseq, 0, n, 4);
+    H2D(5, B.nm, 0, n, 4);
+    if (!(skip & 8)) H2D(6, B.sm, 0, n, 4);
+    H2D(7, B.cigar_off, 0, n + 1, 8); H2D(8, B.cigar, B.cigar_off[0], B.cigar_off[n] - B.cigar_off[0], 4);
+    if (!(skip & 1)) H2D(9, B.seq_off, 0, n + 1, 8);
+    if (!(skip & 2)) H2D(11, B.qual_off, 0, n + 1, 8);
     for (int c = 0; c < n_chunks; ++c) {
         const int64_t a = n * c / n_chunks, b = n * (c + 1) / n_chunks;
-        H2D(e->s_in, 12, B.qual, B.qual_off[a], B.qual_off[b] - B.qual_off[a], 1);
-        H2D(e->s_in, 10, B.seq, B.seq_off[a], B.seq_off[b] - B.seq_off[a], 1);
+        H2D(12, B.qual, B.qual_off[a], B.qual_off[b] - B.qual_off[a], 1);
+        H2D(10, B.seq, B.seq_off[a], B.seq_off[b] - B.seq_off[a], 1);
         CU(cudaEventRecord(e->pipe_ev[2 * c], e->s_in), "event");
     }
     #undef H2D
-    if (tm) CU(cudaEventRecord(e->tm_ev[1], e->s_in), "event");
-    e->h2d_chunks = n_chunks;
     return BRC_OK;
 }
 
 static int compute_pipelined(brc_engine *e) {
-    const bool timing = std::getenv("BRC_PIPE_TIMING") != nullptr;
-    const double t0 = wall_ms();
     const brc_read_batch &B = e->borrowed;
     const int64_t n = B.n_reads;
     const brc_region &rg = e->regions[0];
     const int64_t n_tiles = (int64_t)e->tiles.size();
     const int64_t rs = (int64_t)e->n_rows * e->n_slots;
-    if (e->h2d_chunks == 0) { int rc0 = issue_h2d_chunks(e); if (rc0 != BRC_OK) return rc0; }
-    const int n_chunks = e->h2d_chunks;
-    ReadsDev &R = e->dev_reads;
-    R.n_reads = n; R.pos = e->d_in[0].as<int32_t>(); R.flag = e->d_in[1].as<uint16_t>(); R.mapq = e->d_in[2].as<uint8_t>();
-    R.lib = e->d_in[3].as<uint16_t>(); R.l_qseq = e->d_in[4].as<int32_t>(); R.nm = e->d_in[5].as<int32_t>(); R.sm = e->d_in[6].as<int32_t>();
-    R.cigar_off = e->d_in[7].as<uint64_t>(); R.cigar = e->d_in[8].as<uint32_t>(); R.seq_off = e->d_in[9].as<uint64_t>();
-    R.seq = e->d_in[10].as<uint8_t>(); R.qual_off = e->d_in[11].as<uint64_t>(); R.qual = e->d_in[12].as<uint8_t>();
+    int n_chunks = 0;
+    int rc = issue_h2d_chunks(e, n_chunks);
+    if (rc != BRC_OK) return rc;
+    e->dev_reads = reads_dev(d_in_batch(e, n));
     // host result buffers
     const int64_t rs1 = std::max<int64_t>(rs, 1);
     CU(e->h_words.reserve(rs1 * 4 * N_WORDS), "pin");
@@ -677,7 +658,6 @@ static int compute_pipelined(brc_engine *e) {
         const int64_t a = n * c / n_chunks, b = n * (c + 1) / n_chunks;
         // ---- kernels: K0 on the chunk, K1 on the tiles it completes ----
         CU(cudaStreamWaitEvent(sk, e->pipe_ev[2 * c], 0), "wait");
-        CU(cudaStreamWaitEvent(sk, e->pipe_ev[3 * n_chunks + 2 + c], 0), "wait");
         P0.read_begin = a; P0.read_end = b;
         CU(launch_precompute(P0, sk), "launch read_precompute"); e->launch_count++;
         int64_t tile_to = n_tiles;
@@ -699,14 +679,13 @@ static int compute_pipelined(brc_engine *e) {
             }
             // ---- D2H of the finished slots ----
             CU(cudaStreamWaitEvent(e->s_out, e->pipe_ev[2 * c + 1], 0), "wait");
-            if (timing && tile_done == 0) CU(cudaEventRecord(e->tm_ev[2], e->s_out), "event");
             const int64_t s0 = e->tiles[(size_t)tile_done].slot0;
             const int64_t s1 = tile_to < n_tiles ? e->tiles[(size_t)tile_to].slot0 : e->n_slots;
             const size_t w = (size_t)(s1 - s0);
             const size_t pitch4 = (size_t)e->n_slots * 4;
             const int rows = e->n_rows;
             // the finished slots of all N_WORDS x rows word arrays: one plain copy per array (one strided 2-D copy for many library rows)
-            if (!std::getenv("BRC_D2H_2D") && rows * N_WORDS <= 64) {      // plain copies beat one strided 2-D copy (r02e: 17.0 vs 18.4 ms per window)
+            if (rows * N_WORDS <= 64) {      // plain copies beat one strided 2-D copy (r02e: 17.0 vs 18.4 ms per window)
                 for (int k = 0; k < rows * N_WORDS; ++k)
                     CU(cudaMemcpyAsync((char *)e->h_words.p + (size_t)k * pitch4 + s0 * 4, (char *)e->d_words.p + (size_t)k * pitch4 + s0 * 4, w * 4, cudaMemcpyDeviceToHost, e->s_out), "D2H");
             } else
@@ -714,7 +693,6 @@ static int compute_pipelined(brc_engine *e) {
             tile_done = tile_to;
         }
     }
-    const double t1 = wall_ms();
     CU(cudaEventRecord(e->ev[1], sk), "event");
     CU(cudaEventRecord(e->ev[2], sk), "event");
     // everything is queued: follow the kernels and ship the pool records each chunk finished (their own stream: the word copies
@@ -730,23 +708,11 @@ static int compute_pipelined(brc_engine *e) {
         }
     }
     CU(cudaStreamSynchronize(e->s_in), "sync H2D");
-    CU(cudaStreamSynchronize(e->s_in2), "sync H2D");
-    const double t2 = wall_ms();
     CU(cudaStreamSynchronize(sk), "sync kernels");
-    const double t3 = wall_ms();
     CU(cudaStreamSynchronize(e->s_out), "sync D2H");
-    const double t4 = wall_ms();
-    if (timing) {
-        float h2d_ms = 0, d2h_ms = 0, lag_ms = 0;
-        cudaEventRecord(e->tm_ev[3], e->s_out); cudaEventSynchronize(e->tm_ev[3]);
-        cudaEventElapsedTime(&h2d_ms, e->tm_ev[0], e->tm_ev[1]); cudaEventElapsedTime(&d2h_ms, e->tm_ev[2], e->tm_ev[3]); cudaEventElapsedTime(&lag_ms, e->tm_ev[0], e->tm_ev[2]);
-        std::fprintf(stderr, "[brc pipe] device clocks: H2D stream busy %.2f ms, first D2H starts +%.2f ms after the first H2D, D2H span %.2f ms\n", h2d_ms, lag_ms, d2h_ms);
-    }
-    if (timing) std::fprintf(stderr, "[brc pipe] chunks %d  enqueue %.2f ms  H2D done +%.2f  kernels done +%.2f  D2H done +%.2f (ms since compute start)\n", n_chunks, t1 - t0, t2 - t0, t3 - t0, t4 - t0);
     int32_t cnt = 0;
     CU(cudaMemcpy(&cnt, e->d_sec_count.p, 4, cudaMemcpyDeviceToHost), "D2H sec_count");
     e->h_n_sec = cnt;
-    e->h2d_chunks = 0;
     CU(cudaStreamSynchronize(e->s_sec), "sync D2H sec");
     if ((int64_t)cnt > e->sec_cap) return BRC_E_OVERFLOW;
     return fetch_results(e, sk, true, sec_done);
@@ -766,36 +732,20 @@ int brc_compute(brc_engine *e) {
         const brc_read_batch &b = e->dec.batch;
         rc = alloc_outputs(e, b.n_reads);
         if (rc != BRC_OK) return rc;
-        cudaStream_t sd = e->stream;
-        ReadsDev &R = e->dev_reads;
-        R.n_reads = b.n_reads; R.pos = b.pos; R.flag = b.flag; R.mapq = b.mapq; R.lib = b.lib; R.l_qseq = b.l_qseq; R.nm = b.nm; R.sm = b.sm;
-        R.cigar_off = b.cigar_off; R.cigar = b.cigar; R.seq_off = b.seq_off; R.seq = b.seq; R.qual_off = b.qual_off; R.qual = b.qual;
-        rc = upload_geometry(e, sd);
+        e->dev_reads = reads_dev(b);
+        rc = compute_batch(e, std::max<int64_t>(e->sec_cap, (int64_t)e->n_rows * e->n_slots / 6 + b.n_reads / 8 + 1024), nullptr, e->stream);
         if (rc != BRC_OK) return rc;
-        int64_t capd = std::max<int64_t>(e->sec_cap, (int64_t)e->n_rows * e->n_slots / 6 + b.n_reads / 8 + 1024);
-        for (int attempt = 0; attempt < 8; ++attempt) {
-            rc = alloc_sec(e, capd);
-            if (rc != BRC_OK) return rc;
-            rc = run_kernels(e, nullptr, sd, true);
-            if (rc != BRC_E_OVERFLOW) break;
-            capd = std::max<int64_t>(capd * 2, e->h_n_sec + 1024);
-        }
-        if (rc != BRC_OK) return rc == BRC_E_OVERFLOW ? set_error(e, rc, "secondary key pool overflow") : rc;
-        rc = fetch_results(e, sd);
-        if (rc != BRC_OK) return rc;
-        return brc::fetch_insertion_reads(e, sd);
+        return brc::fetch_insertion_reads(e, e->stream);
     }
-    HostReads &H = e->reads;
     const bool bw = e->is_borrowed;
-    const brc_read_batch &B = e->borrowed;
-    const int64_t n = e->n_host_reads();
-    const int32_t *h_pos = bw ? B.pos : H.pos.data();
+    brc_read_batch src = e->host_batch();
+    const int64_t n = src.n_reads;
     // reference window must cover every read's span (K0 reads it; the emitter reads deletion alleles)
     for (const brc_region &r : e->regions) {
         const HostRef *hr = find_ref(e, r.tid);
         if (!hr) return set_error(e, BRC_E_NO_REFERENCE, "no reference for contig");
         if (r.read_hi > r.read_lo) {
-            int64_t lo = h_pos[(size_t)r.read_lo], hi = (int64_t)r.first_pos + r.n_slots;
+            int64_t lo = src.pos[(size_t)r.read_lo], hi = (int64_t)r.first_pos + r.n_slots;
             lo = std::max<int64_t>(0, std::min<int64_t>(lo, r.first_pos));
             hi = std::min(hi, hr->chrom_len);
             if (lo < hr->win_beg || hi > hr->win_beg + hr->win_len)
@@ -805,56 +755,33 @@ int brc_compute(brc_engine *e) {
     rc = alloc_outputs(e, n);
     if (rc != BRC_OK) return rc;
     cudaStream_t s = e->stream;
+    const int64_t cap = std::max<int64_t>(e->sec_cap, (int64_t)e->n_rows * e->n_slots / 8 + 2 * e->n_indel_ops + 1024);
     if (bw && e->regions.size() == 1 && n > 0 && !e->tiles.empty()) {
         rc = upload_geometry(e, s);
         if (rc != BRC_OK) return rc;
-        int64_t cap0 = std::max<int64_t>(e->sec_cap, (int64_t)e->n_rows * e->n_slots / 8 + 2 * e->n_indel_ops + 1024);
-        rc = alloc_sec(e, cap0);
+        rc = alloc_sec(e, cap);
         if (rc != BRC_OK) return rc;
         rc = compute_pipelined(e);
+        if (rc != BRC_OK && e->s_in) cudaStreamSynchronize(e->s_in);   // on an error return too, no copy from the caller's buffers outlives this call
         if (rc != BRC_E_OVERFLOW) return rc;
-        // pool too small: everything is on the device already; fall through to the plain path with a larger pool
+        // pool too small: fall through to the plain path, which grows the pool
     }
-    if (e->h2d_chunks) { cudaStreamSynchronize(e->s_in); cudaStreamSynchronize(e->s_in2); e->h2d_chunks = 0; }   // a speculative upload is not used on this path
     // H2D of the read arrays (borrowed batches: straight from the caller's buffers)
-    std::vector<uint16_t> zero_lib;
-    const uint16_t *h_lib = bw ? B.lib : H.lib.data();
-    if (bw && !B.lib) { zero_lib.assign((size_t)n, 0); h_lib = zero_lib.data(); }
-    const uint64_t n_cig = bw ? B.cigar_off[n] : (uint64_t)H.cigar.size();
-    const uint64_t n_seq = bw ? B.seq_off[n] : (uint64_t)H.seq.size();
-    const uint64_t n_qual = bw ? B.qual_off[n] : (uint64_t)H.qual.size();
-    const void *src[14] = {h_pos, bw ? (const void *)B.flag : H.flag.data(), bw ? (const void *)B.mapq : H.mapq.data(), h_lib,
-                           bw ? (const void *)B.l_qseq : H.l_qseq.data(), bw ? (const void *)B.nm : H.nm.data(),
-                           bw ? (const void *)B.sm : H.sm.data(), bw ? (const void *)B.cigar_off : H.cigar_off.data(),
-                           bw ? (const void *)B.cigar : H.cigar.data(), bw ? (const void *)B.seq_off : H.seq_off.data(),
-                           bw ? (const void *)B.seq : H.seq.data(), bw ? (const void *)B.qual_off : H.qual_off.data(),
-                           bw ? (const void *)B.qual : H.qual.data(), bw ? nullptr : (const void *)H.region.data()};
+    std::vector<uint16_t> zero_lib;      // a borrowed batch may come without library ids
+    if (!src.lib) { zero_lib.assign((size_t)n, 0); src.lib = zero_lib.data(); }
+    const void *host[14] = {src.pos, src.flag, src.mapq, src.lib, src.l_qseq, src.nm, src.sm, src.cigar_off, src.cigar, src.seq_off,
+                            src.seq, src.qual_off, src.qual, bw ? nullptr : e->reads.region.data()};
     const size_t bytes[14] = {(size_t)n * 4, (size_t)n * 2, (size_t)n, (size_t)n * 2, (size_t)n * 4, (size_t)n * 4, (size_t)n * 4,
-                              (size_t)(n + 1) * 8, (size_t)n_cig * 4, (size_t)(n + 1) * 8, (size_t)n_seq, (size_t)(n + 1) * 8,
-                              (size_t)n_qual, bw ? (size_t)0 : (size_t)n * 4};
+                              (size_t)(n + 1) * 8, (size_t)src.cigar_off[n] * 4, (size_t)(n + 1) * 8, (size_t)src.seq_off[n],
+                              (size_t)(n + 1) * 8, (size_t)src.qual_off[n], bw ? (size_t)0 : (size_t)n * 4};
     e->h2d_bytes_last = 0;
     for (int k = 0; k < 14; ++k) {
         CU(e->d_in[k].reserve(bytes[k] + 16), "cudaMalloc(reads)");
         e->h2d_bytes_last += (int64_t)bytes[k];
-        if (bytes[k]) CU(cudaMemcpyAsync(e->d_in[k].p, src[k], bytes[k], cudaMemcpyHostToDevice, s), "H2D reads");
+        if (bytes[k]) CU(cudaMemcpyAsync(e->d_in[k].p, host[k], bytes[k], cudaMemcpyHostToDevice, s), "H2D reads");
     }
-    ReadsDev &R = e->dev_reads;
-    R.n_reads = n; R.pos = e->d_in[0].as<int32_t>(); R.flag = e->d_in[1].as<uint16_t>(); R.mapq = e->d_in[2].as<uint8_t>();
-    R.lib = e->d_in[3].as<uint16_t>(); R.l_qseq = e->d_in[4].as<int32_t>(); R.nm = e->d_in[5].as<int32_t>(); R.sm = e->d_in[6].as<int32_t>();
-    R.cigar_off = e->d_in[7].as<uint64_t>(); R.cigar = e->d_in[8].as<uint32_t>(); R.seq_off = e->d_in[9].as<uint64_t>();
-    R.seq = e->d_in[10].as<uint8_t>(); R.qual_off = e->d_in[11].as<uint64_t>(); R.qual = e->d_in[12].as<uint8_t>();
-    rc = upload_geometry(e, s);
-    if (rc != BRC_OK) return rc;
-    int64_t cap = std::max<int64_t>(e->sec_cap, (int64_t)e->n_rows * e->n_slots / 8 + 2 * e->n_indel_ops + 1024);
-    for (int attempt = 0; attempt < 8; ++attempt) {
-        rc = alloc_sec(e, cap);
-        if (rc != BRC_OK) return rc;
-        rc = run_kernels(e, e->regions.size() > 1 ? e->d_in[13].as<int32_t>() : nullptr, s, true);
-        if (rc != BRC_E_OVERFLOW) break;
-        cap = std::max<int64_t>(cap * 2, e->h_n_sec + 1024);
-    }
-    if (rc != BRC_OK) return rc == BRC_E_OVERFLOW ? set_error(e, rc, "secondary key pool overflow") : rc;
-    return fetch_results(e, s);
+    e->dev_reads = reads_dev(d_in_batch(e, n));
+    return compute_batch(e, cap, e->regions.size() > 1 ? e->d_in[13].as<int32_t>() : nullptr, s);
 }
 
 int brc_get_results(brc_engine *e, brc_results *out) {
@@ -921,9 +848,7 @@ int brc_run_device(brc_engine *e, const brc_read_batch *b, const int32_t *dev_re
     if (!e->planned) return set_error(e, BRC_E_INVALID, "run_device: call brc_plan_device first");
     if (e->regions.size() > 1 && !dev_region_of_read) return set_error(e, BRC_E_INVALID, "run_device: region_of_read required for >1 region");
     cudaSetDevice(e->cfg.device);
-    ReadsDev &R = e->dev_reads;
-    R.n_reads = b->n_reads; R.pos = b->pos; R.flag = b->flag; R.mapq = b->mapq; R.lib = b->lib; R.l_qseq = b->l_qseq; R.nm = b->nm; R.sm = b->sm;
-    R.cigar_off = b->cigar_off; R.cigar = b->cigar; R.seq_off = b->seq_off; R.seq = b->seq; R.qual_off = b->qual_off; R.qual = b->qual;
+    e->dev_reads = reads_dev(*b);
     if ((size_t)std::max<int64_t>(b->n_reads, 1) * sizeof(ReadDesc) > e->d_desc.cap) return set_error(e, BRC_E_INVALID, "run_device: batch larger than planned n_reads_cap");
     e->results_valid = false;
     return run_kernels(e, dev_region_of_read, (cudaStream_t)stream, false);

@@ -5,6 +5,7 @@
 #include <deque>
 #include <queue>
 #include <string>
+#include <thread>
 #include <vector>
 
 #include <cuda_runtime.h>
@@ -57,6 +58,13 @@ struct HostReads {         // staging SoA of admitted reads, all regions, file o
     std::vector<uint32_t> cigar;
     std::vector<uint8_t> seq, qual;
     int64_t n() const { return (int64_t)pos.size(); }
+    brc_read_batch batch() const {   // the staged reads as a batch (tid NULL: every staged read is on its region's contig)
+        brc_read_batch b{};
+        b.n_reads = n(); b.pos = pos.data(); b.flag = flag.data(); b.mapq = mapq.data(); b.lib = lib.data(); b.l_qseq = l_qseq.data();
+        b.nm = nm.data(); b.sm = sm.data(); b.cigar_off = cigar_off.data(); b.cigar = cigar.data(); b.seq_off = seq_off.data();
+        b.seq = seq.data(); b.qual_off = qual_off.data(); b.qual = qual.data();
+        return b;
+    }
     void clear() {
         pos.clear(); l_qseq.clear(); nm.clear(); sm.clear(); region.clear(); flag.clear(); lib.clear(); mapq.clear();
         cigar_off.assign(1, 0); seq_off.assign(1, 0); qual_off.assign(1, 0); cigar.clear(); seq.clear(); qual.clear();
@@ -83,18 +91,29 @@ struct EmitState {
     bool pending() const { for (auto &d : q) if (!d.empty()) return true; return false; }
 };
 
+// Worker threads for n items: one more per `grain` items, at most `cap` and the core count.
+inline int worker_count(int64_t n, int64_t grain, int cap) {
+    const unsigned hw = std::thread::hardware_concurrency();
+    return (int)std::max<int64_t>(1, std::min<int64_t>({(int64_t)(hw ? hw : 1), (int64_t)cap, n / grain + 1}));
+}
+// Runs work(t) for t in [0, nt): t >= 1 on threads of their own, t = 0 on the calling thread; returns when all are done.
+template <class F> void fan_out(int nt, const F &work) {
+    std::vector<std::thread> th;
+    for (int t = 1; t < nt; ++t) th.emplace_back(work, t);
+    if (nt > 0) work(0);
+    for (auto &x : th) x.join();
+}
+
 }  // namespace brc
 
 struct brc_engine {
     brc_config cfg{};
     int n_rows = 1;
     cudaStream_t stream = nullptr;
-    cudaStream_t s_in = nullptr, s_in2 = nullptr, s_out = nullptr, s_sec = nullptr;   // copy streams of the pipelined push path (reads in, words out, pool records out)
+    cudaStream_t s_in = nullptr, s_out = nullptr, s_sec = nullptr;   // copy streams of the pipelined push path (reads in, words out, pool records out)
     std::vector<cudaEvent_t> pipe_ev;
-    cudaEvent_t tm_ev[4] = {nullptr, nullptr, nullptr, nullptr};   // BRC_PIPE_TIMING: H2D first/last, D2H first/last (timing-enabled)
     int64_t h2d_bytes_last = 0;      // bytes the last push path actually sent over PCIe (after the elision below)
     int skip_h2d = 0;                // borrowed batch: bit0 seq_off, bit1 qual_off arithmetic; bit2 l_qseq, bit3 sm constant -> rebuilt on the device
-    int h2d_chunks = 0;              // >0: the borrowed batch's H2D copies are already in flight on s_in (issued by brc_push_reads)
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
     std::string err;
 
@@ -107,8 +126,7 @@ struct brc_engine {
     bool is_borrowed = false;
     brc_read_batch borrowed{};
     int64_t n_host_reads() const { return is_borrowed ? borrowed.n_reads : reads.n(); }
-    const uint8_t *host_seq() const { return is_borrowed ? borrowed.seq : reads.seq.data(); }
-    const uint64_t *host_seq_off() const { return is_borrowed ? borrowed.seq_off : reads.seq_off.data(); }
+    brc_read_batch host_batch() const { return is_borrowed ? borrowed : reads.batch(); }
     std::vector<brc_region> regions;
     bool region_open = false;
     brc::Admission adm;
@@ -169,7 +187,8 @@ struct brc_engine {
             if (it == dec.ins_reads.end() || *it != r) return nullptr;
             return dec.ins_pool.data() + dec.ins_off[(size_t)(it - dec.ins_reads.begin())];
         }
-        return host_seq() + host_seq_off()[(size_t)r];
+        const brc_read_batch b = host_batch();
+        return b.seq + b.seq_off[(size_t)r];
     }
 
     // deletion queue carried from one formatting pass to the next (brc_set_queue_carry): lets a caller flush argv regions

@@ -16,7 +16,6 @@
 #include <cstring>
 #include <deque>
 #include <string>
-#include <thread>
 #include <vector>
 
 #include <unistd.h>
@@ -68,14 +67,13 @@ struct View {   // raw result arrays of one engine
     int rows; int64_t NS, RS, SC;
     const uint32_t *ncover, *npass, *pstats, *sstats; const uint8_t *flags, *pbase, *skind;
     const int32_t *shead, *snext, *slen, *sqpos; const int64_t *sread;
-    const uint8_t *h_seq; const uint64_t *h_seq_off;
     View(const brc_engine *en, int64_t g) : e(en), rg(&en->regions[(size_t)g]), ref(brc::find_ref(en, rg->tid)) {
         const brc_engine::Wide &W = e->wide;            // full-width view of the packed device records (brc::ensure_wide)
         rows = e->n_rows; NS = e->n_slots; RS = (int64_t)rows * NS; SC = (int64_t)W.sec_next.size();
         ncover = W.ncover.data(); npass = W.npass.data(); pstats = W.pstats.data(); sstats = W.sec_stats.data();
         flags = W.flags.data(); pbase = W.pbase.data(); skind = W.sec_kind.data();
         shead = W.sec_head.data(); snext = W.sec_next.data(); slen = W.sec_len.data(); sqpos = W.sec_qpos.data();
-        sread = W.sec_read.data(); h_seq = e->host_seq(); h_seq_off = e->host_seq_off();
+        sread = W.sec_read.data();
     }
 };
 
@@ -160,8 +158,7 @@ void format_region(const brc_engine *e, int64_t g, int32_t s0, int32_t s1, const
     s0 = std::max(s0, 0); s1 = std::min(s1, rg.n_slots);
     if (s1 <= s0) { if (rg.site_list_mode && s1 >= rg.n_slots) st.clear(); return; }
     const int32_t n = s1 - s0;
-    unsigned hw = std::thread::hardware_concurrency();
-    int nt = (int)std::min<int64_t>({(int64_t)(hw ? hw : 1), (int64_t)32, (int64_t)n / 16384 + 1});
+    int nt = brc::worker_count(n, 16384, 32);
     // The deletion queue carries state across sites.  Inside one region only the site to the left matters, so ranges can be
     // formatted independently — except in the argv loop with several regions, whose queue is never cleared (A.6): keep that sequential.
     if (!rg.site_list_mode && e->regions.size() > 1) nt = 1;
@@ -175,18 +172,14 @@ void format_region(const brc_engine *e, int64_t g, int32_t s0, int32_t s1, const
     } else {
         std::vector<EmitState> states; states.reserve((size_t)nt);
         for (int t = 0; t < nt; ++t) states.emplace_back(e->n_rows);
-        auto work = [&](int t) {
+        brc::fan_out(nt, [&](int t) {
             const int32_t a = s0 + (int32_t)((int64_t)n * t / nt), b = s0 + (int32_t)((int64_t)n * (t + 1) / nt);
             EmitState &ls = t == 0 ? st : states[(size_t)t];
             std::string &dst = parts_out[base + (size_t)t];
             dst.reserve((size_t)(b - a) * 420);
             if ((t > 0 || seed_from_left) && a > 0) { Scratch W; std::string sink; format_site(V, a - 1, lib_names, ls, sink, W, false); }
             format_range(V, a, b, lib_names, ls, dst);
-        };
-        std::vector<std::thread> th;
-        for (int t = 1; t < nt; ++t) th.emplace_back(work, t);
-        work(0);
-        for (auto &x : th) x.join();
+        });
         st.clear();
         for (size_t r = 0; r < st.q.size(); ++r) { st.q[r] = states[(size_t)nt - 1].q[r]; st.q_exists[r] = states[(size_t)nt - 1].q_exists[r]; }
     }
@@ -201,14 +194,13 @@ bool format_many_site_list_regions(const brc_engine *e, const char *const *lib_n
     if (nr < 2) return false;
     int64_t total = 0;
     for (const brc_region &rg : e->regions) { if (!rg.site_list_mode) return false; total += rg.n_slots; }
-    unsigned hw = std::thread::hardware_concurrency();
-    const int nt = (int)std::min<int64_t>({(int64_t)(hw ? hw : 1), (int64_t)32, total / 16384 + 1});
+    const int nt = brc::worker_count(total, 16384, 32);
     std::vector<size_t> cut((size_t)nt + 1, nr);
     cut[0] = 0;
     { int64_t acc = 0; int t = 1; for (size_t g = 0; g < nr && t < nt; ++g) { acc += e->regions[g].n_slots; while (t < nt && acc >= total * t / nt) cut[(size_t)t++] = g + 1; } }
     const size_t base = parts_out.size();
     parts_out.resize(base + (size_t)nt);
-    auto work = [&](int t) {
+    brc::fan_out(nt, [&](int t) {
         EmitState st(e->n_rows);
         std::string &dst = parts_out[base + (size_t)t];
         int64_t slots = 0;
@@ -219,11 +211,7 @@ bool format_many_site_list_regions(const brc_engine *e, const char *const *lib_n
             format_range(V, 0, V.rg->n_slots, lib_names, st, dst);
             st.clear();
         }
-    };
-    std::vector<std::thread> th;
-    for (int t = 1; t < nt; ++t) th.emplace_back(work, t);
-    work(0);
-    for (auto &x : th) x.join();
+    });
     return true;
 }
 
@@ -259,14 +247,10 @@ int64_t serve(brc_engine *e, int64_t k0, int64_t k1, int64_t k2, const char *con
         std::vector<int64_t> off(e->fmt_parts.size() + 1, 0);
         for (size_t i = 0; i < e->fmt_parts.size(); ++i) off[i + 1] = off[i] + (int64_t)e->fmt_parts[i].size();
         const int64_t lim = std::min<int64_t>(n, cap - 1);
-        auto copy = [&](size_t i) {
-            const int64_t a = off[i], b = std::min(off[i + 1], lim);
-            if (b > a) std::memcpy(buf + a, e->fmt_parts[i].data(), (size_t)(b - a));
-        };
-        std::vector<std::thread> th;
-        for (size_t i = 1; i < e->fmt_parts.size(); ++i) th.emplace_back(copy, i);
-        if (!e->fmt_parts.empty()) copy(0);
-        for (auto &x : th) x.join();
+        brc::fan_out((int)e->fmt_parts.size(), [&](int i) {
+            const int64_t a = off[(size_t)i], b = std::min(off[(size_t)i + 1], lim);
+            if (b > a) std::memcpy(buf + a, e->fmt_parts[(size_t)i].data(), (size_t)(b - a));
+        });
         buf[lim] = 0;
         release_parts(e);   // delivered
     }

@@ -707,7 +707,6 @@ __device__ __forceinline__ void site_reset(SiteState &S, const ChunkInfo &ci, in
     }
 }
 
-__device__ __forceinline__ int2 lds_i2(const void *p) { return *reinterpret_cast<const int2 *>(p); }
 // shared-memory loads by 32-bit address: the hot loop walks the staged descriptors with one 32-bit register instead of a
 // generic 64-bit pointer plus its shared-window twin (ncu r02a: three loop values were spilled to local memory)
 __device__ __forceinline__ int2 lds64(uint32_t a) { int2 v; asm volatile("ld.shared.v2.u32 {%0,%1}, [%2];" : "=r"(v.x), "=r"(v.y) : "r"(a)); return v; }
@@ -1140,11 +1139,7 @@ __global__ void __launch_bounds__(K1_THREADS, BRC_K1_CTAS_PER_SM) pileup_kernel(
 #ifdef BRC_K1_PROFILE
         const long long tc0 = clock64();
 #endif
-#ifdef BRC_K1_HINT_WAIT
-        mbar_wait_relaxed(&sm.full[s], ph);          // try_wait with a suspend-time hint: the warp sleeps on the barrier instead of polling
-#else
         mbar_wait_hint<200>(&sm.full[s], ph);        // ncu r02a: this poll loop is 8 % of the issued instructions but 2 % of the stall samples
-#endif
 #ifdef BRC_K1_PROFILE
         const long long tc1 = clock64();
 #endif

@@ -23,9 +23,8 @@ for f in sorted(glob.glob("$O/bench_c3_*.json")):
     except Exception as ex:
         print(f, "FAILED", ex)
 PY
-BRC_PIPE_TIMING=1 timeout 600 python bench.py --config c3 --steps 20 --warmup 3 > $O/bench_c3_full.json 2> $O/bench_c3_full.err
-echo "c3 full rc=$?"; grep "brc pipe" $O/bench_c3_full.err | tail -4
-BRC_EARLY_H2D=1 timeout 300 python bench.py --config c3 --steps 5 --warmup 3 --no-cpu-baseline --no-e2e-text --no-parity > $O/bench_c3_earlyh2d.json 2> $O/bench_c3_earlyh2d.err
+timeout 600 python bench.py --config c3 --steps 20 --warmup 3 > $O/bench_c3_full.json 2> $O/bench_c3_full.err
+echo "c3 full rc=$?"
 timeout 900 python bench.py --steps 5 --warmup 3 > $O/bench_c4.json 2> $O/bench_c4.err
 echo "c4 rc=$?"; tail -c 600 $O/bench_c4.err
 timeout 600 python bench.py --steps 3 --warmup 3 --no-resident $B > $O/bench_c4_noresident.json 2> $O/bench_c4_noresident.err
@@ -34,7 +33,7 @@ echo "c5 rc=$?"; tail -c 400 $O/bench_c5.err
 timeout 300 python bench.py --impl reference --steps 3 --warmup 1 > $O/bench_ref_c4.json 2> $O/bench_ref_c4.err
 python - <<PY
 import json
-for f in ("bench_c3_full","bench_c3_earlyh2d","bench_c4","bench_c4_noresident","bench_c5","bench_ref_c4"):
+for f in ("bench_c3_full","bench_c4","bench_c4_noresident","bench_c5","bench_ref_c4"):
     try:
         d=json.loads(open("$O/"+f+".json").read().strip().splitlines()[-1])
         print(f, "value %.4g ms/step %.3f" % (d["value"], d["ms_per_step"]), "e2e", d.get("e2e",{}).get("ms_per_step"), "parity", d.get("parity",{}).get("identical"), "text", d.get("e2e_text",{}).get("value"), d.get("e2e_text",{}).get("compressed_span",{}).get("ms"))

@@ -9,7 +9,7 @@ echo "pytest done in $(( $(date +%s) - t0 )) s: $(tail -1 $O/pytest.log)"
 t0=$(date +%s); timeout 300 python -c "import __graft_entry__ as g; g.smoke(); print('smoke ok')" > $O/smoke.log 2>&1; echo "smoke rc=$? in $(( $(date +%s) - t0 )) s: $(tail -1 $O/smoke.log)"
 t0=$(date +%s); timeout 900 python bench.py > $O/bench_c4.json 2> $O/bench_c4.err; echo "bench.py (defaults) rc=$? in $(( $(date +%s) - t0 )) s"; tail -c 400 $O/bench_c4.err
 t0=$(date +%s); timeout 600 python bench.py --impl reference > $O/bench_ref_c4.json 2> $O/bench_ref_c4.err; echo "bench.py --impl reference rc=$? in $(( $(date +%s) - t0 )) s"
-t0=$(date +%s); BRC_PIPE_TIMING=1 timeout 600 python bench.py --config c3 --steps 20 --warmup 3 > $O/bench_c3_full.json 2> $O/bench_c3_full.err; echo "c3 rc=$? in $(( $(date +%s) - t0 )) s"; grep "brc pipe" $O/bench_c3_full.err | tail -2
+t0=$(date +%s); timeout 600 python bench.py --config c3 --steps 20 --warmup 3 > $O/bench_c3_full.json 2> $O/bench_c3_full.err; echo "c3 rc=$? in $(( $(date +%s) - t0 )) s"
 t0=$(date +%s); timeout 600 python bench.py --config c5 --steps 2 --warmup 3 > $O/bench_c5.json 2> $O/bench_c5.err; echo "c5 rc=$? in $(( $(date +%s) - t0 )) s"
 python - <<PY
 import json

@@ -13,8 +13,7 @@ for v in bam_readcount_b200/variants/*.so; do
 done
 timeout 600 python bench.py --config c5 --steps 3 --warmup 3 > $O/bench_c5.json 2> $O/bench_c5.err
 echo "c5 rc=$?"; tail -c 400 $O/bench_c5.err
-BRC_PIPE_TIMING=1 timeout 600 python bench.py --config c3 --steps 10 --warmup 3 --no-cpu-baseline > $O/bench_c3_full.json 2> $O/bench_c3_full.err
-grep "brc pipe" $O/bench_c3_full.err | tail -2
+timeout 600 python bench.py --config c3 --steps 10 --warmup 3 --no-cpu-baseline > $O/bench_c3_full.json 2> $O/bench_c3_full.err
 timeout 300 python tools/pcie_numa_probe.py > $O/pcie_probe.txt 2>&1
 python - <<PY
 import json,glob
