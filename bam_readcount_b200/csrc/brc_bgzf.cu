@@ -16,6 +16,7 @@
 
 #include "brc_bgzf.cuh"
 #include "brc_engine_internal.h"
+#include "brc_scan.cuh"
 
 using namespace brc;
 
@@ -136,45 +137,7 @@ __global__ void bam_extract_kernel(ExtractArgs A) {
     }
 }
 
-// three exclusive scans (u32 sizes -> u64 offsets), 256 elements per CTA: partial sums, one-CTA scan of the partials, apply
-constexpr int SCAN_CTA = 256;
-__global__ void __launch_bounds__(SCAN_CTA) scan_partial_kernel(const uint32_t *sz, int64_t n, unsigned long long *partial, int64_t nb) {
-    __shared__ unsigned long long red[SCAN_CTA / 32];
-    const int arr = blockIdx.y;
-    const int64_t i = (int64_t)blockIdx.x * SCAN_CTA + threadIdx.x;
-    unsigned long long v = i < n ? sz[(int64_t)arr * n + i] : 0ull;
-    for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-    __syncthreads();
-    if (threadIdx.x == 0) { unsigned long long t = 0; for (int w = 0; w < SCAN_CTA / 32; ++w) t += red[w]; partial[(int64_t)arr * (nb + 1) + blockIdx.x] = t; }
-}
-__global__ void __launch_bounds__(1024) scan_top_kernel(unsigned long long *partial, int64_t nb) {      // exclusive, in place; [nb] = total
-    __shared__ unsigned long long part[1024];
-    unsigned long long *v = partial + (int64_t)blockIdx.x * (nb + 1);
-    const int t = threadIdx.x;
-    const int64_t per = (nb + 1023) / 1024, lo = min(nb, per * t), hi = min(nb, lo + per);
-    unsigned long long s = 0;
-    for (int64_t i = lo; i < hi; ++i) s += v[i];
-    part[t] = s;
-    __syncthreads();
-    if (t == 0) { unsigned long long acc = 0; for (int i = 0; i < 1024; ++i) { const unsigned long long x = part[i]; part[i] = acc; acc += x; } v[nb] = acc; }
-    __syncthreads();
-    unsigned long long acc = part[t];
-    for (int64_t i = lo; i < hi; ++i) { const unsigned long long x = v[i]; v[i] = acc; acc += x; }
-}
-__global__ void __launch_bounds__(SCAN_CTA) scan_apply_kernel(const uint32_t *sz, int64_t n, const unsigned long long *partial, int64_t nb, uint64_t *off0, uint64_t *off1, uint64_t *off2) {
-    __shared__ unsigned long long sh[SCAN_CTA];
-    const int arr = blockIdx.y;
-    uint64_t *out = arr == 0 ? off0 : (arr == 1 ? off1 : off2);
-    const int64_t i = (int64_t)blockIdx.x * SCAN_CTA + threadIdx.x;
-    const unsigned long long v = i < n ? sz[(int64_t)arr * n + i] : 0ull;
-    sh[threadIdx.x] = v;
-    __syncthreads();
-    for (int o = 1; o < SCAN_CTA; o <<= 1) { const unsigned long long a = threadIdx.x >= o ? sh[threadIdx.x - o] : 0ull; __syncthreads(); sh[threadIdx.x] += a; __syncthreads(); }
-    const unsigned long long base = partial[(int64_t)arr * (nb + 1) + blockIdx.x];
-    if (i < n) out[i] = base + sh[threadIdx.x] - v;
-    if (i == n - 1) out[n] = base + sh[threadIdx.x];
-}
+// pool offsets: the three exclusive scans (u32 sizes -> u64 offsets) of brc_scan.cuh
 
 // one warp per record: CIGAR ops, packed bases, qualities from the inflated bytes into the pools
 __global__ void bam_copy_kernel(const uint8_t *U, const int64_t *src_off, const uint32_t *sz, int64_t n, const uint64_t *cig_off, const uint64_t *seq_off, const uint64_t *qual_off,
@@ -328,7 +291,7 @@ int brc_decode_bam_span(brc_engine *e, const brc_bam_span *sp, brc_read_batch *o
     const size_t per[9] = {n1 * 4, n1 * 2, n1, n1 * 2, n1 * 4, n1 * 4, n1 * 4, n1 * 8, n1 * 12};   // pos flag mapq lib l_qseq nm sm src_off sizes
     for (int k = 0; k < 9; ++k) CUB(D.arr[k].reserve(per[k] + 64), "cudaMalloc(decoded fields)");
     for (int k = 9; k < 12; ++k) CUB(D.arr[k].reserve((n1 + 1) * 8 + 64), "cudaMalloc(decoded offsets)");
-    const int64_t nb = (n + SCAN_CTA - 1) / SCAN_CTA;
+    const int64_t nb = (n + scan::SCAN_CTA - 1) / scan::SCAN_CTA;
     CUB(D.partial.reserve((size_t)(nb + 1) * 8 * 3 + 64), "cudaMalloc(scan partials)");
     ExtractArgs A{};
     A.U = D.u.as<uint8_t>(); A.scratch = D.scratch.as<int64_t>(); A.base = d_base; A.prefix = d_prefix; A.n_entry = sp->n_entry; A.n_reads = n;
@@ -340,9 +303,9 @@ int brc_decode_bam_span(brc_engine *e, const brc_bam_span *sp, brc_read_batch *o
     unsigned long long tot[3] = {0, 0, 0};
     if (n > 0) {
         bam_extract_kernel<<<(unsigned)((n + 127) / 128), 128, 0, s>>>(A);
-        scan_partial_kernel<<<dim3((unsigned)nb, 3), SCAN_CTA, 0, s>>>(A.sz, n, D.partial.as<unsigned long long>(), nb);
-        scan_top_kernel<<<3, 1024, 0, s>>>(D.partial.as<unsigned long long>(), nb);
-        scan_apply_kernel<<<dim3((unsigned)nb, 3), SCAN_CTA, 0, s>>>(A.sz, n, D.partial.as<unsigned long long>(), nb, cig_off, seq_off, qual_off);
+        scan::scan_partial_kernel<<<dim3((unsigned)nb, 3), scan::SCAN_CTA, 0, s>>>(A.sz, n, D.partial.as<unsigned long long>(), nb);
+        scan::scan_top_kernel<<<3, 1024, 0, s>>>(D.partial.as<unsigned long long>(), nb);
+        scan::scan_apply_kernel<<<dim3((unsigned)nb, 3), scan::SCAN_CTA, 0, s>>>(A.sz, n, D.partial.as<unsigned long long>(), nb, cig_off, seq_off, qual_off);
         CUB(cudaGetLastError(), "launch extract/scan");
         for (int k = 0; k < 3; ++k) CUB(cudaMemcpyAsync(&tot[k], D.partial.as<unsigned long long>() + (size_t)k * (nb + 1) + nb, 8, cudaMemcpyDeviceToHost, s), "D2H totals");
     } else {

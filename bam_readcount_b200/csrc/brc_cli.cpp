@@ -10,6 +10,8 @@
 //   -l site list : R:...:574-608  (d.beg=beg-1, d.end=end, queues cleared per region)
 //   argv regions : R:...:641-657  (bam_parse_region; a bare contig name keeps the previous beg/end, A.6)
 #include <algorithm>
+#include <cerrno>
+#include <climits>
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>
@@ -753,7 +755,11 @@ void usage() {
                 "                                        included in per-base counts\n"
                 "  --shard RANK/COUNT                    (this host) compute only shard RANK of COUNT: the regions are cut into COUNT runs of\n"
                 "                                        about equal BAI-estimated coverage, one process per GPU (BRC_DEVICE); outputs\n"
-                "                                        concatenate in rank order\n\n");
+                "                                        concatenate in rank order\n"
+                "  --min-alt-count N                     (this host) print only the sites where an alternative allele (a base other than\n"
+                "                                        the reference base, an insertion or a deletion) has a count of at least N\n"
+                "  --min-alt-fraction F                  (this host) ... and of at least F times the site's depth (0 <= F <= 1; without\n"
+                "                                        --min-alt-count the count must be at least 1).  Printed lines are unchanged\n\n");
 }
 
 // samtools region string "name[:beg[-end]]" as bam_parse_region (V:bam_aux.c:65-75) handles it.  Returns 0 when beg and end were
@@ -791,8 +797,10 @@ int main(int argc, char **argv) {
     std::string fn_pos, fn_fa, dist_arg;
     static option lo[] = {{"help", 0, 0, 'h'}, {"version", 0, 0, 'v'}, {"min-mapping-quality", 1, 0, 'q'}, {"min-base-quality", 1, 0, 'b'},
                           {"max-count", 1, 0, 'd'}, {"site-list", 1, 0, 'l'}, {"reference-fasta", 1, 0, 'f'}, {"print-individual-mapq", 1, 0, 'D'},
-                          {"per-library", 0, 0, 'p'}, {"max-warnings", 1, 0, 'w'}, {"insertion-centric", 0, 0, 'i'}, {"shard", 1, 0, 1000}, {0, 0, 0, 0}};
+                          {"per-library", 0, 0, 'p'}, {"max-warnings", 1, 0, 'w'}, {"insertion-centric", 0, 0, 'i'}, {"shard", 1, 0, 1000},
+                          {"min-alt-count", 1, 0, 1001}, {"min-alt-fraction", 1, 0, 1002}, {0, 0, 0, 0}};
     int shard_rank = 0, shard_count = 1;
+    long min_alt_count = 0; double min_alt_fraction = -1.0;       // site filter (brc_set_site_filter); off unless one is given
     bool help = false, version = false;
     for (int c; (c = getopt_long(argc, argv, "hvq:b:d:l:f:D:pw:i", lo, nullptr)) != -1;) {
         switch (c) {
@@ -801,9 +809,24 @@ int main(int argc, char **argv) {
         case 'l': fn_pos = optarg; break; case 'f': fn_fa = optarg; break; case 'D': dist_arg = optarg; break;
         case 'p': per_lib = true; break; case 'w': max_warn = std::atoll(optarg); break; case 'i': ic = true; break;
         case 1000: if (std::sscanf(optarg, "%d/%d", &shard_rank, &shard_count) != 2 || shard_count < 1 || shard_rank < 0 || shard_rank >= shard_count) { std::fprintf(stderr, "--shard wants RANK/COUNT with 0 <= RANK < COUNT\n"); return 1; } break;
+        case 1001: {
+            char *end = nullptr; errno = 0;
+            min_alt_count = std::strtol(optarg, &end, 10);
+            if (errno || end == optarg || *end || min_alt_count < 1 || min_alt_count > INT32_MAX) { std::fprintf(stderr, "--min-alt-count wants an integer N >= 1\n"); return 1; }
+            break;
+        }
+        case 1002: {
+            char *end = nullptr; errno = 0;
+            min_alt_fraction = std::strtod(optarg, &end);
+            if (errno || end == optarg || *end || !(min_alt_fraction >= 0.0 && min_alt_fraction <= 1.0)) { std::fprintf(stderr, "--min-alt-fraction wants a number F with 0 <= F <= 1\n"); return 1; }
+            break;
+        }
         default: usage(); return 1;
         }
     }
+    const bool site_filter = min_alt_count > 0 || min_alt_fraction >= 0.0;
+    brc_site_filter filter{};
+    filter.min_alt_count = (int32_t)std::max<long>(min_alt_count, 1); filter.min_alt_fraction = std::max(min_alt_fraction, 0.0);
     if (version) { std::printf("bam-readcount version: b200 (engine ABI %d)\n", brc_abi_version()); return 1; }   // R:...:467-470 (exit 1)
     if (help || optind >= argc) { usage(); return 1; }                                                              // R:...:472-475
     const std::string bam_path = argv[optind];
@@ -962,7 +985,11 @@ int main(int argc, char **argv) {
         if (r != BRC_OK) { std::fprintf(stderr, "brc_compute: %s\n", brc_last_error(eng)); return r; }
         brc_results res{};
         const double g0 = now();
-        if ((r = brc_get_results(eng, &res)) != BRC_OK) { std::fprintf(stderr, "brc_get_results: %s\n", brc_last_error(eng)); return r; }
+        if (site_filter) {            // only the selected sites came back: no dense view, the region table is all the loop needs
+            brc_selected_results sel{};
+            if ((r = brc_get_selected_results(eng, &sel)) != BRC_OK) { std::fprintf(stderr, "brc_get_selected_results: %s\n", brc_last_error(eng)); return r; }
+            res.n_regions = sel.n_regions; res.regions = sel.regions;
+        } else if ((r = brc_get_results(eng, &res)) != BRC_OK) { std::fprintf(stderr, "brc_get_results: %s\n", brc_last_error(eng)); return r; }
         std::fflush(stdout);
         const double f0 = now();
         t_results += f0 - g0;
@@ -1030,6 +1057,7 @@ int main(int argc, char **argv) {
     rc = decode_only ? BRC_OK : (warm_rc != BRC_OK ? warm_rc : brc_create(&cfg, &eng));
     if (rc != BRC_OK) { std::fprintf(stderr, "brc_create: %s\n", brc_strerror(rc)); return 1; }
     if (eng) brc_set_queue_carry(eng, 1);
+    if (eng && site_filter && brc_set_site_filter(eng, &filter) != BRC_OK) { std::fprintf(stderr, "brc_set_site_filter: %s\n", brc_last_error(eng)); return 1; }
     const double t_loop0 = now();
     auto next_fbeg = [&](size_t gi) -> int64_t {   // start of the following fetch when it continues this one, else "keep nothing"
         if (gi + 1 >= regions.size() || regions[gi + 1].tid != regions[gi].tid) return INT64_MAX;

@@ -200,6 +200,61 @@ struct PrecomputeParams {
     int32_t min_mapq;      // -q: reads below it (or failing the flag filter) are marked FM_DEAD
 };
 
+// ---- alternative-allele site filter (brc_select.cu on the device, the text emitter on the host; DESIGN.md §10) ----
+// A base class 1..4 ("ACGT") is an alternative allele unless the reference base encodes exactly that one base (seq_nt16 codes
+// 1/2/4/8); a reference N, IUPAC code or missing character makes every base alternative.
+__host__ __device__ inline bool base_is_alt(uint32_t base_class, uint32_t ref_code) {
+    return base_class >= 1u && base_class <= 4u && (1u << (base_class - 1u)) != ref_code;
+}
+// The rule for one printed line: its largest alternative-allele count against min_alt_count and min_alt_fraction * depth (IEEE
+// double; depth = the line's 4th column).  The one predicate both the device selection and the host emitter evaluate.
+__host__ __device__ inline bool site_passes(uint64_t best_alt, uint64_t depth, int32_t min_alt_count, double min_alt_fraction) {
+    return best_alt >= (uint64_t)min_alt_count && (double)best_alt >= min_alt_fraction * (double)depth;
+}
+
+struct SelRegion {         // one region as the selection kernels see it
+    int64_t slot_base;
+    int32_t n_slots;
+    int32_t first_pos;
+    int32_t beg, end;      // printed positions [beg, end)
+    int32_t keep_all_n;    // slots [0, keep_all_n) are shipped whenever they print a line (deletions carried in from other regions)
+    int32_t argv;          // argv region: the last live site of every library row is shipped too (the deletion queue it leaves)
+    int32_t tid_slot;      // index into the RefWin table
+    int32_t ref_on_host;   // 0: the emitter has no reference characters for this contig and prints N, so every base is alternative
+};
+
+struct SelectParams {
+    const uint32_t *words;  // [N_WORDS][rows*slots]
+    int32_t n_rows;
+    int64_t n_slots;
+    const SecRec *sec;
+    const int32_t *sec_count;
+    int64_t sec_cap;
+    const SelRegion *regions;
+    int64_t n_regions;
+    const RefWin *refs;
+    int32_t min_alt_count;
+    double min_alt_fraction;
+    // per-site scratch, [n_slots] each (best .. esc_np and reg_last, counters zeroed before the pool pass)
+    uint32_t *best;         // largest alternative count of the site's pool records
+    uint32_t *dsum;         // deletion counts anchored here that print at the next site (extra depth there)
+    uint32_t *dbest;        // largest such deletion count
+    uint32_t *esc_np;       // npass of the site's escaped primaries
+    uint32_t *reg_last;     // [n_regions][n_rows] 1 + offset of the last live site of an argv region that the row covers
+    unsigned long long *counters;   // [0] pool records shipped, [1] abandoned sites (-p, a read without library)
+    uint8_t *keep;          // bit0 rule holds, bit1 keep-all range, bit2 live (a line is formed at the site)
+    uint8_t *emit;          // emit byte of the shipped site
+    uint32_t *ship;         // 1 = shipped (scan input)
+    unsigned long long *partial;
+    int64_t nb;
+    uint64_t *idx;          // [n_slots+1] compact index of each shipped site; idx[n_slots] = shipped sites
+    // compact outputs
+    uint32_t *c_site;
+    uint8_t *c_emit;
+    uint32_t *c_words;      // [N_WORDS][rows*n_sel]
+    SecRec *c_sec;
+};
+
 // launch wrappers (brc_kernels.cu)
 cudaError_t launch_init_tiles(int32_t *tile_lo, int32_t *tile_hi, int64_t n_tiles, int32_t *sec_count,
                               unsigned long long *warn, cudaStream_t s);
@@ -210,5 +265,9 @@ cudaError_t launch_deep_sites(const PileupParams &p, cudaStream_t s);   // no-op
 cudaError_t launch_fill_offsets(uint64_t *off, int64_t n, uint64_t base, uint64_t stride, cudaStream_t s);   // off[i] = base + i * stride
 cudaError_t launch_fill_i32(int32_t *dst, int64_t n, int32_t v, cudaStream_t s);
 cudaError_t launch_fastmath_selftest(int max_b, unsigned long long *d_bad, cudaStream_t s);
+// brc_select.cu: pool pass, site pass, ship flags, scan, compaction of sites and pool records (SELECT_KERNELS launches)
+constexpr int SELECT_KERNELS = 8;
+constexpr int SELECT_SCAN_CTA = 256;   // sites per scan partial (SelectParams::nb = ceil(n_slots / SELECT_SCAN_CTA))
+cudaError_t launch_select(const SelectParams &p, cudaStream_t s);
 
 }  // namespace brc

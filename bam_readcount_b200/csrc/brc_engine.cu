@@ -129,12 +129,12 @@ void brc_destroy(brc_engine *e) {
     cudaDeviceSynchronize();
     for (auto &r : e->refs) r.dev.release();
     DevBuf *bufs[] = {&e->d_refs, &e->d_desc, &e->d_tiles, &e->d_tile_lo, &e->d_tile_hi, &e->d_regions, &e->d_deep_tiles,
-                      &e->d_words, &e->d_sec, &e->d_sec_count, &e->d_warn};
+                      &e->d_words, &e->d_sec, &e->d_sec_count, &e->d_warn, &e->d_sel, &e->d_sel_regions};
     for (auto *b : bufs) b->release();
     for (auto &b : e->d_in) b.release();
     { brc_engine::Decoded &D = e->dec; DevBuf *db[] = {&D.comp, &D.btab, &D.u, &D.meta, &D.scratch, &D.count, &D.partial, &D.cigar, &D.seq, &D.qual, &D.ins_idx, &D.ins_out};
       for (auto *b : db) b->release(); for (auto &b : D.arr) b.release(); }
-    PinBuf *pins[] = {&e->h_words, &e->h_sec, &e->h_misc};
+    PinBuf *pins[] = {&e->h_words, &e->h_sec, &e->h_misc, &e->h_sel};
     for (auto *b : pins) b->release();
     for (auto &ev : e->ev) if (ev) cudaEventDestroy(ev);
     for (auto &ev : e->pipe_ev) if (ev) cudaEventDestroy(ev);
@@ -172,6 +172,7 @@ int brc_reset(brc_engine *e) {
     if (!e) return BRC_E_INVALID;
     e->reads.clear(); e->is_borrowed = false; e->regions.clear(); e->region_open = false; e->adm.reset(); e->n_indel_ops = 0;
     e->results_valid = false; e->planned = false; e->tiles.clear(); e->regions_dev.clear(); e->n_slots = 0; e->wide.valid = false;
+    e->sparse = false; e->sel_launched = false; e->n_sel = 0;
     e->dec.pushed = false; e->dec.ins_reads.clear(); e->dec.ins_off.clear(); e->dec.ins_pool.clear();
     for (auto &w : e->warn_counts) w = 0;
     return BRC_OK;
@@ -441,6 +442,112 @@ static int upload_geometry(brc_engine *e, cudaStream_t s) {
     return BRC_OK;
 }
 
+// ---------------------------------------------------------------------------------------------
+// alternative-allele site filter: region table, launch, compact fetch (kernels in brc_select.cu)
+// ---------------------------------------------------------------------------------------------
+// Once per brc_compute / brc_run_device.  The emitter's deletion queue is never cleared between argv regions (R:...:650-656),
+// so deletions of one region print in a later one that overlaps or abuts it, where the device cannot see them: the slots of a
+// region up to the last position such a deletion can print at are shipped whole (keep_all_n), and the host rule decides.  Those
+// positions are, per contig, the ends of the earlier argv regions of this batch and, with queue carry on, the positions of the
+// entries the last formatting pass left in the carried queue.  A site-list region empties the queue at its end.
+static void plan_selection(brc_engine *e) {
+    e->sel_regions.clear();
+    if (!e->filter_on) return;
+    std::vector<std::pair<int32_t, int64_t>> hist;        // contig -> last position a queued deletion may print at
+    auto at = [&](int32_t tid) { for (auto &x : hist) if (x.first == tid) return &x; hist.emplace_back(tid, (int64_t)-1); return &hist.back(); };
+    if (e->carry_on)
+        for (const auto &q : e->carry.q)
+            for (const QEnt &x : q) { auto *h = at(x.tid); h->second = std::max<int64_t>(h->second, x.pos); }
+    for (size_t g = 0; g < e->regions.size(); ++g) {
+        const brc_region &r = e->regions[g];
+        const HostRef *ref = find_ref(e, r.tid);
+        SelRegion d{};
+        d.slot_base = r.slot_base; d.n_slots = r.n_slots; d.first_pos = r.first_pos; d.beg = r.beg; d.end = r.end;
+        d.argv = r.site_list_mode ? 0 : 1; d.tid_slot = e->regions_dev[g].tid_slot;
+        d.ref_on_host = ref && !ref->seq.empty();
+        auto *h = at(r.tid);
+        d.keep_all_n = (int32_t)std::max<int64_t>(0, std::min<int64_t>(r.n_slots, h->second - r.first_pos + 1));
+        e->sel_regions.push_back(d);
+        if (r.site_list_mode) hist.clear();
+        else h->second = std::max<int64_t>(h->second, r.end);
+    }
+}
+
+// The selection kernels after the pileup kernels on stream s (ev[3] after them); no-op without a filter.
+static int launch_selection(brc_engine *e, cudaStream_t s) {
+    e->sel_launched = false;
+    if (!e->filter_on) return BRC_OK;
+    const int64_t NS = e->n_slots, rows = e->n_rows, R = (int64_t)e->sel_regions.size();
+    const int64_t nb = std::max<int64_t>(1, (NS + SELECT_SCAN_CTA - 1) / SELECT_SCAN_CTA);
+    size_t off = 0;
+    auto take = [&](size_t bytes) { const size_t o = off; off = (off + bytes + 15) & ~(size_t)15; return o; };
+    const size_t o_best = take((size_t)NS * 16), o_last = take((size_t)R * rows * 4), o_cnt = take(16), zero_end = off;
+    const size_t o_keep = take((size_t)NS), o_emit = take((size_t)NS), o_ship = take((size_t)NS * 4), o_idx = take((size_t)(NS + 1) * 8);
+    const size_t o_part = take((size_t)(nb + 1) * 8), o_site = take((size_t)NS * 4), o_cemit = take((size_t)NS);
+    // The compact outputs are sized for the worst case (every site and record shipped), so the launches need no host round trip
+    // for the count; this doubles the device result footprint of a filtered batch (about 43 B per site and row plus a second
+    // pool).  Sizing them after the count is known would trade that memory for one synchronisation per batch.
+    const size_t o_words = take((size_t)NS * rows * 4 * N_WORDS), o_sec = take((size_t)e->sec_cap * sizeof(SecRec));
+    CU(e->d_sel.reserve(off), "cudaMalloc(selection)");
+    CU(e->d_sel_regions.reserve((size_t)std::max<int64_t>(R, 1) * sizeof(SelRegion)), "cudaMalloc(selection regions)");
+    if (R) CU(cudaMemcpyAsync(e->d_sel_regions.p, e->sel_regions.data(), (size_t)R * sizeof(SelRegion), cudaMemcpyHostToDevice, s), "H2D selection regions");
+    char *b = e->d_sel.as<char>();
+    CU(cudaMemsetAsync(b, 0, zero_end, s), "memset(selection)");
+    SelectParams P{};
+    P.words = e->d_words.as<uint32_t>(); P.n_rows = e->n_rows; P.n_slots = NS;
+    P.sec = e->d_sec.as<SecRec>(); P.sec_count = e->d_sec_count.as<int32_t>(); P.sec_cap = e->sec_cap;
+    P.regions = e->d_sel_regions.as<SelRegion>(); P.n_regions = R; P.refs = e->d_refs.as<RefWin>();
+    P.min_alt_count = e->filter.min_alt_count; P.min_alt_fraction = e->filter.min_alt_fraction;
+    P.best = reinterpret_cast<uint32_t *>(b + o_best); P.dsum = P.best + NS; P.dbest = P.dsum + NS; P.esc_np = P.dbest + NS;
+    P.reg_last = reinterpret_cast<uint32_t *>(b + o_last); P.counters = reinterpret_cast<unsigned long long *>(b + o_cnt);
+    P.keep = reinterpret_cast<uint8_t *>(b + o_keep); P.emit = reinterpret_cast<uint8_t *>(b + o_emit);
+    P.ship = reinterpret_cast<uint32_t *>(b + o_ship); P.idx = reinterpret_cast<uint64_t *>(b + o_idx);
+    P.partial = reinterpret_cast<unsigned long long *>(b + o_part); P.nb = nb;
+    P.c_site = reinterpret_cast<uint32_t *>(b + o_site); P.c_emit = reinterpret_cast<uint8_t *>(b + o_cemit);
+    P.c_words = reinterpret_cast<uint32_t *>(b + o_words); P.c_sec = reinterpret_cast<SecRec *>(b + o_sec);
+    CU(launch_select(P, s), "launch selection");
+    if (NS > 0) e->launch_count += SELECT_KERNELS;
+    CU(cudaEventRecord(e->ev[3], s), "event");
+    e->sel_params = P;
+    e->sel_filter = e->filter;
+    e->sel_launched = true;
+    return BRC_OK;
+}
+
+// The compact selection to the host: the counts first, then exactly the shipped bytes.
+static int fetch_selected(brc_engine *e, cudaStream_t s) {
+    const SelectParams &P = e->sel_params;
+    int32_t cnt = 0;
+    CU(e->h_misc.reserve(64), "pin");
+    uint64_t *hm = e->h_misc.as<uint64_t>();
+    hm[0] = hm[1] = hm[2] = 0;
+    CU(cudaMemcpyAsync(&cnt, e->d_sec_count.p, 4, cudaMemcpyDeviceToHost, s), "D2H sec_count");
+    if (P.n_slots > 0) {
+        CU(cudaMemcpyAsync(hm, P.idx + P.n_slots, 8, cudaMemcpyDeviceToHost, s), "D2H selected sites");
+        CU(cudaMemcpyAsync(hm + 1, P.counters, 16, cudaMemcpyDeviceToHost, s), "D2H selection counters");
+    }
+    CU(cudaStreamSynchronize(s), "sync");
+    if ((int64_t)cnt > e->sec_cap) return set_error(e, BRC_E_OVERFLOW, "secondary key pool overflow (re-plan with a larger n_sec_cap)");
+    const int64_t n = (int64_t)hm[0], ns = (int64_t)hm[1];
+    e->sel_abandoned = (int64_t)hm[2];
+    const size_t wbytes = (size_t)n * e->n_rows * 4 * N_WORDS;
+    CU(e->h_words.reserve(std::max<size_t>(wbytes, 4)), "pin"); CU(e->h_sec.reserve((size_t)std::max<int64_t>(ns, 1) * sizeof(SecRec)), "pin");
+    CU(e->h_sel.reserve((size_t)std::max<int64_t>(n, 1) * 5), "pin");
+    if (n) {
+        CU(cudaMemcpyAsync(e->h_words.p, P.c_words, wbytes, cudaMemcpyDeviceToHost, s), "D2H selected words");
+        CU(cudaMemcpyAsync(e->h_sel.p, P.c_site, (size_t)n * 4, cudaMemcpyDeviceToHost, s), "D2H selected site ids");
+        CU(cudaMemcpyAsync(e->h_sel.as<uint32_t>() + n, P.c_emit, (size_t)n, cudaMemcpyDeviceToHost, s), "D2H selected emit bytes");
+    }
+    if (ns) CU(cudaMemcpyAsync(e->h_sec.p, P.c_sec, (size_t)ns * sizeof(SecRec), cudaMemcpyDeviceToHost, s), "D2H selected records");
+    CU(cudaMemcpyAsync(hm + 4, e->d_warn.p, 16, cudaMemcpyDeviceToHost, s), "D2H warn");
+    CU(cudaStreamSynchronize(s), "sync D2H");
+    e->warn_counts[0] = (int64_t)hm[4]; e->warn_counts[1] = (int64_t)hm[5]; e->warn_counts[2] = 0;
+    e->warn_counts[3] = -1;
+    e->n_sel = n; e->h_n_sec = ns; e->sparse = true;
+    e->results_valid = true; e->fmt_valid = false; e->wide.valid = false;
+    return BRC_OK;
+}
+
 static void make_params(brc_engine *e, const int32_t *d_region_of_read, PrecomputeParams &P0, PileupParams &P1) {
     P0 = PrecomputeParams{};
     P0.reads = e->dev_reads; P0.regions = e->d_regions.as<RegionDev>(); P0.n_regions = (int64_t)e->regions_dev.size();
@@ -470,6 +577,8 @@ static int run_kernels(brc_engine *e, const int32_t *d_region_of_read, cudaStrea
     CU(launch_pileup(P1, s), "launch pileup"); if (P1.n_tiles) e->launch_count++;
     CU(launch_deep_sites(P1, s), "launch deep_sites"); if (P1.n_deep) e->launch_count++;
     CU(cudaEventRecord(e->ev[2], s), "event");
+    const int rs = launch_selection(e, s);
+    if (rs != BRC_OK) return rs;
     if (check_overflow) {
         int32_t cnt = 0;
         CU(cudaMemcpyAsync(&cnt, P1.res.sec_count, 4, cudaMemcpyDeviceToHost, s), "D2H sec_count");
@@ -481,6 +590,7 @@ static int run_kernels(brc_engine *e, const int32_t *d_region_of_read, cudaStrea
 }
 
 static int fetch_results(brc_engine *e, cudaStream_t s, bool slots_already_fetched = false, int64_t sec_done = 0) {
+    if (e->sel_launched) return fetch_selected(e, s);
     const int64_t rs = (int64_t)e->n_rows * e->n_slots;
     int32_t cnt = 0;
     CU(cudaMemcpyAsync(&cnt, e->d_sec_count.p, 4, cudaMemcpyDeviceToHost, s), "D2H sec_count");
@@ -499,6 +609,7 @@ static int fetch_results(brc_engine *e, cudaStream_t s, bool slots_already_fetch
     const unsigned long long *w = e->h_misc.as<unsigned long long>();
     e->warn_counts[0] = (int64_t)w[0]; e->warn_counts[1] = (int64_t)w[1]; e->warn_counts[2] = 0;
     e->warn_counts[3] = -1;          // LIBRARY_UNAVAILABLE: counted from the flag bits on demand (brc_get_warning_counts)
+    e->sparse = false;
     e->results_valid = true; e->fmt_valid = false; e->wide.valid = false;
     return BRC_OK;
 }
@@ -526,7 +637,7 @@ namespace brc {
 void ensure_wide(brc_engine *e) {
     brc_engine::Wide &W = e->wide;
     if (W.valid) return;
-    const int64_t rs = (int64_t)e->n_rows * e->n_slots, ns = e->h_n_sec;
+    const int64_t rs = (int64_t)e->n_rows * e->result_cols(), ns = e->h_n_sec;   // sparse results: the shipped sites' columns
     const uint32_t *words = e->h_words.as<uint32_t>();
     const SecRec *sec = e->h_sec.as<SecRec>();
     W.ncover.resize((size_t)rs); W.npass.resize((size_t)rs); W.flags.resize((size_t)rs); W.pbase.resize((size_t)rs);
@@ -637,9 +748,10 @@ static int compute_pipelined(brc_engine *e) {
     int rc = issue_h2d_chunks(e, n_chunks);
     if (rc != BRC_OK) return rc;
     e->dev_reads = reads_dev(d_in_batch(e, n));
-    // host result buffers
+    // host result buffers (with a site filter only the compacted selection comes back, after the kernels: fetch_selected)
+    const bool sel = e->filter_on;
     const int64_t rs1 = std::max<int64_t>(rs, 1);
-    CU(e->h_words.reserve(rs1 * 4 * N_WORDS), "pin");
+    if (!sel) CU(e->h_words.reserve(rs1 * 4 * N_WORDS), "pin");
     CU(e->h_sec.reserve((size_t)e->sec_cap * sizeof(SecRec)), "pin");          // pool records leave while the kernels run
     CU(e->h_misc.reserve(64 + 4 * 64), "pin");
     if (!e->s_sec) CU(cudaStreamCreateWithFlags(&e->s_sec, cudaStreamNonBlocking), "stream");
@@ -672,12 +784,13 @@ static int compute_pipelined(brc_engine *e) {
             if (P1.work_counter) P1.work_counter = ++k1_launches < N_WORK_COUNTERS ? P1.work_counter + 1 : nullptr;   // next launch: next dispenser
             CU(launch_deep_sites(P1, sk), "launch deep_sites"); if (P1.n_deep) e->launch_count++;
             CU(cudaEventRecord(e->pipe_ev[2 * c + 1], sk), "event");
-            if (c < 64) {   // snapshot of the pool counter: the records allocated so far are final (a tile is computed by exactly one launch)
+            if (!sel && c < 64) {   // snapshot of the pool counter: the records allocated so far are final (a tile is computed by exactly one launch)
                 CU(cudaMemcpyAsync(h_cnt + c, P1.res.sec_count, 4, cudaMemcpyDeviceToHost, sk), "D2H pool counter");
                 CU(cudaEventRecord(e->pipe_ev[2 * n_chunks + 2 + (int)cnt_chunks.size()], sk), "event");
                 cnt_chunks.push_back(c);
             }
             // ---- D2H of the finished slots ----
+            if (sel) { tile_done = tile_to; continue; }
             CU(cudaStreamWaitEvent(e->s_out, e->pipe_ev[2 * c + 1], 0), "wait");
             const int64_t s0 = e->tiles[(size_t)tile_done].slot0;
             const int64_t s1 = tile_to < n_tiles ? e->tiles[(size_t)tile_to].slot0 : e->n_slots;
@@ -695,6 +808,8 @@ static int compute_pipelined(brc_engine *e) {
     }
     CU(cudaEventRecord(e->ev[1], sk), "event");
     CU(cudaEventRecord(e->ev[2], sk), "event");
+    rc = launch_selection(e, sk);
+    if (rc != BRC_OK) return rc;
     // everything is queued: follow the kernels and ship the pool records each chunk finished (their own stream: the word copies
     // of later chunks are already queued on s_out)
     int64_t sec_done = 0;
@@ -725,6 +840,7 @@ int brc_compute(brc_engine *e) {
     cudaSetDevice(e->cfg.device);
     int rc = build_geometry(e, e->regions.data(), (int64_t)e->regions.size());
     if (rc != BRC_OK) return rc;
+    plan_selection(e);
     if (e->dec.pushed) {
         // f-2: the region's reads were inflated and framed on the device (brc_push_bam_span): kernels straight on that batch
         if (!e->dec.valid || e->regions.size() != 1) return set_error(e, BRC_E_INVALID, "compute: the device-decoded batch is gone");
@@ -787,6 +903,7 @@ int brc_compute(brc_engine *e) {
 int brc_get_results(brc_engine *e, brc_results *out) {
     if (!e || !out) return BRC_E_INVALID;
     if (!e->results_valid) return set_error(e, BRC_E_INVALID, "get_results: no results (call brc_compute)");
+    if (e->sparse) return set_error(e, BRC_E_INVALID, "get_results: a site filter is set, there is no dense view (brc_get_selected_results)");
     brc::ensure_wide(e);
     const brc_engine::Wide &W = e->wide;
     out->n_regions = (int64_t)e->regions.size(); out->regions = e->regions.data(); out->n_rows = e->n_rows; out->n_slots = e->n_slots;
@@ -801,6 +918,7 @@ int brc_get_results(brc_engine *e, brc_results *out) {
 int brc_get_packed_results(brc_engine *e, brc_packed_results *out) {
     if (!e || !out) return BRC_E_INVALID;
     if (!e->results_valid) return set_error(e, BRC_E_INVALID, "get_packed_results: no results (call brc_compute)");
+    if (e->sparse) return set_error(e, BRC_E_INVALID, "get_packed_results: a site filter is set, there is no dense view (brc_get_selected_results)");
     out->n_regions = (int64_t)e->regions.size(); out->regions = e->regions.data(); out->n_rows = e->n_rows; out->n_slots = e->n_slots;
     out->words = e->h_words.as<uint32_t>(); out->n_sec = e->h_n_sec; out->sec = e->h_sec.as<brc_sec_record>(); out->sec_count = nullptr;
     return BRC_OK;
@@ -811,7 +929,8 @@ int brc_get_warning_counts(brc_engine *e, int64_t out[4]) {
     if (e->results_valid && e->warn_counts[3] < 0) {
         // LIBRARY_UNAVAILABLE fires once per abandoned site callback (R:bamreadcount.cpp:281-284)
         int64_t lu = 0;
-        if (e->cfg.per_lib) {
+        if (e->cfg.per_lib && e->sparse) lu = e->sel_abandoned;   // counted by the selection's site pass
+        else if (e->cfg.per_lib) {
             const uint32_t *w1 = e->h_words.as<uint32_t>() + (int64_t)e->n_rows * e->n_slots;
             for (int64_t sidx = 0; sidx < e->n_slots; ++sidx) {
                 bool ab = false;
@@ -851,6 +970,7 @@ int brc_run_device(brc_engine *e, const brc_read_batch *b, const int32_t *dev_re
     e->dev_reads = reads_dev(*b);
     if ((size_t)std::max<int64_t>(b->n_reads, 1) * sizeof(ReadDesc) > e->d_desc.cap) return set_error(e, BRC_E_INVALID, "run_device: batch larger than planned n_reads_cap");
     e->results_valid = false;
+    plan_selection(e);
     return run_kernels(e, dev_region_of_read, (cudaStream_t)stream, false);
 }
 
@@ -869,6 +989,25 @@ int brc_fetch_device_results(brc_engine *e, void *stream) {
 }
 
 int brc_last_launch_count(const brc_engine *e) { return e ? e->launch_count : 0; }
+
+int brc_set_site_filter(brc_engine *e, const brc_site_filter *f) {
+    if (!e) return BRC_E_INVALID;
+    if (!f) { e->filter_on = false; e->filter = brc_site_filter{}; return BRC_OK; }
+    if (f->min_alt_count < 1 || f->reserved != 0 || !(f->min_alt_fraction >= 0.0 && f->min_alt_fraction <= 1.0))
+        return set_error(e, BRC_E_INVALID, "set_site_filter: min_alt_count must be >= 1 and min_alt_fraction in [0, 1]");
+    e->filter = *f; e->filter_on = true;
+    return BRC_OK;
+}
+
+int brc_get_selected_results(brc_engine *e, brc_selected_results *out) {
+    if (!e || !out) return BRC_E_INVALID;
+    if (!e->results_valid) return set_error(e, BRC_E_INVALID, "get_selected_results: no results (call brc_compute)");
+    if (!e->sparse) return set_error(e, BRC_E_INVALID, "get_selected_results: the last run had no site filter (brc_get_packed_results)");
+    out->n_regions = (int64_t)e->regions.size(); out->regions = e->regions.data(); out->n_rows = e->n_rows; out->n_slots = e->n_slots;
+    out->n_sites = e->n_sel; out->site = e->sel_site(); out->emit = e->sel_emit(); out->words = e->h_words.as<uint32_t>();
+    out->n_sec = e->h_n_sec; out->sec = e->h_sec.as<brc_sec_record>();
+    return BRC_OK;
+}
 
 int64_t brc_selftest_fastmath(brc_engine *e, int32_t max_b) {
     if (!e || max_b < 1) return BRC_E_INVALID;
@@ -897,11 +1036,13 @@ void brc_host_free(void *p) { if (p) { cudaFreeHost(p); cudaGetLastError(); } }
 int64_t brc_last_h2d_bytes(const brc_engine *e) { return e ? e->h2d_bytes_last : 0; }
 
 float brc_last_stage_ms(const brc_engine *e, int stage) {
-    if (!e || stage < 0 || stage > 2) return 0.0f;
-    // events were recorded on the launching stream around K0 and K1; wait for the last one
-    if (cudaEventSynchronize(e->ev[2]) != cudaSuccess) { cudaGetLastError(); return 0.0f; }
+    if (!e || stage < 0 || stage > 3 || (stage == 3 && !e->sel_launched)) return 0.0f;
+    // events were recorded on the launching stream around K0, K1 and the selection; wait for the last one
+    if (cudaEventSynchronize(e->ev[stage == 3 ? 3 : 2]) != cudaSuccess) { cudaGetLastError(); return 0.0f; }
     float ms = 0.0f;
-    if (cudaEventElapsedTime(&ms, e->ev[stage == 2 ? 0 : stage], e->ev[stage == 2 ? 2 : stage + 1]) != cudaSuccess) { cudaGetLastError(); return 0.0f; }
+    const int a = stage == 2 ? 0 : stage, b = stage == 2 ? 2 : (stage == 3 ? 3 : stage + 1);
+    if (stage == 3 && cudaEventElapsedTime(&ms, e->ev[2], e->ev[3]) != cudaSuccess) { cudaGetLastError(); return 0.0f; }
+    if (stage != 3 && cudaEventElapsedTime(&ms, e->ev[a], e->ev[b]) != cudaSuccess) { cudaGetLastError(); return 0.0f; }
     return ms;
 }
 

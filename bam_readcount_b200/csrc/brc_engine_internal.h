@@ -196,6 +196,24 @@ struct brc_engine {
     bool carry_on = false;
     brc::EmitState carry;
 
+    // alternative-allele site filter (brc_set_site_filter, brc_select.cu).  With it set, the kernels' records are compacted on
+    // the device to the sites that print a passing line plus their context, and only those cross PCIe.
+    bool filter_on = false;
+    brc_site_filter filter{};
+    std::vector<brc::SelRegion> sel_regions;   // the selection's region table of the current batch
+    brc::DevBuf d_sel, d_sel_regions;          // scratch + compact outputs; region table
+    bool sel_launched = false;                 // the last kernel run ended with the selection
+    brc::SelectParams sel_params{};            // ... on these buffers
+    brc_site_filter sel_filter{};              // the filter the selection ran with
+    // host results are SPARSE: n_sel shipped sites (ids ascending, emit bytes in h_sel), their words in h_words as
+    // [N_WORDS][rows*n_sel], their pool records in h_sec with slot = row * n_sel + compact index
+    bool sparse = false;
+    int64_t n_sel = 0, sel_abandoned = 0;
+    brc::PinBuf h_sel;
+    const uint32_t *sel_site() const { return h_sel.as<uint32_t>(); }
+    const uint8_t *sel_emit() const { return reinterpret_cast<const uint8_t *>(h_sel.as<uint32_t>() + n_sel); }
+    int64_t result_cols() const { return sparse ? n_sel : n_slots; }   // columns of the host word / wide arrays
+
     int launch_count = 0;
 };
 

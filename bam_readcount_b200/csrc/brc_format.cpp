@@ -67,9 +67,12 @@ struct View {   // raw result arrays of one engine
     int rows; int64_t NS, RS, SC;
     const uint32_t *ncover, *npass, *pstats, *sstats; const uint8_t *flags, *pbase, *skind;
     const int32_t *shead, *snext, *slen, *sqpos; const int64_t *sread;
+    // site filter: the arrays hold only the shipped sites (column i = site csite[i], emit byte cemit[i]); null when dense
+    const uint32_t *csite = nullptr; const uint8_t *cemit = nullptr; int64_t n_sel = 0;
     View(const brc_engine *en, int64_t g) : e(en), rg(&en->regions[(size_t)g]), ref(brc::find_ref(en, rg->tid)) {
         const brc_engine::Wide &W = e->wide;            // full-width view of the packed device records (brc::ensure_wide)
-        rows = e->n_rows; NS = e->n_slots; RS = (int64_t)rows * NS; SC = (int64_t)W.sec_next.size();
+        rows = e->n_rows; NS = e->result_cols(); RS = (int64_t)rows * NS; SC = (int64_t)W.sec_next.size();
+        if (e->sparse) { csite = e->sel_site(); cemit = e->sel_emit(); n_sel = e->n_sel; }
         ncover = W.ncover.data(); npass = W.npass.data(); pstats = W.pstats.data(); sstats = W.sec_stats.data();
         flags = W.flags.data(); pbase = W.pbase.data(); skind = W.sec_kind.data();
         shead = W.sec_head.data(); snext = W.sec_next.data(); slen = W.sec_len.data(); sqpos = W.sec_qpos.data();
@@ -80,17 +83,28 @@ struct View {   // raw result arrays of one engine
 struct Indel { std::string allele; Stat st; };
 struct Scratch { std::string rec; std::vector<Indel> indels; };
 
+// seq_nt16 code of a reference character (1/2/4/8 for one base; 15 for N, IUPAC codes and anything else)
+inline uint32_t nt16(char c) {
+    switch (c) { case 'A': case 'a': return 1; case 'C': case 'c': return 2; case 'G': case 'g': return 4; case 'T': case 't': return 8; default: return 15; }
+}
+
 // One site: pileup_func's print section.  emit=false only replays the deletion pushes (used to seed a thread's first site).
-void format_site(const View &V, int32_t s, const char *const *lib_names, EmitState &st, std::string &out, Scratch &W, bool emit) {
+// `slot` is the site's column in the result arrays (dense: rg.slot_base + s; sparse: its index among the shipped sites).  With
+// a site filter the line is printed only when the filter's rule holds on it (brc::site_passes, the device selection's rule).
+void format_site(const View &V, int32_t s, int64_t slot, const char *const *lib_names, EmitState &st, std::string &out, Scratch &W, bool emit) {
     const brc_region &rg = *V.rg;
     const int rows = V.rows; const int64_t NS = V.NS;
-    const int64_t slot = rg.slot_base + s;
     const int64_t pos = (int64_t)rg.first_pos + s;
     uint64_t n_total = 0, mapq_n = 0; bool abandoned = false;
     for (int r = 0; r < rows; ++r) { n_total += V.ncover[r * NS + slot]; mapq_n += V.npass[r * NS + slot]; abandoned |= (V.flags[r * NS + slot] & 1) != 0; }
     if (n_total == 0 || abandoned) return;   // no callback / -p with a read lacking a library: `return 0` before anything is kept
     std::string &rec = W.rec; rec.clear();
     int64_t extra_depth = 0;
+    char rb = 'N';
+    if (emit && V.ref && pos < V.ref->chrom_len && pos >= V.ref->win_beg && pos < V.ref->win_beg + (int64_t)V.ref->seq.size()) rb = V.ref->seq[(size_t)(pos - V.ref->win_beg)];   // a device-only reference window (brc_set_reference_device) has no characters here
+    const bool gate = emit && V.csite;
+    const uint32_t rcode = gate ? nt16(rb) : 15u;
+    uint64_t best_alt = 0;
     for (int r = 0; r < rows; ++r) {
         const int64_t idx = r * NS + slot;
         if (V.ncover[idx] == 0) continue;
@@ -117,10 +131,11 @@ void format_site(const View &V, int32_t s, const char *const *lib_names, EmitSta
             W.indels.push_back(std::move(in));
         }
         if (emit) for (int j = 0; j < 6; ++j) { rec += '\t'; rec += kNt[j]; rec += ':'; put_stat(rec, have[j] ? &base[j] : nullptr, false); }
+        if (gate) for (int j = 1; j <= 4; ++j) if (have[j] && brc::base_is_alt((uint32_t)j, rcode)) best_alt = std::max<uint64_t>(best_alt, base[j].v[BRC_S_COUNT]);
         if (W.indels.size() > 1) std::sort(W.indels.begin(), W.indels.end(), [](const Indel &a, const Indel &b) { return a.allele < b.allele; });
         for (auto &in : W.indels) {
             if (in.allele[0] == '-') { st.q[(size_t)r].push_back(make_qent(rg.tid, pos + 1, in.st, in.allele)); st.q_exists[(size_t)r] = 1; }
-            else if (emit) { rec += '\t'; rec += in.allele; rec += ':'; put_stat(rec, &in.st, true); }
+            else if (emit) { rec += '\t'; rec += in.allele; rec += ':'; put_stat(rec, &in.st, true); best_alt = std::max<uint64_t>(best_alt, in.st.v[BRC_S_COUNT]); }
         }
         if (emit && st.q_exists[(size_t)r]) {          // IndelQueue::process(tid, pos, record)
             auto &q = st.q[(size_t)r];
@@ -128,14 +143,14 @@ void format_site(const View &V, int32_t s, const char *const *lib_names, EmitSta
             while (!q.empty() && q.front().tid == rg.tid && q.front().pos == pos) {
                 rec += '\t'; rec += q.front().allele; rec += ':'; put_stat(rec, qstat(q.front()), true);
                 extra_depth += q.front().st[BRC_S_COUNT];
+                best_alt = std::max<uint64_t>(best_alt, q.front().st[BRC_S_COUNT]);
                 q.pop_front();
             }
         }
         if (emit && V.e->cfg.per_lib) rec += "\t}";
     }
-    if (emit && pos >= rg.beg && pos < rg.end) {
-        char rb = 'N';
-        if (V.ref && pos < V.ref->chrom_len && pos >= V.ref->win_beg && pos < V.ref->win_beg + (int64_t)V.ref->seq.size()) rb = V.ref->seq[(size_t)(pos - V.ref->win_beg)];   // a device-only reference window (brc_set_reference_device) has no characters here
+    if (emit && pos >= rg.beg && pos < rg.end &&
+        (!gate || brc::site_passes(best_alt, mapq_n + (uint64_t)extra_depth, V.e->sel_filter.min_alt_count, V.e->sel_filter.min_alt_fraction))) {
         if (V.ref) out += V.ref->name; else out += '?';
         out += '\t'; put_u(out, (uint64_t)(pos + 1)); out += '\t'; out += rb; out += '\t';
         put_u(out, (uint64_t)((int64_t)mapq_n + extra_depth));
@@ -143,10 +158,23 @@ void format_site(const View &V, int32_t s, const char *const *lib_names, EmitSta
     }
 }
 
-// sites [s0, s1) of region g, sequentially, with the caller's queue state
-void format_range(const View &V, int32_t s0, int32_t s1, const char *const *lib_names, EmitState &st, std::string &out) {
+// sites [s0, s1) of region g, sequentially, with the caller's queue state; seed: first replay the deletion pushes of site s0-1.
+// Sparse results walk the shipped sites of the range: emit byte 0 (context) only replays pushes, the others form their line.
+void format_range(const View &V, int32_t s0, int32_t s1, const char *const *lib_names, EmitState &st, std::string &out, bool seed) {
     Scratch W;
-    for (int32_t s = s0; s < s1; ++s) format_site(V, s, lib_names, st, out, W, true);
+    const int64_t base = V.rg->slot_base;
+    if (!V.csite) {
+        if (seed && s0 > 0) { std::string sink; format_site(V, s0 - 1, base + s0 - 1, lib_names, st, sink, W, false); }
+        for (int32_t s = s0; s < s1; ++s) format_site(V, s, base + s, lib_names, st, out, W, true);
+        return;
+    }
+    const uint32_t *c = V.csite, *ce = V.csite + V.n_sel;
+    const int64_t from = base + s0 - (seed && s0 > 0 ? 1 : 0);
+    for (const uint32_t *p = std::lower_bound(c, ce, (uint32_t)from); p < ce && (int64_t)*p < base + s1; ++p) {
+        const int64_t i = p - c;
+        const int32_t s = (int32_t)((int64_t)*p - base);
+        format_site(V, s, i, lib_names, st, out, W, s >= s0 && V.cemit[i] != 0);
+    }
 }
 
 // Formats sites [s0, s1) of region g.  The text is appended to `parts` as one string per worker thread (in site order), so
@@ -166,9 +194,8 @@ void format_region(const brc_engine *e, int64_t g, int32_t s0, int32_t s1, const
     const size_t base = parts_out.size();
     parts_out.resize(base + (size_t)nt);
     if (nt <= 1) {
-        if (seed_from_left && s0 > 0) { Scratch W; std::string sink; format_site(V, s0 - 1, lib_names, st, sink, W, false); }
-        parts_out[base].reserve((size_t)n * 96);
-        format_range(V, s0, s1, lib_names, st, parts_out[base]);
+        parts_out[base].reserve((size_t)(V.csite ? 0 : n) * 96);
+        format_range(V, s0, s1, lib_names, st, parts_out[base], seed_from_left);
     } else {
         std::vector<EmitState> states; states.reserve((size_t)nt);
         for (int t = 0; t < nt; ++t) states.emplace_back(e->n_rows);
@@ -176,9 +203,8 @@ void format_region(const brc_engine *e, int64_t g, int32_t s0, int32_t s1, const
             const int32_t a = s0 + (int32_t)((int64_t)n * t / nt), b = s0 + (int32_t)((int64_t)n * (t + 1) / nt);
             EmitState &ls = t == 0 ? st : states[(size_t)t];
             std::string &dst = parts_out[base + (size_t)t];
-            dst.reserve((size_t)(b - a) * 420);
-            if ((t > 0 || seed_from_left) && a > 0) { Scratch W; std::string sink; format_site(V, a - 1, lib_names, ls, sink, W, false); }
-            format_range(V, a, b, lib_names, ls, dst);
+            if (!V.csite) dst.reserve((size_t)(b - a) * 420);
+            format_range(V, a, b, lib_names, ls, dst, t > 0 || seed_from_left);
         });
         st.clear();
         for (size_t r = 0; r < st.q.size(); ++r) { st.q[r] = states[(size_t)nt - 1].q[r]; st.q_exists[r] = states[(size_t)nt - 1].q_exists[r]; }
@@ -205,10 +231,10 @@ bool format_many_site_list_regions(const brc_engine *e, const char *const *lib_n
         std::string &dst = parts_out[base + (size_t)t];
         int64_t slots = 0;
         for (size_t g = cut[(size_t)t]; g < cut[(size_t)t + 1]; ++g) slots += e->regions[g].n_slots;
-        dst.reserve((size_t)slots * 200);
+        if (!e->sparse) dst.reserve((size_t)slots * 200);
         for (size_t g = cut[(size_t)t]; g < cut[(size_t)t + 1]; ++g) {
             const View V(e, (int64_t)g);
-            format_range(V, 0, V.rg->n_slots, lib_names, st, dst);
+            format_range(V, 0, V.rg->n_slots, lib_names, st, dst, false);
             st.clear();
         }
     });

@@ -75,6 +75,17 @@ class CPackedResults(C.Structure):
                 ("words", C.c_void_p), ("n_sec", C.c_int64), ("sec", C.c_void_p), ("sec_count", C.c_void_p)]
 
 
+class CSiteFilter(C.Structure):
+    _fields_ = [("min_alt_count", C.c_int32), ("reserved", C.c_int32), ("min_alt_fraction", C.c_double)]
+
+
+class CSelectedResults(C.Structure):
+    """brc_selected_results: the sites a site filter shipped (include/brc_engine.h)."""
+    _fields_ = [("n_regions", C.c_int64), ("regions", C.POINTER(CRegion)), ("n_rows", C.c_int32), ("n_slots", C.c_int64),
+                ("n_sites", C.c_int64), ("site", C.c_void_p), ("emit", C.c_void_p), ("words", C.c_void_p), ("n_sec", C.c_int64),
+                ("sec", C.c_void_p)]
+
+
 N_WORDS = 8
 SEC_RECORD_BYTES = 72
 
@@ -83,6 +94,7 @@ EXPORTS = [
     "brc_begin_region", "brc_push_read", "brc_push_reads", "brc_end_region", "brc_decode_bam_span", "brc_push_bam_span", "brc_fetch_decoded_batch", "brc_compute", "brc_get_results",
     "brc_get_warning_counts", "brc_format_text", "brc_format_window", "brc_write_text", "brc_set_queue_carry", "brc_plan_device", "brc_run_device", "brc_device_packed_results", "brc_get_packed_results",
     "brc_fetch_device_results", "brc_last_launch_count", "brc_last_h2d_bytes", "brc_host_alloc", "brc_host_free", "brc_last_stage_ms", "brc_selftest_fastmath",
+    "brc_set_site_filter", "brc_get_selected_results",
 ]
 
 _lib = None
@@ -138,6 +150,8 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
     lib.brc_last_h2d_bytes.restype = C.c_int64
     lib.brc_last_stage_ms.argtypes = [C.c_void_p, C.c_int]
     lib.brc_last_stage_ms.restype = C.c_float
+    lib.brc_set_site_filter.argtypes = [C.c_void_p, C.POINTER(CSiteFilter)]
+    lib.brc_get_selected_results.argtypes = [C.c_void_p, C.POINTER(CSelectedResults)]
     if path is None:
         _lib = lib
     return lib
@@ -313,6 +327,35 @@ class PackedResults:
         return ncover, npass, flags, pbase, ps
 
 
+class SelectedResults:
+    """Host copy of a filtered run's sparse results (brc_get_selected_results): the shipped sites' global slot ids (ascending),
+    their emit bytes (1 = the line passes, 2 = shipped for the deletion queue, 0 = context), packed words
+    [N_WORDS][rows][n_sites] and secondary records (slot = row * n_sites + index into ``site``)."""
+
+    def __init__(self, r: CSelectedResults):
+        self.n_rows, self.n_slots, self.n_sites = int(r.n_rows), int(r.n_slots), int(r.n_sites)
+        self.regions = [dict(tid=g.tid, beg=g.beg, end=g.end, site_list_mode=g.site_list_mode, slot_base=g.slot_base,
+                             first_pos=g.first_pos, n_slots=g.n_slots) for g in (r.regions[i] for i in range(int(r.n_regions)))]
+        n = self.n_sites
+        self.site = _np_view(r.site, n, np.uint32).copy()
+        self.emit = _np_view(r.emit, n, np.uint8).copy()
+        self.words = _np_view(r.words, self.n_rows * n * N_WORDS, np.uint32).reshape(N_WORDS, self.n_rows, n).copy()
+        self.n_sec = int(r.n_sec)
+        self.sec = _np_view(r.sec, self.n_sec * (SEC_RECORD_BYTES // 4), np.uint32).reshape(self.n_sec, SEC_RECORD_BYTES // 4).copy()
+
+    def nbytes(self) -> int:
+        """What crossed PCIe for these results: site ids, emit bytes, words and records."""
+        return int(self.site.nbytes + self.emit.nbytes + self.words.nbytes + self.sec.nbytes)
+
+    def positions(self, emit: int = 1):
+        """0-based reference positions of the sites with the given emit byte, in slot order."""
+        starts = np.array([g["slot_base"] for g in self.regions], dtype=np.int64)
+        s = self.site[self.emit == emit].astype(np.int64)
+        g = np.searchsorted(starts, s, side="right") - 1                 # last region starting at or before the slot
+        first = np.array([g_["first_pos"] for g_ in self.regions], dtype=np.int64)
+        return (first[g] + s - starts[g]).tolist()
+
+
 class Engine:
     """One engine handle == one bam-readcount "process" on one GPU."""
 
@@ -411,8 +454,10 @@ class Engine:
     def end_region(self):
         self._check(self.lib.brc_end_region(self.h))
 
-    def compute(self) -> Results:
+    def compute(self) -> Optional[Results]:
         self._check(self.lib.brc_compute(self.h))
+        if getattr(self, "filtered", False):
+            return None
         r = CResults()
         self._check(self.lib.brc_get_results(self.h, C.byref(r)))
         res = Results(r)
@@ -449,8 +494,10 @@ class Engine:
         self._check(self.lib.brc_device_packed_results(self.h, C.byref(r)))
         return r
 
-    def fetch_device_results(self, stream_ptr: int) -> Results:
+    def fetch_device_results(self, stream_ptr: int) -> Optional[Results]:
         self._check(self.lib.brc_fetch_device_results(self.h, stream_ptr))
+        if getattr(self, "filtered", False):
+            return None
         r = CResults()
         self._check(self.lib.brc_get_results(self.h, C.byref(r)))
         res = Results(r)
@@ -461,6 +508,23 @@ class Engine:
         r = CPackedResults()
         self._check(self.lib.brc_get_packed_results(self.h, C.byref(r)))
         return PackedResults(r)
+
+    # ---- alternative-allele site filter (include/brc_engine.h brc_set_site_filter) ----------------------------------------
+    def set_site_filter(self, min_alt_count: int, min_alt_fraction: float = 0.0):
+        """Print only lines with an alternative allele of count >= min_alt_count and >= min_alt_fraction * depth (from the next
+        compute() on); while set, compute() returns None (no dense view) and selected() is the sparse result."""
+        f = CSiteFilter(int(min_alt_count), 0, float(min_alt_fraction))
+        self._check(self.lib.brc_set_site_filter(self.h, C.byref(f)))
+        self.filtered = True
+
+    def clear_site_filter(self):
+        self._check(self.lib.brc_set_site_filter(self.h, None))
+        self.filtered = False
+
+    def selected(self) -> SelectedResults:
+        r = CSelectedResults()
+        self._check(self.lib.brc_get_selected_results(self.h, C.byref(r)))
+        return SelectedResults(r)
 
     def stage_ms(self, stage: int) -> float:
         return float(self.lib.brc_last_stage_ms(self.h, stage))

@@ -288,6 +288,47 @@ BRC_API int64_t brc_format_window(brc_engine *e, int64_t region_index, int64_t f
  * ignored); otherwise the window [first, first+count) of that region (count < 0: to its end).  Returns bytes written. */
 BRC_API int64_t brc_write_text(brc_engine *e, int64_t region_index, int64_t first, int64_t count, const char *const *lib_names, int fd);
 
+/* ---- alternative-allele site filter ----------------------------------------------------------
+ * Prints only the lines a user would keep when looking for non-reference alleles: a line is printed iff one of its allele
+ * entries (any library block with -p) is an ALTERNATIVE allele whose count c satisfies c >= min_alt_count and
+ * c >= min_alt_fraction * depth (IEEE double; depth = the line's 4th column).  Alternative alleles: every insertion (+...)
+ * and deletion (-...) entry printed on the line, and an A/C/G/T entry whose seq_nt16 code differs from the reference base's
+ * (a reference N, IUPAC code or missing character makes all four alternative; case is ignored).  "=" and "N" never are.
+ * The reference base is the one the text prints: for a contig set only with brc_set_reference_device that is N.
+ * Every printed line is byte-identical to the line the unfiltered run prints for that site; the filter only removes lines.
+ *
+ * The sites are selected on the device right after the pileup kernels (brc_compute, brc_run_device) and only the selected
+ * sites' records are copied to the host.  While a filter is set there is no dense view: brc_get_results and
+ * brc_get_packed_results return BRC_E_INVALID; brc_get_selected_results is the sparse view. */
+typedef struct {
+    int32_t min_alt_count;        /* >= 1 */
+    int32_t reserved;             /* 0 */
+    double min_alt_fraction;      /* in [0, 1] */
+} brc_site_filter;
+/* f == NULL turns the filter off (the unfiltered path, exactly as without this call); takes effect at the next brc_compute /
+ * brc_run_device.  Out-of-range values: BRC_E_INVALID. */
+BRC_API int brc_set_site_filter(brc_engine *e, const brc_site_filter *f);
+/* Sparse host view of a filtered run: the shipped sites (global slot ids, ascending) with their emit byte
+ *   1: the line passes the filter   2: shipped for the deletion queue (a range whose lines may carry deletions queued by an
+ *      earlier region, or the last site of an argv region that forms a line and that a library row covers); the emitter forms
+ *      the line and evaluates the rule on it   0: context only (the left neighbour of a site with emit byte 1 or 2: its
+ *      deletions print on that line)
+ * their packed words [BRC_N_WORDS][n_rows * n_sites] (the packed layout with n_sites columns) and their secondary-pool
+ * records, whose slot is row * n_sites + index into site[]. */
+typedef struct {
+    int64_t n_regions;
+    const brc_region *regions;
+    int32_t n_rows;
+    int64_t n_slots;              /* dense slots of the batch (site[] indexes them) */
+    int64_t n_sites;
+    const uint32_t *site;
+    const uint8_t *emit;
+    const uint32_t *words;
+    int64_t n_sec;
+    const brc_sec_record *sec;
+} brc_selected_results;
+BRC_API int brc_get_selected_results(brc_engine *e, brc_selected_results *out);
+
 /* ---- device-resident path (bench "value": inputs already in HBM) -------------------------
  * brc_plan_device: fix the region geometry (host array of n_regions regions with read_lo/hi,
  * slot_base, first_pos, n_slots filled) and size the outputs.  brc_run_device: launch the
@@ -316,7 +357,8 @@ BRC_API int brc_last_launch_count(const brc_engine *e);
  * fixed-length reads are rebuilt on the device and do not count) */
 BRC_API int64_t brc_last_h2d_bytes(const brc_engine *e);
 /* elapsed GPU milliseconds of the named stage of the last run, measured with CUDA events on the
- * launching stream: 0 = per-read precompute kernel, 1 = pileup kernel, 2 = whole device step */
+ * launching stream: 0 = per-read precompute kernel, 1 = pileup kernel, 2 = whole device step (without the selection),
+ * 3 = site selection + compaction (0 when no filter was set) */
 BRC_API float brc_last_stage_ms(const brc_engine *e, int stage);
 
 #ifdef __cplusplus
