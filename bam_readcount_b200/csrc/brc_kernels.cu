@@ -1598,7 +1598,9 @@ __global__ void fastmath_selftest_kernel(int max_b, unsigned long long *bad) {
     if (b > max_b) return;
     const float fb = (float)b, rcp = __frcp_rn(fb);
     unsigned long long nbad = 0;
-    for (int a = threadIdx.x; a <= 2 * b + 2; a += blockDim.x) {
+    // every numerator the hot path can form for any divisor: |2 (qpos - left_clip) - clipped_length| reaches 2 (l_qseq - 1) when a
+    // soft clip after a hard clip counts as a right clip (5H100S10M: 190..208 over 10)
+    for (int a = threadIdx.x; a <= 2 * FASTDIV_MAX + 2; a += blockDim.x) {
         const float fa = (float)a;
         const float want = __fdiv_rn(fa, fb), got = div_small(fa, fb, rcp);
         if (__float_as_uint(want) != __float_as_uint(got)) nbad++;

@@ -9,6 +9,9 @@ the UNMODIFIED reference binary oracle/_ref/bam-readcount (oracle/build_ref.sh).
   ref_<case>_<flags>.txt.gz        reference-binary STDOUT on the deterministic synthetic cases
                                    of tests/cases.py (deletions, insertions, -q/-b, -i, -p, -d)
   edge_*.txt.gz                    reference-binary STDOUT on the hand-built edge-case reads
+  fresh_fuzz_sha256.json, boundary_sha256.json
+                                   SHA-256 of the reference binary's STDOUT on the fuzz seeds of test_differential_fuzz.py and
+                                   on the capacity-boundary cases of boundary_cases.py (--boundary-only: only the latter)
 """
 import gzip
 import hashlib
@@ -49,14 +52,30 @@ def decode_fixture(bam, out):
 
 def write_case_files(case, d):
     name, L, seq, wb = case["contigs"][0]
-    assert wb == 0
+    if wb:      # the engine and the oracle get a window of the contig; the reference binary reads all of it
+        seq = case["full_ref"]
     synth.write_fasta(os.path.join(d, "ref.fa"), name, np.frombuffer(seq, dtype=np.uint8))
     synth.write_sam(os.path.join(d, "s.sam"), case["batch"], [(name, L)], n_libs=len(case["lib_names"]),
                     read_group=case.get("read_group", True))
-    if "sam_header_extra" in case:
-        pass
+    _missing_qual_as_star(os.path.join(d, "s.sam"))
     subprocess.check_call([REF_SAMTOOLS, "view", "-b", "-o", os.path.join(d, "s.bam"), os.path.join(d, "s.sam")])
     subprocess.check_call([REF_SAMTOOLS, "index", os.path.join(d, "s.bam")])
+
+
+def _missing_qual_as_star(path):
+    """Quality bytes of 0xFF (a read stored with QUAL '*') come out of write_sam as spaces: write them as '*'.  SAM has no way to
+    write 0xFF for only some bases of a read, so a batch holding such a read is refused."""
+    with open(path) as fh:
+        lines = fh.read().split("\n")
+    for i, ln in enumerate(lines):
+        f = ln.split("\t")
+        if len(f) > 10 and not ln.startswith("@") and " " in f[10]:
+            if f[10].strip(" "):
+                raise ValueError(f"{f[0]}: quality 0xFF on some bases only cannot be written as SAM")
+            f[10] = "*"
+            lines[i] = "\t".join(f)
+    with open(path, "w") as fh:
+        fh.write("\n".join(lines))
 
 
 def reference_stdout(case, flags, d, site_list):
@@ -85,8 +104,28 @@ def fresh_fuzz_jobs():
     return jobs
 
 
+def boundary_jobs():
+    """The capacity-boundary cases of tests/boundary_cases.py: every flag set, in each region mode the case runs in."""
+    import boundary_cases
+    return boundary_cases.jobs()
+
+
+def write_sha_file(jobs, out):
+    sums, dirs = {}, {}
+    for case, fname, fl, sl, key in jobs:
+        if case["name"] not in dirs:
+            dirs[case["name"]] = tempfile.mkdtemp()
+            write_case_files(case, dirs[case["name"]])
+        sums[key] = hashlib.sha256(reference_stdout(case, fl, dirs[case["name"]], sl).encode("latin-1")).hexdigest()
+    with open(os.path.join(HERE, out), "w") as fh:
+        json.dump(sums, fh, indent=1, sort_keys=True)
+
+
 def main():
     assert os.path.exists(REF_BIN), "run oracle/build_ref.sh first"
+    if "--boundary-only" in sys.argv:
+        write_sha_file(boundary_jobs(), "boundary_sha256.json")
+        return
     for f in ("expected_all_lib", "expected_per_lib", "expected_insertion_centric_all_lib",
               "expected_insertion_centric_per_lib"):
         shutil.copy(os.path.join(TD, f), os.path.join(HERE, f))
@@ -123,15 +162,9 @@ def main():
             fh.write(txt.encode("latin-1"))
         print(outname, len(txt.splitlines()), "lines")
 
-    # the fuzz seeds: only the SHA-256 of the reference's STDOUT is kept
-    sums, dirs = {}, {}
-    for case, fname, fl, sl, key in fresh_fuzz_jobs():
-        if case["name"] not in dirs:
-            dirs[case["name"]] = tempfile.mkdtemp()
-            write_case_files(case, dirs[case["name"]])
-        sums[key] = hashlib.sha256(reference_stdout(case, fl, dirs[case["name"]], sl).encode("latin-1")).hexdigest()
-    with open(os.path.join(HERE, "fresh_fuzz_sha256.json"), "w") as fh:
-        json.dump(sums, fh, indent=1, sort_keys=True)
+    # the fuzz seeds and the boundary cases: only the SHA-256 of the reference's STDOUT is kept
+    write_sha_file(fresh_fuzz_jobs(), "fresh_fuzz_sha256.json")
+    write_sha_file(boundary_jobs(), "boundary_sha256.json")
 
 
 if __name__ == "__main__":
