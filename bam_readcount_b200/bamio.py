@@ -45,39 +45,60 @@ class BamHeader:
         return self.lib_id[lb]
 
 
-_AUX_SIZE = {"c": 1, "C": 1, "s": 2, "S": 2, "i": 4, "I": 4, "f": 4, "A": 1}
-_AUX_FMT = {"c": "<b", "C": "<B", "s": "<h", "S": "<H", "i": "<i", "I": "<I"}
+_AUX_SIZE = {"A": 1, "c": 1, "C": 1, "s": 2, "S": 2, "i": 4, "I": 4, "f": 4, "d": 8}
+_AUX_INT = {"c": "<b", "C": "<B", "s": "<h", "S": "<H", "i": "<i", "I": "<i"}   # I: bam_aux2i kept in an int32_t, as the reference does
 
 
-def _scan_aux(aux: bytes) -> Tuple[Optional[int], Optional[int], Optional[str]]:
-    """Return (NM, SM, RG): first occurrence of each, like bam_aux_get's linear scan."""
-    nm = sm = rg = None
-    i, n = 0, len(aux)
-    while i + 3 <= n:
-        tag = aux[i:i + 2]
-        typ = chr(aux[i + 2])
-        i += 3
-        if typ in _AUX_SIZE:
-            sz = _AUX_SIZE[typ]
-            if typ in _AUX_FMT and tag in (b"NM", b"SM"):
-                v = struct.unpack_from(_AUX_FMT[typ], aux, i)[0]
-                if tag == b"NM" and nm is None:
-                    nm = v
-                elif tag == b"SM" and sm is None:
-                    sm = v
-            i += sz
-        elif typ in "ZH":
-            j = aux.index(b"\0", i)
-            if tag == b"RG" and rg is None and typ == "Z":
-                rg = aux[i:j].decode()
-            i = j + 1
-        elif typ == "B":
-            sub = chr(aux[i])
-            cnt = struct.unpack_from("<I", aux, i + 1)[0]
-            i += 5 + cnt * _AUX_SIZE[sub]
-        else:
+def _skip_aux(d: bytes, o: int, end: int) -> int:
+    """Offset past the value whose type byte is at d[o], or -1 when it cannot be skipped (csrc/brc_aux.cuh: skip)."""
+    t = chr(d[o]); o += 1
+    if t in "ZH":
+        j = d.find(b"\0", o, end)
+        return end if j < 0 else j + 1
+    if t == "B":
+        if end - o < 5:
+            return -1
+        es = _AUX_SIZE.get(chr(d[o]), 0)
+        n = struct.unpack_from("<I", d, o + 1)[0]
+        o += 5
+        return -1 if es == 0 or end - o < es * n else o + es * n
+    sz = _AUX_SIZE.get(t, 0)
+    return -1 if sz == 0 or end - o < sz else o + sz
+
+
+def _scan_aux(d: bytes, aux_o: int, end: int):
+    """(NM, SM, RG ID bytes, CG type offset) of the record body d[..end) whose tags start at aux_o, by the rules of
+    csrc/brc_aux.cuh: the first tag of each name; the walk stops at a value that cannot be skipped; a non-integer NM/SM is
+    present and worth 0; the first RG names the read group whatever its type."""
+    nm = sm = rg = cg = None
+    o = aux_o
+    while end - o >= 3:
+        tag = d[o:o + 2]; o += 2
+        e = _skip_aux(d, o, end)
+        if e >= 0 and chr(d[o]) in "ZH" and d[e - 1] != 0:
+            e = -2                                           # a wanted Z/H without its NUL is absent; the walk ends here anyway
+        if tag in (b"NM", b"SM") and (nm if tag == b"NM" else sm) is None:
+            v = False
+            if e >= 0:
+                t = chr(d[o])
+                v = struct.unpack_from(_AUX_INT[t], d, o + 1)[0] if t in _AUX_INT else 0
+            if tag == b"NM":
+                nm = v
+            else:
+                sm = v
+        elif tag == b"RG" and rg is None:
+            if e >= 0:
+                z = d.find(b"\0", o + 1, end)
+                rg = d[o + 1:end if z < 0 else z]
+            else:
+                rg = False
+        elif tag == b"CG" and cg is None:
+            cg = o if e >= 0 else False
+        if e < 0:
             break
-    return nm, sm, rg
+        o = e
+    # False: the first tag of that name could not be read, so the read has none
+    return tuple(None if x is False else x for x in (nm, sm, rg, cg))
 
 
 def read_bam(path: str) -> Tuple[BamHeader, ReadBatch]:
@@ -107,10 +128,16 @@ def read_bam(path: str) -> Tuple[BamHeader, ReadBatch]:
         cig = np.frombuffer(raw, dtype="<u4", count=n_cig, offset=q); q += 4 * n_cig
         sq = np.frombuffer(raw, dtype=np.uint8, count=(l_seq + 1) // 2, offset=q); q += (l_seq + 1) // 2
         ql = np.frombuffer(raw, dtype=np.uint8, count=l_seq, offset=q); q += l_seq
-        a_nm, a_sm, a_rg = _scan_aux(raw[q:o + bs])
+        a_nm, a_sm, a_rg, a_cg = _scan_aux(raw, q, o + bs)
+        # a long CIGAR kept in CG:B:I behind a <l_qseq>S placeholder (csrc/brc_aux.cuh: scan)
+        if (a_cg is not None and raw[a_cg:a_cg + 2] == b"BI" and n_cig > 0 and refid >= 0 and p >= 0
+                and int(cig[0]) == (l_seq << 4 | 4)):
+            n_cg = struct.unpack_from("<I", raw, a_cg + 2)[0]
+            if n_cig <= n_cg < 1 << 29:
+                cig = np.frombuffer(raw, dtype="<u4", count=n_cg, offset=a_cg + 6)
         o += bs
         tid.append(refid); pos.append(p); flag.append(fl); mapq.append(mq); lq.append(l_seq)
-        lib.append(hdr.lib_of_rg(a_rg))
+        lib.append(hdr.lib_of_rg(None if a_rg is None else a_rg.decode("utf-8", "surrogateescape")))
         nm.append(int(TAG_ABSENT) if a_nm is None else a_nm)
         sm.append(int(TAG_ABSENT) if a_sm is None else a_sm)
         cig_parts.append(cig); seq_parts.append(sq); qual_parts.append(ql)

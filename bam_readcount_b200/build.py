@@ -10,7 +10,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libbrc_engine.so")
 SOURCES = ["brc_kernels.cu", "brc_engine.cu", "brc_bgzf.cu", "brc_select.cu", "brc_format.cpp"]
-HEADERS = ["brc_device.cuh", "brc_engine_internal.h", "brc_fmt_num.h", "brc_bgzf.cuh", "brc_scan.cuh", os.path.join("..", "..", "include", "brc_engine.h")]
+HEADERS = ["brc_device.cuh", "brc_engine_internal.h", "brc_fmt_num.h", "brc_aux.cuh", "brc_bgzf.cuh", "brc_scan.cuh", os.path.join("..", "..", "include", "brc_engine.h")]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
@@ -93,7 +93,7 @@ def build_cli(force: bool = False) -> str:
     """The C++ host binary (same CLI / STDOUT as bam-readcount) on top of libbrc_engine.so."""
     src = os.path.join(CSRC, "brc_cli.cpp")
     hts_a = os.path.join(HERE, "third_party", "htslib", "libhts.a")
-    newest = max([os.path.getmtime(src), os.path.getmtime(LIB)] + ([os.path.getmtime(hts_a)] if os.path.exists(hts_a) else []))
+    newest = max([os.path.getmtime(src), os.path.getmtime(os.path.join(CSRC, "brc_aux.cuh")), os.path.getmtime(LIB)] + ([os.path.getmtime(hts_a)] if os.path.exists(hts_a) else []))
     if not force and os.path.exists(CLI) and os.path.getmtime(CLI) >= newest:
         return CLI
     cmd = ["g++", "-O2", "-std=c++17", "-Wall", "-o", CLI, src, "-I", os.path.join(HERE, "..", "include"),

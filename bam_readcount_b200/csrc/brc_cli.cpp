@@ -33,6 +33,7 @@
 #include <unistd.h>
 
 #include "../../include/brc_engine.h"
+#include "brc_aux.cuh"
 #ifdef BRC_WITH_HTSLIB
 #include <functional>
 #include <htslib/sam.h>
@@ -247,15 +248,6 @@ struct Rec {   // one decoded alignment (the bam1_t fields the path reads)
     const uint32_t *cigar; const uint8_t *seq, *qual; std::string rg; bool has_rg;
 };
 
-int64_t aux_int(const uint8_t *p, char t) {
-    switch (t) {
-    case 'c': return (int8_t)p[0]; case 'C': return p[0];
-    case 's': { int16_t v; std::memcpy(&v, p, 2); return v; } case 'S': { uint16_t v; std::memcpy(&v, p, 2); return v; }
-    case 'i': { int32_t v; std::memcpy(&v, p, 4); return v; } case 'I': { uint32_t v; std::memcpy(&v, p, 4); return v; }
-    default: return 0;
-    }
-}
-
 bool read_record(Bgzf &bz, Rec &r) {
     int32_t bs;
     if (!bz.read(&bs, 4)) return false;                                   // EOF (clean unless bz.error)
@@ -266,28 +258,15 @@ bool read_record(Bgzf &bz, Rec &r) {
     int32_t refid, pos, l_seq; uint8_t l_rn, mapq; uint16_t n_cig, flag;
     std::memcpy(&refid, d, 4); std::memcpy(&pos, d + 4, 4); l_rn = d[8]; mapq = d[9];
     std::memcpy(&n_cig, d + 12, 2); std::memcpy(&flag, d + 14, 2); std::memcpy(&l_seq, d + 16, 4);
-    r.tid = refid; r.pos = pos; r.mapq = mapq; r.flag = flag; r.n_cigar = n_cig; r.l_qseq = l_seq;
-    size_t o = 32 + l_rn;
-    r.cigar = (const uint32_t *)(d + o); o += 4 * (size_t)n_cig;
+    r.tid = refid; r.pos = pos; r.mapq = mapq; r.flag = flag; r.l_qseq = l_seq;
+    size_t o = 32 + l_rn + 4 * (size_t)n_cig;
     r.seq = d + o; o += ((size_t)l_seq + 1) / 2;
     r.qual = d + o; o += (size_t)l_seq;
-    r.nm = BRC_TAG_ABSENT; r.sm = BRC_TAG_ABSENT; r.has_rg = false;
-    bool got_nm = false, got_sm = false;
-    while (o + 3 <= (size_t)bs) {          // bam_aux_get's linear scan: first occurrence wins
-        const uint8_t *t = d + o; const char ty = (char)t[2]; o += 3;
-        size_t sz = 0;
-        switch (ty) {
-        case 'A': case 'c': case 'C': sz = 1; break;
-        case 's': case 'S': sz = 2; break;
-        case 'i': case 'I': case 'f': sz = 4; break;
-        case 'Z': case 'H': { size_t e = o; while (e < (size_t)bs && d[e]) ++e; if (ty == 'Z' && t[0] == 'R' && t[1] == 'G' && !r.has_rg) { r.rg.assign((const char *)d + o, e - o); r.has_rg = true; } o = e + 1; continue; }
-        case 'B': { const char st = (char)d[o]; uint32_t cnt; std::memcpy(&cnt, d + o + 1, 4); size_t es = (st == 'c' || st == 'C') ? 1 : (st == 's' || st == 'S') ? 2 : 4; o += 5 + es * cnt; continue; }
-        default: o = (size_t)bs; continue;
-        }
-        if (t[0] == 'N' && t[1] == 'M' && !got_nm && ty != 'A' && ty != 'f') { r.nm = (int32_t)aux_int(d + o, ty); got_nm = true; }
-        if (t[0] == 'S' && t[1] == 'M' && !got_sm && ty != 'A' && ty != 'f') { r.sm = (int32_t)aux_int(d + o, ty); got_sm = true; }
-        o += sz;
-    }
+    const brc::aux::RecAux ax = brc::aux::scan(d, bs, (int64_t)o, 32 + l_rn, n_cig);     // NM, SM, RG, CG (brc_aux.cuh)
+    r.cigar = (const uint32_t *)(d + ax.cig_o); r.n_cigar = ax.n_cigar;
+    r.nm = ax.nm; r.sm = ax.sm;
+    r.has_rg = ax.rg_o >= 0;
+    if (r.has_rg) r.rg.assign((const char *)d + ax.rg_o, (size_t)ax.rg_len);
     return true;
 }
 
@@ -434,8 +413,8 @@ struct HtsSource {
             uint8_t *p;
             r.nm = (p = bam_aux_get(b, "NM")) ? (int32_t)bam_aux2i(p) : BRC_TAG_ABSENT;
             r.sm = (p = bam_aux_get(b, "SM")) ? (int32_t)bam_aux2i(p) : BRC_TAG_ABSENT;
-            r.has_rg = (p = bam_aux_get(b, "RG")) != nullptr && *p == 'Z';
-            if (r.has_rg) r.rg = (const char *)(p + 1);
+            r.has_rg = (p = bam_aux_get(b, "RG")) != nullptr;                                        // bam_get_library: the first RG, any type
+            if (r.has_rg) r.rg.assign((const char *)(p + 1), strnlen((const char *)(p + 1), (size_t)(b->data + b->l_data - (p + 1))));
             r.endpos = rec_endpos(r);
             emit(r);
         }

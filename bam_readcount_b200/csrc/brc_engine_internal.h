@@ -175,6 +175,7 @@ struct brc_engine {
         int kernels = 0;
         bool valid = false;              // a decoded batch is resident
         bool pushed = false;             // ... and it is the open / only region's read stream (brc_push_bam_span)
+        cudaStream_t stream = nullptr;   // the stream the decode kernels ran on
         std::vector<std::vector<uint8_t>> host;   // brc_fetch_decoded_batch
         // packed bases of the reads that carry an insertion allele (the text emitter prints them), fetched after the kernels
         std::vector<int64_t> ins_reads; std::vector<uint64_t> ins_off; std::vector<uint8_t> ins_pool;

@@ -12,6 +12,8 @@ the UNMODIFIED reference binary oracle/_ref/bam-readcount (oracle/build_ref.sh).
   fresh_fuzz_sha256.json, boundary_sha256.json
                                    SHA-256 of the reference binary's STDOUT on the fuzz seeds of test_differential_fuzz.py and
                                    on the capacity-boundary cases of boundary_cases.py (--boundary-only: only the latter)
+  decode_sha256.json               SHA-256 of the reference binary's STDOUT and STDERR on the crafted BAMs of bam_craft.py
+                                   (--decode-only: only this)
 """
 import gzip
 import hashlib
@@ -121,8 +123,29 @@ def write_sha_file(jobs, out):
         json.dump(sums, fh, indent=1, sort_keys=True)
 
 
+def write_decode_sha():
+    """SHA-256 of the reference binary's STDOUT and STDERR on every crafted BAM of bam_craft.py that it reads as stored, per
+    flag set of the decode tests."""
+    import bam_craft
+    sums = {}
+    d = tempfile.mkdtemp()
+    for f in bam_craft.write_corpus(d, REF_SAMTOOLS):
+        if not f["vs_reference"]:
+            continue
+        for fname, argv in bam_craft.FLAG_SETS.items():
+            out, err, rc = run_reference_binary(["-w", "1"] + argv + ["-f", f["fasta"], f["bam"]] + f["regions"])
+            assert rc == 0, err[-2000:]
+            sums[f"{f['name']}_{fname}"] = dict(stdout=hashlib.sha256(out.encode("latin-1")).hexdigest(),
+                                                stderr=hashlib.sha256(err.encode("latin-1")).hexdigest())
+    with open(os.path.join(HERE, "decode_sha256.json"), "w") as fh:
+        json.dump(sums, fh, indent=1, sort_keys=True)
+
+
 def main():
     assert os.path.exists(REF_BIN), "run oracle/build_ref.sh first"
+    if "--decode-only" in sys.argv:
+        write_decode_sha()
+        return
     if "--boundary-only" in sys.argv:
         write_sha_file(boundary_jobs(), "boundary_sha256.json")
         return
@@ -165,6 +188,7 @@ def main():
     # the fuzz seeds and the boundary cases: only the SHA-256 of the reference's STDOUT is kept
     write_sha_file(fresh_fuzz_jobs(), "fresh_fuzz_sha256.json")
     write_sha_file(boundary_jobs(), "boundary_sha256.json")
+    write_decode_sha()
 
 
 if __name__ == "__main__":
