@@ -9,8 +9,10 @@
 // Mirrors, region by region, the reference's two loops:
 //   -l site list : R:...:574-608  (d.beg=beg-1, d.end=end, queues cleared per region)
 //   argv regions : R:...:641-657  (bam_parse_region; a bare contig name keeps the previous beg/end, A.6)
+// With --bam-list the same per-sample run is repeated over a list of inputs in one process (DESIGN.md §11).
 #include <algorithm>
 #include <cerrno>
+#include <cstdarg>
 #include <climits>
 #include <cstdint>
 #include <cstdio>
@@ -19,6 +21,8 @@
 #include <fstream>
 #include <getopt.h>
 #include <deque>
+#include <fcntl.h>
+#include <filesystem>
 #include <map>
 #include <set>
 #include <sstream>
@@ -440,6 +444,7 @@ struct Warner {
     long long max_per_type; bool unlimited; int min_mapq, min_bq; bool per_lib, ic;
     long long counts[NT] = {0, 0, 0, 0};
     std::vector<Cand> cands; std::vector<Reg> regs;
+    FILE *err = stderr;           // the sample's message stream
     Warner(long long mw, int q, int b, bool p, bool i) : max_per_type(mw < 0 ? 1000 : mw), unlimited(mw < 0), min_mapq(q), min_bq(b), per_lib(p), ic(i) {}
     bool budget_left() const { return counts[SM] < max_per_type || counts[NM] < max_per_type || (per_lib && counts[LIB] < max_per_type); }
     bool collecting() const { return max_per_type > 0 && budget_left(); }
@@ -466,8 +471,8 @@ struct Warner {
                                       "Library unavailable. Check to make sure the LB tag is present in the @RG entries of the header."};
         ++counts[type];
         if (counts[type] > max_per_type) return;
-        std::fprintf(stderr, "WARNING: In read %s: %s\n", qname.c_str(), msg[type]);
-        if (!unlimited && counts[type] == max_per_type) std::fprintf(stderr, "The previous warning has been emitted %lld times and will be disabled.\n", counts[type]);
+        std::fprintf(err, "WARNING: In read %s: %s\n", qname.c_str(), msg[type]);
+        if (!unlimited && counts[type] == max_per_type) std::fprintf(err, "The previous warning has been emitted %lld times and will be disabled.\n", counts[type]);
     }
     // stateless resolve_cigar2 (V:htslib-1.10/sam.c:3964-4041): qpos / is_del / indel of `site` in a read
     static bool resolve(const Cand &c, int64_t site, int &qpos, int &indel) {
@@ -518,7 +523,7 @@ struct Warner {
     void finish(const int64_t engine_counts[4]) const {
         if (!unlimited) return;
         static const char *nm[NT] = {"SM tag missing", "NM tag missing", "generated tag missing", "library unavailable"};
-        for (int t = 0; t < NT; ++t) if (engine_counts[t] > max_per_type) std::fprintf(stderr, "WARNING: %s: %lld events in total (only the first %lld are listed)\n", nm[t], (long long)engine_counts[t], max_per_type);
+        for (int t = 0; t < NT; ++t) if (engine_counts[t] > max_per_type) std::fprintf(err, "WARNING: %s: %lld events in total (only the first %lld are listed)\n", nm[t], (long long)engine_counts[t], max_per_type);
     }
 };
 
@@ -564,6 +569,7 @@ struct WindowJob {   // one decoded window: the slices and the concatenated batc
     brc_read_batch batch{};
     uint64_t n_decoded = 0; bool error = false, cand_overflow = false;
     int tid = -1; int64_t fbeg = 0, fend = 0;
+    std::string timing;           // BRC_CLI_TIMING line, printed to the sample's stream by the thread that takes the job
 };
 
 struct ParallelFetcher {
@@ -623,7 +629,7 @@ struct ParallelFetcher {
 
     // decode [fbeg, fend) of `tid` into job.slices and job.batch; false when a reader could not be opened
     bool run(int tid, int64_t fbeg, int64_t fend, bool collect, WindowJob &job) {
-        job.tid = tid; job.fbeg = fbeg; job.fend = fend; job.error = false; job.cand_overflow = false; job.n_decoded = 0;
+        job.tid = tid; job.fbeg = fbeg; job.fend = fend; job.error = false; job.cand_overflow = false; job.n_decoded = 0; job.timing.clear();
         const int64_t w0 = fbeg >> 14, w1 = (fend + 16383) >> 14;
         const int T = (int)std::max<int64_t>(1, std::min<int64_t>(n_threads, (w1 - w0) / 4));
         while ((int)readers.size() < T) { readers.emplace_back(new Bgzf()); if (!readers.back()->open_worker(path)) return false; }
@@ -676,7 +682,11 @@ struct ParallelFetcher {
             copy(0);
             for (auto &x : th) x.join();
         }
-        if (timing) std::fprintf(stderr, "[brc timing] window %d:%lld-%lld: %d threads decode %.3fs, concatenate %.3fs (%zu reads)\n", tid, (long long)fbeg, (long long)fend, T, t1 - t0, clk() - t1, n);
+        if (timing) {
+            char line[256];
+            std::snprintf(line, sizeof line, "[brc timing] window %d:%lld-%lld: %d threads decode %.3fs, concatenate %.3fs (%zu reads)\n", tid, (long long)fbeg, (long long)fend, T, t1 - t0, clk() - t1, n);
+            job.timing = line;
+        }
         brc_read_batch &b = job.batch;
         b = brc_read_batch{};
         b.n_reads = (int64_t)n; b.tid = nullptr; b.pos = pos; b.flag = flag; b.mapq = mapq; b.lib = lib; b.l_qseq = lq; b.nm = nm; b.sm = sm;
@@ -738,7 +748,12 @@ void usage() {
                 "  --min-alt-count N                     (this host) print only the sites where an alternative allele (a base other than\n"
                 "                                        the reference base, an insertion or a deletion) has a count of at least N\n"
                 "  --min-alt-fraction F                  (this host) ... and of at least F times the site's depth (0 <= F <= 1; without\n"
-                "                                        --min-alt-count the count must be at least 1).  Printed lines are unchanged\n\n");
+                "                                        --min-alt-count the count must be at least 1).  Printed lines are unchanged\n"
+                "  --bam-list FILE                       (this host) run many samples in one process.  Each line of FILE is\n"
+                "                                        INPUT<TAB>OUT or INPUT<TAB>OUT<TAB>ERR (ERR defaults to OUT.log); OUT and ERR get\n"
+                "                                        exactly what `brc-readcount <options> INPUT <regions>` prints on STDOUT and\n"
+                "                                        STDERR.  Every positional argument is a region; a failed sample does not stop\n"
+                "                                        the others (exit status 1 at the end)\n\n");
 }
 
 // samtools region string "name[:beg[-end]]" as bam_parse_region (V:bam_aux.c:65-75) handles it.  Returns 0 when beg and end were
@@ -768,126 +783,179 @@ int parse_region(const BamFile &bam, const std::string &s, int &tid, int &beg, i
     return 0;
 }
 
-}  // namespace
-
-int main(int argc, char **argv) {
-    const double t_main0 = std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count();
+// ------------------------------------------------------------------------------------------
+// One sample = what a run on one BAM/CRAM does.  The run is split in two so that a cohort (--bam-list) can open sample k+1
+// on a worker thread while sample k computes:
+//   open_sample : the input, its header, @RG/LB map, BAI/CRAI, the FASTA index, the region list and its windows, and the
+//                 decode of the first window.  Its messages go to Sample::log (Messages).
+//   run_sample  : the region loop on the engine handle for the sample's library count; text to a given fd, messages to
+//                 stderr, which a cohort points at the sample's ERR file for the time of the sample (htslib writes there too).
+// A run on one input calls the same two functions with STDOUT_FILENO and the process's stderr, so each sample of a cohort
+// prints exactly the bytes its own run prints.
+// ------------------------------------------------------------------------------------------
+struct Options {   // everything on the command line except the inputs: the same for every sample
     int min_mapq = 0, min_bq = 0, max_cnt = 10000000; bool per_lib = false, ic = false; long long max_warn = -1;
     std::string fn_pos, fn_fa, dist_arg;
-    static option lo[] = {{"help", 0, 0, 'h'}, {"version", 0, 0, 'v'}, {"min-mapping-quality", 1, 0, 'q'}, {"min-base-quality", 1, 0, 'b'},
-                          {"max-count", 1, 0, 'd'}, {"site-list", 1, 0, 'l'}, {"reference-fasta", 1, 0, 'f'}, {"print-individual-mapq", 1, 0, 'D'},
-                          {"per-library", 0, 0, 'p'}, {"max-warnings", 1, 0, 'w'}, {"insertion-centric", 0, 0, 'i'}, {"shard", 1, 0, 1000},
-                          {"min-alt-count", 1, 0, 1001}, {"min-alt-fraction", 1, 0, 1002}, {0, 0, 0, 0}};
+    std::vector<std::string> region_args;
     int shard_rank = 0, shard_count = 1;
-    long min_alt_count = 0; double min_alt_fraction = -1.0;       // site filter (brc_set_site_filter); off unless one is given
-    bool help = false, version = false;
-    for (int c; (c = getopt_long(argc, argv, "hvq:b:d:l:f:D:pw:i", lo, nullptr)) != -1;) {
-        switch (c) {
-        case 'h': help = true; break; case 'v': version = true; break;
-        case 'q': min_mapq = std::atoi(optarg); break; case 'b': min_bq = std::atoi(optarg); break; case 'd': max_cnt = std::atoi(optarg); break;
-        case 'l': fn_pos = optarg; break; case 'f': fn_fa = optarg; break; case 'D': dist_arg = optarg; break;
-        case 'p': per_lib = true; break; case 'w': max_warn = std::atoll(optarg); break; case 'i': ic = true; break;
-        case 1000: if (std::sscanf(optarg, "%d/%d", &shard_rank, &shard_count) != 2 || shard_count < 1 || shard_rank < 0 || shard_rank >= shard_count) { std::fprintf(stderr, "--shard wants RANK/COUNT with 0 <= RANK < COUNT\n"); return 1; } break;
-        case 1001: {
-            char *end = nullptr; errno = 0;
-            min_alt_count = std::strtol(optarg, &end, 10);
-            if (errno || end == optarg || *end || min_alt_count < 1 || min_alt_count > INT32_MAX) { std::fprintf(stderr, "--min-alt-count wants an integer N >= 1\n"); return 1; }
-            break;
-        }
-        case 1002: {
-            char *end = nullptr; errno = 0;
-            min_alt_fraction = std::strtod(optarg, &end);
-            if (errno || end == optarg || *end || !(min_alt_fraction >= 0.0 && min_alt_fraction <= 1.0)) { std::fprintf(stderr, "--min-alt-fraction wants a number F with 0 <= F <= 1\n"); return 1; }
-            break;
-        }
-        default: usage(); return 1;
-        }
+    bool site_filter = false; brc_site_filter filter{};
+    bool decode_only = false, device_decode = false, timing = false;
+    bool dist_refused() const { return dist_arg == "1" || dist_arg == "true"; }
+};
+
+double now() { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
+
+// The messages of open_sample.  A run on one input prints them as they come (`live` = stderr), between whatever the libraries
+// it calls print themselves; a cohort opening the next sample under the current one holds them until that sample runs.
+struct Messages {
+    FILE *live = nullptr;
+    std::string held;
+    void say(const char *fmt, ...) __attribute__((format(printf, 2, 3))) {
+        va_list ap;
+        if (live) { va_start(ap, fmt); std::vfprintf(live, fmt, ap); va_end(ap); return; }
+        va_start(ap, fmt); const int n = std::vsnprintf(nullptr, 0, fmt, ap); va_end(ap);
+        if (n <= 0) return;
+        std::string line((size_t)n + 1, '\0');
+        va_start(ap, fmt); std::vsnprintf(&line[0], line.size(), fmt, ap); va_end(ap);
+        line.pop_back();
+        held += line;
     }
-    const bool site_filter = min_alt_count > 0 || min_alt_fraction >= 0.0;
-    brc_site_filter filter{};
-    filter.min_alt_count = (int32_t)std::max<long>(min_alt_count, 1); filter.min_alt_fraction = std::max(min_alt_fraction, 0.0);
-    if (version) { std::printf("bam-readcount version: b200 (engine ABI %d)\n", brc_abi_version()); return 1; }   // R:...:467-470 (exit 1)
-    if (help || optind >= argc) { usage(); return 1; }                                                              // R:...:472-475
-    const std::string bam_path = argv[optind];
-    std::vector<std::string> region_args(argv + optind + 1, argv + argc);
-    std::fprintf(stderr, "Minimum mapping quality is set to %d\n", min_mapq);
-    if (dist_arg == "1" || dist_arg == "true") { std::fprintf(stderr, "Not currently supporting distributions\n"); return 1; }
+};
 
-    // CUDA context creation takes a second or two: do it while the BAM header, index and FASTA index are read
-    brc_config cfg{}; cfg.min_mapq = min_mapq; cfg.min_bq = min_bq; cfg.max_cnt = max_cnt; cfg.per_lib = per_lib; cfg.insertion_centric = ic;
-    cfg.n_libs = 0; cfg.device = std::getenv("BRC_DEVICE") ? std::atoi(std::getenv("BRC_DEVICE")) : 0;
-    const bool decode_only = std::getenv("BRC_CLI_DECODE_ONLY") != nullptr;   // test hook: exercise BGZF/BAI/region fetch without a GPU
-    int warm_rc = BRC_OK;
-    brc_config warm_cfg = cfg; warm_cfg.per_lib = 0;
-    std::thread warm([&warm_rc, warm_cfg, decode_only] { if (decode_only) return; brc_engine *tmp = nullptr; warm_rc = brc_create(&warm_cfg, &tmp); if (tmp) brc_destroy(tmp); });
+struct Region { int tid, beg, end; bool site_list; bool cont = false; };   // cont: a later window of a cut region (its halo site belongs to the window before)
 
+struct Sample {
+    const Options &o;
+    std::string path; bool is_cram = false;
+    Messages log;                 // the run's STDERR up to its region loop (held when opened ahead of its turn)
+    int status = 1;               // 0 once open_sample got to the end; otherwise the run exits 1 after printing `log`
+    double t0 = 0;                // when opening began
     BamFile bam;
-    struct Joiner { std::thread &t; ~Joiner() { if (t.joinable()) t.join(); } } joiner{warm};
-    const bool is_cram = bam_path.size() > 5 && bam_path.substr(bam_path.size() - 5) == ".cram";
 #ifdef BRC_WITH_HTSLIB
     HtsSource hts;
-    if (is_cram) { if (!hts.open(bam_path, fn_fa, bam)) { std::fprintf(stderr, "Fail to open BAM file %s\n", bam_path.c_str()); return 1; } }
+#endif
+    Fasta fa; bool have_fa = false;
+    std::map<std::string, std::string> rg_lb;                   // @RG ID -> LB
+    std::map<std::string, uint16_t> lib_rank;
+    std::vector<std::string> lib_names; std::vector<const char *> lib_ptrs;
+    std::vector<Region> regions;
+    Warner warner;
+    // big fetches (windows of a cut region) are decoded by several threads, one window ahead of the engine (ParallelFetcher)
+    ParallelFetcher pf;
+    bool allow_parallel = false;
+    WindowJob *jobs;              // the process's two window jobs (page-locked buffers), used by one sample at a time
+    std::future<bool> ahead; size_t ahead_gi = (size_t)-1; int ahead_slot = 0;   // waited for when the sample goes
+    bool par_decode_error = false; uint64_t par_decoded = 0, par_windows = 0;
+
+    Sample(const Options &opt, const std::string &p, WindowJob *pool)
+        : o(opt), path(p), warner(opt.max_warn, opt.min_mapq, opt.min_bq, opt.per_lib, opt.ic), pf(bam, p, opt.per_lib, !opt.decode_only), jobs(pool) {}
+    Sample(const Sample &) = delete; Sample &operator=(const Sample &) = delete;
+
+    void fetch_range(size_t gi, int64_t &fb, int64_t &fe) const {
+        const Region &g = regions[gi];
+        const int64_t clen = bam.lens[(size_t)g.tid];
+        fb = std::max<int64_t>((int64_t)g.beg - 1, 0);
+        fe = std::min<int64_t>(g.end, std::max<int64_t>(clen, (int64_t)g.beg + 1));
+    }
+    bool par_ok(size_t gi) const {
+        if (!allow_parallel || gi >= regions.size()) return false;
+        int64_t fb, fe; fetch_range(gi, fb, fe);
+        return ParallelFetcher::eligible(fb, fe);
+    }
+    std::future<bool> start_decode(size_t gi, int slot) {
+        int64_t fb, fe; fetch_range(gi, fb, fe);
+        const int tid = regions[gi].tid; const bool collect = warner.collecting();
+        WindowJob *job = &jobs[slot]; ParallelFetcher *pfp = &pf;
+        return std::async(std::launch::async, [pfp, job, tid, fb, fe, collect] { return pfp->run(tid, fb, fe, collect, *job); });
+    }
+    // the decoded window for region gi (prefetched or decoded now); nullptr = take the sequential path
+    WindowJob *decoded_window(size_t gi) {
+        int slot = 0; bool ok;
+        if (ahead.valid() && ahead_gi == gi) { ok = ahead.get(); slot = ahead_slot; }
+        else { if (ahead.valid()) ahead.get(); ok = start_decode(gi, 0).get(); }
+        ahead_gi = (size_t)-1;
+        WindowJob *job = &jobs[slot];
+        if (!job->timing.empty()) { std::fputs(job->timing.c_str(), warner.err); job->timing.clear(); }
+        if (ok && gi + 1 < regions.size() && par_ok(gi + 1)) { ahead_slot = slot ^ 1; ahead_gi = gi + 1; ahead = start_decode(gi + 1, ahead_slot); }
+        if (!ok) return nullptr;
+        if (job->cand_overflow && warner.collecting()) return nullptr;      // a BAM full of untagged reads: the per-read warning replay wants them all
+        par_decode_error = par_decode_error || job->error; par_decoded += job->n_decoded; ++par_windows;
+        return job;
+    }
+    bool uses_windows() const { for (size_t gi = 0; gi < regions.size(); ++gi) if (par_ok(gi)) return true; return false; }
+    int64_t next_fbeg(size_t gi) const {   // start of the following fetch when it continues this one, else "keep nothing"
+        if (gi + 1 >= regions.size() || regions[gi + 1].tid != regions[gi].tid) return INT64_MAX;
+        return std::max<int64_t>((int64_t)regions[gi + 1].beg - 1, 0);
+    }
+};
+
+bool is_cram_path(const std::string &p) { return p.size() > 5 && p.substr(p.size() - 5) == ".cram"; }
+
+// `live`: print the messages as they come (else hold them in s.log).  `first_window`: start decoding the first window into
+// `pool` (only when no other sample is using it).
+std::unique_ptr<Sample> open_sample(const Options &o, const std::string &bam_path, double t0, FILE *live, WindowJob *pool, bool first_window) {
+    std::unique_ptr<Sample> sp(new Sample(o, bam_path, pool));
+    Sample &s = *sp; Messages &log = s.log; BamFile &bam = s.bam;
+    s.t0 = t0; log.live = live;
+    log.say("Minimum mapping quality is set to %d\n", o.min_mapq);
+    if (o.dist_refused()) { log.say("Not currently supporting distributions\n"); return sp; }
+    s.is_cram = is_cram_path(bam_path);
+#ifdef BRC_WITH_HTSLIB
+    if (s.is_cram) { if (!s.hts.open(bam_path, o.fn_fa, bam)) { log.say("Fail to open BAM file %s\n", bam_path.c_str()); return sp; } }
     else
 #else
-    if (is_cram) { std::fprintf(stderr, "CRAM input needs a host built with htslib (tools/build_htslib.sh, then python -m bam_readcount_b200.build); convert to BAM\n"); return 1; }
+    if (s.is_cram) { log.say("CRAM input needs a host built with htslib (tools/build_htslib.sh, then python -m bam_readcount_b200.build); convert to BAM\n"); return sp; }
 #endif
-    if (!bam.open(bam_path)) { std::fprintf(stderr, "Fail to open BAM file %s\n", bam_path.c_str()); return 1; }
-    Fasta fa;
-    const bool have_fa = !fn_fa.empty() && fa.open(fn_fa);
-    if (!fn_fa.empty() && !have_fa) { std::fprintf(stderr, "Fail to open reference file %s\n", fn_fa.c_str()); return 1; }
+    if (!bam.open(bam_path)) { log.say("Fail to open BAM file %s\n", bam_path.c_str()); return sp; }
+    s.have_fa = !o.fn_fa.empty() && s.fa.open(o.fn_fa);
+    if (!o.fn_fa.empty() && !s.have_fa) { log.say("Fail to open reference file %s\n", o.fn_fa.c_str()); return sp; }
 
     // @RG ID -> LB; libraries in std::set order (R:...:92-111, 526-529)
-    std::map<std::string, std::string> rg_lb; std::set<std::string> libs;
+    std::set<std::string> libs;
     {
         std::istringstream ss(bam.text); std::string line;
         while (std::getline(ss, line)) {
             if (line.compare(0, 3, "@RG") != 0) continue;
             std::istringstream ls(line); std::string tok, id, lb; bool has_lb = false;
             while (std::getline(ls, tok, '\t')) { if (tok.compare(0, 3, "ID:") == 0) id = tok.substr(3); else if (tok.compare(0, 3, "LB:") == 0) { lb = tok.substr(3); has_lb = true; } }
-            if (has_lb) { libs.insert(lb); if (!id.empty() && !rg_lb.count(id)) rg_lb[id] = lb; }
+            if (has_lb) { libs.insert(lb); if (!id.empty() && !s.rg_lb.count(id)) s.rg_lb[id] = lb; }
         }
     }
-    for (const auto &l : libs) std::fprintf(stderr, "Expect library: %s in BAM\n", l.c_str());
-    std::vector<std::string> lib_names(libs.begin(), libs.end());
-    std::map<std::string, uint16_t> lib_rank;
-    for (size_t i = 0; i < lib_names.size(); ++i) lib_rank[lib_names[i]] = (uint16_t)i;
-    std::vector<const char *> lib_ptrs; for (auto &s : lib_names) lib_ptrs.push_back(s.c_str());
-    if (lib_ptrs.empty()) lib_ptrs.push_back("");
+    for (const auto &l : libs) log.say("Expect library: %s in BAM\n", l.c_str());
+    s.lib_names.assign(libs.begin(), libs.end());
+    for (size_t i = 0; i < s.lib_names.size(); ++i) s.lib_rank[s.lib_names[i]] = (uint16_t)i;
+    for (auto &n : s.lib_names) s.lib_ptrs.push_back(n.c_str());
+    if (s.lib_ptrs.empty()) s.lib_ptrs.push_back("");
 
-    if (fn_pos.empty() && region_args.empty()) {
-        std::fprintf(stderr, "Whole-file mode is not supported (the reference skips its per-read pre-processing there, R:...:624); give regions or -l\n");
-        return 1;
+    if (o.fn_pos.empty() && o.region_args.empty()) {
+        log.say("Whole-file mode is not supported (the reference skips its per-read pre-processing there, R:...:624); give regions or -l\n");
+        return sp;
     }
 #ifdef BRC_WITH_HTSLIB
-    if (is_cram) { if (!hts.load_index(bam_path)) { std::fprintf(stderr, "BAM indexing file is not available.\n"); return 1; } }
+    if (s.is_cram) { if (!s.hts.load_index(bam_path)) { log.say("BAM indexing file is not available.\n"); return sp; } }
     else
 #endif
-    if (!bam.load_index(bam_path)) { std::fprintf(stderr, "BAM indexing file is not available.\n"); return 1; }
-    if (!have_fa && !decode_only) { std::fprintf(stderr, "A reference FASTA (-f) is required in region / site-list mode\n"); return 1; }
+    if (!bam.load_index(bam_path)) { log.say("BAM indexing file is not available.\n"); return sp; }
+    if (!s.have_fa && !o.decode_only) { log.say("A reference FASTA (-f) is required in region / site-list mode\n"); return sp; }
 
-    cfg.n_libs = (int32_t)lib_names.size();
-    brc_engine *eng = nullptr;      // created below, once the first window is already being decoded (the CUDA context is still coming up)
-    int rc = BRC_OK;
-
-    struct Region { int tid, beg, end; bool site_list; bool cont = false; };   // cont: a later window of a cut region (its halo site belongs to the window before)
-    std::vector<Region> regions;
-    if (!fn_pos.empty()) {
-        std::ifstream fp(fn_pos);
-        if (!fp) { std::fprintf(stderr, "Failed to open region list file: %s\n", fn_pos.c_str()); return 1; }
+    std::vector<Region> &regions = s.regions;
+    if (!o.fn_pos.empty()) {
+        std::ifstream fp(o.fn_pos);
+        if (!fp) { log.say("Failed to open region list file: %s\n", o.fn_pos.c_str()); return sp; }
         std::string line;
         while (std::getline(fp, line)) {
             std::istringstream ss(line); std::string name; int b, e;
             if (!(ss >> name >> b >> e)) continue;
             auto it = bam.tid_of.find(name);
-            if (it == bam.tid_of.end()) { std::fprintf(stderr, "%s not found in bam file. Region %s %i %i skipped.\n", name.c_str(), name.c_str(), b, e); continue; }
+            if (it == bam.tid_of.end()) { log.say("%s not found in bam file. Region %s %i %i skipped.\n", name.c_str(), name.c_str(), b, e); continue; }
             regions.push_back({it->second, b - 1, e, true});
         }
     } else {
         int beg = 0, end = 0x7fffffff;
-        for (const auto &rs : region_args) {
+        for (const auto &rs : o.region_args) {
             int tid;
             parse_region(bam, rs, tid, beg, end);
-            if (tid < 0) { std::fprintf(stderr, "Invalid region %s\n", rs.c_str()); brc_destroy(eng); return 1; }
+            if (tid < 0) { log.say("Invalid region %s\n", rs.c_str()); return sp; }
             regions.push_back({tid, beg, end, false});
         }
     }
@@ -899,9 +967,9 @@ int main(int argc, char **argv) {
     {
         // 2 Mb windows: each is decoded by all threads in ~40 ms one window ahead of the engine and needs 110 MB of page-locked memory
         // (8 Mb windows were 0.6 s slower on a 10 Mb BAM, r02t); the record-by-record paths (CRAM, BRC_CLI_SEQUENTIAL) keep 8 Mb
-        const bool par_windows_ok = !is_cram && std::getenv("BRC_CLI_DEVICE_DECODE") == nullptr && std::getenv("BRC_CLI_SEQUENTIAL") == nullptr;
+        const bool par_windows_ok = !s.is_cram && std::getenv("BRC_CLI_DEVICE_DECODE") == nullptr && std::getenv("BRC_CLI_SEQUENTIAL") == nullptr;
         int64_t W = std::getenv("BRC_CLI_WINDOW") ? std::atoll(std::getenv("BRC_CLI_WINDOW")) : (par_windows_ok ? 2000000 : 8000000);
-        if (shard_count > 1 && !std::getenv("BRC_CLI_WINDOW")) W = 1000000;      // finer units so the shards can balance
+        if (o.shard_count > 1 && !std::getenv("BRC_CLI_WINDOW")) W = 1000000;      // finer units so the shards can balance
         std::vector<Region> cut;
         for (const Region &g : regions) {
             const int64_t clen = bam.lens[(size_t)g.tid];
@@ -922,7 +990,8 @@ int main(int argc, char **argv) {
     // — and the units are cut into COUNT contiguous runs of about equal weight; this process computes run RANK.  Units are
     // independent (every window recomputes its left halo site), so the concatenation of the ranks' outputs in rank order is the
     // unsharded output; only the reference's never-cleared argv deletion queue does not cross a shard boundary.
-    if (shard_count > 1) {
+    if (o.shard_count > 1) {
+        const int shard_rank = o.shard_rank, shard_count = o.shard_count;
         std::vector<double> wgt(regions.size(), 1.0);
         for (size_t i = 0; i < regions.size(); ++i) {
             const Region &g = regions[i];
@@ -941,35 +1010,88 @@ int main(int argc, char **argv) {
         std::vector<size_t> cutpt((size_t)shard_count + 1, regions.size()); cutpt[0] = 0;
         { double acc = 0; int r = 1; for (size_t i = 0; i < regions.size() && r < shard_count; ++i) { acc += wgt[i]; while (r < shard_count && acc >= tot * r / shard_count) cutpt[(size_t)r++] = i + 1; } }
         std::vector<Region> mine(regions.begin() + (long)cutpt[(size_t)shard_rank], regions.begin() + (long)cutpt[(size_t)shard_rank + 1]);
-        if (std::getenv("BRC_CLI_TIMING")) std::fprintf(stderr, "[brc shard] %d/%d: units %zu..%zu of %zu\n", shard_rank, shard_count, cutpt[(size_t)shard_rank], cutpt[(size_t)shard_rank + 1], regions.size());
+        if (o.timing) log.say("[brc shard] %d/%d: units %zu..%zu of %zu\n", shard_rank, shard_count, cutpt[(size_t)shard_rank], cutpt[(size_t)shard_rank + 1], regions.size());
         regions.swap(mine);
     }
 
-    std::set<int> ref_loaded;
+    for (const auto &kv : s.rg_lb) s.pf.rg_lib[kv.first] = s.lib_rank[kv.second];
+    s.allow_parallel = !s.is_cram && !o.device_decode && std::getenv("BRC_CLI_SEQUENTIAL") == nullptr;
+    // decode under the CUDA start-up (first sample) or under the previous sample's compute (cohort)
+    if (first_window && !regions.empty() && s.par_ok(0)) { s.ahead_slot = 0; s.ahead_gi = 0; s.ahead = s.start_decode(0, 0); }
+    s.status = 0;
+    return sp;
+}
+
+// ------------------------------------------------------------------------------------------
+// The engine handles of a process.  One CUDA context, brought up once by a throw-away engine on a thread of its own while the
+// first sample is opened.  A handle's library rows are fixed at brc_create, so under -p there is one handle per library count,
+// kept and reused by the later samples with that count (brc_create allocates nothing on the device until first use); without
+// -p every sample shares one handle.  Each handle remembers which contig it holds the reference of for every tid: tids are
+// per-header, so the reference is uploaded again only when a sample's tid names another contig.
+// ------------------------------------------------------------------------------------------
+struct Engines {
+    brc_config cfg{};
+    std::thread warm; int warm_rc = BRC_OK;
+    struct Handle { brc_engine *eng = nullptr; std::unordered_map<int, std::string> ref_name; };
+    std::map<int32_t, Handle> handles;
+
+    void start_warm() {
+        brc_config w = cfg; w.per_lib = 0;
+        warm = std::thread([this, w] { brc_engine *tmp = nullptr; warm_rc = brc_create(&w, &tmp); if (tmp) brc_destroy(tmp); });
+    }
+    // the handle for a sample with n_libs libraries; nullptr (message on err) when it cannot be created
+    Handle *get(int32_t n_libs, const Options &o, FILE *err) {
+        if (warm.joinable()) warm.join();
+        const int32_t key = cfg.per_lib ? n_libs : 0;
+        auto it = handles.find(key);
+        if (it != handles.end()) return &it->second;
+        brc_config c = cfg; c.n_libs = n_libs;
+        brc_engine *eng = nullptr;
+        const int rc = warm_rc != BRC_OK ? warm_rc : brc_create(&c, &eng);
+        if (rc != BRC_OK) { std::fprintf(err, "brc_create: %s\n", brc_strerror(rc)); return nullptr; }
+        if (o.site_filter && brc_set_site_filter(eng, &o.filter) != BRC_OK) { std::fprintf(err, "brc_set_site_filter: %s\n", brc_last_error(eng)); brc_destroy(eng); return nullptr; }
+        Handle &h = handles[key]; h.eng = eng;
+        return &h;
+    }
+    void destroy() { for (auto &kv : handles) brc_destroy(kv.second.eng); handles.clear(); }
+    ~Engines() { if (warm.joinable()) warm.join(); }
+};
+
+// One sample's region loop (the two loops of the reference, R:...:574-608 and 641-657): text to out_fd, messages to err.
+// Returns the exit status of the run on this input alone (0 or 1), or -1 when no engine could be created.
+int run_sample(const Options &o, Engines &engines, Sample &s, int out_fd, FILE *err, double t_main0) {
+    std::fputs(s.log.held.c_str(), err);
+    if (s.status != 0) return 1;
+    s.warner.err = err;
+    BamFile &bam = s.bam; const std::vector<Region> &regions = s.regions; Warner &warner = s.warner;
+    const std::vector<const char *> &lib_ptrs = s.lib_ptrs;
+    Engines::Handle *h = nullptr; brc_engine *eng = nullptr;
+    if (!o.decode_only) {
+        if (!(h = engines.get((int32_t)s.lib_names.size(), o, err))) return -1;
+        eng = h->eng;
+        // nothing left from an earlier sample: no pushed reads (a sample that failed mid-way) and no queued deletion
+        // (switching the carry empties the queue); the argv loop's queue is then carried across this sample's flushes
+        brc_reset(eng); brc_set_queue_carry(eng, 0); brc_set_queue_carry(eng, 1);
+    }
+
     std::string chrom;
-    const bool timing = std::getenv("BRC_CLI_TIMING") != nullptr;
-    auto now = [] { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); };
     double t_decode = 0, t_compute = 0, t_format = 0, t_write = 0, t_ref = 0, t_results = 0, t_reset = 0;
     // BRC_CLI_DEVICE_DECODE=1: BGZF inflate + BAM framing on the GPU (per-read warning lines need host-decoded reads: counts only)
-    const bool device_decode = std::getenv("BRC_CLI_DEVICE_DECODE") != nullptr && !decode_only;
-    std::vector<std::string> rg_id_store; std::vector<const char *> rg_ids; std::vector<uint16_t> rg_libs;
-    for (const auto &kv : rg_lb) rg_id_store.push_back(kv.first);
-    for (const auto &id : rg_id_store) { rg_ids.push_back(id.c_str()); rg_libs.push_back(lib_rank[rg_lb[id]]); }
-    Warner warner(max_warn, min_mapq, min_bq, per_lib, ic);
+    std::vector<const char *> rg_ids; std::vector<uint16_t> rg_libs;
+    for (const auto &kv : s.rg_lb) { rg_ids.push_back(kv.first.c_str()); rg_libs.push_back(s.lib_rank[kv.second]); }
     int64_t warn_total[4] = {0, 0, 0, 0};
     auto flush = [&]() -> int {
         const double c0 = now();
         int r = brc_compute(eng);
         t_compute += now() - c0;
-        if (r != BRC_OK) { std::fprintf(stderr, "brc_compute: %s\n", brc_last_error(eng)); return r; }
+        if (r != BRC_OK) { std::fprintf(err, "brc_compute: %s\n", brc_last_error(eng)); return r; }
         brc_results res{};
         const double g0 = now();
-        if (site_filter) {            // only the selected sites came back: no dense view, the region table is all the loop needs
+        if (o.site_filter) {          // only the selected sites came back: no dense view, the region table is all the loop needs
             brc_selected_results sel{};
-            if ((r = brc_get_selected_results(eng, &sel)) != BRC_OK) { std::fprintf(stderr, "brc_get_selected_results: %s\n", brc_last_error(eng)); return r; }
+            if ((r = brc_get_selected_results(eng, &sel)) != BRC_OK) { std::fprintf(err, "brc_get_selected_results: %s\n", brc_last_error(eng)); return r; }
             res.n_regions = sel.n_regions; res.regions = sel.regions;
-        } else if ((r = brc_get_results(eng, &res)) != BRC_OK) { std::fprintf(stderr, "brc_get_results: %s\n", brc_last_error(eng)); return r; }
-        std::fflush(stdout);
+        } else if ((r = brc_get_results(eng, &res)) != BRC_OK) { std::fprintf(err, "brc_get_results: %s\n", brc_last_error(eng)); return r; }
         const double f0 = now();
         t_results += f0 - g0;
         const bool argv_chain = res.n_regions > 1 && !res.regions[0].site_list_mode;   // never-cleared deletion queue: one sequential pass
@@ -977,12 +1099,12 @@ int main(int argc, char **argv) {
         for (int64_t g = 0; g < res.n_regions; ++g) total_slots += res.regions[g].n_slots;
         const bool many_small = res.n_regions > 1 && total_slots <= (int64_t(1) << 22);  // a site list: all regions in one formatting pass
         if (argv_chain || many_small) {
-            if (brc_write_text(eng, -1, 0, -1, lib_ptrs.data(), STDOUT_FILENO) < 0) { std::fprintf(stderr, "format: %s\n", brc_last_error(eng)); return -1; }
+            if (brc_write_text(eng, -1, 0, -1, lib_ptrs.data(), out_fd) < 0) { std::fprintf(err, "format: %s\n", brc_last_error(eng)); return -1; }
         } else {
             const int64_t WIN = 1 << 21;   // stream big regions in 2M-site windows (each formatted by several threads)
             for (int64_t g = 0; g < res.n_regions; ++g)
                 for (int64_t first = 0; first < res.regions[g].n_slots; first += WIN)
-                    if (brc_write_text(eng, g, first, WIN, lib_ptrs.data(), STDOUT_FILENO) < 0) { std::fprintf(stderr, "format: %s\n", brc_last_error(eng)); return -1; }
+                    if (brc_write_text(eng, g, first, WIN, lib_ptrs.data(), out_fd) < 0) { std::fprintf(err, "format: %s\n", brc_last_error(eng)); return -1; }
         }
         t_format += now() - f0;
         { int64_t wc[4]; if (brc_get_warning_counts(eng, wc) == BRC_OK) for (int k = 0; k < 4; ++k) warn_total[k] += wc[k]; }
@@ -994,62 +1116,15 @@ int main(int argc, char **argv) {
     };
     int64_t pushed = 0;
     RegionFetcher fetcher(bam);
-    // big fetches (windows of a cut region) are decoded by several threads, one window ahead of the engine (ParallelFetcher)
-    ParallelFetcher pf(bam, bam_path, per_lib, !decode_only);
-    for (const auto &kv : rg_lb) pf.rg_lib[kv.first] = lib_rank[kv.second];
-    const bool allow_parallel = !is_cram && !device_decode && std::getenv("BRC_CLI_SEQUENTIAL") == nullptr;
-    std::unique_ptr<WindowJob[]> jobs(new WindowJob[2]);
-    std::future<bool> ahead; size_t ahead_gi = (size_t)-1; int ahead_slot = 0;
-    bool par_decode_error = false; uint64_t par_decoded = 0, par_windows = 0;
-    auto fetch_range = [&](size_t gi, int64_t &fb, int64_t &fe) {
-        const Region &g = regions[gi];
-        const int64_t clen = bam.lens[(size_t)g.tid];
-        fb = std::max<int64_t>((int64_t)g.beg - 1, 0);
-        fe = std::min<int64_t>(g.end, std::max<int64_t>(clen, (int64_t)g.beg + 1));
-    };
-    auto par_ok = [&](size_t gi) {
-        if (!allow_parallel || gi >= regions.size()) return false;
-        int64_t fb, fe; fetch_range(gi, fb, fe);
-        return ParallelFetcher::eligible(fb, fe);
-    };
-    auto start_decode = [&](size_t gi, int slot) {
-        int64_t fb, fe; fetch_range(gi, fb, fe);
-        const int tid = regions[gi].tid; const bool collect = warner.collecting();
-        WindowJob *job = &jobs[slot]; ParallelFetcher *pfp = &pf;
-        return std::async(std::launch::async, [pfp, job, tid, fb, fe, collect] { return pfp->run(tid, fb, fe, collect, *job); });
-    };
-    // the decoded window for region gi (prefetched or decoded now); nullptr = take the sequential path
-    auto decoded_window = [&](size_t gi) -> WindowJob * {
-        int slot = 0; bool ok;
-        if (ahead.valid() && ahead_gi == gi) { ok = ahead.get(); slot = ahead_slot; }
-        else { if (ahead.valid()) ahead.get(); ok = start_decode(gi, 0).get(); }
-        ahead_gi = (size_t)-1;
-        WindowJob *job = &jobs[slot];
-        if (ok && gi + 1 < regions.size() && par_ok(gi + 1)) { ahead_slot = slot ^ 1; ahead_gi = gi + 1; ahead = start_decode(gi + 1, ahead_slot); }
-        if (!ok) return nullptr;
-        if (job->cand_overflow && warner.collecting()) return nullptr;      // a BAM full of untagged reads: the per-read warning replay wants them all
-        par_decode_error = par_decode_error || job->error; par_decoded += job->n_decoded; ++par_windows;
-        return job;
-    };
-    if (!regions.empty() && par_ok(0)) { ahead_slot = 0; ahead_gi = 0; ahead = start_decode(0, 0); }   // decode under the CUDA start-up
-    warm.join();
-    rc = decode_only ? BRC_OK : (warm_rc != BRC_OK ? warm_rc : brc_create(&cfg, &eng));
-    if (rc != BRC_OK) { std::fprintf(stderr, "brc_create: %s\n", brc_strerror(rc)); return 1; }
-    if (eng) brc_set_queue_carry(eng, 1);
-    if (eng && site_filter && brc_set_site_filter(eng, &filter) != BRC_OK) { std::fprintf(stderr, "brc_set_site_filter: %s\n", brc_last_error(eng)); return 1; }
     const double t_loop0 = now();
-    auto next_fbeg = [&](size_t gi) -> int64_t {   // start of the following fetch when it continues this one, else "keep nothing"
-        if (gi + 1 >= regions.size() || regions[gi + 1].tid != regions[gi].tid) return INT64_MAX;
-        return std::max<int64_t>((int64_t)regions[gi + 1].beg - 1, 0);
-    };
     for (size_t gi = 0; gi < regions.size(); ++gi) {
         const Region &g = regions[gi];
         const double d0 = now();
-        if (decode_only) {
+        if (o.decode_only) {
             const int64_t fbeg = std::max<int64_t>((int64_t)g.beg - 1, 0), fend = g.end;
             int64_t n = 0, psum = 0, qsum = 0;
             auto count = [&](const Rec &r) { if (r.flag & 4) return; ++n; psum += r.pos; for (int k = 0; k < r.l_qseq; ++k) qsum += r.qual[k]; };
-            WindowJob *job = par_ok(gi) ? decoded_window(gi) : nullptr;
+            WindowJob *job = s.par_ok(gi) ? s.decoded_window(gi) : nullptr;
             if (job) {
                 const brc_read_batch &b = job->batch;
                 n = b.n_reads;
@@ -1058,36 +1133,39 @@ int main(int argc, char **argv) {
                 fetcher.active = false;
             } else
 #ifdef BRC_WITH_HTSLIB
-            if (is_cram) hts.fetch(g.tid, fbeg, fend, count); else
+            if (s.is_cram) s.hts.fetch(g.tid, fbeg, fend, count); else
 #endif
-            fetcher.fetch(g.tid, fbeg, fend, next_fbeg(gi), count);
-            std::printf("%d\t%d\t%d\t%lld\t%lld\t%lld\n", g.tid, g.beg, g.end, (long long)n, (long long)psum, (long long)qsum);
+            fetcher.fetch(g.tid, fbeg, fend, s.next_fbeg(gi), count);
+            dprintf(out_fd, "%d\t%d\t%d\t%lld\t%lld\t%lld\n", g.tid, g.beg, g.end, (long long)n, (long long)psum, (long long)qsum);
             continue;
         }
-        if (!ref_loaded.count(g.tid)) {   // load_reference: whole chromosome
-            if (!fa.fetch(bam.names[(size_t)g.tid], chrom)) { std::fprintf(stderr, "Failed to fetch %s from %s\n", bam.names[(size_t)g.tid].c_str(), fn_fa.c_str()); brc_destroy(eng); return 1; }
-            rc = brc_set_reference(eng, g.tid, bam.names[(size_t)g.tid].c_str(), (int64_t)chrom.size(), 0, chrom.data(), (int64_t)chrom.size());
-            if (rc != BRC_OK) { std::fprintf(stderr, "brc_set_reference: %s\n", brc_last_error(eng)); brc_destroy(eng); return 1; }
-            ref_loaded.insert(g.tid);
+        const std::string &contig = bam.names[(size_t)g.tid];
+        auto loaded = h->ref_name.find(g.tid);
+        if (loaded == h->ref_name.end() || loaded->second != contig) {   // load_reference: whole chromosome
+            h->ref_name.erase(g.tid);
+            if (!s.fa.fetch(contig, chrom)) { std::fprintf(err, "Failed to fetch %s from %s\n", contig.c_str(), o.fn_fa.c_str()); return 1; }
+            const int rc = brc_set_reference(eng, g.tid, contig.c_str(), (int64_t)chrom.size(), 0, chrom.data(), (int64_t)chrom.size());
+            if (rc != BRC_OK) { std::fprintf(err, "brc_set_reference: %s\n", brc_last_error(eng)); return 1; }
+            h->ref_name[g.tid] = contig;
             t_ref += now() - d0;
         }
         const double d1 = now();
-        if (par_ok(gi)) {
+        if (s.par_ok(gi)) {
             // one window = one batch: whatever smaller regions are pending goes out first, then the window is pushed as ONE borrowed
             // batch (the engine streams it to the GPU in chunks) while the next window is already being decoded
-            if (pushed > 0) { if (flush() != BRC_OK) { brc_destroy(eng); return 1; } pushed = 0; }
-            if (WindowJob *job = decoded_window(gi)) {
+            if (pushed > 0) { if (flush() != BRC_OK) return 1; pushed = 0; }
+            if (WindowJob *job = s.decoded_window(gi)) {
                 brc_begin_region(eng, g.tid, g.beg, g.end, g.site_list ? 1 : 0);
                 warner.begin_region(g.tid, g.beg, g.end, g.cont);
                 for (Slice &sl : job->slices) warner.take(sl.cands);
                 if (job->batch.n_reads > 0) {
                     const int prc = brc_push_reads(eng, &job->batch);
-                    if (prc != BRC_OK) { std::fprintf(stderr, "brc_push_reads: %s\n", brc_last_error(eng)); brc_destroy(eng); return 1; }
+                    if (prc != BRC_OK) { std::fprintf(err, "brc_push_reads: %s\n", brc_last_error(eng)); return 1; }
                 }
                 brc_end_region(eng);
                 fetcher.active = false;
                 t_decode += now() - d1;
-                if (flush() != BRC_OK) { brc_destroy(eng); return 1; }     // the batch is borrowed until the text is out
+                if (flush() != BRC_OK) return 1;     // the batch is borrowed until the text is out
                 pushed = 0;
                 continue;
             }
@@ -1097,27 +1175,27 @@ int main(int argc, char **argv) {
         // samfetch(in, idx, ref, d.beg-1, d.end): records with tid, endpos > max(beg-1,0), pos < end, in file order
         const int64_t fbeg = std::max<int64_t>((int64_t)g.beg - 1, 0), fend = g.end;
         int push_rc = BRC_OK;
-        if (device_decode && !is_cram) {
+        if (o.device_decode && !s.is_cram) {
             // f-2: hand the engine the compressed span; it inflates, frames and computes on the device.  One span per batch.
             SpanBuilder sb;
             if (sb.build(bam, g.tid, fbeg, fend)) {
                 brc_bam_span sp{}; sp.comp = sb.comp.data(); sp.comp_len = (int64_t)sb.comp.size(); sp.n_entry = (int64_t)sb.entries.size(); sp.entry = sb.entries.data();
                 sp.end_voff = sb.end_voff; sp.tid = g.tid; sp.n_rg = (int32_t)rg_ids.size(); sp.rg_id = rg_ids.data(); sp.rg_lib = rg_libs.data();
                 const int prc = brc_push_bam_span(eng, &sp);
-                if (prc != BRC_OK) { std::fprintf(stderr, "brc_push_bam_span: %s\n", brc_last_error(eng)); brc_destroy(eng); return 1; }
+                if (prc != BRC_OK) { std::fprintf(err, "brc_push_bam_span: %s\n", brc_last_error(eng)); return 1; }
             }
             fetcher.active = false;
             brc_end_region(eng);
             t_decode += now() - d1;
-            if (flush() != BRC_OK) { brc_destroy(eng); return 1; }
+            if (flush() != BRC_OK) return 1;
             pushed = 0;
             continue;
         }
         auto push = [&](const Rec &r) {
             uint16_t lib = 0;
-            if (per_lib) {
+            if (o.per_lib) {
                 lib = (uint16_t)BRC_LIB_NONE;
-                if (r.has_rg) { auto it = rg_lb.find(r.rg); if (it != rg_lb.end()) lib = lib_rank[it->second]; }
+                if (r.has_rg) { auto it = s.rg_lb.find(r.rg); if (it != s.rg_lb.end()) lib = s.lib_rank[it->second]; }
             }
             warner.consider(r, lib == (uint16_t)BRC_LIB_NONE);
             const int prc = brc_push_read(eng, r.tid, r.pos, r.flag, r.mapq, lib, r.l_qseq, r.nm, r.sm, r.n_cigar, r.cigar, r.seq, r.qual);
@@ -1125,35 +1203,215 @@ int main(int argc, char **argv) {
             ++pushed;
         };
 #ifdef BRC_WITH_HTSLIB
-        if (is_cram) hts.fetch(g.tid, fbeg, fend, push); else
+        if (s.is_cram) s.hts.fetch(g.tid, fbeg, fend, push); else
 #endif
-        fetcher.fetch(g.tid, fbeg, fend, next_fbeg(gi), push);
-        if (push_rc != BRC_OK) { std::fprintf(stderr, "brc_push_read: %s\n", brc_last_error(eng)); brc_destroy(eng); return 1; }
+        fetcher.fetch(g.tid, fbeg, fend, s.next_fbeg(gi), push);
+        if (push_rc != BRC_OK) { std::fprintf(err, "brc_push_read: %s\n", brc_last_error(eng)); return 1; }
         brc_end_region(eng);
         t_decode += now() - d1;
         // flush in batches at region boundaries; the deletion queue of the argv loop is carried by the engine (brc_set_queue_carry)
-        if (gi + 1 == regions.size() || pushed > 1500000) { if (flush() != BRC_OK) { brc_destroy(eng); return 1; } pushed = 0; }
+        if (gi + 1 == regions.size() || pushed > 1500000) { if (flush() != BRC_OK) return 1; pushed = 0; }
     }
     warner.finish(warn_total);
 #ifdef BRC_WITH_HTSLIB
-    const bool decode_error = bam.bz.error || hts.error || par_decode_error;
+    const bool decode_error = bam.bz.error || s.hts.error || s.par_decode_error;
 #else
-    const bool decode_error = bam.bz.error || par_decode_error;
+    const bool decode_error = bam.bz.error || s.par_decode_error;
 #endif
-    if (ahead.valid()) ahead.get();
-    if (decode_error) std::fprintf(stderr, "[E::bgzf_read] %s: truncated or corrupt BGZF block / BAM record — the output above is incomplete\n", bam_path.c_str());
-    if (timing) std::fprintf(stderr, "[brc timing] index seeks %llu  records decoded %llu  (+ %llu records in %llu windows decoded by %d threads)\n", (unsigned long long)fetcher.n_seeks,
-                             (unsigned long long)fetcher.n_decoded, (unsigned long long)par_decoded, (unsigned long long)par_windows, pf.n_threads);
-    if (decode_only) return decode_error ? 1 : 0;
-    if (timing) std::fprintf(stderr, "[brc timing] reference %.3fs  decode+push %.3fs  compute %.3fs  results %.3fs  format %.3fs  reset %.3fs  write %.3fs  | region loop %.3fs, since main() %.3fs\n",
-                             t_ref, t_decode, t_compute, t_results, t_format, t_reset, t_write, now() - t_loop0, now() - t_main0);
-    if (timing) std::fprintf(stderr, "[brc timing] startup (CUDA context, header, index, first window) %.3fs\n", t_loop0 - t_main0);
-    if (!std::getenv("BRC_CLI_CLEAN_EXIT")) {
-        // everything is printed: leave without tearing down the CUDA context, the page-locked buffers and the thread pools one by
-        // one (a teardown that takes a noticeable part of a second) — the kernel reclaims them
-        std::fflush(nullptr);
-        _exit(decode_error ? 1 : 0);
-    }
-    brc_destroy(eng);
+    if (s.ahead.valid()) s.ahead.get();
+    if (decode_error) std::fprintf(err, "[E::bgzf_read] %s: truncated or corrupt BGZF block / BAM record — the output above is incomplete\n", s.path.c_str());
+    if (o.timing) std::fprintf(err, "[brc timing] index seeks %llu  records decoded %llu  (+ %llu records in %llu windows decoded by %d threads)\n", (unsigned long long)fetcher.n_seeks,
+                               (unsigned long long)fetcher.n_decoded, (unsigned long long)s.par_decoded, (unsigned long long)s.par_windows, s.pf.n_threads);
+    if (o.decode_only) return decode_error ? 1 : 0;
+    if (o.timing) std::fprintf(err, "[brc timing] reference %.3fs  decode+push %.3fs  compute %.3fs  results %.3fs  format %.3fs  reset %.3fs  write %.3fs  | region loop %.3fs, since main() %.3fs\n",
+                               t_ref, t_decode, t_compute, t_results, t_format, t_reset, t_write, now() - t_loop0, now() - t_main0);
+    if (o.timing) std::fprintf(err, "[brc timing] startup (CUDA context, header, index, first window) %.3fs\n", t_loop0 - s.t0);
     return decode_error ? 1 : 0;
+}
+
+// Everything is printed: leave without tearing down the CUDA context, the page-locked buffers and the thread pools one by
+// one (a teardown that takes a noticeable part of a second) — the kernel reclaims them.  BRC_CLI_CLEAN_EXIT=1 tears down.
+// A run that failed before it asked for an engine still waits for the CUDA start-up thread, as returning from main() would.
+int leave(Engines &engines, std::unique_ptr<Sample> &last, int status) {
+    if (engines.warm.joinable()) engines.warm.join();
+    if (!std::getenv("BRC_CLI_CLEAN_EXIT")) {
+        std::fflush(nullptr);
+        _exit(status);
+    }
+    last.reset();
+    engines.destroy();
+    return status;
+}
+
+// OUT and ERR of one cohort sample.  Nothing is created or emptied until both are open: a sample that cannot have both
+// leaves no new file behind and no earlier file truncated.
+bool open_outputs(const std::string &out, const std::string &err, int &out_fd, int &err_fd, std::string &why) {
+    const std::string *path[2] = {&out, &err};
+    int fd[2] = {-1, -1}; bool made[2] = {false, false};
+    auto undo = [&](int n) { for (int j = 0; j < n; ++j) { ::close(fd[j]); if (made[j]) ::unlink(path[j]->c_str()); } };
+    for (int i = 0; i < 2; ++i) {
+        fd[i] = ::open(path[i]->c_str(), O_WRONLY | O_CREAT | O_EXCL | O_CLOEXEC, 0666);
+        if (fd[i] >= 0) made[i] = true;
+        else if (errno == EEXIST) fd[i] = ::open(path[i]->c_str(), O_WRONLY | O_CLOEXEC);
+        if (fd[i] < 0) { why = "cannot open " + *path[i] + ": " + std::strerror(errno); undo(i); return false; }
+    }
+    for (int i = 0; i < 2; ++i)
+        if (::ftruncate(fd[i], 0) != 0) { why = "cannot truncate " + *path[i] + ": " + std::strerror(errno); undo(2); return false; }
+    out_fd = fd[0]; err_fd = fd[1];
+    return true;
+}
+
+// --bam-list FILE: a cohort in one process.  Each non-empty line of FILE is INPUT<TAB>OUT[<TAB>ERR] (ERR defaults to OUT.log);
+// OUT and ERR receive exactly what a run on INPUT alone with the same options and regions prints on STDOUT and STDERR.  A
+// sample whose own run would exit 1 is reported on this process's STDERR and the batch goes on; the exit status is 1 when any
+// sample failed.  The list is checked whole before any sample runs.
+//
+// While a sample runs, file descriptor 2 is its ERR file, so whatever a library prints there (htslib's CRAM and index messages)
+// lands in that sample's ERR in the order its own run prints it.  The next sample is opened on a worker thread while the current
+// one computes, holding its messages until its turn, unless it is a CRAM: htslib prints while it opens one, so a CRAM is opened
+// at its turn.  Its first window is decoded ahead only when the current sample does not use the process's two window jobs, so
+// page-locked window memory stays at two jobs, reused from sample to sample.
+int run_cohort(const Options &o, Engines &engines, const std::string &list_path, double t_main0) {
+    struct Entry { std::string in, out, err; };
+    std::vector<Entry> list;
+    {
+        std::ifstream f(list_path);
+        if (!f) { std::fprintf(stderr, "Failed to open sample list file: %s\n", list_path.c_str()); return 1; }
+        std::set<std::string> outputs;
+        std::string line; int ln = 0;
+        while (std::getline(f, line)) {
+            ++ln;
+            if (!line.empty() && line.back() == '\r') line.pop_back();
+            if (line.empty()) continue;
+            std::vector<std::string> fld; size_t p = 0;
+            for (size_t t; (t = line.find('\t', p)) != std::string::npos; p = t + 1) fld.push_back(line.substr(p, t - p));
+            fld.push_back(line.substr(p));
+            const bool empty_field = std::any_of(fld.begin(), fld.end(), [](const std::string &x) { return x.empty(); });
+            if ((fld.size() != 2 && fld.size() != 3) || empty_field) {
+                std::fprintf(stderr, "%s:%d: a sample line is INPUT<TAB>OUT or INPUT<TAB>OUT<TAB>ERR\n", list_path.c_str(), ln);
+                return 1;
+            }
+            Entry e{fld[0], fld[1], fld.size() == 3 ? fld[2] : fld[1] + ".log"};
+            for (const std::string *path : {&e.out, &e.err}) {
+                std::error_code ec;
+                std::filesystem::path abs = std::filesystem::absolute(*path, ec);
+                if (ec) abs = *path;
+                if (!outputs.insert(abs.lexically_normal().string()).second) {
+                    std::fprintf(stderr, "%s:%d: %s is already the output of an earlier sample\n", list_path.c_str(), ln, path->c_str());
+                    return 1;
+                }
+            }
+            list.push_back(std::move(e));
+        }
+        if (list.empty()) { std::fprintf(stderr, "%s lists no sample\n", list_path.c_str()); return 1; }
+    }
+    std::unique_ptr<WindowJob[]> pool(new WindowJob[2]);
+    auto open_ahead = [&](size_t k, bool first_window) {
+        return std::async(std::launch::async, open_sample, std::cref(o), list[k].in, now(), nullptr, pool.get(), first_window);
+    };
+    if (!o.decode_only && !o.dist_refused()) engines.start_warm();
+    std::future<std::unique_ptr<Sample>> ahead;                          // sample k, opened ahead of its turn
+    if (!is_cram_path(list[0].in)) ahead = open_ahead(0, true);          // under the CUDA start-up
+    std::unique_ptr<Sample> cur;
+    int n_failed = 0;
+    for (size_t k = 0; k < list.size(); ++k) {
+        const Entry &e = list[k];
+        const bool next_ahead = k + 1 < list.size() && !is_cram_path(list[k + 1].in);
+        int out_fd = -1, err_fd = -1; std::string why;
+        if (!open_outputs(e.out, e.err, out_fd, err_fd, why)) {
+            if (ahead.valid()) ahead.get();
+            std::fprintf(stderr, "sample %zu (%s) failed: %s\n", k + 1, e.in.c_str(), why.c_str());
+            ++n_failed;
+            if (next_ahead) ahead = open_ahead(k + 1, true);
+            continue;
+        }
+        std::fflush(stderr);
+        const int saved_fd2 = ::dup(2);
+        ::dup2(err_fd, 2);
+        cur = ahead.valid() ? ahead.get() : open_sample(o, e.in, now(), stderr, pool.get(), true);
+        if (next_ahead) ahead = open_ahead(k + 1, !cur->uses_windows());
+        const int rc = run_sample(o, engines, *cur, out_fd, stderr, t_main0);
+        cur.reset();                                                     // htslib's closing lines still go to this ERR
+        if (std::fflush(stderr) != 0) why = e.err + ": " + std::strerror(errno);
+        else if (std::ferror(stderr)) why = e.err + ": write error";
+        std::clearerr(stderr);
+        ::dup2(saved_fd2, 2);
+        ::close(saved_fd2);
+        if (::close(err_fd) != 0 && why.empty()) why = e.err + ": " + std::strerror(errno);
+        if (::close(out_fd) != 0 && why.empty()) why = e.out + ": " + std::strerror(errno);
+        if (rc < 0) {
+            std::fprintf(stderr, "sample %zu (%s): no engine could be created (see %s); the remaining samples are not run\n", k + 1, e.in.c_str(), e.err.c_str());
+            return leave(engines, cur, 1);
+        }
+        if (rc != 0 || !why.empty()) {
+            ++n_failed;
+            if (!why.empty()) std::fprintf(stderr, "sample %zu (%s) failed: writing %s\n", k + 1, e.in.c_str(), why.c_str());
+            else std::fprintf(stderr, "sample %zu (%s) failed: see %s\n", k + 1, e.in.c_str(), e.err.c_str());
+        }
+    }
+    if (o.timing) std::fprintf(stderr, "[brc timing] cohort: %zu samples (%d failed) in %.3fs since main()\n", list.size(), n_failed, now() - t_main0);
+    return leave(engines, cur, n_failed ? 1 : 0);
+}
+
+}  // namespace
+
+int main(int argc, char **argv) {
+    const double t_main0 = now();
+    Options o;
+    std::string bam_list; bool shard_given = false;
+    static option lo[] = {{"help", 0, 0, 'h'}, {"version", 0, 0, 'v'}, {"min-mapping-quality", 1, 0, 'q'}, {"min-base-quality", 1, 0, 'b'},
+                          {"max-count", 1, 0, 'd'}, {"site-list", 1, 0, 'l'}, {"reference-fasta", 1, 0, 'f'}, {"print-individual-mapq", 1, 0, 'D'},
+                          {"per-library", 0, 0, 'p'}, {"max-warnings", 1, 0, 'w'}, {"insertion-centric", 0, 0, 'i'}, {"shard", 1, 0, 1000},
+                          {"min-alt-count", 1, 0, 1001}, {"min-alt-fraction", 1, 0, 1002}, {"bam-list", 1, 0, 1003}, {0, 0, 0, 0}};
+    long min_alt_count = 0; double min_alt_fraction = -1.0;       // site filter (brc_set_site_filter); off unless one is given
+    bool help = false, version = false;
+    for (int c; (c = getopt_long(argc, argv, "hvq:b:d:l:f:D:pw:i", lo, nullptr)) != -1;) {
+        switch (c) {
+        case 'h': help = true; break; case 'v': version = true; break;
+        case 'q': o.min_mapq = std::atoi(optarg); break; case 'b': o.min_bq = std::atoi(optarg); break; case 'd': o.max_cnt = std::atoi(optarg); break;
+        case 'l': o.fn_pos = optarg; break; case 'f': o.fn_fa = optarg; break; case 'D': o.dist_arg = optarg; break;
+        case 'p': o.per_lib = true; break; case 'w': o.max_warn = std::atoll(optarg); break; case 'i': o.ic = true; break;
+        case 1000: if (std::sscanf(optarg, "%d/%d", &o.shard_rank, &o.shard_count) != 2 || o.shard_count < 1 || o.shard_rank < 0 || o.shard_rank >= o.shard_count) { std::fprintf(stderr, "--shard wants RANK/COUNT with 0 <= RANK < COUNT\n"); return 1; }
+                   shard_given = true; break;
+        case 1001: {
+            char *end = nullptr; errno = 0;
+            min_alt_count = std::strtol(optarg, &end, 10);
+            if (errno || end == optarg || *end || min_alt_count < 1 || min_alt_count > INT32_MAX) { std::fprintf(stderr, "--min-alt-count wants an integer N >= 1\n"); return 1; }
+            break;
+        }
+        case 1002: {
+            char *end = nullptr; errno = 0;
+            min_alt_fraction = std::strtod(optarg, &end);
+            if (errno || end == optarg || *end || !(min_alt_fraction >= 0.0 && min_alt_fraction <= 1.0)) { std::fprintf(stderr, "--min-alt-fraction wants a number F with 0 <= F <= 1\n"); return 1; }
+            break;
+        }
+        case 1003: bam_list = optarg; break;
+        default: usage(); return 1;
+        }
+    }
+    o.site_filter = min_alt_count > 0 || min_alt_fraction >= 0.0;
+    o.filter.min_alt_count = (int32_t)std::max<long>(min_alt_count, 1); o.filter.min_alt_fraction = std::max(min_alt_fraction, 0.0);
+    if (version) { std::printf("bam-readcount version: b200 (engine ABI %d)\n", brc_abi_version()); return 1; }   // R:...:467-470 (exit 1)
+    if (help || (optind >= argc && bam_list.empty())) { usage(); return 1; }                                        // R:...:472-475
+    if (!bam_list.empty() && shard_given) { std::fprintf(stderr, "--bam-list and --shard cannot be combined: shard a cohort by splitting its list\n"); return 1; }
+    o.decode_only = std::getenv("BRC_CLI_DECODE_ONLY") != nullptr;   // test hook: exercise BGZF/BAI/region fetch without a GPU
+    o.device_decode = std::getenv("BRC_CLI_DEVICE_DECODE") != nullptr && !o.decode_only;
+    o.timing = std::getenv("BRC_CLI_TIMING") != nullptr;
+
+    Engines engines;
+    brc_config &cfg = engines.cfg;
+    cfg.min_mapq = o.min_mapq; cfg.min_bq = o.min_bq; cfg.max_cnt = o.max_cnt; cfg.per_lib = o.per_lib; cfg.insertion_centric = o.ic;
+    cfg.n_libs = 0; cfg.device = std::getenv("BRC_DEVICE") ? std::atoi(std::getenv("BRC_DEVICE")) : 0;
+    if (!bam_list.empty()) {
+        o.region_args.assign(argv + optind, argv + argc);          // every positional argument is a region of every sample
+        return run_cohort(o, engines, bam_list, t_main0);
+    }
+    const std::string bam_path = argv[optind];
+    o.region_args.assign(argv + optind + 1, argv + argc);
+    // CUDA context creation takes a second or two: do it while the BAM header, index and FASTA index are read
+    if (!o.decode_only && !o.dist_refused()) engines.start_warm();
+    std::unique_ptr<WindowJob[]> pool(new WindowJob[2]);
+    std::unique_ptr<Sample> s = open_sample(o, bam_path, t_main0, stderr, pool.get(), true);
+    const int rc = run_sample(o, engines, *s, STDOUT_FILENO, stderr, t_main0);
+    return leave(engines, s, rc < 0 ? 1 : rc);
 }
