@@ -283,6 +283,16 @@ int64_t rec_endpos(const Rec &r) {   // bam_endpos
     return (int64_t)r.pos + 1;
 }
 
+using RgLib = std::unordered_map<std::string, uint16_t>;   // @RG ID -> library rank
+
+// the library the engine counts a record under: 0 without -p; under -p the rank of its read group's LB, or BRC_LIB_NONE
+// where bam_get_library finds none (no RG tag, or an ID without an LB in the header)
+uint16_t rec_lib(const Rec &r, const RgLib &rg_lib, bool per_lib) {
+    if (!per_lib) return 0;
+    if (r.has_rg) { auto it = rg_lib.find(r.rg); if (it != rg_lib.end()) return it->second; }
+    return (uint16_t)BRC_LIB_NONE;
+}
+
 // ------------------------------------------------------------------------------------------
 // SURVEY.md §8 f-2: the compressed bytes + index entry points covering samfetch(tid, fbeg, fend), for brc_push_bam_span — the
 // records are inflated and framed on the device, only compressed bytes cross PCIe.  The BAI's chunk begins and linear-index
@@ -342,12 +352,12 @@ struct RegionFetcher {
     BamFile &bam;
     std::deque<Rec> win;          // decoded records that may overlap a later region, file order
     std::vector<Rec> spare;       // recycled records (keeps their heap buffers)
-    bool active = false, stream_done = false, merge = true;
+    bool active = false, stream_done = false;
     int cur_tid = -1;
     int64_t last_fbeg = -1, keep_floor = -1, last_pos = -1;
     uint64_t n_seeks = 0, n_decoded = 0;
 
-    explicit RegionFetcher(BamFile &b) : bam(b) { merge = std::getenv("BRC_CLI_NO_MERGE") == nullptr; }
+    explicit RegionFetcher(BamFile &b) : bam(b) {}
 
     Rec take() { if (spare.empty()) return Rec(); Rec r = std::move(spare.back()); spare.pop_back(); return r; }
     void give(Rec &&r) { if (spare.size() < 4096) spare.push_back(std::move(r)); }
@@ -355,7 +365,7 @@ struct RegionFetcher {
     template <class Emit> void fetch(int tid, int64_t fbeg, int64_t fend, int64_t next_fbeg, Emit &&emit) {
         uint64_t voff;
         if (!bam.query_offset(tid, fbeg, voff)) return;
-        const bool cont = merge && active && tid == cur_tid && fbeg >= last_fbeg && fbeg >= keep_floor && voff <= bam.bz.tell();
+        const bool cont = active && tid == cur_tid && fbeg >= last_fbeg && fbeg >= keep_floor && voff <= bam.bz.tell();
         if (!cont) {
             while (!win.empty()) { give(std::move(win.back())); win.pop_back(); }
             stream_done = false; last_pos = -1; ++n_seeks;
@@ -449,13 +459,20 @@ struct Warner {
     bool budget_left() const { return counts[SM] < max_per_type || counts[NM] < max_per_type || (per_lib && counts[LIB] < max_per_type); }
     bool collecting() const { return max_per_type > 0 && budget_left(); }
     void begin_region(int tid, int beg, int end, bool skip_halo) { regs.push_back({tid, beg, end, skip_halo, cands.size(), cands.size()}); }
-    void consider(const Rec &r, bool no_lib) {
-        if (!collecting() || (r.flag & 4) || regs.empty()) return;
-        const bool no_nm = r.nm == BRC_TAG_ABSENT, no_sm = (r.flag & 2) && r.sm == BRC_TAG_ABSENT;
-        if (!no_nm && !no_sm && !(per_lib && no_lib)) return;
-        Cand c; c.pos = r.pos; c.endpos = r.endpos; c.flag = r.flag; c.mapq = r.mapq; c.no_nm = no_nm; c.no_sm = no_sm; c.no_lib = per_lib && no_lib;
+    // a record that can warn at all (no NM tag, proper pair without SM tag, or `lib` == BRC_LIB_NONE) becomes `c`
+    static bool candidate(const Rec &r, uint16_t lib, Cand &c) {
+        const bool no_nm = r.nm == BRC_TAG_ABSENT, no_sm = (r.flag & 2) && r.sm == BRC_TAG_ABSENT, no_lib = lib == (uint16_t)BRC_LIB_NONE;
+        if (!no_nm && !no_sm && !no_lib) return false;
+        c.pos = r.pos; c.endpos = rec_endpos(r); c.flag = r.flag; c.mapq = r.mapq; c.no_nm = no_nm; c.no_sm = no_sm; c.no_lib = no_lib;
         c.cigar.assign(r.cigar, r.cigar + r.n_cigar); c.qual.assign(r.qual, r.qual + r.l_qseq);
         c.qname = (const char *)(r.data.data() + 32);
+        return true;
+    }
+    // a record of the record stream, in file order
+    void consider(const Rec &r, uint16_t lib) {
+        if (!collecting() || (r.flag & 4) || regs.empty()) return;
+        Cand c;
+        if (!candidate(r, lib, c)) return;
         cands.push_back(std::move(c)); regs.back().c1 = cands.size();
     }
     // candidates collected by a parallel decode (ParallelFetcher), already in file order
@@ -546,6 +563,13 @@ struct Slice {
         cands.clear(); cand_overflow = false; error = false; n_decoded = 0;
     }
     size_t n() const { return pos.size(); }
+    void append(const Rec &r, uint16_t l) {
+        pos.push_back(r.pos); flag.push_back(r.flag); mapq.push_back(r.mapq); lib.push_back(l); l_qseq.push_back(r.l_qseq);
+        nm.push_back(r.nm); sm.push_back(r.sm);
+        cigar.insert(cigar.end(), r.cigar, r.cigar + r.n_cigar); cigar_off.push_back(cigar.size());
+        seq.insert(seq.end(), r.seq, r.seq + ((size_t)r.l_qseq + 1) / 2); seq_off.push_back(seq.size());
+        qual.insert(qual.end(), r.qual, r.qual + r.l_qseq); qual_off.push_back(qual.size());
+    }
 };
 
 struct PinnedBuf {   // grow-only host buffer: page-locked through the engine when there is one (brc_host_alloc), plain otherwise
@@ -573,12 +597,11 @@ struct WindowJob {   // one decoded window: the slices and the concatenated batc
 };
 
 struct ParallelFetcher {
-    const BamFile &bam; std::string path; int n_threads; bool per_lib, want_pinned;
-    std::unordered_map<std::string, uint16_t> rg_lib;      // @RG ID -> library rank
+    const BamFile &bam; const RgLib &rg_lib; std::string path; int n_threads; bool per_lib, want_pinned;
     std::vector<std::unique_ptr<Bgzf>> readers;
     static constexpr size_t MAX_CANDS = 65536;
 
-    ParallelFetcher(const BamFile &b, const std::string &p, bool pl, bool pin) : bam(b), path(p), per_lib(pl), want_pinned(pin) {
+    ParallelFetcher(const BamFile &b, const RgLib &rl, const std::string &p, bool pl, bool pin) : bam(b), rg_lib(rl), path(p), per_lib(pl), want_pinned(pin) {
         unsigned hw = std::thread::hardware_concurrency();
         n_threads = (int)std::max(1u, std::min(hw ? hw : 1u, 16u));
         if (const char *ov = std::getenv("BRC_CLI_DECODE_THREADS")) n_threads = std::max(1, std::atoi(ov));
@@ -602,28 +625,15 @@ struct ParallelFetcher {
                 if (r.endpos <= fbeg) continue;
             }
             if (r.flag & 4) continue;
-            uint16_t lib = 0; bool no_lib = false;
-            if (per_lib) {
-                lib = (uint16_t)BRC_LIB_NONE;
-                if (r.has_rg) { auto it = rg_lib.find(r.rg); if (it != rg_lib.end()) lib = it->second; }
-                no_lib = lib == (uint16_t)BRC_LIB_NONE;
-            }
+            const uint16_t lib = rec_lib(r, rg_lib, per_lib);
             if (collect && !out.cand_overflow) {
-                const bool no_nm = r.nm == BRC_TAG_ABSENT, no_sm = (r.flag & 2) && r.sm == BRC_TAG_ABSENT;
-                if (no_nm || no_sm || no_lib) {
+                Warner::Cand c;
+                if (Warner::candidate(r, lib, c)) {
                     if (out.cands.size() >= MAX_CANDS) out.cand_overflow = true;
-                    else {
-                        Warner::Cand c; c.pos = r.pos; c.endpos = rec_endpos(r); c.flag = r.flag; c.mapq = r.mapq; c.no_nm = no_nm; c.no_sm = no_sm; c.no_lib = no_lib;
-                        c.cigar.assign(r.cigar, r.cigar + r.n_cigar); c.qual.assign(r.qual, r.qual + r.l_qseq); c.qname = (const char *)(r.data.data() + 32);
-                        out.cands.push_back(std::move(c));
-                    }
+                    else out.cands.push_back(std::move(c));
                 }
             }
-            out.pos.push_back(r.pos); out.flag.push_back(r.flag); out.mapq.push_back(r.mapq); out.lib.push_back(lib); out.l_qseq.push_back(r.l_qseq);
-            out.nm.push_back(r.nm); out.sm.push_back(r.sm);
-            out.cigar.insert(out.cigar.end(), r.cigar, r.cigar + r.n_cigar); out.cigar_off.push_back(out.cigar.size());
-            out.seq.insert(out.seq.end(), r.seq, r.seq + ((size_t)r.l_qseq + 1) / 2); out.seq_off.push_back(out.seq.size());
-            out.qual.insert(out.qual.end(), r.qual, r.qual + r.l_qseq); out.qual_off.push_back(out.qual.size());
+            out.append(r, lib);
         }
     }
 
@@ -824,6 +834,11 @@ struct Messages {
 
 struct Region { int tid, beg, end; bool site_list; bool cont = false; };   // cont: a later window of a cut region (its halo site belongs to the window before)
 
+// the end of region g's fetch, clamped to the contig's length (a region that starts beyond the contig keeps one base)
+int64_t fetch_end(const BamFile &bam, const Region &g) {
+    return std::min<int64_t>(g.end, std::max<int64_t>(bam.lens[(size_t)g.tid], (int64_t)g.beg + 1));
+}
+
 struct Sample {
     const Options &o;
     std::string path; bool is_cram = false;
@@ -835,12 +850,12 @@ struct Sample {
     HtsSource hts;
 #endif
     Fasta fa; bool have_fa = false;
-    std::map<std::string, std::string> rg_lb;                   // @RG ID -> LB
-    std::map<std::string, uint16_t> lib_rank;
+    RgLib rg_lib;
     std::vector<std::string> lib_names; std::vector<const char *> lib_ptrs;
     std::vector<Region> regions;
     Warner warner;
-    // big fetches (windows of a cut region) are decoded by several threads, one window ahead of the engine (ParallelFetcher)
+    // big fetches (windows of a cut region) of a BAM are decoded by several threads, one window ahead of the engine
+    // (ParallelFetcher), unless the engine decodes the file itself (BRC_CLI_DEVICE_DECODE)
     ParallelFetcher pf;
     bool allow_parallel = false;
     WindowJob *jobs;              // the process's two window jobs (page-locked buffers), used by one sample at a time
@@ -848,14 +863,12 @@ struct Sample {
     bool par_decode_error = false; uint64_t par_decoded = 0, par_windows = 0;
 
     Sample(const Options &opt, const std::string &p, WindowJob *pool)
-        : o(opt), path(p), warner(opt.max_warn, opt.min_mapq, opt.min_bq, opt.per_lib, opt.ic), pf(bam, p, opt.per_lib, !opt.decode_only), jobs(pool) {}
+        : o(opt), path(p), warner(opt.max_warn, opt.min_mapq, opt.min_bq, opt.per_lib, opt.ic), pf(bam, rg_lib, p, opt.per_lib, !opt.decode_only), jobs(pool) {}
     Sample(const Sample &) = delete; Sample &operator=(const Sample &) = delete;
 
     void fetch_range(size_t gi, int64_t &fb, int64_t &fe) const {
-        const Region &g = regions[gi];
-        const int64_t clen = bam.lens[(size_t)g.tid];
-        fb = std::max<int64_t>((int64_t)g.beg - 1, 0);
-        fe = std::min<int64_t>(g.end, std::max<int64_t>(clen, (int64_t)g.beg + 1));
+        fb = std::max<int64_t>((int64_t)regions[gi].beg - 1, 0);
+        fe = fetch_end(bam, regions[gi]);
     }
     bool par_ok(size_t gi) const {
         if (!allow_parallel || gi >= regions.size()) return false;
@@ -910,20 +923,21 @@ std::unique_ptr<Sample> open_sample(const Options &o, const std::string &bam_pat
     s.have_fa = !o.fn_fa.empty() && s.fa.open(o.fn_fa);
     if (!o.fn_fa.empty() && !s.have_fa) { log.say("Fail to open reference file %s\n", o.fn_fa.c_str()); return sp; }
 
-    // @RG ID -> LB; libraries in std::set order (R:...:92-111, 526-529)
-    std::set<std::string> libs;
+    // @RG ID -> rank of its LB: the first @RG line of an ID wins, libraries in std::set order (R:...:92-111, 526-529)
+    std::set<std::string> libs; std::vector<std::pair<std::string, std::string>> id_lb;
     {
         std::istringstream ss(bam.text); std::string line;
         while (std::getline(ss, line)) {
             if (line.compare(0, 3, "@RG") != 0) continue;
             std::istringstream ls(line); std::string tok, id, lb; bool has_lb = false;
             while (std::getline(ls, tok, '\t')) { if (tok.compare(0, 3, "ID:") == 0) id = tok.substr(3); else if (tok.compare(0, 3, "LB:") == 0) { lb = tok.substr(3); has_lb = true; } }
-            if (has_lb) { libs.insert(lb); if (!id.empty() && !s.rg_lb.count(id)) s.rg_lb[id] = lb; }
+            if (has_lb) { libs.insert(lb); if (!id.empty()) id_lb.emplace_back(id, lb); }
         }
     }
     for (const auto &l : libs) log.say("Expect library: %s in BAM\n", l.c_str());
     s.lib_names.assign(libs.begin(), libs.end());
-    for (size_t i = 0; i < s.lib_names.size(); ++i) s.lib_rank[s.lib_names[i]] = (uint16_t)i;
+    for (const auto &p : id_lb)
+        s.rg_lib.emplace(p.first, (uint16_t)(std::lower_bound(s.lib_names.begin(), s.lib_names.end(), p.second) - s.lib_names.begin()));
     for (auto &n : s.lib_names) s.lib_ptrs.push_back(n.c_str());
     if (s.lib_ptrs.empty()) s.lib_ptrs.push_back("");
 
@@ -964,16 +978,15 @@ std::unique_ptr<Sample> open_sample(const Options &o, const std::string &bam_pat
     // at 30x would otherwise need tens of GB).  A window is just a region of the -l loop: it recomputes the site to its left
     // (the 1-site halo), so the concatenated output equals the unsplit region's.  Only the last window of an argv region keeps
     // argv semantics.  (With a tiny -d the max-count rule sees the window's own fetch order; SURVEY.md §8e.)
+    s.allow_parallel = !s.is_cram && !o.device_decode;
     {
         // 2 Mb windows: each is decoded by all threads in ~40 ms one window ahead of the engine and needs 110 MB of page-locked memory
-        // (8 Mb windows were 0.6 s slower on a 10 Mb BAM, r02t); the record-by-record paths (CRAM, BRC_CLI_SEQUENTIAL) keep 8 Mb
-        const bool par_windows_ok = !s.is_cram && std::getenv("BRC_CLI_DEVICE_DECODE") == nullptr && std::getenv("BRC_CLI_SEQUENTIAL") == nullptr;
-        int64_t W = std::getenv("BRC_CLI_WINDOW") ? std::atoll(std::getenv("BRC_CLI_WINDOW")) : (par_windows_ok ? 2000000 : 8000000);
+        // (8 Mb windows were 0.6 s slower on a 10 Mb BAM, r02t); the record-by-record paths (CRAM, device decode) keep 8 Mb
+        int64_t W = std::getenv("BRC_CLI_WINDOW") ? std::atoll(std::getenv("BRC_CLI_WINDOW")) : (s.allow_parallel ? 2000000 : 8000000);
         if (o.shard_count > 1 && !std::getenv("BRC_CLI_WINDOW")) W = 1000000;      // finer units so the shards can balance
         std::vector<Region> cut;
         for (const Region &g : regions) {
-            const int64_t clen = bam.lens[(size_t)g.tid];
-            const int64_t e_eff = std::min<int64_t>(g.end, std::max<int64_t>(clen, (int64_t)g.beg + 1));
+            const int64_t e_eff = fetch_end(bam, g);
             if (e_eff - g.beg <= W) { cut.push_back(g); continue; }
             for (int64_t b = g.beg; b < e_eff; b += W) {
                 const bool last = b + W >= e_eff;
@@ -995,8 +1008,7 @@ std::unique_ptr<Sample> open_sample(const Options &o, const std::string &bam_pat
         std::vector<double> wgt(regions.size(), 1.0);
         for (size_t i = 0; i < regions.size(); ++i) {
             const Region &g = regions[i];
-            const int64_t clen = bam.lens[(size_t)g.tid];
-            const int64_t e_eff = std::min<int64_t>(g.end, std::max<int64_t>(clen, (int64_t)g.beg + 1));
+            const int64_t e_eff = fetch_end(bam, g);
             double w = (double)std::max<int64_t>(e_eff - g.beg, 1) * 0.05;                 // no index information: 0.05 bytes per base
             if (g.tid < (int)bam.idx.size() && !bam.idx[(size_t)g.tid].linear.empty()) {
                 const auto &lin = bam.idx[(size_t)g.tid].linear;
@@ -1014,8 +1026,6 @@ std::unique_ptr<Sample> open_sample(const Options &o, const std::string &bam_pat
         regions.swap(mine);
     }
 
-    for (const auto &kv : s.rg_lb) s.pf.rg_lib[kv.first] = s.lib_rank[kv.second];
-    s.allow_parallel = !s.is_cram && !o.device_decode && std::getenv("BRC_CLI_SEQUENTIAL") == nullptr;
     // decode under the CUDA start-up (first sample) or under the previous sample's compute (cohort)
     if (first_window && !regions.empty() && s.par_ok(0)) { s.ahead_slot = 0; s.ahead_gi = 0; s.ahead = s.start_decode(0, 0); }
     s.status = 0;
@@ -1075,10 +1085,10 @@ int run_sample(const Options &o, Engines &engines, Sample &s, int out_fd, FILE *
     }
 
     std::string chrom;
-    double t_decode = 0, t_compute = 0, t_format = 0, t_write = 0, t_ref = 0, t_results = 0, t_reset = 0;
+    double t_decode = 0, t_compute = 0, t_format = 0, t_ref = 0, t_results = 0, t_reset = 0;
     // BRC_CLI_DEVICE_DECODE=1: BGZF inflate + BAM framing on the GPU (per-read warning lines need host-decoded reads: counts only)
     std::vector<const char *> rg_ids; std::vector<uint16_t> rg_libs;
-    for (const auto &kv : s.rg_lb) { rg_ids.push_back(kv.first.c_str()); rg_libs.push_back(s.lib_rank[kv.second]); }
+    for (const auto &kv : s.rg_lib) { rg_ids.push_back(kv.first.c_str()); rg_libs.push_back(kv.second); }
     int64_t warn_total[4] = {0, 0, 0, 0};
     auto flush = [&]() -> int {
         const double c0 = now();
@@ -1120,63 +1130,48 @@ int run_sample(const Options &o, Engines &engines, Sample &s, int out_fd, FILE *
     for (size_t gi = 0; gi < regions.size(); ++gi) {
         const Region &g = regions[gi];
         const double d0 = now();
-        if (o.decode_only) {
-            const int64_t fbeg = std::max<int64_t>((int64_t)g.beg - 1, 0), fend = g.end;
-            int64_t n = 0, psum = 0, qsum = 0;
-            auto count = [&](const Rec &r) { if (r.flag & 4) return; ++n; psum += r.pos; for (int k = 0; k < r.l_qseq; ++k) qsum += r.qual[k]; };
-            WindowJob *job = s.par_ok(gi) ? s.decoded_window(gi) : nullptr;
-            if (job) {
-                const brc_read_batch &b = job->batch;
+        if (!o.decode_only) {
+            const std::string &contig = bam.names[(size_t)g.tid];
+            auto loaded = h->ref_name.find(g.tid);
+            if (loaded == h->ref_name.end() || loaded->second != contig) {   // load_reference: whole chromosome
+                h->ref_name.erase(g.tid);
+                if (!s.fa.fetch(contig, chrom)) { std::fprintf(err, "Failed to fetch %s from %s\n", contig.c_str(), o.fn_fa.c_str()); return 1; }
+                const int rc = brc_set_reference(eng, g.tid, contig.c_str(), (int64_t)chrom.size(), 0, chrom.data(), (int64_t)chrom.size());
+                if (rc != BRC_OK) { std::fprintf(err, "brc_set_reference: %s\n", brc_last_error(eng)); return 1; }
+                h->ref_name[g.tid] = contig;
+                t_ref += now() - d0;
+            }
+        }
+        const double d1 = now();
+        // the source: a window decoded by ParallelFetcher, the compressed span (device decode), or the record stream.  A window
+        // or a span is a batch of its own: whatever smaller regions are pending goes out first.
+        const bool window = s.par_ok(gi), span = !window && o.device_decode && !s.is_cram;
+        if ((window || span) && pushed > 0) { if (flush() != BRC_OK) return 1; pushed = 0; }
+        WindowJob *job = window ? s.decoded_window(gi) : nullptr;      // nullptr: the record stream after all
+        if (!o.decode_only) {
+            brc_begin_region(eng, g.tid, g.beg, g.end, g.site_list ? 1 : 0);
+            warner.begin_region(g.tid, g.beg, g.end, g.cont);
+        }
+        // samfetch(in, idx, ref, d.beg-1, d.end): records with tid, endpos > max(beg-1,0), pos < end, in file order
+        const int64_t fbeg = std::max<int64_t>((int64_t)g.beg - 1, 0), fend = g.end;
+        int64_t n = 0, psum = 0, qsum = 0;                             // decode-only: what the region received
+        if (job) {
+            // ONE borrowed batch (the engine streams it to the GPU in chunks) while the next window is already being decoded
+            const brc_read_batch &b = job->batch;
+            if (o.decode_only) {
                 n = b.n_reads;
                 for (int64_t i = 0; i < b.n_reads; ++i) psum += b.pos[i];
                 for (uint64_t k = b.qual_off[0]; k < b.qual_off[b.n_reads]; ++k) qsum += b.qual[k];
-                fetcher.active = false;
-            } else
-#ifdef BRC_WITH_HTSLIB
-            if (s.is_cram) s.hts.fetch(g.tid, fbeg, fend, count); else
-#endif
-            fetcher.fetch(g.tid, fbeg, fend, s.next_fbeg(gi), count);
-            dprintf(out_fd, "%d\t%d\t%d\t%lld\t%lld\t%lld\n", g.tid, g.beg, g.end, (long long)n, (long long)psum, (long long)qsum);
-            continue;
-        }
-        const std::string &contig = bam.names[(size_t)g.tid];
-        auto loaded = h->ref_name.find(g.tid);
-        if (loaded == h->ref_name.end() || loaded->second != contig) {   // load_reference: whole chromosome
-            h->ref_name.erase(g.tid);
-            if (!s.fa.fetch(contig, chrom)) { std::fprintf(err, "Failed to fetch %s from %s\n", contig.c_str(), o.fn_fa.c_str()); return 1; }
-            const int rc = brc_set_reference(eng, g.tid, contig.c_str(), (int64_t)chrom.size(), 0, chrom.data(), (int64_t)chrom.size());
-            if (rc != BRC_OK) { std::fprintf(err, "brc_set_reference: %s\n", brc_last_error(eng)); return 1; }
-            h->ref_name[g.tid] = contig;
-            t_ref += now() - d0;
-        }
-        const double d1 = now();
-        if (s.par_ok(gi)) {
-            // one window = one batch: whatever smaller regions are pending goes out first, then the window is pushed as ONE borrowed
-            // batch (the engine streams it to the GPU in chunks) while the next window is already being decoded
-            if (pushed > 0) { if (flush() != BRC_OK) return 1; pushed = 0; }
-            if (WindowJob *job = s.decoded_window(gi)) {
-                brc_begin_region(eng, g.tid, g.beg, g.end, g.site_list ? 1 : 0);
-                warner.begin_region(g.tid, g.beg, g.end, g.cont);
+            } else {
                 for (Slice &sl : job->slices) warner.take(sl.cands);
-                if (job->batch.n_reads > 0) {
-                    const int prc = brc_push_reads(eng, &job->batch);
+                if (b.n_reads > 0) {
+                    const int prc = brc_push_reads(eng, &b);
                     if (prc != BRC_OK) { std::fprintf(err, "brc_push_reads: %s\n", brc_last_error(eng)); return 1; }
                 }
-                brc_end_region(eng);
-                fetcher.active = false;
-                t_decode += now() - d1;
-                if (flush() != BRC_OK) return 1;     // the batch is borrowed until the text is out
-                pushed = 0;
-                continue;
             }
-        }
-        brc_begin_region(eng, g.tid, g.beg, g.end, g.site_list ? 1 : 0);
-        warner.begin_region(g.tid, g.beg, g.end, g.cont);
-        // samfetch(in, idx, ref, d.beg-1, d.end): records with tid, endpos > max(beg-1,0), pos < end, in file order
-        const int64_t fbeg = std::max<int64_t>((int64_t)g.beg - 1, 0), fend = g.end;
-        int push_rc = BRC_OK;
-        if (o.device_decode && !s.is_cram) {
-            // f-2: hand the engine the compressed span; it inflates, frames and computes on the device.  One span per batch.
+            fetcher.active = false;
+        } else if (span) {
+            // f-2: hand the engine the compressed span; it inflates, frames and computes on the device
             SpanBuilder sb;
             if (sb.build(bam, g.tid, fbeg, fend)) {
                 brc_bam_span sp{}; sp.comp = sb.comp.data(); sp.comp_len = (int64_t)sb.comp.size(); sp.n_entry = (int64_t)sb.entries.size(); sp.entry = sb.entries.data();
@@ -1185,32 +1180,39 @@ int run_sample(const Options &o, Engines &engines, Sample &s, int out_fd, FILE *
                 if (prc != BRC_OK) { std::fprintf(err, "brc_push_bam_span: %s\n", brc_last_error(eng)); return 1; }
             }
             fetcher.active = false;
-            brc_end_region(eng);
-            t_decode += now() - d1;
-            if (flush() != BRC_OK) return 1;
-            pushed = 0;
+        } else {
+            auto stream = [&](auto &&sink) {
+#ifdef BRC_WITH_HTSLIB
+                if (s.is_cram) { s.hts.fetch(g.tid, fbeg, fend, sink); return; }
+#endif
+                fetcher.fetch(g.tid, fbeg, fend, s.next_fbeg(gi), sink);
+            };
+            int push_rc = BRC_OK;
+            auto push = [&](const Rec &r) {
+                const uint16_t lib = rec_lib(r, s.rg_lib, o.per_lib);
+                warner.consider(r, lib);
+                const int prc = brc_push_read(eng, r.tid, r.pos, r.flag, r.mapq, lib, r.l_qseq, r.nm, r.sm, r.n_cigar, r.cigar, r.seq, r.qual);
+                if (prc != BRC_OK && push_rc == BRC_OK) push_rc = prc;
+                ++pushed;
+            };
+            auto count = [&](const Rec &r) {
+                if (r.flag & 4) return;
+                int64_t q = 0;             // a local sum: the quality bytes may alias qsum, which would be stored once per byte
+                for (int k = 0; k < r.l_qseq; ++k) q += r.qual[k];
+                ++n; psum += r.pos; qsum += q;
+            };
+            if (o.decode_only) stream(count); else stream(push);
+            if (push_rc != BRC_OK) { std::fprintf(err, "brc_push_read: %s\n", brc_last_error(eng)); return 1; }
+        }
+        if (o.decode_only) {
+            dprintf(out_fd, "%d\t%d\t%d\t%lld\t%lld\t%lld\n", g.tid, g.beg, g.end, (long long)n, (long long)psum, (long long)qsum);
             continue;
         }
-        auto push = [&](const Rec &r) {
-            uint16_t lib = 0;
-            if (o.per_lib) {
-                lib = (uint16_t)BRC_LIB_NONE;
-                if (r.has_rg) { auto it = s.rg_lb.find(r.rg); if (it != s.rg_lb.end()) lib = s.lib_rank[it->second]; }
-            }
-            warner.consider(r, lib == (uint16_t)BRC_LIB_NONE);
-            const int prc = brc_push_read(eng, r.tid, r.pos, r.flag, r.mapq, lib, r.l_qseq, r.nm, r.sm, r.n_cigar, r.cigar, r.seq, r.qual);
-            if (prc != BRC_OK && push_rc == BRC_OK) push_rc = prc;
-            ++pushed;
-        };
-#ifdef BRC_WITH_HTSLIB
-        if (s.is_cram) s.hts.fetch(g.tid, fbeg, fend, push); else
-#endif
-        fetcher.fetch(g.tid, fbeg, fend, s.next_fbeg(gi), push);
-        if (push_rc != BRC_OK) { std::fprintf(err, "brc_push_read: %s\n", brc_last_error(eng)); return 1; }
         brc_end_region(eng);
         t_decode += now() - d1;
-        // flush in batches at region boundaries; the deletion queue of the argv loop is carried by the engine (brc_set_queue_carry)
-        if (gi + 1 == regions.size() || pushed > 1500000) { if (flush() != BRC_OK) return 1; pushed = 0; }
+        // a window's batch is borrowed until its text is out, and a span is one batch; record-stream regions go out in batches
+        // at region boundaries (the deletion queue of the argv loop is carried by the engine, brc_set_queue_carry)
+        if (job || span || gi + 1 == regions.size() || pushed > 1500000) { if (flush() != BRC_OK) return 1; pushed = 0; }
     }
     warner.finish(warn_total);
 #ifdef BRC_WITH_HTSLIB
@@ -1223,8 +1225,8 @@ int run_sample(const Options &o, Engines &engines, Sample &s, int out_fd, FILE *
     if (o.timing) std::fprintf(err, "[brc timing] index seeks %llu  records decoded %llu  (+ %llu records in %llu windows decoded by %d threads)\n", (unsigned long long)fetcher.n_seeks,
                                (unsigned long long)fetcher.n_decoded, (unsigned long long)s.par_decoded, (unsigned long long)s.par_windows, s.pf.n_threads);
     if (o.decode_only) return decode_error ? 1 : 0;
-    if (o.timing) std::fprintf(err, "[brc timing] reference %.3fs  decode+push %.3fs  compute %.3fs  results %.3fs  format %.3fs  reset %.3fs  write %.3fs  | region loop %.3fs, since main() %.3fs\n",
-                               t_ref, t_decode, t_compute, t_results, t_format, t_reset, t_write, now() - t_loop0, now() - t_main0);
+    if (o.timing) std::fprintf(err, "[brc timing] reference %.3fs  decode+push %.3fs  compute %.3fs  results %.3fs  format %.3fs  reset %.3fs  | region loop %.3fs, since main() %.3fs\n",
+                               t_ref, t_decode, t_compute, t_results, t_format, t_reset, now() - t_loop0, now() - t_main0);
     if (o.timing) std::fprintf(err, "[brc timing] startup (CUDA context, header, index, first window) %.3fs\n", t_loop0 - s.t0);
     return decode_error ? 1 : 0;
 }

@@ -160,10 +160,10 @@ def _make_bam(case, d):
     return os.path.join(d, "s.bam"), os.path.join(d, "ref.fa")
 
 
-def test_cli_site_list_fetch_merging_yields_samfetch_records(tmp_path):
+def test_cli_site_list_fetch_merging_yields_samfetch_records_in_one_pass(tmp_path):
     """CPU (SURVEY.md §8 f-3): consecutive site-list lines share one forward pass over the BAM instead of one index seek
-    each; every region must still receive exactly the records samfetch yields.  Checked against the per-region seek path
-    (BRC_CLI_NO_MERGE) and against the Python decoder."""
+    each; every region must still receive exactly the records samfetch yields (checked against the Python decoder), and the
+    fetch must seek and decode about as little as one pass over the file."""
     from oracle.oracle import REF_SAMTOOLS
     if not os.path.exists(REF_SAMTOOLS):
         pytest.skip("oracle/_ref/samtools not built")
@@ -173,19 +173,19 @@ def test_cli_site_list_fetch_merging_yields_samfetch_records(tmp_path):
     regs = _site_list_regions(60000, np.random.default_rng(5))
     sl = tmp_path / "sites"
     sl.write_text("".join(f"chr1\t{s}\t{e}\n" for s, e in regs))
-    outs, stats = [], []
-    for extra in ({}, {"BRC_CLI_NO_MERGE": "1"}):
-        p = subprocess.run([exe, "-l", str(sl), bam], capture_output=True, env=dict(os.environ, BRC_CLI_DECODE_ONLY="1", BRC_CLI_TIMING="1", **extra))
-        assert p.returncode == 0, p.stderr.decode()
-        outs.append(p.stdout.decode())
-        line = [ln for ln in p.stderr.decode().splitlines() if "index seeks" in ln][0].split()
-        stats.append((int(line[4]), int(line[7])))
-    assert outs[0] == outs[1]
-    assert stats[0][0] < 20 and stats[1][0] == len(regs)          # a handful of seeks instead of one per line
-    assert stats[0][1] * 20 < stats[1][1]                          # and far fewer records decoded
+    p = subprocess.run([exe, "-l", str(sl), bam], capture_output=True, env=dict(os.environ, BRC_CLI_DECODE_ONLY="1", BRC_CLI_TIMING="1"))
+    assert p.returncode == 0, p.stderr.decode()
+    line = [ln for ln in p.stderr.decode().splitlines() if "index seeks" in ln][0].split()
+    seeks, decoded = int(line[4]), int(line[7])
     b = case["batch"]
+    assert seeks < 20                                              # a handful of seeks instead of one per line (658)
+    # One forward pass decodes every record once.  Only the lines that go back (to 3000 and to 1) seek backwards, into the first
+    # 16 kb linear-index window, and re-decode the records in front of them: together less than one more pass over this 60 kb
+    # contig.  One seek per line decodes about 50 times the file here.
+    assert decoded < 2 * b.n_reads
     qo = b.qual_off.astype(np.int64)
-    got = [tuple(int(x) for x in line.split("\t")) for line in outs[0].strip().splitlines()]
+    got = [tuple(int(x) for x in line.split("\t")) for line in p.stdout.decode().strip().splitlines()]
+    assert len(got) == len(regs)
     for (s, e), g in zip(regs, got):
         idx = b.fetch(0, max(s - 2, 0), e)
         want = (0, s - 1, e, len(idx), int(b.pos[idx].astype(np.int64).sum()), int(sum(int(b.qual[qo[i]:qo[i + 1]].astype(np.int64).sum()) for i in idx)))
@@ -207,18 +207,14 @@ def test_cli_dense_site_list_matches_oracle(tmp_path):
     sl.write_text("".join(f"chr1\t{s}\t{e}\n" for s, e in regs))
     for fl, argv in ((dict(min_mapq=20, min_bq=20), ["-q", "20", "-b", "20"]), (dict(per_lib=True), ["-p"])):
         want, _, _ = cases.run_oracle(case, fl, site_list=True)
-        outs = []
-        for extra in ({}, {"BRC_CLI_NO_MERGE": "1"}):
-            p = subprocess.run([exe, "-w", "0", "-f", ref] + argv + ["-l", str(sl), bam], capture_output=True, env=dict(os.environ, **extra))
-            assert p.returncode == 0, p.stderr.decode()[-2000:]
-            outs.append(p.stdout.decode("latin-1"))
-        assert outs[0] == outs[1]
-        assert outs[0] == want
+        p = subprocess.run([exe, "-w", "0", "-f", ref] + argv + ["-l", str(sl), bam], capture_output=True)
+        assert p.returncode == 0, p.stderr.decode()[-2000:]
+        assert p.stdout.decode("latin-1") == want
 
 
 def test_cli_fetch_merging_two_contigs_unsorted_and_past_the_end(tmp_path):
     """CPU: the merged fetch across contig changes, lines that go backwards, duplicates, a line past the contig's last read
-    and an unknown contig — record sets identical to the one-seek-per-line path and to the Python decoder."""
+    and an unknown contig — record sets identical to the Python decoder's samfetch."""
     from oracle.oracle import REF_SAMTOOLS
     if not os.path.exists(REF_SAMTOOLS):
         pytest.skip("oracle/_ref/samtools not built")
@@ -238,14 +234,10 @@ def test_cli_fetch_merging_two_contigs_unsorted_and_past_the_end(tmp_path):
              ("chrB", 19990, 25000), ("chrA", 29999, 30000), ("chrZ", 5, 6), ("chrB", 1, 1), ("chrB", 2, 2), ("chrB", 3, 400)]
     sl = tmp_path / "sites"
     sl.write_text("".join(f"{c}\t{s}\t{e}\n" for c, s, e in lines))
-    outs = []
-    for extra in ({}, {"BRC_CLI_NO_MERGE": "1"}):
-        p = subprocess.run([exe, "-l", str(sl), os.path.join(d, "s.bam")], capture_output=True, env=dict(os.environ, BRC_CLI_DECODE_ONLY="1", **extra))
-        assert p.returncode == 0, p.stderr.decode()
-        outs.append(p.stdout.decode())
-        assert b"chrZ not found in bam file" in p.stderr
-    assert outs[0] == outs[1]
-    got = [tuple(int(x) for x in ln.split("\t")) for ln in outs[0].strip().splitlines()]
+    p = subprocess.run([exe, "-l", str(sl), os.path.join(d, "s.bam")], capture_output=True, env=dict(os.environ, BRC_CLI_DECODE_ONLY="1"))
+    assert p.returncode == 0, p.stderr.decode()
+    assert b"chrZ not found in bam file" in p.stderr
+    got = [tuple(int(x) for x in ln.split("\t")) for ln in p.stdout.decode().strip().splitlines()]
     known = [ln for ln in lines if ln[0] != "chrZ"]
     assert len(got) == len(known)
     qo = both.qual_off.astype(np.int64)
@@ -454,37 +446,74 @@ def test_cli_sharded_output_concatenates_to_the_unsharded_output(tmp_path):
     assert multi.stdout == whole.stdout and len(whole.stdout.splitlines()) == 378000
 
 
-def test_cli_parallel_window_decode_yields_samfetch_records(tmp_path):
+def _samfetch_sums(b, tid, beg, end):
+    """(count, position sum, quality sum) of the mapped records samfetch(tid, max(beg-1, 0), end) yields for a region whose
+    0-based start is beg: what a decode-only run prints for it."""
+    qo = b.qual_off.astype(np.int64)
+    idx = [i for i in b.fetch(tid, max(beg - 1, 0), end) if not b.flag[i] & 4]
+    return (len(idx), int(b.pos[idx].astype(np.int64).sum()) if idx else 0, int(sum(int(b.qual[qo[i]:qo[i + 1]].astype(np.int64).sum()) for i in idx)))
+
+
+def test_cli_parallel_window_decode_yields_python_decoder_records(tmp_path):
     """Big fetches are decoded by several threads over position sub-ranges (ParallelFetcher) and concatenated: record count,
-    position sum and quality sum per region must equal the sequential reader's, whatever the thread count and window size
-    (decode-only, no device)."""
+    position sum and quality sum per region must equal the Python decoder's samfetch, whatever the thread count and window size.
+    A region under 256 kb takes the record stream instead (decode-only, no device)."""
     from oracle.oracle import REF_SAMTOOLS
     if not os.path.exists(REF_SAMTOOLS):
         pytest.skip("oracle/_ref/samtools not built")
     from bam_readcount_b200 import synth_cb
+    from bam_readcount_b200.bamio import read_bam
     exe = _cli()
     sp = synth_cb.Spec(seed=5, contig_len=1280 * 700)
     info = synth_cb.write_sample_bam(sp, 0, 0, 700, str(tmp_path), REF_SAMTOOLS)
+    _, rb = read_bam(info["bam"])
     regions = ["chr1:1-896000", "chr1:100001-700000", "chr1:5-300", "chr1"]
-    outs = []
-    for extra in ({"BRC_CLI_SEQUENTIAL": "1"}, {}, {"BRC_CLI_DECODE_THREADS": "3"}, {"BRC_CLI_DECODE_THREADS": "16", "BRC_CLI_WINDOW": "300000"},
-                  {"BRC_CLI_SEQUENTIAL": "1", "BRC_CLI_WINDOW": "300000"}):
-        p = subprocess.run([exe, "-w", "0", info["bam"]] + regions, capture_output=True, env=dict(os.environ, BRC_CLI_DECODE_ONLY="1", BRC_CLI_TIMING="1", **extra))
+    for extra, regs in (({}, regions), ({"BRC_CLI_DECODE_THREADS": "3"}, regions),
+                        ({"BRC_CLI_DECODE_THREADS": "16", "BRC_CLI_WINDOW": "300000"}, regions), ({}, ["chr1:100001-300000"])):
+        p = subprocess.run([exe, "-w", "0", info["bam"]] + regs, capture_output=True, env=dict(os.environ, BRC_CLI_DECODE_ONLY="1", BRC_CLI_TIMING="1", **extra))
         assert p.returncode == 0, p.stderr.decode()[-1000:]
-        outs.append((p.stdout, p.stderr.decode()))
-    assert outs[0][0] == outs[1][0] == outs[2][0] and outs[3][0] == outs[4][0]
-    assert len(outs[0][0].splitlines()) == 4 and int(outs[0][0].split()[3]) > 170000
-    assert "windows decoded by" in outs[1][1] and "(+ 0 records in 0 windows" in outs[0][1] and "(+ 0 records in 0 windows" not in outs[1][1]
+        got = [tuple(int(x) for x in ln.split("\t")) for ln in p.stdout.decode().strip().splitlines()]
+        for g in got:
+            assert g[3:] == _samfetch_sums(rb, *g[:3]), (extra, g)
+        through_windows = "(+ 0 records in 0 windows" not in p.stderr.decode()
+        if regs is regions:
+            assert through_windows
+            if "BRC_CLI_WINDOW" in extra:
+                assert len(got) > len(regs)                      # one line per 300 kb window
+            else:
+                assert len(got) == len(regs) and got[0][3] > 170000
+        else:
+            assert not through_windows and len(got) == 1 and got[0][3] > 0
+
+
+_WARNING_TYPES = (("Couldn't find single-end mapping quality.", "SM tag missing"), ("Couldn't find number of mismatches.", "NM tag missing"),
+                  ("Couldn't find the generated tag.", "generated tag missing"), ("Library unavailable.", "library unavailable"))
+
+
+def _capped_warnings(stderr, cap=1000):
+    """The reference binary's STDERR under -w -1 as brc-readcount prints it (DESIGN.md §8): the first `cap` warning lines of
+    each type, then for every type that had more a line with its total."""
+    counts = [0] * len(_WARNING_TYPES)
+    out = []
+    for ln in stderr.splitlines(keepends=True):
+        t = next((k for k, (msg, _) in enumerate(_WARNING_TYPES) if ln.startswith("WARNING: In read ") and msg in ln), None)
+        if t is not None:
+            counts[t] += 1
+            if counts[t] > cap:
+                continue
+        out.append(ln)
+    out += [f"WARNING: {name}: {n} events in total (only the first {cap} are listed)\n" for (_, name), n in zip(_WARNING_TYPES, counts) if n > cap]
+    return "".join(out)
 
 
 @pytest.mark.gpu
-def test_cli_parallel_window_decode_text_and_warnings_equal_sequential(tmp_path):
-    """The parallel window path (one borrowed, page-locked batch per window, next window decoded ahead) against the record-by-record
-    path: STDOUT and the per-read warning lines on STDERR must be identical, also when a window boundary falls inside the region."""
-    from oracle.oracle import REF_SAMTOOLS
-    if not os.path.exists(REF_SAMTOOLS):
-        pytest.skip("oracle/_ref/samtools not built")
-    from bam_readcount_b200 import synth
+def test_cli_parallel_window_decode_text_and_warnings_match_the_reference_binary(tmp_path):
+    """The parallel window path (one borrowed, page-locked batch per window, next window decoded ahead) against the unmodified
+    reference binary: STDOUT and the per-read warning lines on STDERR must be identical, also when a window boundary falls inside
+    the region.  Without -w the reference prints every warning event; brc-readcount prints the first 1000 per type and the total."""
+    from oracle.oracle import REF_BIN, REF_SAMTOOLS, have_reference_binary
+    if not have_reference_binary() or not os.path.exists(REF_SAMTOOLS):
+        pytest.skip("oracle/_ref not built")
     from bam_readcount_b200.batch import TAG_ABSENT
     exe = _cli()
     case = cases.synthetic_case(L=300000, depth=12, seed=97, regions=((0, 1, 300000),), site_list=False)
@@ -496,22 +525,26 @@ def test_cli_parallel_window_decode_text_and_warnings_equal_sequential(tmp_path)
     d = str(tmp_path)
     _make_bam(case, d)
     for args in (["-w", "0", "-i"], ["-p", "-q", "20", "-b", "20"], ["-w", "7", "-p"]):
-        outs = []
-        for extra in ({"BRC_CLI_SEQUENTIAL": "1"}, {}, {"BRC_CLI_DECODE_THREADS": "3", "BRC_CLI_WINDOW": "280000"}):
-            p = subprocess.run([exe] + args + ["-f", os.path.join(d, "ref.fa"), os.path.join(d, "s.bam"), "chr1:1-300000", "chr1:1001-2000"],
-                               capture_output=True, env=dict(os.environ, **extra))
-            assert p.returncode == 0, p.stderr.decode()[-2000:]
-            outs.append((p.stdout, p.stderr))
-        assert outs[0][0] == outs[1][0] == outs[2][0] and outs[0][0].count(b"\n") > 299000
-        assert outs[0][1] == outs[1][1] == outs[2][1]
+        argv = args + ["-f", os.path.join(d, "ref.fa"), os.path.join(d, "s.bam"), "chr1:1-300000", "chr1:1001-2000"]
+        r = subprocess.run([REF_BIN] + argv, capture_output=True)
+        assert r.returncode == 0, r.stderr.decode()[-2000:]
+        want_err = r.stderr.decode("latin-1")
+        if "-w" not in args:                                       # the default, -w -1
+            want_err = _capped_warnings(want_err)
+        assert r.stdout.count(b"\n") > 299000
         if args[1] != "0":
-            assert b"WARNING: In read" in outs[0][1]
+            assert "WARNING: In read" in want_err
+        for extra in ({}, {"BRC_CLI_DECODE_THREADS": "3", "BRC_CLI_WINDOW": "280000"}):
+            p = subprocess.run([exe] + argv, capture_output=True, env=dict(os.environ, **extra))
+            assert p.returncode == 0, p.stderr.decode()[-2000:]
+            assert p.stdout == r.stdout, (args, extra)
+            assert p.stderr.decode("latin-1") == want_err, (args, extra)
 
 
 def test_cli_parallel_window_decode_two_contigs_unmapped_and_edges(tmp_path):
     """CPU: the parallel window decode on a two-contig BAM with placed-but-unmapped records, a fetch that starts inside a read,
     a fetch past the last read, a site-list line long enough to be cut into windows, and a contig without reads behind it:
-    per-region (count, position sum, quality sum) identical to the sequential reader and to the Python decoder's samfetch."""
+    per-region (count, position sum, quality sum) identical to the Python decoder's samfetch, uncut and cut into windows."""
     from oracle.oracle import REF_SAMTOOLS
     if not os.path.exists(REF_SAMTOOLS):
         pytest.skip("oracle/_ref/samtools not built")
@@ -535,21 +568,18 @@ def test_cli_parallel_window_decode_two_contigs_unmapped_and_edges(tmp_path):
     sl = tmp_path / "sites"
     sl.write_text("".join(f"{c}\t{s}\t{e}\n" for c, s, e in lines))
     outs = []
-    for extra in ({"BRC_CLI_SEQUENTIAL": "1"}, {}, {"BRC_CLI_DECODE_THREADS": "5", "BRC_CLI_WINDOW": "270000"}, {"BRC_CLI_SEQUENTIAL": "1", "BRC_CLI_WINDOW": "270000"}):
+    for extra in ({}, {"BRC_CLI_DECODE_THREADS": "5", "BRC_CLI_WINDOW": "270000"}):
         p = subprocess.run([exe, "-l", str(sl), os.path.join(d, "s.bam")], capture_output=True, env=dict(os.environ, BRC_CLI_DECODE_ONLY="1", BRC_CLI_TIMING="1", **extra))
         assert p.returncode == 0, p.stderr.decode()[-1500:]
         outs.append((p.stdout.decode(), p.stderr.decode()))
-    assert outs[0][0] == outs[1][0] and outs[2][0] == outs[3][0]
-    assert "(+ 0 records in 0 windows" not in outs[1][1] and "(+ 0 records in 0 windows" not in outs[2][1]
+        assert "(+ 0 records in 0 windows" not in outs[-1][1]
     got = [tuple(int(x) for x in ln.split("\t")) for ln in outs[0][0].strip().splitlines()]
     assert len(got) == len(lines)
-    qo = both.qual_off.astype(np.int64)
-    mapped = (both.flag & 4) == 0
     for (c, s, e), g in zip(lines, got):
         tid = {"chrA": 0, "chrB": 1, "chrC": 2}[c]
-        idx = [i for i in both.fetch(tid, max(s - 2, 0), e) if mapped[i]]
-        want = (tid, s - 1, e, len(idx), int(both.pos[idx].astype(np.int64).sum()) if idx else 0, int(sum(int(both.qual[qo[i]:qo[i + 1]].astype(np.int64).sum()) for i in idx)))
-        assert g == want, (c, s, e, g, want)
-    # the cut form prints one line per window: their sums are the uncut line's
-    cut = [tuple(int(x) for x in ln.split("\t")) for ln in outs[2][0].strip().splitlines()]
+        assert g == (tid, s - 1, e) + _samfetch_sums(both, tid, s - 1, e), (c, s, e, g)
+    # the cut form prints one line per window, each with the records of its own fetch
+    cut = [tuple(int(x) for x in ln.split("\t")) for ln in outs[1][0].strip().splitlines()]
     assert len(cut) > len(lines)
+    for g in cut:
+        assert g[3:] == _samfetch_sums(both, *g[:3]), g

@@ -22,8 +22,6 @@ run() { name=$1; shift
   done
 }
 run par X=1
-run seq BRC_CLI_SEQUENTIAL=1
 run par_w4m BRC_CLI_WINDOW=4000000
 run par_w2m BRC_CLI_WINDOW=2000000
 s=$(date +%s.%N); bam_readcount_b200/brc-readcount -w 0 -i -f /tmp/brc_txt/ref.fa /tmp/brc_txt/s.bam chr1:1-$N 2>/dev/null | md5sum; e=$(date +%s.%N); echo "par to md5sum: $(python -c "print('%.3f' % ($e - $s))") s"
-BRC_CLI_SEQUENTIAL=1 bam_readcount_b200/brc-readcount -w 0 -i -f /tmp/brc_txt/ref.fa /tmp/brc_txt/s.bam chr1:1-$N 2>/dev/null | md5sum

@@ -1,5 +1,5 @@
-"""Site-list mode (-l) wall-clock: brc-readcount (merged fetch, and the per-line seek path) vs the reference binary on
-the same synthetic BAM and the same list of single-base sites.  usage: sitelist_bench.py [contig_len] [site_step] [ref_sites]"""
+"""Site-list mode (-l) wall-clock: brc-readcount vs the reference binary on the same synthetic BAM and the same list of
+single-base sites.  usage: sitelist_bench.py [contig_len] [site_step] [ref_sites]"""
 import os, subprocess, sys, tempfile, time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -20,18 +20,15 @@ with open(d + "/sites_ref", "w") as fh:
     fh.write("".join(f"chr1\t{p}\t{p}\n" for p in sites[:ref_sites]))
 print(f"BAM: {b.n_reads} reads; {len(sites)} sites every {step} bp")
 exe = build.build_cli()
-outs = {}
-for tag, extra in (("merged fetch", {}), ("per-line seek", {"BRC_CLI_NO_MERGE": "1"})):
-    t0 = time.time()
-    with open(d + f"/out_{len(outs)}.txt", "wb") as fh:
-        p = subprocess.run([exe, "-w", "0", "-q", "20", "-b", "20", "-f", d + "/ref.fa", "-l", d + "/sites", d + "/s.bam"], stdout=fh, stderr=subprocess.PIPE,
-                           env=dict(os.environ, BRC_CLI_TIMING="1", **extra))
-    dt = time.time() - t0
-    outs[tag] = open(d + f"/out_{len(outs)}.txt", "rb").read()
-    print(f"brc-readcount ({tag}): {dt:.2f}s  {len(sites)/dt:.3e} sites/s rc={p.returncode}\n   " + "\n   ".join(p.stderr.decode().strip().splitlines()[-2:]))
-print("merged == per-line:", outs["merged fetch"] == outs["per-line seek"])
+t0 = time.time()
+with open(d + "/out.txt", "wb") as fh:
+    p = subprocess.run([exe, "-w", "0", "-q", "20", "-b", "20", "-f", d + "/ref.fa", "-l", d + "/sites", d + "/s.bam"], stdout=fh, stderr=subprocess.PIPE,
+                       env=dict(os.environ, BRC_CLI_TIMING="1"))
+dt = time.time() - t0
+out = open(d + "/out.txt", "rb").read()
+print(f"brc-readcount: {dt:.2f}s  {len(sites)/dt:.3e} sites/s rc={p.returncode}\n   " + "\n   ".join(p.stderr.decode().strip().splitlines()[-2:]))
 t0 = time.time()
 r = subprocess.run([REF_BIN, "-w", "0", "-q", "20", "-b", "20", "-f", d + "/ref.fa", "-l", d + "/sites_ref", d + "/s.bam"], stdout=subprocess.PIPE, stderr=subprocess.DEVNULL)
 dt = time.time() - t0
 print(f"reference binary on the first {ref_sites} sites: {dt:.2f}s  {ref_sites/dt:.3e} sites/s")
-print("byte-identical on those sites:", outs["merged fetch"].startswith(r.stdout))
+print("byte-identical on those sites:", out.startswith(r.stdout))
