@@ -9,9 +9,10 @@ the UNMODIFIED reference binary oracle/_ref/bam-readcount (oracle/build_ref.sh).
   ref_<case>_<flags>.txt.gz        reference-binary STDOUT on the deterministic synthetic cases
                                    of tests/cases.py (deletions, insertions, -q/-b, -i, -p, -d)
   edge_*.txt.gz                    reference-binary STDOUT on the hand-built edge-case reads
-  fresh_fuzz_sha256.json, boundary_sha256.json
-                                   SHA-256 of the reference binary's STDOUT on the fuzz seeds of test_differential_fuzz.py and
-                                   on the capacity-boundary cases of boundary_cases.py (--boundary-only: only the latter)
+  fresh_fuzz_sha256.json, boundary_sha256.json, pipeline_sha256.json
+                                   SHA-256 of the reference binary's STDOUT on the fuzz seeds of test_differential_fuzz.py, on
+                                   the capacity-boundary cases of boundary_cases.py (--boundary-only: only these) and on the
+                                   chunk-cut, deep-site and pool-offset cases of pipeline_cases.py (--pipeline-only: only these)
   decode_sha256.json               SHA-256 of the reference binary's STDOUT and STDERR on the crafted BAMs of bam_craft.py
                                    (--decode-only: only this)
 """
@@ -112,6 +113,12 @@ def boundary_jobs():
     return boundary_cases.jobs()
 
 
+def pipeline_jobs():
+    """The cases of tests/pipeline_cases.py (pipelined push path, pools past 2^32 bytes)."""
+    import pipeline_cases
+    return pipeline_cases.jobs()
+
+
 def write_sha_file(jobs, out):
     sums, dirs = {}, {}
     for case, fname, fl, sl, key in jobs:
@@ -148,6 +155,9 @@ def main():
         return
     if "--boundary-only" in sys.argv:
         write_sha_file(boundary_jobs(), "boundary_sha256.json")
+        return
+    if "--pipeline-only" in sys.argv:
+        write_sha_file(pipeline_jobs(), "pipeline_sha256.json")
         return
     for f in ("expected_all_lib", "expected_per_lib", "expected_insertion_centric_all_lib",
               "expected_insertion_centric_per_lib"):
@@ -188,6 +198,7 @@ def main():
     # the fuzz seeds and the boundary cases: only the SHA-256 of the reference's STDOUT is kept
     write_sha_file(fresh_fuzz_jobs(), "fresh_fuzz_sha256.json")
     write_sha_file(boundary_jobs(), "boundary_sha256.json")
+    write_sha_file(pipeline_jobs(), "pipeline_sha256.json")
     write_decode_sha()
 
 
