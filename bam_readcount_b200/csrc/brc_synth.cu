@@ -149,34 +149,116 @@ HD Slot deep_slot(const brc_synth_spec &S, int64_t site_lo, int64_t idx, int64_t
 // ------------------------------------------------------------------------------------------------
 struct DevArgs { brc_synth_spec S; int32_t contig; int64_t blk_lo, n_reads; brc_synth_out O; unsigned long long *blk_cig; };
 
-__device__ void bitonic256(uint32_t *k, int t) {
+static_assert(RL % 2 == 0 && RL % 8 != 0 && BR == 256, "the fill writes whole quality groups and bytes of two bases");
+constexpr int NG = (RL + 7) / 8;   // quality groups of 8 per read: one sub_stream word each, the fill's unit of work
+constexpr int NWIN = 48;           // reference words staged per CTA: a WGS block's reads touch at most 45 (1280 + 152 bp)
+
+// ascending sort of 256 unique keys, one per thread (key of thread t on return = rank t).  Strides below 32 exchange by
+// shuffle; the six larger ones go through `xs` (256 words).
+__device__ uint32_t bitonic256(uint32_t key, uint32_t *xs, int t) {
     for (int size = 2; size <= BR; size <<= 1)
         for (int stride = size >> 1; stride > 0; stride >>= 1) {
-            __syncthreads();
-            const int p = t ^ stride;
-            if (p > t) {
-                const uint32_t a = k[t], b = k[p];
-                const bool up = (t & size) == 0;
-                if ((a > b) == up) { k[t] = b; k[p] = a; }
-            }
+            uint32_t other;
+            if (stride >= 32) { __syncthreads(); xs[t] = key; __syncthreads(); other = xs[t ^ stride]; }
+            else other = __shfl_xor_sync(0xffffffffu, key, stride);
+            key = (((t & stride) == 0) == ((t & size) == 0)) ? min(key, other) : max(key, other);
         }
-    __syncthreads();
+    return key;
 }
 
-__device__ Slot dev_slot(const DevArgs &A, uint32_t *keys, int t) {
-    const int64_t b = blockIdx.x;
-    if (A.S.mode == BRC_SYNTH_DEEP) return deep_slot(A.S, A.blk_lo, b * BR + t, A.n_reads);
-    const int64_t block = A.blk_lo + b;
-    {
-        const Hdr h = make_hdr(A.S.seed, (uint64_t)A.contig, (uint64_t)block, (uint64_t)t);
-        keys[t] = ((uint32_t)(wgs_start(A.S, block, h.off) - block * BBP + BRC_SYNTH_MAX_SPAN) << 8) | (uint32_t)t;   // (start, j): unique
+// exclusive prefix sum over the CTA (256 threads); `ws` holds 8 warp totals
+__device__ uint32_t cta_exclusive_scan(uint32_t v, uint32_t *ws, int t) {
+    uint32_t x = v;
+    for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xffffffffu, x, o); if ((t & 31) >= o) x += y; }
+    if ((t & 31) == 31) ws[t >> 5] = x;
+    __syncthreads();
+    for (int w = 0; w < (t >> 5); ++w) x += ws[w];
+    return x - v;
+}
+
+// the substitutions make_body applies, as a list: entry k (bits 10k..10k+9) = position | shift << 8, the count in bits 60..63.
+// Same draw and the same rule: distinct positions, first occurrence wins, and a position is remembered before the check that it
+// came from the reference.  Returns NM.
+__device__ int32_t sub_list(const Hdr &h, uint64_t &list) {
+    int32_t nm = h.kind == 1 ? 2 : (h.kind == 2 ? 3 : 0);
+    uint64_t l = 0; int n = 0;
+    if (h.n_subs > 0) {
+        const uint64_t h2 = sub_stream(h.rk, 2), h3 = sub_stream(h.rk, 3);
+        uint64_t seen = ~0ull;
+        for (int t = 0; t < 6; ++t) {
+            if (t >= h.n_subs) break;
+            const uint64_t src = t < 3 ? h2 >> (20 * t) : h3 >> (20 * (t - 3));
+            const uint32_t p = (uint32_t)(src & 0xFFFFu) % (uint32_t)RL;
+            const uint32_t sft = 1u + ((uint32_t)((src >> 16) & 0xFu) % 3u);
+            bool dup = false;
+            for (int k = 0; k < 6; ++k) dup = dup || ((uint32_t)(seen >> (8 * k)) & 0xFFu) == p;
+            if (dup) continue;
+            seen = (seen << 8) | p;
+            if (ref_off(h.kind, (int)p) < 0) continue;
+            l |= (uint64_t)(p | (sft << 8)) << (10 * n);
+            ++n; ++nm;
+        }
     }
-    bitonic256(keys, t);
-    Slot s; s.valid = true; s.unit = (uint64_t)A.contig; s.blk = (uint64_t)block; s.j = keys[t] & 255u;
-    s.h = make_hdr(A.S.seed, s.unit, s.blk, s.j);
-    s.start = wgs_start(A.S, block, s.h.off);
-    s.lib = (int32_t)((block * BR + t) % A.S.n_libs); s.region = 0;
-    return s;
+    list = l | ((uint64_t)n << 60);
+    return nm;
+}
+
+// 4 quality bytes from 4 bytes b of a quality word: {37,37,37,30,25,12,2}[(b * 7) >> 8], two bytes per 16-bit lane, one byte permute
+__device__ __forceinline__ uint32_t qual4(uint32_t w) {
+    const uint32_t e = (((w & 0x00FF00FFu) * 7u) >> 8) & 0x00070007u, o = ((((w >> 8) & 0x00FF00FFu) * 7u) >> 8) & 0x00070007u;
+    return __byte_perm(0x1E252525u, 0x00020C19u, (e | (e >> 8) | (o << 4) | (o >> 4)) & 0x7777u);
+}
+
+// 4 packed sequence bytes from 8 base codes (2 bits each, base k at bits 2k): byte j = (1 << b[2j]) << 4 | 1 << b[2j+1]
+__device__ __forceinline__ uint32_t seq4(uint32_t c) {
+    uint32_t x = (c | (c << 8)) & 0x00FF00FFu;
+    x = (x | (x << 4)) & 0x0F0F0F0Fu;
+    x = (x | (x << 2)) & 0x33333333u;                       // base k in bits 4k, 4k+1
+    const uint32_t b0 = x & 0x11111111u, b1 = (x >> 1) & 0x11111111u;
+    const uint32_t nib = (~(b0 | b1) & 0x11111111u) | ((b0 & ~b1) << 1) | ((b1 & ~b0) << 2) | ((b0 & b1) << 3);
+    return ((nib & 0x0F0F0F0Fu) << 4) | ((nib >> 4) & 0x0F0F0F0Fu);
+}
+
+// quality group g (query positions 8g .. 8g+7) of a read: 8 quality bytes (little-endian) and 8 base codes (2 bits each), the
+// substitutions applied.  The values make_body computes, position for position.
+__device__ __forceinline__ void fill_group(const Hdr &h, int64_t start, uint64_t subs, int g, const uint64_t *win, int64_t w_lo,
+                                           uint64_t seed, uint64_t unit, uint64_t &qual8, uint32_t &codes) {
+    const int q0 = 8 * g;
+    const uint64_t hq = sub_stream(h.rk, 8 + (uint64_t)g);
+    uint64_t qv = (uint64_t)qual4((uint32_t)hq) | (uint64_t)qual4((uint32_t)(hq >> 32)) << 32;
+    const int tail_from = RL - h.tail - q0;              // bytes k >= tail_from are the Q2 tail
+    if (tail_from < 8) {
+        const uint64_t m = tail_from <= 0 ? ~0ull : ~0ull << (8 * tail_from);
+        qv = (qv & ~m) | (0x0202020202020202ull & m);
+    }
+    qual8 = qv;
+    // the group's reference bases lie within 11 bp from its first one (a 3 bp deletion at most): 32 bases from there
+    const int ro0 = max(ref_off(h.kind, q0), 0);
+    const int64_t p0 = start + ro0, w0 = p0 >> 5;
+    auto word = [&](int64_t w) { const int64_t k = w - w_lo; return (uint64_t)k < (uint64_t)NWIN ? win[k] : ref_word(seed, unit, (uint64_t)w); };
+    const int s = 2 * (int)(p0 & 31);
+    const uint64_t wa = word(w0);
+    const uint64_t bases = s ? (wa >> s) | (word(w0 + 1) << (64 - s)) : wa;
+    uint32_t c = (uint32_t)bases & 0xFFFFu;                // the group's bases are the 8 from its first one ...
+    const bool clipped = (h.kind == 1 && g == 8) || (h.kind == 3 && g <= 1);
+    if (clipped || (h.kind == 2 && g == 7)) {               // ... unless it holds an insertion, the clip or the deletion
+        const uint64_t hb = clipped ? sub_stream(h.rk, 4) : 0;
+        c = 0;
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+            const int q = q0 + k, ro = ref_off(h.kind, q);
+            const uint32_t b = ro >= 0 ? (uint32_t)(bases >> (2 * (ro - ro0))) & 3u : (uint32_t)(hb >> (2 * (q & 31))) & 3u;
+            c |= b << (2 * k);
+        }
+    }
+    for (int k = 0; k < (int)(subs >> 60); ++k) {
+        const uint32_t e = (uint32_t)(subs >> (10 * k)), p = e & 0xFFu;
+        if ((int)(p >> 3) != g) continue;
+        const int sh = 2 * (int)(p & 7u);
+        const uint32_t b = (c >> sh) & 3u;
+        c ^= (b ^ ((b + ((e >> 8) & 3u)) & 3u)) << sh;
+    }
+    codes = c;
 }
 
 __global__ void __launch_bounds__(BR) synth_count_kernel(DevArgs A) {
@@ -192,36 +274,70 @@ __global__ void __launch_bounds__(BR) synth_count_kernel(DevArgs A) {
 }
 
 __global__ void __launch_bounds__(1024) synth_scan_kernel(unsigned long long *v, int64_t n) {   // exclusive scan, one CTA; v[n] = total
-    __shared__ unsigned long long part[1024];
+    __shared__ unsigned long long ws[32];
     const int t = threadIdx.x;
     const int64_t per = (n + 1023) / 1024, lo = imin64(n, per * t), hi = imin64(n, lo + per);
     unsigned long long s = 0;
     for (int64_t i = lo; i < hi; ++i) s += v[i];
-    part[t] = s;
+    unsigned long long x = s;                            // CTA-inclusive scan of the 1024 partial sums
+    for (int o = 1; o < 32; o <<= 1) { const unsigned long long y = __shfl_up_sync(0xffffffffu, x, o); if ((t & 31) >= o) x += y; }
+    if ((t & 31) == 31) ws[t >> 5] = x;
     __syncthreads();
-    if (t == 0) { unsigned long long acc = 0; for (int i = 0; i < 1024; ++i) { const unsigned long long x = part[i]; part[i] = acc; acc += x; } v[n] = acc; }
+    if (t < 32) {
+        unsigned long long w = ws[t];
+        for (int o = 1; o < 32; o <<= 1) { const unsigned long long y = __shfl_up_sync(0xffffffffu, w, o); if (t >= o) w += y; }
+        ws[t] = w;
+    }
     __syncthreads();
-    unsigned long long acc = part[t];
-    for (int64_t i = lo; i < hi; ++i) { const unsigned long long x = v[i]; v[i] = acc; acc += x; }
+    unsigned long long acc = x - s + ((t >> 5) ? ws[(t >> 5) - 1] : 0ull);
+    if (t == 1023) v[n] = acc + s;
+    for (int64_t i = lo; i < hi; ++i) { const unsigned long long y = v[i]; v[i] = acc; acc += y; }
 }
 
+// One CTA = one block of 256 reads.  Each read's header is hashed once and kept in shared memory; its metadata and substitution
+// list are made by one thread, its bases and qualities by all: the CTA's 256 x 19 quality groups are spread over the 256 threads,
+// consecutive lanes on consecutive groups of a read, the reference bases taken from words staged once per CTA.  The rows are staged
+// in shared memory and leave with 16-byte stores.
 __global__ void __launch_bounds__(BR) synth_fill_kernel(DevArgs A) {
     extern __shared__ __align__(16) uint8_t smem[];
-    uint8_t *seq_s = smem, *qual_s = smem + BR * SB;                         // 19200 + 38400 bytes
-    uint32_t *keys = reinterpret_cast<uint32_t *>(smem + BR * (SB + RL));    // 256 keys, then reused for the cigar scan
+    uint8_t *seq_s = smem, *qual_s = smem + BR * SB;                                          // 19200 + 38400 bytes
+    Hdr *hs = reinterpret_cast<Hdr *>(smem + BR * (SB + RL));                                 // headers: by j, then by row
+    int64_t *start_s = reinterpret_cast<int64_t *>(hs + BR);
+    uint64_t *subs_s = reinterpret_cast<uint64_t *>(start_s + BR);
+    uint64_t *win = subs_s + BR;                                                              // NWIN reference words from w_lo
+    uint32_t *xs = reinterpret_cast<uint32_t *>(win + NWIN);                                  // sort exchange / scan totals
+    __shared__ int64_t w_lo_s;
     const int t = threadIdx.x;
     const int64_t b = blockIdx.x, i = b * BR + t;
-    const Slot s = dev_slot(A, keys, t);
-    __syncthreads();
+    const bool deep = A.S.mode == BRC_SYNTH_DEEP;
+    const uint64_t seed = A.S.seed, unit = deep ? 0 : (uint64_t)A.contig;
+    const int64_t block = A.blk_lo + b;
+    Slot s;
+    if (deep) {
+        s = deep_slot(A.S, A.blk_lo, i, A.n_reads);
+        if (t == 0) w_lo_s = s.start >> 5;                            // the CTA's first read starts leftmost
+        __syncthreads();
+    } else {
+        if (t < NWIN) win[t] = ref_word(seed, unit, (uint64_t)((block * BBP >> 5) + t));   // every start is >= block * BBP
+        const Hdr h = make_hdr(seed, unit, (uint64_t)block, (uint64_t)t);
+        hs[t] = h;
+        const uint32_t key = bitonic256(((uint32_t)(wgs_start(A.S, block, h.off) - block * BBP + BRC_SYNTH_MAX_SPAN) << 8) | (uint32_t)t, xs, t);
+        __syncthreads();
+        s.valid = true; s.unit = unit; s.blk = (uint64_t)block; s.j = key & 255u;     // (start, j): unique, so any sort gives this order
+        s.h = hs[s.j];
+        s.start = wgs_start(A.S, block, s.h.off);
+        s.lib = (int32_t)((block * BR + t) % A.S.n_libs); s.region = 0;
+    }
+    const int64_t w_lo = deep ? w_lo_s : block * BBP >> 5;
+    if (deep && t < NWIN) win[t] = ref_word(seed, unit, (uint64_t)(w_lo + t));
     // block-exclusive scan of the CIGAR op counts
     const int nc = s.valid ? n_cigar_of(s.h.kind) : 0;
-    keys[t] = (uint32_t)nc;
-    __syncthreads();
-    for (int o = 1; o < BR; o <<= 1) { const uint32_t v = t >= o ? keys[t - o] : 0u; __syncthreads(); keys[t] += v; __syncthreads(); }
-    const unsigned long long coff = A.blk_cig[b] + keys[t] - (uint32_t)nc;
+    const unsigned long long coff = A.blk_cig[b] + cta_exclusive_scan((uint32_t)nc, xs, t);   // its barrier: every header read by j
     const brc_synth_out &O = A.O;
     if (s.valid) {
-        const int32_t nm = make_body(A.S.seed, s.unit, s.h, s.start, seq_s + t * SB, qual_s + t * RL);
+        uint64_t subs;
+        const int32_t nm = sub_list(s.h, subs);
+        hs[t] = s.h; start_s[t] = s.start; subs_s[t] = subs;
         if (O.tid) O.tid[i] = A.contig;
         O.pos[i] = (int32_t)s.start; O.flag[i] = (uint16_t)(s.h.reverse ? 16 : 0); O.mapq[i] = (uint8_t)s.h.mapq; O.lib[i] = (uint16_t)s.lib;
         O.l_qseq[i] = RL; O.nm[i] = nm; O.sm[i] = TAG_ABSENT;
@@ -232,8 +348,24 @@ __global__ void __launch_bounds__(BR) synth_fill_kernel(DevArgs A) {
         if (i == A.n_reads - 1) { O.cigar_off[i + 1] = coff + nc; O.seq_off[i + 1] = (uint64_t)(i + 1) * SB; O.qual_off[i + 1] = (uint64_t)(i + 1) * RL; }
     }
     __syncthreads();
+    // bases and qualities: item it = quality group g of row r
+    const int rows = (int)imin64(BR, A.n_reads - b * BR);
+#pragma unroll 2
+    for (int it = t; it < rows * NG; it += BR) {
+        const int r = it / NG, g = it - r * NG;
+        uint64_t qv; uint32_t codes;
+        fill_group(hs[r], start_s[r], subs_s[r], g, win, w_lo, seed, unit, qv, codes);
+        const int nq = g == NG - 1 ? RL - 8 * (NG - 1) : 8;
+        uint16_t *qd = reinterpret_cast<uint16_t *>(qual_s + r * RL + 8 * g);                  // rows and groups start at even bytes
+        uint8_t *sd = seq_s + r * SB + 4 * g;
+        const uint32_t sq = seq4(codes);
+        for (int k = 0; k < nq / 2; ++k) {
+            qd[k] = (uint16_t)(qv >> (16 * k));
+            sd[k] = (uint8_t)(sq >> (8 * k));
+        }
+    }
+    __syncthreads();
     // coalesced copy of the staged rows (the CTA's rows are contiguous in the pools; 256 rows start 16-byte aligned)
-    const int64_t rows = imin64(BR, A.n_reads - b * BR);
     {
         const int64_t nb = rows * SB; uint8_t *dst = O.seq + b * BR * SB;
         for (int64_t k = t; k < nb / 16; k += BR) reinterpret_cast<int4 *>(dst)[k] = reinterpret_cast<const int4 *>(seq_s)[k];
@@ -395,7 +527,7 @@ int brc_synth_fill_device(const brc_synth_spec *S, int32_t contig, int64_t lo, i
     if (O->n_reads != n) return BRC_E_INVALID;
     if (n == 0) return BRC_OK;
     const int64_t nblk = (n + BR - 1) / BR;
-    const int smem = BR * (SB + RL) + BR * 4;
+    const int smem = BR * (SB + RL) + BR * (int)(sizeof(Hdr) + 2 * sizeof(uint64_t)) + NWIN * (int)sizeof(uint64_t) + BR * 4;
     if (cudaFuncSetAttribute(synth_fill_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) return BRC_E_CUDA;
     DevArgs A; A.S = *S; A.contig = contig; A.blk_lo = lo; A.n_reads = n; A.O = *O; A.blk_cig = reinterpret_cast<unsigned long long *>(scratch_dev);
     cudaStream_t s = (cudaStream_t)stream;
