@@ -35,7 +35,7 @@ constexpr int FASTDIV_MAX = 2048;
 struct __align__(16) ReadDesc {
     // q0
     int32_t pos;        // leftmost reference position
-    int32_t end;        // bam_endpos (== pos for reads the pileup buffer never admits)
+    int32_t end;        // bam_endpos clamped to INT32_MAX (== pos for reads the pileup buffer never admits)
     uint32_t fm;        // flag | mapq<<16 | FM_* bits
     uint32_t lib_nc;    // lib[0:16) | min(n_cigar,0xFFFF)<<16
     // q1 : four of the five values of fetch_func (R:bamreadcount.cpp:248-253)
@@ -51,7 +51,7 @@ struct __align__(16) ReadDesc {
     // q3
     uint32_t qual32;    // low 32 bits of the read's byte offset in the qual pool
     uint32_t seq32;     // low 32 bits of the read's byte offset in the seq pool
-    uint32_t cig;       // SIMPLE: qoff (qpos = site - pos + qoff); else index of the first CIGAR op
+    uint32_t cig;       // SIMPLE: qoff (qpos = site - pos + qoff); else low 32 bits of the index of the first CIGAR op
     uint32_t n_cigar;
     // q4
     float rcp_l;        // RN(1 / (float)l_qseq)         (FM_FASTDIV only)

@@ -403,7 +403,9 @@ __global__ void __launch_bounds__(K0_READS) read_precompute_kernel(PrecomputePar
     if (unmapped) end = pos;      // never admitted to the pileup: covers nothing
 
     ReadDesc d;
-    d.pos = pos; d.end = (int32_t)end; d.fl = (float)l_qseq;
+    // a read overhanging a contig of length close to 2^31 - 1 ends past INT32_MAX: every site is below it, so the clamp keeps
+    // site < end exact
+    d.pos = pos; d.end = (int32_t)min(end, (int64_t)INT32_MAX); d.fl = (float)l_qseq;
     uint32_t fm = (flag & 0xFFFFu) | (mapq << 16);
     if (simple) fm |= FM_SIMPLE;
     const int32_t sm = smtag;
@@ -839,6 +841,9 @@ __device__ __forceinline__ void process_chunk(const PileupParams &P, const Stage
     const uint32_t qual_s = smem_u32(sb.qual) - ci.qbase32;   // staged bytes are addressed with the reads' low-32 pool offsets
     const uint32_t seq_s = smem_u32(sb.seq) - ci.sbase32;
     const int32_t wfirst = S.wfirst;
+    // last position of the warp's window, kept below the sentinel's INT_MAX: on a contig of length close to 2^31 - 1 the window
+    // [wfirst, wfirst + 31] can reach past it, and a read starts at most at 2^31 - 2
+    const int32_t wlast = min(wfirst, 0x7fffffff - 32) + 31;
     {   // vectorised skip of the leading reads that end before this warp's first site (32 reads per ballot):
         // keeps the 8 warps of a tile in step — the last warp would otherwise walk ~45 dead reads one by one
         const int n_in = ci.r1 - ci.r0, lane = tid & 31;
@@ -859,14 +864,14 @@ __device__ __forceinline__ void process_chunk(const PileupParams &P, const Stage
         const int2 fl2 = lds64(da + 8u);                          // fm, lib_nc
         // the next read's: when `pe` is the sentinel this is the spare record behind it in desc[], loaded and never used
         const int2 pe_b = lds64(da + DSZ), fl_b = lds64(da + DSZ + 8u);
-        if (pe.x - wfirst > 31) { if (pe.x != 0x7fffffff) S.warp_done = true; break; }   // reads are position-sorted within a region; INT_MAX = end of chunk
+        if (pe.x > wlast) { if (pe.x != 0x7fffffff) S.warp_done = true; break; }   // reads are position-sorted within a region; INT_MAX = end of chunk
         if (STAGED) {
             // Two FM_HOT reads (A = this one, B = the next) in one predicated body; the test is uniform across the warp.  -p: a
             // read without a library (which stops the site's accumulation) is never part of a pair.  B is never the sentinel.
             bool pair = ((uint32_t)fl2.x & (uint32_t)fl_b.x & FM_HOT) != 0u;
             if (PER_LIB) pair = pair && ((uint32_t)fl2.y & 0xFFFFu) != LIB_NONE && ((uint32_t)fl_b.y & 0xFFFFu) != LIB_NONE;
             if (pair) {
-                const bool b_in = pe_b.x - wfirst <= 31;          // B beyond the warp's window: it covers no lane and ends the walk
+                const bool b_in = pe_b.x <= wlast;                // B beyond the warp's window: it covers no lane and ends the walk
                 hot_pair<PER_LIB>(P, sacc, ci, S, tid, da, desc_s, qual_s, seq_s, pe, (uint32_t)fl2.x, (uint32_t)fl2.y,
                                   b_in ? pe_b : make_int2(0x7fffffff, 0), (uint32_t)fl_b.x, (uint32_t)fl_b.y, pk3, pkmb);
                 if (!b_in) { S.warp_done = true; break; }
@@ -927,11 +932,14 @@ __device__ __forceinline__ void process_chunk(const PileupParams &P, const Stage
             // ---- general path ----
             if (fm & FM_SIMPLE) qpos = S.site - pe.x + q3.z;
             else {
-                // staged ops are indexed with the reads' pool op indices; their address derives from desc_s, which the loop
-                // keeps anyway (not from the ring slot's index, which would be reloaded from local memory)
-                const uint32_t *cig_base = (ci.flags & 16u)
-                    ? static_cast<const uint32_t *>(__cvta_shared_to_generic(desc_s + (uint32_t)offsetof(StageBuf, cigar))) - ci.cbase32 : P.cigar;
-                const int3 rr = resolve_general(cig_base + (uint32_t)q3.z, (uint32_t)q3.w, pe.x, S.site);
+                // staged ops: the read's op index relative to the chunk's first staged op, in 32 bits (exact: the staged window
+                // spans fewer than STAGE_CIGAR ops, also where it crosses a multiple of 2^32); the address derives from desc_s,
+                // which the loop keeps anyway (not from the ring slot's index, which would be reloaded from local memory).
+                // Unstaged: the full 64-bit op offset, as the unstaged quality loads do
+                const uint32_t *cig = (ci.flags & 16u)
+                    ? static_cast<const uint32_t *>(__cvta_shared_to_generic(desc_s + (uint32_t)offsetof(StageBuf, cigar) + 4u * ((uint32_t)q3.z - ci.cbase32)))
+                    : P.cigar + P.cigar_off[ci.r0 + (int)((da - desc_s) / DSZ)];
+                const int3 rr = resolve_general(cig, (uint32_t)q3.w, pe.x, S.site);
                 if (rr.z) continue;                              // is_del
                 qpos = rr.x; indel = rr.y;
             }
@@ -1372,7 +1380,7 @@ __global__ void __launch_bounds__(DEEP_THREADS, 2) deep_site_kernel(PileupParams
             const int32_t site = ti.pos0 + sg;
             if (fm & FM_SIMPLE) eq[sg] = site - d.pos + (int)d.cig;
             else {
-                const int3 rr = resolve_general(P.cigar + d.cig, d.n_cigar, d.pos, site);
+                const int3 rr = resolve_general(P.cigar + P.cigar_off[r], d.n_cigar, d.pos, site);   // d.cig: low 32 bits only
                 if (rr.z) continue;
                 eq[sg] = rr.x; ei[sg] = rr.y;
             }

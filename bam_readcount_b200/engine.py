@@ -245,7 +245,8 @@ class Results:
                         al += NT[_CANON[(b & 15) if (i & 1) else (b >> 4)]]
                 else:
                     wb, seq = refs[tid]
-                    al = "-" + seq[pos + 1 - wb: pos + 1 - wb + ln].decode("latin-1")
+                    # positions outside the window (past the contig end) print as N, as the emitter does
+                    al = "-" + "".join(chr(seq[p - wb]) if 0 <= p - wb < len(seq) else "N" for p in range(pos + 1, pos + 1 + ln))
                 indels.append((al.encode("latin-1"), al, st))
             j = int(self.sec_next[j])
         indels.sort(key=lambda x: x[0])

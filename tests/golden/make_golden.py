@@ -9,10 +9,11 @@ the UNMODIFIED reference binary oracle/_ref/bam-readcount (oracle/build_ref.sh).
   ref_<case>_<flags>.txt.gz        reference-binary STDOUT on the deterministic synthetic cases
                                    of tests/cases.py (deletions, insertions, -q/-b, -i, -p, -d)
   edge_*.txt.gz                    reference-binary STDOUT on the hand-built edge-case reads
-  fresh_fuzz_sha256.json, boundary_sha256.json, pipeline_sha256.json
+  fresh_fuzz_sha256.json, boundary_sha256.json, pipeline_sha256.json, edge32_sha256.json
                                    SHA-256 of the reference binary's STDOUT on the fuzz seeds of test_differential_fuzz.py, on
-                                   the capacity-boundary cases of boundary_cases.py (--boundary-only: only these) and on the
+                                   the capacity-boundary cases of boundary_cases.py (--boundary-only: only these), on the
                                    chunk-cut, deep-site and pool-offset cases of pipeline_cases.py (--pipeline-only: only these)
+                                   and on the contigs of length close to 2^31 of edge32_cases.py (--edge32-only: only these)
   decode_sha256.json               SHA-256 of the reference binary's STDOUT and STDERR on the crafted BAMs of bam_craft.py
                                    (--decode-only: only this)
 """
@@ -55,14 +56,35 @@ def decode_fixture(bam, out):
 
 def write_case_files(case, d):
     name, L, seq, wb = case["contigs"][0]
-    if wb:      # the engine and the oracle get a window of the contig; the reference binary reads all of it
-        seq = case["full_ref"]
-    synth.write_fasta(os.path.join(d, "ref.fa"), name, np.frombuffer(seq, dtype=np.uint8))
+    if wb and "full_ref" in case:       # the engine and the oracle get a window of the contig; the reference binary reads all of it
+        synth.write_fasta(os.path.join(d, "ref.fa"), name, np.frombuffer(case["full_ref"], dtype=np.uint8))
+    elif wb:                            # a contig too long to hold (edge32_cases): N up to the window, then the window's bases
+        _write_window_fasta(os.path.join(d, "ref.fa"), name, L, wb, seq)
+    else:
+        synth.write_fasta(os.path.join(d, "ref.fa"), name, np.frombuffer(seq, dtype=np.uint8))
     synth.write_sam(os.path.join(d, "s.sam"), case["batch"], [(name, L)], n_libs=len(case["lib_names"]),
                     read_group=case.get("read_group", True))
     _missing_qual_as_star(os.path.join(d, "s.sam"))
     subprocess.check_call([REF_SAMTOOLS, "view", "-b", "-o", os.path.join(d, "s.bam"), os.path.join(d, "s.sam")])
-    subprocess.check_call([REF_SAMTOOLS, "index", os.path.join(d, "s.bam")])
+    # BAI addresses positions below 2^29 only: a longer contig takes a CSI index, which sam_index_load3 finds as well
+    subprocess.check_call([REF_SAMTOOLS, "index"] + (["-c"] if L > 1 << 29 else []) + [os.path.join(d, "s.bam")])
+
+
+def _write_window_fasta(path, name, L, wb, win, width=60):
+    """FASTA of a contig of length L that is N except for `win` at [wb, L), written a block of lines at a time."""
+    block = 1 << 16
+    n_line = (b"N" * width + b"\n") * block
+    with open(path, "wb") as fh:
+        fh.write(f">{name}\n".encode())
+        p = 0
+        head = (wb // width) * width                    # lines wholly before the window
+        while p + width * block <= head:
+            fh.write(n_line)
+            p += width * block
+        fh.write((b"N" * width + b"\n") * ((head - p) // width))
+        tail = b"N" * (wb - head) + bytes(win)
+        assert head + len(tail) == L
+        fh.write(b"".join(tail[i:i + width] + b"\n" for i in range(0, len(tail), width)))
 
 
 def _missing_qual_as_star(path):
@@ -119,6 +141,12 @@ def pipeline_jobs():
     return pipeline_cases.jobs()
 
 
+def edge32_jobs():
+    """The contigs of length close to 2^31 of tests/edge32_cases.py."""
+    import edge32_cases
+    return edge32_cases.jobs()
+
+
 def write_sha_file(jobs, out):
     sums, dirs = {}, {}
     for case, fname, fl, sl, key in jobs:
@@ -158,6 +186,9 @@ def main():
         return
     if "--pipeline-only" in sys.argv:
         write_sha_file(pipeline_jobs(), "pipeline_sha256.json")
+        return
+    if "--edge32-only" in sys.argv:
+        write_sha_file(edge32_jobs(), "edge32_sha256.json")
         return
     for f in ("expected_all_lib", "expected_per_lib", "expected_insertion_centric_all_lib",
               "expected_insertion_centric_per_lib"):
@@ -199,6 +230,7 @@ def main():
     write_sha_file(fresh_fuzz_jobs(), "fresh_fuzz_sha256.json")
     write_sha_file(boundary_jobs(), "boundary_sha256.json")
     write_sha_file(pipeline_jobs(), "pipeline_sha256.json")
+    write_sha_file(edge32_jobs(), "edge32_sha256.json")
     write_decode_sha()
 
 

@@ -17,7 +17,8 @@ GPU, each asserting that it reached its path
   test_multi_chunk_pool_overflow_falls_back  compute_pipelined overflows its pool and the plain path recomputes.
   test_multi_chunk_deep_site                 the deep-site kernel launched from the chunk loop.
   test_multi_chunk_carried_queue             brc_set_queue_carry, one brc_compute per argv region, several chunks each.
-  test_starved_pileup_grid                   one CTA per SM (BRC_K1_RESERVE_CTAS, in a fresh process) on more tiles than CTAs.
+  test_starved_pileup_grid                   one CTA per SM (BRC_K1_RESERVE_CTAS, in a fresh process) on more tiles than CTAs,
+                                             on the plain path and in every pileup launch of 2 and 3 chunks.
   test_device_pools_past_2_31_and_2_32       brc_run_device with quality or base pools whose offsets cross 2^31 / 2^32."""
 import functools
 import hashlib
@@ -294,20 +295,32 @@ def _starved_jobs():
     import boundary_cases
     big = selection_cases()[0]
     big = dict(big, regions=big["regions"][:1])               # one argv region of 300 000 sites
-    return [("300k_sites", big, dict(), False), ("pool_perlib", pool_case(), dict(per_lib=True), True),
-            ("chunk_geometry", boundary_cases.chunk_geometry(), dict(per_lib=True), True),
-            ("chunk_geometry_alllib", boundary_cases.chunk_geometry(), dict(), True)]
+    jobs = [("300k_sites", big, dict(), False, 0), ("pool_perlib", pool_case(), dict(per_lib=True), True, 0),
+            ("chunk_geometry", boundary_cases.chunk_geometry(), dict(per_lib=True), True, 0),
+            ("chunk_geometry_alllib", boundary_cases.chunk_geometry(), dict(), True, 0)]
+    # the chunked push path on the same starved grid: every pileup launch of these plans has several tiles per CTA
+    for n_chunks in (2, 3):
+        jobs += [(f"300k_sites_chunks{n_chunks}", big, dict(), False, n_chunks),
+                 (f"300k_sites_perlib_chunks{n_chunks}", big, dict(per_lib=True), False, n_chunks)]
+    return jobs
 
 
 def starved_child():
     """Runs in a fresh process with BRC_K1_RESERVE_CTAS set (launch_pileup reads it once per process): each job's dump, text and
-    warnings against the oracle; prints one JSON line."""
+    warnings against the oracle, and for the chunked jobs (BRC_PIPE_CHUNKS) the launch count; prints one JSON line."""
     out = {}
-    for name, case, flags, sl in _starved_jobs():
+    for name, case, flags, sl, n_chunks in _starved_jobs():
         otext, odump, owarn = cases.run_oracle(case, flags, site_list=sl)
-        etext, edump, ewarn, _ = cases.run_engine(case, flags, site_list=sl)
+        if n_chunks:
+            os.environ["BRC_PIPE_CHUNKS"] = str(n_chunks)
+            try:
+                etext, edump, ewarn, launches, _ = _engine(case, flags, sl)
+            finally:
+                del os.environ["BRC_PIPE_CHUNKS"]
+        else:
+            (etext, edump, ewarn, _), launches = cases.run_engine(case, flags, site_list=sl), 0
         out[name] = dict(dump=edump == odump, text=etext == otext, warn=[ewarn[0], ewarn[1], ewarn[3]] == list(owarn),
-                         diff="" if edump == odump else _first_diff(edump, odump))
+                         launches=launches, diff="" if edump == odump else _first_diff(edump, odump))
     print("STARVED " + json.dumps(out))
 
 
@@ -317,13 +330,20 @@ def test_starved_pileup_grid():
     many tiles from the dispenser and carries site_reset, its shared second-class cells, the stage ring's parity and its warning
     slots from one tile to the next (the 300 000-site region: 1172 tiles on 132 CTAs of an H100).  That region without -p, the
     random-base pool case and chunk_geometry (each fewer work items than SMs: one CTA per item under the same grid rule) equal
-    the oracle."""
+    the oracle.  The 300 000-site region also runs through the chunked push path at 2 and 3 chunks, with and without -p: every
+    pileup launch of those plans has more than two tiles per CTA, so each CTA takes several tiles inside one chunk's launch, and
+    the launch count is the plan's."""
     import torch
     sms = torch.cuda.get_device_properties(0).multi_processor_count
     reserve = 1 << 20
     grid = max(3 * sms - reserve, sms)                        # launch_pileup: max(SMs x BRC_K1_CTAS_PER_SM - reserve, SMs)
-    _, _, _, n_tiles = _geometry(_starved_jobs()[0][1], _starved_jobs()[0][1]["regions"][0])
+    big = _starved_jobs()[0][1]
+    _, _, _, n_tiles = _geometry(big, big["regions"][0])
     assert n_tiles > 8 * grid, (n_tiles, grid)               # 300 000 sites: every CTA takes at least eight tiles
+    plans = {n: _plan(big, n) for n in (2, 3)}
+    for n, plan in plans.items():
+        k1 = [t1 - t0 for _, _, t0, t1 in plan if t1 > t0]
+        assert len(k1) == n and min(k1) > 2 * grid, (n, k1, grid)
     env = dict(os.environ, BRC_K1_RESERVE_CTAS=str(reserve))
     cmd = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + [
         "-c", f"import sys; sys.path[:0] = [{ROOT!r}, {os.path.join(ROOT, 'tests')!r}]; import test_pipeline_scale as t; t.starved_child()"]
@@ -333,8 +353,11 @@ def test_starved_pileup_grid():
     assert line, p.stdout[-2000:]
     res = json.loads(line[-1][len("STARVED "):])
     assert set(res) == {j[0] for j in _starved_jobs()}
-    for name, r in res.items():
+    for name, case, flags, sl, n_chunks in _starved_jobs():
+        r = res[name]
         assert r["dump"] and r["text"] and r["warn"], (name, r)
+        if n_chunks:
+            assert r["launches"] == pc.pipe_launches(plans[n_chunks]), (name, r["launches"])
 
 
 # ---------------------------------------------------------------------------------------------------------------------------
