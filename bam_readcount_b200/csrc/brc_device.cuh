@@ -12,10 +12,12 @@
 #include <cstdint>
 #include <cuda_runtime.h>
 
+#include "../../include/brc_engine.h"
+
 namespace brc {
 
 constexpr int TILE = 256;            // sites per CTA of the pileup kernel (threads = sites)
-constexpr int N_STATS = 13;
+constexpr int N_STATS = BRC_N_STATS; // a 13-vector of statistics is indexed by the BRC_S_* names (print order)
 constexpr uint32_t LIB_NONE = 0xFFFFu;
 constexpr int KIND_INS = 6, KIND_DEL = 7;
 constexpr uint8_t NO_BASE = 255;
@@ -166,11 +168,11 @@ struct PileupParams {
     const int32_t *deep_tiles;
     int32_t n_deep;
     int32_t deep_min_reads;
-    // tile dispenser of THIS launch (ResultsDev::warn + WARN_WORDS + k, zeroed by init_tiles_kernel); nullptr = fixed stride
+    // tile dispenser of THIS launch (ResultsDev::warn + WARN_WORDS + k, zeroed by init_tiles_kernel)
     unsigned long long *work_counter;
 };
-constexpr int WARN_WORDS = 4;          // ResultsDev::warn: [0] SM missing, [1] NM missing, [2..3] spare
-constexpr int N_WORK_COUNTERS = 64;    // followed by one tile dispenser per pileup launch of a run
+constexpr int WARN_WORDS = 4;          // ResultsDev::warn: [0] SM missing, [1] NM missing, [2..3] spare; followed by one tile
+                                       // dispenser per pileup launch of a run
 
 constexpr int DEEP_MAX_SITES = 2;
 constexpr int DEEP_THREADS = 256;
@@ -257,7 +259,7 @@ struct SelectParams {
 
 // launch wrappers (brc_kernels.cu)
 cudaError_t launch_init_tiles(int32_t *tile_lo, int32_t *tile_hi, int64_t n_tiles, int32_t *sec_count,
-                              unsigned long long *warn, cudaStream_t s);
+                              unsigned long long *warn, int n_dispensers, cudaStream_t s);
 cudaError_t launch_precompute(const PrecomputeParams &p, cudaStream_t s);
 cudaError_t launch_ref_encode(const char *d_ascii, uint8_t *d_code, int64_t n, cudaStream_t s);
 cudaError_t launch_pileup(const PileupParams &p, cudaStream_t s);

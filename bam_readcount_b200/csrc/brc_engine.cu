@@ -412,7 +412,7 @@ static int alloc_outputs(brc_engine *e, int64_t n_reads_cap) {
     if (rs >= 0xFFFFFFFFll) return set_error(e, BRC_E_INVALID, "more than 2^32 (library, site) slots in one batch: window the region");
     CU(e->d_words.reserve(rs1 * 4 * N_WORDS), "cudaMalloc(words)");
     CU(e->d_sec_count.reserve(16), "cudaMalloc(sec_count)");
-    CU(e->d_warn.reserve((WARN_WORDS + N_WORK_COUNTERS) * 8), "cudaMalloc(warn)");
+    CU(e->d_warn.reserve((WARN_WORDS + 1) * 8), "cudaMalloc(warn)");   // one tile dispenser; compute_pipelined makes room for one per chunk
     return BRC_OK;
 }
 
@@ -561,7 +561,7 @@ static void make_params(brc_engine *e, const int32_t *d_region_of_read, Precompu
     P1.tiles = e->d_tiles.as<TileInfo>(); P1.tile_lo = P0.tile_lo; P1.tile_hi = P0.tile_hi; P1.n_tiles = (int64_t)e->tiles.size(); P1.tile_begin = 0; P1.tile_count = P1.n_tiles;
     P1.res = results_dev(e);
     P1.deep_tiles = e->deep_tiles.empty() ? nullptr : e->d_deep_tiles.as<int32_t>(); P1.n_deep = (int32_t)e->deep_tiles.size(); P1.deep_min_reads = e->deep_min_reads;
-    P1.work_counter = P1.res.warn + WARN_WORDS;                 // launch k of a run takes dispenser k
+    P1.work_counter = P1.res.warn + WARN_WORDS;                 // pileup launch k of a run takes dispenser k
 }
 
 // K(init) + K0 + K1 on stream s.  Returns BRC_E_OVERFLOW (after syncing) if the secondary pool was too small.
@@ -571,7 +571,7 @@ static int run_kernels(brc_engine *e, const int32_t *d_region_of_read, cudaStrea
 
     e->launch_count = 0;
     CU(cudaEventRecord(e->ev[0], s), "event");
-    CU(launch_init_tiles(P0.tile_lo, P0.tile_hi, P1.n_tiles, P1.res.sec_count, P1.res.warn, s), "launch init_tiles"); e->launch_count++;
+    CU(launch_init_tiles(P0.tile_lo, P0.tile_hi, P1.n_tiles, P1.res.sec_count, P1.res.warn, 1, s), "launch init_tiles"); e->launch_count++;
     CU(launch_precompute(P0, s), "launch read_precompute"); if (P0.reads.n_reads) e->launch_count++;
     CU(cudaEventRecord(e->ev[1], s), "event");
     CU(launch_pileup(P1, s), "launch pileup"); if (P1.n_tiles) e->launch_count++;
@@ -652,10 +652,10 @@ void ensure_wide(brc_engine *e) {
             W.ncover[(size_t)i] = w0 & 0xFFu; W.npass[(size_t)i] = (w0 >> 8) & 0xFFu;
             W.flags[(size_t)i] = (uint8_t)((w1 >> 3) & 1u); W.pbase[(size_t)i] = (uint8_t)(pc < 6u ? pc : BRC_NO_BASE);
             W.sec_head[(size_t)i] = -1;
-            ps[0 * rs + i] = count; ps[1 * rs + i] = w1 >> 16; ps[2 * rs + i] = w2 & 0xFFFFu; ps[3 * rs + i] = w2 >> 16;
-            ps[4 * rs + i] = plus; ps[5 * rs + i] = count - plus; ps[6 * rs + i] = words[4 * rs + i]; ps[7 * rs + i] = words[5 * rs + i];
-            ps[8 * rs + i] = w3 >> 16; ps[9 * rs + i] = (w1 >> 8) & 0xFFu; ps[10 * rs + i] = words[6 * rs + i]; ps[11 * rs + i] = w3 & 0xFFFFu;
-            ps[12 * rs + i] = words[7 * rs + i];
+            ps[BRC_S_COUNT * rs + i] = count; ps[BRC_S_MAPQ * rs + i] = w1 >> 16; ps[BRC_S_BASEQ * rs + i] = w2 & 0xFFFFu; ps[BRC_S_SE_MAPQ * rs + i] = w2 >> 16;
+            ps[BRC_S_PLUS * rs + i] = plus; ps[BRC_S_MINUS * rs + i] = count - plus; ps[BRC_S_POS_FRAC * rs + i] = words[4 * rs + i]; ps[BRC_S_NM_FRAC * rs + i] = words[5 * rs + i];
+            ps[BRC_S_MMQS * rs + i] = w3 >> 16; ps[BRC_S_NQ2 * rs + i] = (w1 >> 8) & 0xFFu; ps[BRC_S_Q2_DIST * rs + i] = words[6 * rs + i]; ps[BRC_S_CLIP_LEN * rs + i] = w3 & 0xFFFFu;
+            ps[BRC_S_3P_DIST * rs + i] = words[7 * rs + i];
         }
     });
     // secondary records: keys are chained per slot (order is immaterial to every consumer); escaped primaries fill their slot
@@ -758,14 +758,14 @@ static int compute_pipelined(brc_engine *e) {
     int32_t *h_cnt = e->h_misc.as<int32_t>() + 16;                              // pool counter after each chunk's kernels
     std::vector<int> cnt_chunks;
 
+    CU(e->d_warn.reserve((size_t)(WARN_WORDS + n_chunks) * 8), "cudaMalloc(warn)");   // at most one pileup launch per chunk
     PrecomputeParams P0; PileupParams P1;
     make_params(e, nullptr, P0, P1);
     cudaStream_t sk = e->stream;
     e->launch_count = 0;
     CU(cudaEventRecord(e->ev[0], sk), "event");
-    CU(launch_init_tiles(P0.tile_lo, P0.tile_hi, n_tiles, P1.res.sec_count, P1.res.warn, sk), "launch init_tiles"); e->launch_count++;
+    CU(launch_init_tiles(P0.tile_lo, P0.tile_hi, n_tiles, P1.res.sec_count, P1.res.warn, n_chunks, sk), "launch init_tiles"); e->launch_count++;
     int64_t tile_done = 0;
-    int k1_launches = 0;
     for (int c = 0; c < n_chunks; ++c) {
         const int64_t a = n * c / n_chunks, b = n * (c + 1) / n_chunks;
         // ---- kernels: K0 on the chunk, K1 on the tiles it completes ----
@@ -781,7 +781,7 @@ static int compute_pipelined(brc_engine *e) {
         if (tile_to > tile_done) {
             P1.tile_begin = tile_done; P1.tile_count = tile_to - tile_done;
             CU(launch_pileup(P1, sk), "launch pileup"); e->launch_count++;
-            if (P1.work_counter) P1.work_counter = ++k1_launches < N_WORK_COUNTERS ? P1.work_counter + 1 : nullptr;   // next launch: next dispenser
+            P1.work_counter++;                                  // next launch: next dispenser
             CU(launch_deep_sites(P1, sk), "launch deep_sites"); if (P1.n_deep) e->launch_count++;
             CU(cudaEventRecord(e->pipe_ev[2 * c + 1], sk), "event");
             if (!sel && c < 64) {   // snapshot of the pool counter: the records allocated so far are final (a tile is computed by exactly one launch)

@@ -69,17 +69,18 @@ __device__ __forceinline__ uint32_t seq_nib(const uint8_t *seq, uint64_t off, in
 // init: tile read ranges + counters
 // ---------------------------------------------------------------------------------------------
 __global__ void init_tiles_kernel(int32_t *tile_lo, int32_t *tile_hi, int64_t n_tiles, int32_t *sec_count,
-                                  unsigned long long *warn) {
+                                  unsigned long long *warn, int n_dispensers) {
     int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
     if (i < n_tiles) { tile_lo[i] = 0x7fffffff; tile_hi[i] = 0; }
     if (i == 0) { *sec_count = 0; warn[0] = 0; warn[1] = 0; }
-    if (i < N_WORK_COUNTERS) warn[WARN_WORDS + i] = 0ull;   // tile dispensers of this run's pileup launches
+    if (i < n_dispensers) warn[WARN_WORDS + i] = 0ull;   // tile dispensers of this run's pileup launches
 }
 
 cudaError_t launch_init_tiles(int32_t *tile_lo, int32_t *tile_hi, int64_t n_tiles, int32_t *sec_count,
-                              unsigned long long *warn, cudaStream_t s) {
-    int64_t n = n_tiles > 1 ? n_tiles : 1;
-    init_tiles_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(tile_lo, tile_hi, n_tiles, sec_count, warn);
+                              unsigned long long *warn, int n_dispensers, cudaStream_t s) {
+    // a region of few tiles cut into many chunks still gets every dispenser zeroed
+    const int64_t n = std::max<int64_t>(n_tiles, n_dispensers);
+    init_tiles_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(tile_lo, tile_hi, n_tiles, sec_count, warn, n_dispensers);
     return cudaGetLastError();
 }
 
@@ -225,7 +226,7 @@ __device__ __forceinline__ uint32_t nib8_smem(uint32_t addr, int t) {
     if (t & 1) x = (x << 4) | ((__byte_perm(w0, w1, sh + 4u) >> 4) & 0xFu);
     return x;
 }
-__device__ __forceinline__ uint32_t lds_u8_k0(uint32_t addr) {
+__device__ __forceinline__ uint32_t lds_u8(uint32_t addr) {
     uint32_t v;
     asm volatile("ld.shared.u8 %0, [%1];" : "=r"(v) : "r"(addr));
     return v;
@@ -366,7 +367,7 @@ __global__ void __launch_bounds__(K0_READS) read_precompute_kernel(PrecomputePar
                     const int k8 = __clz(m) >> 2;          // flag of symbol i sits at bit 28-4i
                     m &= ~(0x10000000u >> (4 * k8));
                     const int cur = read_position + j + k8;
-                    const int q = staged ? (int)lds_u8_k0(qual_sa + (uint32_t)cur) : (int)qual[cur];
+                    const int q = staged ? (int)lds_u8(qual_sa + (uint32_t)cur) : (int)qual[cur];
                     if (last_mm_pos != -1) {
                         if (last_mm_pos + 1 != cur) { sum_mmq += (uint32_t)last_mm_qual; last_mm_qual = q; }
                         else if (last_mm_qual < q) last_mm_qual = q;
@@ -391,7 +392,7 @@ __global__ void __launch_bounds__(K0_READS) read_precompute_kernel(PrecomputePar
     if (reverse) { kk = tpi = 0; inc = 1; if (tpi < left_clip) tpi = left_clip; }
     else { kk = tpi = l_qseq - 1; inc = -1; if (tpi > right_clip) tpi = right_clip; }
     while (kk >= 0 && kk < l_qseq) {
-        if ((staged ? lds_u8_k0(qual_sa + (uint32_t)kk) : (uint32_t)qual[kk]) != 2u) { q2_pos = kk - 1; break; }
+        if ((staged ? lds_u8(qual_sa + (uint32_t)kk) : (uint32_t)qual[kk]) != 2u) { q2_pos = kk - 1; break; }
         kk += inc;
     }
     if (reverse) { if (tpi < q2_pos) tpi = q2_pos; }
@@ -540,6 +541,67 @@ __device__ __forceinline__ Terms event_terms(bool fast, int qpos, int q2pos, int
     return t;
 }
 
+// event_terms for an FM_HOT read, from its staged descriptor words q1 (mmq,clen,lclip,tpi), q2 (q2,nmfrac,se,fl) and
+// q4 (rcp_l,rcp_clen,fclen,inc).  The Q2 term only counts when the read has a Q2 position, which for most forward reads IS the
+// effective 3' end (R:...:229-238); it is not tested here, a read without one never adds the term.
+__device__ __forceinline__ Terms hot_terms(const int4 &q1, const int4 &q2, const int4 &q4, int qpos) {
+    Terms t;
+    const float fl = __int_as_float(q2.w), rcp_l = __int_as_float(q4.x);
+    t.d3pterm = div_small((float)abs(qpos - q1.w), fl, rcp_l);
+    t.posf = div_small((float)abs(2 * (qpos - q1.z) - q1.y), __int_as_float(q4.z), __int_as_float(q4.y));
+    t.q2term = q2.x == q1.w ? t.d3pterm : div_small((float)abs(qpos - q2.x), fl, rcp_l);
+    t.posterm = __dsub_rn(1.0, f32_to_f64_nonneg(t.posf));
+    return t;
+}
+
+// What one event adds to each of the 13 statistics of its key: the integers, and the bit patterns of the float terms
+// (BRC_S_POS_FRAC carries posf; the sum takes 1 - posf in double).  `bq` is 0 for an indel key.  Returns whether the read has a
+// Q2 position: without one the two Q2 words are 0 and the event leaves the Q2 count and sum alone.
+__device__ __forceinline__ bool event_words(uint32_t (&w)[N_STATS], uint32_t fm, int32_t se, float nmfrac, int32_t mmq, int32_t clen,
+                                            int32_t q2pos, uint32_t bq, const Terms &t) {
+    const uint32_t plus = (fm & 16u) ? 0u : 1u;
+    const bool has_q2 = q2pos > -1;
+    w[BRC_S_COUNT] = 1u; w[BRC_S_MAPQ] = (fm >> 16) & 0xFFu; w[BRC_S_BASEQ] = bq; w[BRC_S_SE_MAPQ] = (uint32_t)se;
+    w[BRC_S_PLUS] = plus; w[BRC_S_MINUS] = 1u - plus;
+    w[BRC_S_POS_FRAC] = __float_as_uint(t.posf); w[BRC_S_NM_FRAC] = __float_as_uint(nmfrac); w[BRC_S_MMQS] = (uint32_t)mmq;
+    w[BRC_S_NQ2] = has_q2 ? 1u : 0u; w[BRC_S_Q2_DIST] = has_q2 ? __float_as_uint(t.q2term) : 0u;
+    w[BRC_S_CLIP_LEN] = (uint32_t)clen; w[BRC_S_3P_DIST] = __float_as_uint(t.d3pterm);
+    return has_q2;
+}
+// Adds an event_words vector into the 13 cells cell(k) of a key (a pool record's stats[k], a column of shared memory): the exact
+// IEEE form of BasicStat::process_read, one float32 add per float sum and one double add rounded to float32 for the location.
+template <class Cell>
+__device__ __forceinline__ void stats_add(Cell cell, const uint32_t (&w)[N_STATS], bool has_q2) {
+    const auto fadd = [&](int k) { cell(k) = __float_as_uint(__fadd_rn(__uint_as_float(cell(k)), __uint_as_float(w[k]))); };
+    cell(BRC_S_COUNT) += w[BRC_S_COUNT]; cell(BRC_S_MAPQ) += w[BRC_S_MAPQ]; cell(BRC_S_BASEQ) += w[BRC_S_BASEQ];
+    cell(BRC_S_SE_MAPQ) += w[BRC_S_SE_MAPQ]; cell(BRC_S_PLUS) += w[BRC_S_PLUS]; cell(BRC_S_MINUS) += w[BRC_S_MINUS];
+    cell(BRC_S_POS_FRAC) = __float_as_uint(__double2float_rn(__dadd_rn((double)__uint_as_float(cell(BRC_S_POS_FRAC)),
+                                                                       __dsub_rn(1.0, (double)__uint_as_float(w[BRC_S_POS_FRAC])))));
+    fadd(BRC_S_NM_FRAC);
+    cell(BRC_S_MMQS) += w[BRC_S_MMQS];
+    if (has_q2) { cell(BRC_S_NQ2) += w[BRC_S_NQ2]; fadd(BRC_S_Q2_DIST); }
+    cell(BRC_S_CLIP_LEN) += w[BRC_S_CLIP_LEN];
+    fadd(BRC_S_3P_DIST);
+}
+// What an event of the site's primary base class adds to the register accumulators and to the chunk's packed counters (pk3:
+// count | plus << 8 | nq2 << 16 | ncover << 24, all three in the descriptor's `inc`; pkmb: baseq | mapq << 16), applied only
+// when `take` holds.  A dropped event adds 0 to the integer sums, which is exact, and keeps the old value of a float sum: it
+// never adds +-0 to one.  Two calls in a row apply their events to every accumulator in call order, which is what keeps file
+// order when hot_pair takes read A and then read B.  With a literal `true` the selects fold to straight adds.
+__device__ __forceinline__ void acc_primary(Acc &a, uint32_t &pk3, uint32_t &pkmb, bool take, uint32_t fm, uint32_t bq,
+                                            const int4 &q1, const int4 &q2, const int4 &q4, const Terms &t) {
+    const bool take_q2 = take && (q4.w & 0x10000);             // K0 sets the bit iff q2_pos > -1
+    pk3 += take ? (uint32_t)q4.w : 0u;
+    pkmb += take ? (fm & 0x00FF0000u) + bq : 0u;
+    a.mmqs += take ? (uint32_t)q1.x : 0u;
+    a.clip += take ? (uint32_t)q1.y : 0u;
+    a.se += take ? (uint32_t)q2.z : 0u;
+    a.q2d = take_q2 ? __fadd_rn(a.q2d, t.q2term) : a.q2d;
+    a.d3p = take ? __fadd_rn(a.d3p, t.d3pterm) : a.d3p;
+    a.posd = take ? round_to_f32_precision(__dadd_rn(a.posd, t.posterm)) : a.posd;
+    a.nmf = take ? __fadd_rn(a.nmf, __int_as_float(q2.y)) : a.nmf;
+}
+
 // stateless resolve_cigar2.  Returns {qpos, indel, is_del}.
 __device__ __noinline__ int3 resolve_general(const uint32_t *cig, uint32_t n_cigar, int32_t pos, int32_t site) {
     int64_t x = pos; int y = 0; uint32_t k = 0; uint32_t op = 0; int len = 0;
@@ -581,7 +643,7 @@ struct RareCtx {
     const ReadDesc *desc;
     const uint8_t *seq;
     const uint64_t *seq_off;
-    SecRec *sec;
+    SecRec *sec;             // the pool, under the names ResultsDev gives it (sec_append takes either)
     int32_t *sec_count;
     int64_t sec_cap;
 };
@@ -596,34 +658,27 @@ __device__ __forceinline__ bool same_insertion(const RareCtx &C, int32_t read_a,
         same = canonical16(seq_nib(C.seq, oa, qpos_a + k)) == canonical16(seq_nib(C.seq, ob, qpos_b + k));
     return same;
 }
-__device__ __forceinline__ void sec_init(SecRec &r, uint32_t slot, int32_t next, uint32_t kind, uint32_t len, int32_t read, int32_t qpos) {
-    r.slot = slot; r.next = next; r.kind_len = kind | (len << 8); r.read = read; r.qpos = qpos;
-#pragma unroll
-    for (int k = 0; k < N_STATS; ++k) r.stats[k] = 0u;
+// Takes the next record of the pool R (a ResultsDev or a RareCtx) and writes its header; the caller stores the 13 statistics.
+// Returns the record's index.  An index >= sec_cap is the overflow: nothing was written, the caller skips its stores, and the host
+// sees sec_count > sec_cap and runs again with a larger pool.
+template <class Pool>
+__device__ __forceinline__ int32_t sec_append(const Pool &R, uint32_t slot, int32_t next, uint32_t kind_len, int32_t read, int32_t qpos) {
+    const int32_t j = atomicAdd(R.sec_count, 1);
+    if ((int64_t)j < R.sec_cap) {
+        SecRec &r = R.sec[j];
+        r.slot = slot; r.next = next; r.kind_len = kind_len; r.read = read; r.qpos = qpos;
+    }
+    return j;
 }
 // one event of BasicStat::process_read into a pool record (slow, exact IEEE path)
 __device__ __forceinline__ void sec_accumulate(const ReadDesc *desc, SecRec &r, int32_t read, int qpos, uint32_t bq, bool is_indel) {
     const ReadDesc d = desc[read];
     const Terms t = event_terms(false, qpos, d.q2, d.tpi, d.lclip, d.clen, d.fl, d.fclen, 0.f, 0.f);
-    uint32_t v[N_STATS];
-#pragma unroll
-    for (int k = 0; k < N_STATS; ++k) v[k] = r.stats[k];
-    v[0] += 1u;
-    v[1] += (d.fm >> 16) & 0xFFu;
-    if (!is_indel) v[2] += bq;
-    v[3] += (uint32_t)d.se;
-    if (d.fm & 16u) v[5] += 1u; else v[4] += 1u;
-    v[6] = __float_as_uint(__double2float_rn(__dadd_rn((double)__uint_as_float(v[6]), t.posterm)));
-    v[7] = __float_as_uint(__fadd_rn(__uint_as_float(v[7]), d.nmfrac));
-    v[8] += (uint32_t)d.mmq;
-    if (d.q2 > -1) { v[9] += 1u; v[10] = __float_as_uint(__fadd_rn(__uint_as_float(v[10]), t.q2term)); }
-    v[11] += (uint32_t)d.clen;
-    v[12] = __float_as_uint(__fadd_rn(__uint_as_float(v[12]), t.d3pterm));
-#pragma unroll
-    for (int k = 0; k < N_STATS; ++k) r.stats[k] = v[k];
+    uint32_t w[N_STATS];
+    const bool has_q2 = event_words(w, d.fm, d.se, d.nmfrac, d.mmq, d.clen, d.q2, is_indel ? 0u : bq, t);
+    stats_add([&](int k) -> uint32_t & { return r.stats[k]; }, w, has_q2);
 }
-// find-or-append of the allele's record in the chain starting at `head`; returns the record index (>= sec_cap on overflow:
-// the host sees sec_count > cap and retries with a larger pool)
+// find-or-append of the allele's record in the chain starting at `head`; returns the record index (>= sec_cap on overflow)
 __device__ __noinline__ int32_t rare_find_or_append(const RareCtx C, int32_t &head, uint32_t slot, int kind, int len, int32_t read, int qpos) {
     const uint32_t want = (uint32_t)kind | ((uint32_t)len << 8);
     int32_t j = head;
@@ -633,9 +688,10 @@ __device__ __noinline__ int32_t rare_find_or_append(const RareCtx C, int32_t &he
         j = r.next;
     }
     if (j < 0) {
-        j = atomicAdd(C.sec_count, 1);
+        j = sec_append(C, slot, head, want, read, qpos);
         if ((int64_t)j >= C.sec_cap) return j;
-        sec_init(C.sec[j], slot, head, (uint32_t)kind, (uint32_t)len, read, qpos);
+#pragma unroll
+        for (int k = 0; k < N_STATS; ++k) C.sec[j].stats[k] = 0u;
         head = j;
     }
     return j;
@@ -671,12 +727,6 @@ struct __align__(128) PileupSmem {
     ChunkInfo info[NSTAGE];
     uint64_t full[NSTAGE], empty[NSTAGE];
 };
-
-__device__ __forceinline__ uint32_t lds_u8(uint32_t addr) {
-    uint32_t v;
-    asm volatile("ld.shared.u8 %0, [%1];" : "=r"(v) : "r"(addr));
-    return v;
-}
 
 // per-thread (= per-site) state of a consumer, all in registers
 struct SiteState {
@@ -719,6 +769,19 @@ __device__ __forceinline__ uint32_t slot_index(const PileupParams &P, const Chun
     return (uint32_t)((PER_LIB ? (int64_t)S.row * P.res.n_slots : 0) + ci.slot0 + (S.site - ci.pos0));
 }
 constexpr uint32_t DSZ = (uint32_t)sizeof(ReadDesc);
+// index of the read whose staged descriptor sits at shared address `da` (desc_s = the chunk's first descriptor)
+__device__ __forceinline__ int32_t read_index(const ChunkInfo &ci, uint32_t da, uint32_t desc_s) { return ci.r0 + (int)((da - desc_s) / DSZ); }
+// base quality and base class ("=ACGTN" index) at `qpos` of a read: from the staged bytes (qual_s / seq_s + the read's low-32
+// pool offset), or from the pools for a chunk too long for the stage (`read` is only used then)
+template <bool STAGED>
+__device__ __forceinline__ uint32_t load_bq(const PileupParams &P, uint32_t qual_s, uint32_t qual32, int32_t read, int qpos) {
+    return STAGED ? lds_u8(qual_s + qual32 + (uint32_t)qpos) : (uint32_t)P.qual[P.qual_off[read] + (uint32_t)qpos];
+}
+__device__ __forceinline__ uint32_t base_class(uint32_t byte, int qpos) { return canonical16((byte >> ((~qpos & 1) << 2)) & 0xFu); }
+template <bool STAGED>
+__device__ __forceinline__ uint32_t load_base(const PileupParams &P, uint32_t seq_s, uint32_t seq32, int32_t read, int qpos) {
+    return base_class(STAGED ? lds_u8(seq_s + seq32 + ((uint32_t)qpos >> 1)) : (uint32_t)P.seq[P.seq_off[read] + ((uint32_t)qpos >> 1)], qpos);
+}
 
 // A passing event whose base is not the site's primary class: the site's second base class accumulates in shared memory,
 // a third one in the record pool.  `da` = the read's staged descriptor, `read` its index.
@@ -734,25 +797,19 @@ __device__ __forceinline__ void off_primary_event(const PileupParams &P, uint32_
     const int4 q4 = lds128(da + 64u);                            // rcp_l, rcp_clen, fclen
     const Terms t = event_terms(fast, qpos, q2.x, q1.w, q1.z, q1.y, __int_as_float(q2.w), __int_as_float(q4.z),
                                 __int_as_float(q4.x), __int_as_float(q4.y));
-    const uint32_t plus = (fm & 16u) ? 0u : 1u;
+    uint32_t w[N_STATS];
+    const bool has_q2 = event_words(w, fm, q2.z, __int_as_float(q2.y), q1.x, q1.y, q2.x, bq, t);
     if (S.sbase == NO_BASE) {
         S.sbase = base;
 #pragma unroll
         for (int k = 0; k < N_STATS; ++k) sacc[k][tid] = 0u;
     }
-    sacc[0][tid] += 1u; sacc[1][tid] += (fm >> 16) & 0xFFu; sacc[2][tid] += bq; sacc[3][tid] += (uint32_t)q2.z;
-    sacc[4][tid] += plus; sacc[5][tid] += 1u - plus;
-    sacc[6][tid] = __float_as_uint(__double2float_rn(__dadd_rn((double)__uint_as_float(sacc[6][tid]), t.posterm)));
-    sacc[7][tid] = __float_as_uint(__fadd_rn(__uint_as_float(sacc[7][tid]), __int_as_float(q2.y)));
-    sacc[8][tid] += (uint32_t)q1.x;
-    if (q2.x > -1) { sacc[9][tid] += 1u; sacc[10][tid] = __float_as_uint(__fadd_rn(__uint_as_float(sacc[10][tid]), t.q2term)); }
-    sacc[11][tid] += (uint32_t)q1.y;
-    sacc[12][tid] = __float_as_uint(__fadd_rn(__uint_as_float(sacc[12][tid]), t.d3pterm));
+    stats_add([&](int k) -> uint32_t & { return sacc[k][tid]; }, w, has_q2);
 }
 
 // Two consecutive staged FM_HOT reads A (descriptor at `da`) and B (at da + DSZ) in one body without branches: every lane
-// computes both events (a lane off a read loads a valid byte of it and drops the result) and applies them as predicated
-// updates, A before B, so each accumulator still sees file order.  Only the rare event that is not the site's primary class
+// computes both events (a lane off a read loads a valid byte of it and drops the result) and applies them through
+// acc_primary, A before B.  Only the rare event that is not the site's primary class
 // (a second or third base class, ~0.5 % of events) branches, again A before B.  -p: neither read is library-less, so the
 // site's library-less flag cannot change here; a lane whose flag is already set takes neither read.
 template <bool PER_LIB>
@@ -761,6 +818,7 @@ __device__ __forceinline__ void hot_pair(const PileupParams &P, uint32_t (*sacc)
                                          int2 pe_a, uint32_t fm_a, uint32_t lib_a, int2 pe_b, uint32_t fm_b, uint32_t lib_b,
                                          uint32_t &pk3, uint32_t &pkmb) {
     const uint32_t db = da + DSZ;
+    const int32_t read_a = read_index(ci, da, desc_s);
     const int4 q3a = lds128(da + 48u), q3b = lds128(db + 48u);    // qual32,seq32,qoff,n_cigar
     bool cov_a = S.site >= pe_a.x && S.site < pe_a.y;
     bool cov_b = S.site >= pe_b.x && S.site < pe_b.y;
@@ -772,15 +830,13 @@ __device__ __forceinline__ void hot_pair(const PileupParams &P, uint32_t (*sacc)
     pk3 += ((uint32_t)cov_a + (uint32_t)cov_b) << 24;
     const int qpos_a = cov_a ? S.site - pe_a.x + q3a.z : 0;        // FM_HOT reads have l_qseq >= 1: byte 0 exists
     const int qpos_b = cov_b ? S.site - pe_b.x + q3b.z : 0;
-    const uint32_t bq_a = lds_u8(qual_s + (uint32_t)q3a.x + (uint32_t)qpos_a);
-    const uint32_t bq_b = lds_u8(qual_s + (uint32_t)q3b.x + (uint32_t)qpos_b);
-    const uint32_t byte_a = lds_u8(seq_s + (uint32_t)q3a.y + ((uint32_t)qpos_a >> 1));
-    const uint32_t byte_b = lds_u8(seq_s + (uint32_t)q3b.y + ((uint32_t)qpos_b >> 1));
+    const uint32_t bq_a = load_bq<true>(P, qual_s, (uint32_t)q3a.x, read_a, qpos_a);
+    const uint32_t bq_b = load_bq<true>(P, qual_s, (uint32_t)q3b.x, read_a + 1, qpos_b);
+    const uint32_t base_a = load_base<true>(P, seq_s, (uint32_t)q3a.y, read_a, qpos_a);
+    const uint32_t base_b = load_base<true>(P, seq_s, (uint32_t)q3b.y, read_a + 1, qpos_b);
     const bool pass_a = cov_a && !(fm_a & FM_DEAD) && (int)bq_a >= P.min_bq;
     const bool pass_b = cov_b && !(fm_b & FM_DEAD) && (int)bq_b >= P.min_bq;
     S.npass += (uint32_t)pass_a + (uint32_t)pass_b;
-    const uint32_t base_a = canonical16((byte_a >> ((~qpos_a & 1) << 2)) & 0xFu);
-    const uint32_t base_b = canonical16((byte_b >> ((~qpos_b & 1) << 2)) & 0xFu);
     if (pass_a && S.pbase == NO_BASE) S.pbase = base_a;
     const bool prim_a = pass_a && base_a == S.pbase;
     if (pass_b && S.pbase == NO_BASE) S.pbase = base_b;
@@ -789,37 +845,12 @@ __device__ __forceinline__ void hot_pair(const PileupParams &P, uint32_t (*sacc)
     const int4 q1a = lds128(da + 16u), q1b = lds128(db + 16u);    // mmq,clen,lclip,tpi
     const int4 q2a = lds128(da + 32u), q2b = lds128(db + 32u);    // q2,nmfrac,se,fl
     const int4 q4a = lds128(da + 64u), q4b = lds128(db + 64u);    // rcp_l, rcp_clen, fclen, inc
-    const float fl_a = __int_as_float(q2a.w), rcp_la = __int_as_float(q4a.x);
-    const float fl_b = __int_as_float(q2b.w), rcp_lb = __int_as_float(q4b.x);
-    const float d3_a = div_small((float)abs(qpos_a - q1a.w), fl_a, rcp_la);
-    const float d3_b = div_small((float)abs(qpos_b - q1b.w), fl_b, rcp_lb);
-    const float f_a = div_small((float)abs(2 * (qpos_a - q1a.z) - q1a.y), __int_as_float(q4a.z), __int_as_float(q4a.y));
-    const float f_b = div_small((float)abs(2 * (qpos_b - q1b.z) - q1b.y), __int_as_float(q4b.z), __int_as_float(q4b.y));
-    // the Q2 term only counts when the read has a Q2 position, which for most forward reads IS the effective 3' end
-    const float q2t_a = q2a.x == q1a.w ? d3_a : div_small((float)abs(qpos_a - q2a.x), fl_a, rcp_la);
-    const float q2t_b = q2b.x == q1b.w ? d3_b : div_small((float)abs(qpos_b - q2b.x), fl_b, rcp_lb);
-    const bool q2_a = prim_a && (q4a.w & 0x10000), q2_b = prim_b && (q4b.w & 0x10000);
-
-    // integer sums: adding 0 for a dropped event is exact
-    pk3 += (prim_a ? (uint32_t)q4a.w : 0u) + (prim_b ? (uint32_t)q4b.w : 0u);
-    pkmb += (prim_a ? (fm_a & 0x00FF0000u) + bq_a : 0u) + (prim_b ? (fm_b & 0x00FF0000u) + bq_b : 0u);
-    Acc &a = S.acc;
-    a.mmqs += (prim_a ? (uint32_t)q1a.x : 0u) + (prim_b ? (uint32_t)q1b.x : 0u);
-    a.clip += (prim_a ? (uint32_t)q1a.y : 0u) + (prim_b ? (uint32_t)q1b.y : 0u);
-    a.se += (prim_a ? (uint32_t)q2a.z : 0u) + (prim_b ? (uint32_t)q2b.z : 0u);
-    // float sums: a dropped event keeps the old value (never "+ 0"), A's add before B's
-    a.q2d = q2_a ? __fadd_rn(a.q2d, q2t_a) : a.q2d;
-    a.q2d = q2_b ? __fadd_rn(a.q2d, q2t_b) : a.q2d;
-    a.d3p = prim_a ? __fadd_rn(a.d3p, d3_a) : a.d3p;
-    a.d3p = prim_b ? __fadd_rn(a.d3p, d3_b) : a.d3p;
-    a.posd = prim_a ? round_to_f32_precision(__dadd_rn(a.posd, __dsub_rn(1.0, f32_to_f64_nonneg(f_a)))) : a.posd;
-    a.posd = prim_b ? round_to_f32_precision(__dadd_rn(a.posd, __dsub_rn(1.0, f32_to_f64_nonneg(f_b)))) : a.posd;
-    a.nmf = prim_a ? __fadd_rn(a.nmf, __int_as_float(q2a.y)) : a.nmf;
-    a.nmf = prim_b ? __fadd_rn(a.nmf, __int_as_float(q2b.y)) : a.nmf;
+    const Terms t_a = hot_terms(q1a, q2a, q4a, qpos_a), t_b = hot_terms(q1b, q2b, q4b, qpos_b);
+    acc_primary(S.acc, pk3, pkmb, prim_a, fm_a, bq_a, q1a, q2a, q4a, t_a);
+    acc_primary(S.acc, pk3, pkmb, prim_b, fm_b, bq_b, q1b, q2b, q4b, t_b);
 
     const bool off_a = pass_a && !prim_a, off_b = pass_b && !prim_b;
     if (off_a || off_b) {
-        const int32_t read_a = ci.r0 + (int)((da - desc_s) / DSZ);
         if (off_a) off_primary_event<PER_LIB>(P, sacc, ci, S, tid, da, read_a, true, fm_a, qpos_a, bq_a, base_a);
         if (off_b) off_primary_event<PER_LIB>(P, sacc, ci, S, tid, db, read_a + 1, true, fm_b, qpos_b, bq_b, base_b);
     }
@@ -899,33 +930,16 @@ __device__ __forceinline__ void process_chunk(const PileupParams &P, const Stage
             // ---- straight-line path: filters decided by K0, single match op, exact reciprocal divisions ----
             if (fm & FM_DEAD) continue;
             qpos = S.site - pe.x + q3.z;
-            if (STAGED) bq = lds_u8(qual_s + (uint32_t)q3.x + (uint32_t)qpos);
-            else bq = P.qual[P.qual_off[ci.r0 + (int)((da - desc_s) / (uint32_t)sizeof(ReadDesc))] + (uint32_t)qpos];
+            bq = load_bq<STAGED>(P, qual_s, (uint32_t)q3.x, read_index(ci, da, desc_s), qpos);
             if ((int)bq < P.min_bq) continue;
             S.npass++;
-            uint32_t byte;
-            if (STAGED) byte = lds_u8(seq_s + (uint32_t)q3.y + ((uint32_t)qpos >> 1));
-            else byte = P.seq[P.seq_off[ci.r0 + (int)((da - desc_s) / (uint32_t)sizeof(ReadDesc))] + ((uint32_t)qpos >> 1)];
-            base = canonical16((byte >> ((~qpos & 1) << 2)) & 0xFu);
+            base = load_base<STAGED>(P, seq_s, (uint32_t)q3.y, read_index(ci, da, desc_s), qpos);
             if (S.pbase == NO_BASE) S.pbase = base;
             if (base == S.pbase) {
                 const int4 q1 = lds128(da + 16u);                // mmq,clen,lclip,tpi
                 const int4 q2 = lds128(da + 32u);                // q2,nmfrac,se,fl
                 const int4 q4 = lds128(da + 64u);                // rcp_l, rcp_clen, fclen, inc
-                const float fl = __int_as_float(q2.w), rcp_l = __int_as_float(q4.x);
-                const float d3 = div_small((float)abs(qpos - q1.w), fl, rcp_l);
-                const float f = div_small((float)abs(2 * (qpos - q1.z) - q1.y), __int_as_float(q4.z), __int_as_float(q4.y));
-                Acc &a = S.acc;
-                pk3 += (uint32_t)q4.w;
-                pkmb += (fm & 0x00FF0000u) + bq;
-                a.mmqs += (uint32_t)q1.x; a.clip += (uint32_t)q1.y; a.se += (uint32_t)q2.z;
-                if (q4.w & 0x10000) {                            // the read has a Q2 position (usually == the effective 3' end, R:...:229-238)
-                    const float q2t = q2.x == q1.w ? d3 : div_small((float)abs(qpos - q2.x), fl, rcp_l);
-                    a.q2d = __fadd_rn(a.q2d, q2t);
-                }
-                a.d3p = __fadd_rn(a.d3p, d3);
-                a.posd = round_to_f32_precision(__dadd_rn(a.posd, __dsub_rn(1.0, f32_to_f64_nonneg(f))));
-                a.nmf = __fadd_rn(a.nmf, __int_as_float(q2.y));
+                acc_primary(S.acc, pk3, pkmb, true, fm, bq, q1, q2, q4, hot_terms(q1, q2, q4, qpos));
                 continue;
             }
         } else {
@@ -938,50 +952,37 @@ __device__ __forceinline__ void process_chunk(const PileupParams &P, const Stage
                 // Unstaged: the full 64-bit op offset, as the unstaged quality loads do
                 const uint32_t *cig = (ci.flags & 16u)
                     ? static_cast<const uint32_t *>(__cvta_shared_to_generic(desc_s + (uint32_t)offsetof(StageBuf, cigar) + 4u * ((uint32_t)q3.z - ci.cbase32)))
-                    : P.cigar + P.cigar_off[ci.r0 + (int)((da - desc_s) / DSZ)];
+                    : P.cigar + P.cigar_off[read_index(ci, da, desc_s)];
                 const int3 rr = resolve_general(cig, (uint32_t)q3.w, pe.x, S.site);
                 if (rr.z) continue;                              // is_del
                 qpos = rr.x; indel = rr.y;
             }
             if (fm & FM_DEAD) continue;                          // mapq / flag filter (R:...:288-310)
-            if (STAGED) bq = lds_u8(qual_s + (uint32_t)q3.x + (uint32_t)qpos);
-            else bq = P.qual[P.qual_off[ci.r0 + (int)((da - desc_s) / (uint32_t)sizeof(ReadDesc))] + (uint32_t)qpos];
+            bq = load_bq<STAGED>(P, qual_s, (uint32_t)q3.x, read_index(ci, da, desc_s), qpos);
             if ((int)bq < P.min_bq) continue;
             S.npass++;
             const bool warns = (fm & (FM_NM_ABSENT | FM_SM_MISSING)) != 0;   // a tag the reference warns about is missing
             if (indel != 0) {
-                const int32_t r = ci.r0 + (int)((da - desc_s) / (uint32_t)sizeof(ReadDesc));
-                S.sec_head = rare_event(rare_ctx(P), S.sec_head, slot_index<PER_LIB>(P, ci, S), indel > 0 ? KIND_INS : KIND_DEL, indel > 0 ? indel : -indel, r, qpos, bq, true);
+                S.sec_head = rare_event(rare_ctx(P), S.sec_head, slot_index<PER_LIB>(P, ci, S), indel > 0 ? KIND_INS : KIND_DEL, indel > 0 ? indel : -indel,
+                                        read_index(ci, da, desc_s), qpos, bq, true);
                 if (warns) { warn[0][tid] += (fm >> 25) & 1u; warn[1][tid] += (fm >> 26) & 1u; }
                 if (indel > 0 && P.insertion_centric) continue;
             }
             if (warns) { warn[0][tid] += (fm >> 25) & 1u; warn[1][tid] += (fm >> 26) & 1u; }
-            uint32_t byte;
-            if (STAGED) byte = lds_u8(seq_s + (uint32_t)q3.y + ((uint32_t)qpos >> 1));
-            else byte = P.seq[P.seq_off[ci.r0 + (int)((da - desc_s) / (uint32_t)sizeof(ReadDesc))] + ((uint32_t)qpos >> 1)];
-            base = canonical16((byte >> ((~qpos & 1) << 2)) & 0xFu);
+            base = load_base<STAGED>(P, seq_s, (uint32_t)q3.y, read_index(ci, da, desc_s), qpos);
             if (S.pbase == NO_BASE) S.pbase = base;
         }
         // ---- an event that is not (hot, primary): full-width accumulation ----
         if (base != S.pbase) {
-            off_primary_event<PER_LIB>(P, sacc, ci, S, tid, da, ci.r0 + (int)((da - desc_s) / DSZ), (fm & FM_FASTDIV) != 0, fm, qpos, bq, base);
+            off_primary_event<PER_LIB>(P, sacc, ci, S, tid, da, read_index(ci, da, desc_s), (fm & FM_FASTDIV) != 0, fm, qpos, bq, base);
             continue;
         }
         const int4 q1 = lds128(da + 16u);                        // mmq,clen,lclip,tpi
         const int4 q2 = lds128(da + 32u);                        // q2,nmfrac,se,fl
-        const int4 q4 = lds128(da + 64u);                        // rcp_l, rcp_clen, fclen
+        const int4 q4 = lds128(da + 64u);                        // rcp_l, rcp_clen, fclen, inc
         const Terms t = event_terms((fm & FM_FASTDIV) != 0, qpos, q2.x, q1.w, q1.z, q1.y, __int_as_float(q2.w), __int_as_float(q4.z),
                                     __int_as_float(q4.x), __int_as_float(q4.y));
-        Acc &a = S.acc;
-        pk3 += (uint32_t)q4.w;                                   // count, plus, nq2: the packed counters, as on the hot path
-        pkmb += (fm & 0x00FF0000u) + bq;
-        a.mmqs += (uint32_t)q1.x;
-        if (q2.x > -1) a.q2d = __fadd_rn(a.q2d, t.q2term);
-        a.d3p = __fadd_rn(a.d3p, t.d3pterm);
-        a.clip += (uint32_t)q1.y;
-        a.posd = round_to_f32_precision(__dadd_rn(a.posd, t.posterm));
-        a.se += (uint32_t)q2.z;
-        a.nmf = __fadd_rn(a.nmf, __int_as_float(q2.y));
+        acc_primary(S.acc, pk3, pkmb, true, fm, bq, q1, q2, q4, t);
     }
     // flush the chunk's packed counters of the primary class
     S.acc.count += pk3 & 0xFFu; S.acc.plus += (pk3 >> 8) & 0xFFu; S.acc.nq2 += (pk3 >> 16) & 0xFFu; S.ncover += pk3 >> 24;
@@ -989,25 +990,24 @@ __device__ __forceinline__ void process_chunk(const PileupParams &P, const Stage
 }
 
 // Packs one site's header + primary accumulators into the 8-word narrow record, or escapes it to a full-width pool record
-// (brc_device.cuh).  `st` = the 13 accumulators in print order.  Returns false when the pool overflowed (host retries).
+// (brc_device.cuh).  `st` = the 13 accumulators in print order.
 __device__ __forceinline__ void emit_packed(const ResultsDev &R, int64_t idx, uint32_t ncover, uint32_t npass, uint32_t flags, uint32_t pbase,
                                             int32_t sec_head, const uint32_t (&st)[N_STATS]) {
     const uint32_t pcode = pbase < 6u ? pbase : PB_NONE;
-    const bool narrow = ncover <= 255u && st[1] <= 0xFFFFu && st[2] <= 0xFFFFu && st[3] <= 0xFFFFu && st[11] <= 0xFFFFu && st[8] <= 0xFFFFu;
+    const bool narrow = ncover <= 255u && st[BRC_S_MAPQ] <= 0xFFFFu && st[BRC_S_BASEQ] <= 0xFFFFu && st[BRC_S_SE_MAPQ] <= 0xFFFFu &&
+                        st[BRC_S_CLIP_LEN] <= 0xFFFFu && st[BRC_S_MMQS] <= 0xFFFFu;
     uint32_t w[N_WORDS];
     if (narrow) {
-        w[0] = ncover | (npass << 8) | (st[0] << 16) | (st[4] << 24);
-        w[1] = pcode | ((flags & 1u) << 3) | (sec_head >= 0 ? 16u : 0u) | (st[9] << 8) | (st[1] << 16);
-        w[2] = st[2] | (st[3] << 16);
-        w[3] = st[11] | (st[8] << 16);
-        w[4] = st[6]; w[5] = st[7]; w[6] = st[10]; w[7] = st[12];
+        w[0] = ncover | (npass << 8) | (st[BRC_S_COUNT] << 16) | (st[BRC_S_PLUS] << 24);
+        w[1] = pcode | ((flags & 1u) << 3) | (sec_head >= 0 ? 16u : 0u) | (st[BRC_S_NQ2] << 8) | (st[BRC_S_MAPQ] << 16);
+        w[2] = st[BRC_S_BASEQ] | (st[BRC_S_SE_MAPQ] << 16);
+        w[3] = st[BRC_S_CLIP_LEN] | (st[BRC_S_MMQS] << 16);
+        w[4] = st[BRC_S_POS_FRAC]; w[5] = st[BRC_S_NM_FRAC]; w[6] = st[BRC_S_Q2_DIST]; w[7] = st[BRC_S_3P_DIST];
     } else {
-        const int32_t j = atomicAdd(R.sec_count, 1);
+        const int32_t j = sec_append(R, (uint32_t)idx, sec_head, (KIND_WIDE + pcode) | (ncover << 8), (int32_t)flags, (int32_t)npass);
         if ((int64_t)j < R.sec_cap) {
-            SecRec &r = R.sec[j];
-            r.slot = (uint32_t)idx; r.next = sec_head; r.kind_len = (KIND_WIDE + pcode) | (ncover << 8); r.read = (int32_t)flags; r.qpos = (int32_t)npass;
 #pragma unroll
-            for (int k = 0; k < N_STATS; ++k) r.stats[k] = st[k];
+            for (int k = 0; k < N_STATS; ++k) R.sec[j].stats[k] = st[k];
         }
         w[0] = 0u; w[1] = PB_ESCAPE | ((flags & 1u) << 3) | 16u; w[2] = w[3] = w[4] = w[5] = w[6] = w[7] = 0u;
     }
@@ -1025,19 +1025,29 @@ __device__ __forceinline__ void site_emit(const PileupParams &P, uint32_t (*sacc
     int32_t sec_head = S.sec_head;
     const int64_t idx = (PER_LIB ? (int64_t)S.row * R.n_slots : 0) + ci.slot0 + (S.site - ci.pos0);
     if (S.sbase != NO_BASE) {   // move the second base class into the record pool
-        const int32_t j = atomicAdd(R.sec_count, 1);
+        const int32_t j = sec_append(R, (uint32_t)idx, sec_head, S.sbase, 0, 0);
         if ((int64_t)j < R.sec_cap) {
-            SecRec &r = R.sec[j];
-            r.slot = (uint32_t)idx; r.next = sec_head; r.kind_len = S.sbase; r.read = 0; r.qpos = 0;
 #pragma unroll
-            for (int k = 0; k < N_STATS; ++k) r.stats[k] = sacc[k][tid];
+            for (int k = 0; k < N_STATS; ++k) R.sec[j].stats[k] = sacc[k][tid];
             sec_head = j;
         }
     }
     const Acc &a = S.acc;
-    const uint32_t st[N_STATS] = {a.count, a.mapq, a.baseq, a.se, a.plus, a.count - a.plus, __float_as_uint(__double2float_rn(a.posd)),
-                                  __float_as_uint(a.nmf), a.mmqs, a.nq2, __float_as_uint(a.q2d), a.clip, __float_as_uint(a.d3p)};
+    uint32_t st[N_STATS];
+    st[BRC_S_COUNT] = a.count; st[BRC_S_MAPQ] = a.mapq; st[BRC_S_BASEQ] = a.baseq; st[BRC_S_SE_MAPQ] = a.se;
+    st[BRC_S_PLUS] = a.plus; st[BRC_S_MINUS] = a.count - a.plus; st[BRC_S_POS_FRAC] = __float_as_uint(__double2float_rn(a.posd));
+    st[BRC_S_NM_FRAC] = __float_as_uint(a.nmf); st[BRC_S_MMQS] = a.mmqs; st[BRC_S_NQ2] = a.nq2; st[BRC_S_Q2_DIST] = __float_as_uint(a.q2d);
+    st[BRC_S_CLIP_LEN] = a.clip; st[BRC_S_3P_DIST] = __float_as_uint(a.d3p);
     emit_packed(R, idx, S.ncover, S.npass, PER_LIB ? S.flags : 0u, S.pbase, sec_head, st);
+}
+
+// a thread's two warning counters into the run's: warp-reduce, then one atomic per warp (called by whole warps)
+__device__ __forceinline__ void flush_warnings(unsigned long long *warn, uint32_t warn_nm, uint32_t warn_sm) {
+    for (int o = 16; o; o >>= 1) { warn_sm += __shfl_xor_sync(0xffffffffu, warn_sm, o); warn_nm += __shfl_xor_sync(0xffffffffu, warn_nm, o); }
+    if ((threadIdx.x & 31) == 0) {
+        if (warn_sm) atomicAdd(warn + 0, (unsigned long long)warn_sm);
+        if (warn_nm) atomicAdd(warn + 1, (unsigned long long)warn_nm);
+    }
 }
 
 template <bool PER_LIB>
@@ -1062,9 +1072,8 @@ __global__ void __launch_bounds__(K1_THREADS, BRC_K1_CTAS_PER_SM) pileup_kernel(
         // another stream's CTAs (the NCCL send/recv kernels of the ordered-emit gather, a neighbouring window's K0) run their tiles
         // slower, and with a fixed stride the slowest SM set the launch time (r02m8: 2.8 -> 4.2 ms per window at 4 GPUs).  The
         // producer runs up to NSTAGE chunks ahead of the consumers, which hides the atomic's round trip.
-        int64_t w_static = blockIdx.x;
-        for (;; w_static += gridDim.x) {
-            const int64_t w = P.work_counter ? (int64_t)atomicAdd(P.work_counter, 1ull) : w_static;
+        for (;;) {
+            const int64_t w = (int64_t)atomicAdd(P.work_counter, 1ull);
             const bool done = w >= n_work;
             int32_t lo = 0, hi = 0; TileInfo ti{0, 0, 0}; uint32_t row = 0;
             bool narrow = false;
@@ -1165,13 +1174,7 @@ __global__ void __launch_bounds__(K1_THREADS, BRC_K1_CTAS_PER_SM) pileup_kernel(
 #endif
         if (lane == 0) mbar_arrive(&sm.empty[s]);   // this warp is done with the slot
     }
-    // warning counters: warp-reduce then one atomic per warp
-    uint32_t warn_nm = sm.warn[0][tid], warn_sm = sm.warn[1][tid];
-    for (int o = 16; o; o >>= 1) { warn_sm += __shfl_xor_sync(0xffffffffu, warn_sm, o); warn_nm += __shfl_xor_sync(0xffffffffu, warn_nm, o); }
-    if (lane == 0) {
-        if (warn_sm) atomicAdd(P.res.warn + 0, (unsigned long long)warn_sm);
-        if (warn_nm) atomicAdd(P.res.warn + 1, (unsigned long long)warn_nm);
-    }
+    flush_warnings(P.res.warn, sm.warn[0][tid], sm.warn[1][tid]);
 }
 
 static std::atomic<int> g_sm_count[64];
@@ -1323,9 +1326,9 @@ __global__ void __launch_bounds__(DEEP_THREADS, 2) deep_site_kernel(PileupParams
     bool owner = false; int og = 0, oj = 0, kind = 0;   // kind 0 integer, 1 float, 2 double-rounded
     {
         const int fb = deep_flt_base(G), db = deep_dbl_base(G);
-        if (tid < 9 * G) { const int k = tid / G; og = tid - k * G; oj = k < 6 ? k : (k == 6 ? 8 : (k == 7 ? 9 : 11)); kind = 0; owner = true; }
-        else if (tid >= fb && tid < fb + 3 * G) { const int k = (tid - fb) / G; og = tid - fb - k * G; oj = k == 0 ? 7 : (k == 1 ? 10 : 12); kind = 1; owner = true; }
-        else if (tid >= db && tid < db + G) { og = tid - db; oj = 6; kind = 2; owner = true; }
+        if (tid < 9 * G) { const int k = tid / G; og = tid - k * G; oj = k < 6 ? k : (k == 6 ? BRC_S_MMQS : (k == 7 ? BRC_S_NQ2 : BRC_S_CLIP_LEN)); kind = 0; owner = true; }   // k < 6: BRC_S_COUNT .. BRC_S_MINUS
+        else if (tid >= fb && tid < fb + 3 * G) { const int k = (tid - fb) / G; og = tid - fb - k * G; oj = k == 0 ? BRC_S_NM_FRAC : (k == 1 ? BRC_S_Q2_DIST : BRC_S_3P_DIST); kind = 1; owner = true; }
+        else if (tid >= db && tid < db + G) { og = tid - db; oj = BRC_S_POS_FRAC; kind = 2; owner = true; }
     }
     uint32_t acc_u = 0u; float acc_f = 0.0f; double acc_d = 0.0;
     uint32_t pbase = NO_BASE; int32_t sec_head = -1;
@@ -1405,14 +1408,10 @@ __global__ void __launch_bounds__(DEEP_THREADS, 2) deep_site_kernel(PileupParams
             const bool base_part = !(indel > 0 && P.insertion_centric);
             const uint32_t nw = (indel != 0 ? 1u : 0u) + (base_part ? 1u : 0u);   // process_read calls that warn
             warn_nm += nw * ((fm >> 25) & 1u); warn_sm += nw * ((fm >> 26) & 1u);
-            const uint32_t base = canonical16((bytev[sg] >> ((~qpos & 1) << 2)) & 0xFu);
+            const uint32_t base = base_class(bytev[sg], qpos);
             const Terms t = event_terms((fm & FM_FASTDIV) != 0, qpos, d.q2, d.tpi, d.lclip, d.clen, d.fl, d.fclen, d.rcp_l, d.rcp_clen);
-            const uint32_t plus = (fm & 16u) ? 0u : 1u;
-            const bool has_q2 = d.q2 > -1;
-            w[sg][0] = 1u; w[sg][1] = mapq; w[sg][2] = bq; w[sg][3] = (uint32_t)d.se; w[sg][4] = plus; w[sg][5] = 1u - plus;
-            w[sg][6] = __float_as_uint(t.posf); w[sg][7] = __float_as_uint(d.nmfrac); w[sg][8] = (uint32_t)d.mmq;
-            w[sg][9] = has_q2 ? 1u : 0u; w[sg][10] = has_q2 ? __float_as_uint(t.q2term) : 0u;   // + 0.0f leaves the sum unchanged
-            w[sg][11] = (uint32_t)d.clen; w[sg][12] = __float_as_uint(t.d3pterm);
+            // phase 2 adds every word: for a read without a Q2 position the Q2 words are 0, and + 0.0f leaves the sum unchanged
+            event_words(w[sg], fm, d.se, d.nmfrac, d.mmq, d.clen, d.q2, bq, t);
             emeta[sg] = base | (indel != 0 ? 8u : 0u) | (base_part ? 16u : 0u) | (bq << 8);
         }
 #ifdef BRC_DEEP_PROFILE
@@ -1472,7 +1471,7 @@ __global__ void __launch_bounds__(DEEP_THREADS, 2) deep_site_kernel(PileupParams
                 for (; i < n; ++i) { const uint32_t m = mp[i]; if (m & 16u) { pbase = m & 7u; break; } }
             }
             const uint32_t want = 16u | pbase;  // (m & 0x17) == want  <=>  base event of the primary class
-            const bool is0 = oj == 0;
+            const bool is0 = oj == BRC_S_COUNT;
             // indel-only events before the first base event (insertion-centric): still the read_count owner's to replay
             if (is0) for (uint32_t k = 0; k < i; ++k) { const uint32_t m = mp[k]; if (m & 8u) deep_indel_event(P, sm, og, oslot, sec_head, sm.eindel[b0 + k], sm.eread[b0 + k], sm.eqpos[b0 + k], m >> 8); }
             // 32 events at a time, branch-free: a non-primary event adds 0 (exact: the sums are non-negative) and sets a bit;
@@ -1530,14 +1529,9 @@ __global__ void __launch_bounds__(DEEP_THREADS, 2) deep_site_kernel(PileupParams
     // ---- emit: non-primary base classes become pool records (what site_emit does with its second class) ----
     for (int c = 0; c < 6; ++c) {
         const bool present = owner && (uint32_t)c != pbase && (uint32_t)sm.other[c][og] != 0u;   // thread og owns read_count of group og
-        if (present && oj == 0) {
-            const ResultsDev &R = P.res;
-            const int32_t j = atomicAdd(R.sec_count, 1);
-            if ((int64_t)j < R.sec_cap) {
-                SecRec &r = R.sec[j];
-                r.slot = oslot; r.next = sec_head; r.kind_len = (uint32_t)c; r.read = 0; r.qpos = 0;
-                sec_head = j;
-            }
+        if (present && oj == BRC_S_COUNT) {
+            const int32_t j = sec_append(P.res, oslot, sec_head, (uint32_t)c, 0, 0);
+            if ((int64_t)j < P.res.sec_cap) sec_head = j;
             sm.recj[og] = j;
         }
         __syncthreads();
@@ -1554,18 +1548,14 @@ __global__ void __launch_bounds__(DEEP_THREADS, 2) deep_site_kernel(PileupParams
     uint32_t *scr = sm.meta;                                   // free after the last block: [group][16] scratch
     if (owner) scr[og * 16 + oj] = kind == 2 ? __float_as_uint(__double2float_rn(acc_d)) : (kind == 1 ? __float_as_uint(acc_f) : acc_u);
     __syncthreads();
-    if (owner && oj == 0) {
+    if (owner && oj == BRC_S_COUNT) {
         const int sg = og / n_rows;
         uint32_t st[N_STATS];
 #pragma unroll
         for (int k = 0; k < N_STATS; ++k) st[k] = scr[og * 16 + k];
         emit_packed(P.res, (int64_t)oslot, sm.ncover[og], sm.npass[og], (PER_LIB && sm.first_libless[sg] != 0x7fffffff) ? 1u : 0u, pbase, sec_head, st);
     }
-    for (int o = 16; o; o >>= 1) { warn_sm += __shfl_xor_sync(0xffffffffu, warn_sm, o); warn_nm += __shfl_xor_sync(0xffffffffu, warn_nm, o); }
-    if (lane == 0) {
-        if (warn_sm) atomicAdd(P.res.warn + 0, (unsigned long long)warn_sm);
-        if (warn_nm) atomicAdd(P.res.warn + 1, (unsigned long long)warn_nm);
-    }
+    flush_warnings(P.res.warn, warn_nm, warn_sm);
 #ifdef BRC_DEEP_PROFILE
     if (tid == 0) for (int k = 0; k < 6; ++k) atomicAdd(&g_deepprof[k], (unsigned long long)prof[k]);
 #endif

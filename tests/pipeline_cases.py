@@ -15,8 +15,8 @@ import numpy as np
 from boundary_cases import K1_TILE, _case, _ref, _Reads
 
 TILE = K1_TILE
-# chunk counts of the cut tests.  65: one chunk past the 64 tile dispensers, so any 65th pileup launch of a run takes the static
-# stride; 200: enough chunks that finish a tile for the chunk-cut case to make more than 64 pileup launches in one run.
+# chunk counts of the cut tests.  A run cuts its own input into at most 32 chunks; every pileup launch takes a tile dispenser of
+# its own.  65: a 65th one; 200: enough chunks that finish a tile for the chunk-cut case to make more than 64 pileup launches in one run.
 CHUNK_COUNTS = (1, 2, 3, 7, 32, 64, 65, 200)
 CUT_KINDS = ("in_run", "on_edge", "off_edge", "before_region", "no_tile", "later_tile")
 _CIGARS = ("100M", "100M", "100M", "48M3D52M", "30M2I68M", "5S95M", "90M10S", "60M1D40M")

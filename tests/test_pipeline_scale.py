@@ -11,7 +11,7 @@ CPU
 GPU, each asserting that it reached its path
   test_chunk_cuts_equal_the_oracle           every chunk count x cases.FLAG_SETS: K0 per chunk, the pileup kernel on the
                                              tiles a chunk finishes, per-chunk word copies at s0 > 0, pool records shipped
-                                             in pieces, the static-stride dispenser past 64 launches.  Launch count = plan.
+                                             in pieces, a tile dispenser for each of more than 64 launches.  Launch count = plan.
   test_multi_chunk_per_library_rows          -p with 3 rows (per-array copies) and 12 rows (one strided 2-D copy at s0 > 0).
   test_multi_chunk_site_filter               the site selection after a chunked run (no per-chunk copies).
   test_multi_chunk_pool_overflow_falls_back  compute_pipelined overflows its pool and the plain path recomputes.
@@ -121,7 +121,7 @@ def test_chunk_cuts_reach_every_edge_of_the_chunk_rule():
         # no tile of <= 2 sites: no deep-site tile, so the launch count of a plan is 1 + chunks + pileup launches
         assert n_slots % pc.TILE > 2
         k1 = {n: sum(1 for _, _, t0, t1 in pc.pipe_plan(sub.pos, first_pos, n_tiles, n) if t1 > t0) for n in pc.CHUNK_COUNTS}
-        assert k1[200] > 64, k1                     # the 65th pileup launch of a run has no dispenser: static stride
+        assert k1[200] > 64, k1                     # every pileup launch of a run has its own tile dispenser, the 65th and later ones too
         assert all(k1[n] > 1 for n in pc.CHUNK_COUNTS if n > 1), k1
     carry = pc.carried_regions()
     for region in carry["regions"]:
