@@ -196,10 +196,9 @@ class Results:
         (``S``/``A``/``L``/``K``/``Q``/``D`` records).  ``pushed``: the admitted reads in push order;
         ``refs``: tid -> (win_beg, bytes)."""
         out: List[str] = []
-        per_lib = self.n_rows > 1 or getattr(self, "_per_lib", False)
         for g in self.regions:
             queues = [[] for _ in range(self.n_rows)]   # site-list semantics: fresh queue per region
-            self._dump_region(g, pushed, refs, out, queues, per_lib)
+            self._dump_region(g, pushed, refs, out, queues, 0)
         return "".join(out)
 
     def dump_range(self, pushed: ReadBatch, refs: dict, region_index: int, pos_lo: int, pos_hi: int, read_offset: int = 0) -> str:
@@ -213,17 +212,13 @@ class Results:
         g["first_pos"] = pos_lo
         g["n_slots"] = pos_hi - pos_lo
         out: List[str] = []
-        self._read_offset = read_offset
-        try:
-            self._dump_region(g, pushed, refs, out, [[] for _ in range(self.n_rows)], self.n_rows > 1 or getattr(self, "_per_lib", False))
-        finally:
-            self._read_offset = 0
+        self._dump_region(g, pushed, refs, out, [[] for _ in range(self.n_rows)], read_offset)
         return "".join(out)
 
     def _stat_str(self, v) -> str:
         return " ".join((f"{int(x):08x}" if k in _FLOAT_STATS else str(int(x))) for k, x in enumerate(v))
 
-    def _keys(self, row, slot, pos, pushed, refs, tid):
+    def _keys(self, row, slot, pos, pushed, refs, tid, read_offset):
         bases, indels = {}, []
         if self.pbase[row, slot] < 6:
             bases[int(self.pbase[row, slot])] = self.pstats[:, row, slot]
@@ -236,7 +231,7 @@ class Results:
             else:
                 ln = int(self.sec_len[j])
                 if k == KIND_INS:
-                    rd, qp = int(self.sec_read[j]) - getattr(self, "_read_offset", 0), int(self.sec_qpos[j])
+                    rd, qp = int(self.sec_read[j]) - read_offset, int(self.sec_qpos[j])
                     so = int(pushed.seq_off[rd])
                     al = "+"
                     for t in range(1, ln + 1):
@@ -252,7 +247,7 @@ class Results:
         indels.sort(key=lambda x: x[0])
         return bases, indels
 
-    def _dump_region(self, g, pushed, refs, out, queues, per_lib):
+    def _dump_region(self, g, pushed, refs, out, queues, read_offset):
         tid = g["tid"]
         for s in range(g["n_slots"]):
             slot = g["slot_base"] + s
@@ -270,7 +265,7 @@ class Results:
                 if nc[row] == 0:
                     continue
                 out.append(f"L {row} {int(nc[row])}\n")
-                bases, indels = self._keys(row, slot, pos, pushed, refs, tid)
+                bases, indels = self._keys(row, slot, pos, pushed, refs, tid, read_offset)
                 for b in range(6):
                     if b in bases and int(bases[b][0]) > 0:
                         out.append(f"K {row} {NT[b]} {self._stat_str(bases[b])}\n")
@@ -457,18 +452,25 @@ class Engine:
 
     def compute(self) -> Optional[Results]:
         self._check(self.lib.brc_compute(self.h))
+        return self._results()
+
+    def _results(self) -> Optional[Results]:
+        """The dense results of the last run; None while a site filter is set."""
         if getattr(self, "filtered", False):
             return None
         r = CResults()
         self._check(self.lib.brc_get_results(self.h, C.byref(r)))
-        res = Results(r)
-        res._per_lib = self.per_lib
-        return res
+        return Results(r)
 
     def warnings(self):
         out = (C.c_int64 * 4)()
         self._check(self.lib.brc_get_warning_counts(self.h, out))
         return tuple(int(x) for x in out)
+
+    def set_queue_carry(self, on: bool):
+        """Carry the argv deletion queue from one compute() to the next (brc_set_queue_carry), as the reference's never-cleared
+        queue does across argv regions; off, every compute() starts with an empty queue."""
+        self._check(self.lib.brc_set_queue_carry(self.h, int(on)))
 
     def format_text(self, region: int = -1) -> str:
         n = self.lib.brc_format_text(self.h, region, self._names_arr, None, 0)
@@ -497,13 +499,7 @@ class Engine:
 
     def fetch_device_results(self, stream_ptr: int) -> Optional[Results]:
         self._check(self.lib.brc_fetch_device_results(self.h, stream_ptr))
-        if getattr(self, "filtered", False):
-            return None
-        r = CResults()
-        self._check(self.lib.brc_get_results(self.h, C.byref(r)))
-        res = Results(r)
-        res._per_lib = self.per_lib
-        return res
+        return self._results()
 
     def packed(self) -> "PackedResults":
         r = CPackedResults()

@@ -18,6 +18,7 @@ import re
 
 import numpy as np
 
+import cases
 import edge_cases
 from bam_readcount_b200.batch import BatchBuilder
 
@@ -305,6 +306,44 @@ def queue_rows(seed=408):
     c = _case("queue_rows", ref, R.build(), regions, site_list=False, modes=(False,), n_libs=40, targets=["queue_rows"])
     c["probe"] = dict(anchors=(1099, 1399), low_anchors=(1699,))   # 0-based region ends: deletions only from rows >= 32 / < 32
     return c
+
+
+
+@functools.lru_cache(maxsize=None)
+def pool_case():
+    """About 3000 sites at depth 60 whose reads carry random bases: every site holds four or five base classes, so the secondary
+    pool needs several times the initial capacity brc_compute gives it."""
+    c = cases.synthetic_case(L=3500, depth=60, seed=61, regions=((0, 201, 3200),), site_list=True, n_libs=8)
+    b = c["batch"]
+    rng = np.random.default_rng(61)
+    codes = np.array([1, 2, 4, 8, 15], np.uint8)
+    nib_hi, nib_lo = rng.choice(codes, b.seq.shape[0]), rng.choice(codes, b.seq.shape[0])
+    b.seq = ((nib_hi << 4) | nib_lo).astype(np.uint8)
+    return dict(c, name="pool")
+
+
+def initial_pool_cap(case, flags, n_slots):
+    """The secondary pool's initial capacity in brc_compute: an eighth of the (row, site) cells, two records per indel op, 1024."""
+    b = case["batch"]
+    n_indel = int(np.isin(b.cigar & 0xF, (1, 2)).sum())
+    rows = len(case["lib_names"]) if flags.get("per_lib") else 1
+    return rows * n_slots // 8 + 2 * n_indel + 1024
+
+
+@functools.lru_cache(maxsize=None)
+def selection_cases():
+    """The site selection at scale: one argv region of 300 000 sites (more than 1024 scan partials) followed by adjacent and
+    overlapping ones; and 300 adjacent argv regions over 40 libraries with 1 % library-less reads."""
+    big = cases.synthetic_case(L=302000, depth=3, seed=71, n_libs=4,
+                               regions=((0, 1, 300000), (0, 300001, 300100), (0, 300050, 300200), (0, 300201, 300300)), site_list=False)
+    big = dict(big, name="sel_big")
+    many = cases.synthetic_case(L=14000, depth=40, seed=72, n_libs=40, regions=tuple((0, 1000 + 40 * k, 1039 + 40 * k) for k in range(300)),
+                                site_list=False)
+    b = many["batch"]
+    rng = np.random.default_rng(72)
+    b.lib = b.lib.copy()
+    b.lib[rng.random(b.n_reads) < 0.01] = 0xFFFF                # library-less reads
+    return big, dict(many, name="sel_40libs")
 
 
 # the flag sets every boundary case runs with

@@ -3,12 +3,23 @@
 A case is a dict: contigs [(name, length, ref_bytes, win_beg)], batch (all reads, file order),
 regions [(contig_index, beg1, end1)] in 1-based inclusive coordinates as a user would write
 them, ``site_list`` (True: -l loop, False: argv regions), flags, lib_names.
+
+The harness every parity test goes through: ``run_oracle`` / ``run_oracle_cached``, ``run_engine`` (one brc_compute over the
+case's regions) and ``run_engine_per_region`` (one per region, deletion queue carried), ``assert_same`` and ``first_diff`` to
+compare them, ``device_batch`` / ``run_device`` for the device-resident path, ``assert_anchor`` for the reference binary's
+SHA-256, and ``cli`` / ``samtools`` / ``inflate_check`` for the executables the tests run.
 """
 from __future__ import annotations
 
+import contextlib
+import dataclasses
 import gzip
+import hashlib
+import json
 import os
+import subprocess
 import sys
+from typing import NamedTuple, Optional
 
 import numpy as np
 
@@ -91,7 +102,13 @@ def region_reads(case, ci, beg1, end1):
     return tid, beg, end, case["batch"].select(idx)
 
 
-def run_oracle(case, flags, site_list=None):
+class OracleRun(NamedTuple):
+    text: str
+    dump: str
+    warnings: tuple
+
+
+def run_oracle(case, flags, site_list=None) -> OracleRun:
     from oracle.oracle import Oracle
     sl = case["site_list"] if site_list is None else site_list
     o = Oracle(lib_names=case["lib_names"], **flags)
@@ -99,35 +116,212 @@ def run_oracle(case, flags, site_list=None):
         name, clen, seq, wb = case["contigs"][ci]
         tid, beg, end, sub = region_reads(case, ci, b1, e1)
         o.region(sub, tid=tid, beg=beg, end=end, contig=name, chrom_len=clen, ref_seq=seq, ref_win_beg=wb, site_list_mode=sl)
-    return o.text(), o.dump(), o.warnings()
+    return OracleRun(o.text(), o.dump(), o.warnings())
 
 
-def run_engine(case, flags, site_list=None, want_dump=True):
-    from bam_readcount_b200.engine import Engine, admitted
+_ORACLE_RUNS: dict = {}
+
+
+def run_oracle_cached(case, flags, site_list=None) -> OracleRun:
+    """run_oracle, computed once per case name, flags and region mode (a case's name identifies it)."""
     sl = case["site_list"] if site_list is None else site_list
-    e = Engine(lib_names=case["lib_names"], **flags)
+    key = (case["name"], tuple(sorted(flags.items())), sl)
+    if key not in _ORACLE_RUNS:
+        _ORACLE_RUNS[key] = run_oracle(case, flags, site_list=sl)
+    return _ORACLE_RUNS[key]
+
+
+@dataclasses.dataclass
+class EngineRun:
+    """What one brc_compute left: the text, the raw accumulator dump ("" when not asked for or under a site filter), the warning
+    counters, the kernel launch count, the pool record count of packed() (-1 under a site filter) and, under a site filter, the
+    selected sites."""
+    text: str
+    dump: str
+    warnings: tuple
+    launches: int
+    n_sec: int
+    selected: object = None
+
+
+@contextlib.contextmanager
+def open_engine(case, flags=None):
+    """An engine with the case's libraries and the reference of every contig of the case."""
+    from bam_readcount_b200.engine import Engine
+    e = Engine(lib_names=case["lib_names"], **(flags or {}))
     try:
-        refs = {}
         for ci, (name, clen, seq, wb) in enumerate(case["contigs"]):
-            tid = case_tid(case, ci)
-            e.set_reference(tid, name, clen, seq, wb)
-            refs[tid] = (wb, seq)
-        pushed = []
-        for (ci, b1, e1) in case["regions"]:
-            tid, beg, end, sub = region_reads(case, ci, b1, e1)
-            e.begin_region(tid, beg, end, sl)
-            e.push_reads(sub)
-            e.end_region()
-            if want_dump:
-                pushed.append(sub.select(admitted(sub, tid, flags.get("max_cnt", 10_000_000))))
-        res = e.compute()
-        text = e.format_text(-1)
-        dump = res.dump(ReadBatch.concat(pushed), refs) if want_dump and pushed else ""
-        warn = e.warnings()
-        timing = (e.stage_ms(0), e.stage_ms(1))
-        return text, dump, warn, timing
+            e.set_reference(case_tid(case, ci), name, clen, seq, wb)
+        yield e
     finally:
         e.close()
+
+
+def push_regions(e, case, site_list, regions=None, push="one"):
+    """begin_region / push / end_region for each region (default: the case's).  ``push``: "one" pushes a region's reads at
+    once (borrowed by the engine), "halves" in two pushes (the engine copies them), a callable push(e, tid, beg, end, sub) as it
+    likes.  Returns (tid, reads) per region."""
+    pushed = []
+    for (ci, b1, e1) in case["regions"] if regions is None else regions:
+        tid, beg, end, sub = region_reads(case, ci, b1, e1)
+        e.begin_region(tid, beg, end, site_list)
+        if push == "one":
+            e.push_reads(sub)
+        elif push == "halves":
+            h = sub.n_reads // 2
+            e.push_reads(sub.select(np.arange(0, h)))
+            e.push_reads(sub.select(np.arange(h, sub.n_reads)))
+        else:
+            push(e, tid, beg, end, sub)
+        e.end_region()
+        pushed.append((tid, sub))
+    return pushed
+
+
+def _compute(e, case, flags, pushed, dump) -> EngineRun:
+    from bam_readcount_b200.engine import admitted
+    res = e.compute()
+    text = e.format_text(-1)
+    d = ""
+    if dump and res is not None and pushed:
+        cnt = flags.get("max_cnt", 10_000_000)
+        reads = ReadBatch.concat([sub.select(admitted(sub, tid, cnt)) for tid, sub in pushed])
+        d = res.dump(reads, {case_tid(case, ci): (wb, seq) for ci, (_, _, seq, wb) in enumerate(case["contigs"])})
+    return EngineRun(text=text, dump=d, warnings=e.warnings(), launches=e.launch_count(),
+                     n_sec=e.packed().n_sec if res is not None else -1, selected=e.selected() if res is None else None)
+
+
+def run_engine(case, flags, site_list=None, *, dump=True, site_filter=None, push="one") -> EngineRun:
+    """The case's regions as one batch, one brc_compute.  site_filter: (min_alt_count, min_alt_fraction); push: push_regions."""
+    sl = case["site_list"] if site_list is None else site_list
+    with open_engine(case, flags) as e:
+        if site_filter:
+            e.set_site_filter(*site_filter)
+        return _compute(e, case, flags, push_regions(e, case, sl, push=push), dump)
+
+
+def run_engine_per_region(case, flags, site_list=None, *, dump=False) -> list:
+    """One brc_compute per region with the deletion queue carried from one to the next (what brc-readcount does to bound its
+    memory): an EngineRun per region, whose texts joined are the output."""
+    sl = case["site_list"] if site_list is None else site_list
+    with open_engine(case, flags) as e:
+        e.set_queue_carry(True)
+        runs = []
+        for region in case["regions"]:
+            e.reset()
+            runs.append(_compute(e, case, flags, push_regions(e, case, sl, [region]), dump))
+        e.set_queue_carry(False)
+        return runs
+
+
+def first_diff(got: str, want: str) -> str:
+    """The first line where two texts differ (keeps pytest from diffing megabytes of text)."""
+    la, lb = got.splitlines(), want.splitlines()
+    for i, (x, y) in enumerate(zip(la, lb)):
+        if x != y:
+            return f"line {i}:\n got: {x[:300]}\nwant: {y[:300]}"
+    return f"length differs: got {len(la)} lines, want {len(lb)}"
+
+
+def assert_same(got: EngineRun, want: OracleRun, what: str = "", *, fields=("dump", "text", "warnings")):
+    """The engine run equals the oracle's in the named fields (warnings: the engine's counters 0, 1 and 3, the oracle's three)."""
+    pre = f"{what}: " if what else ""
+    if "dump" in fields:
+        assert got.dump == want.dump, pre + first_diff(got.dump, want.dump)
+    if "text" in fields:
+        assert got.text == want.text, pre + first_diff(got.text, want.text)
+    if "warnings" in fields:
+        w = got.warnings
+        assert (w[0], w[1], w[3]) == want.warnings, f"{pre}warnings {w}, oracle {want.warnings}"
+
+
+def region_geometry(case, region):
+    """(tid, beg, end, reads, first_pos, n_slots, n_tiles) of one region as brc_begin_region / brc_end_region form them."""
+    from kernel_model import kernel_constants
+    tile = kernel_constants()["TILE"]
+    tid, beg, end, sub = region_reads(case, *region)
+    first_pos = max(beg - 1, 0)
+    n_slots = max(0, min(end, int(sub.ref_end().max())) - first_pos) if sub.n_reads else 0
+    return tid, beg, end, sub, first_pos, n_slots, (n_slots + tile - 1) // tile
+
+
+_TORCH_VIEW = {np.dtype(np.uint16): np.int16, np.dtype(np.uint32): np.int32, np.dtype(np.uint64): np.int64}
+
+
+def device_batch(batch, device, *, lead=None, cigar_pool=None):
+    """The batch's arrays on the device: a CReadBatch of device pointers and the tensors that own them.  64 zero bytes follow
+    the base and quality pools.  lead=("qual" or "seq", n): that pool starts n bytes into an allocation whose first n bytes are
+    never written, its offsets shifted by n.  cigar_pool=(int32 tensor, n): the CIGAR ops are copied into the caller's tensor
+    at op n, their offsets shifted by n."""
+    import torch
+    from bam_readcount_b200.engine import CReadBatch
+    at = dict([lead]) if lead else {}
+    pool = None
+    if cigar_pool is not None:
+        pool, at["cigar"] = cigar_pool
+    keep = []
+
+    def dev(a, pad=0, start=0, into=None):
+        a = np.ascontiguousarray(a)
+        a = torch.from_numpy(a.view(_TORCH_VIEW.get(a.dtype, a.dtype)))
+        if into is None:
+            into = torch.empty(start + a.shape[0] + pad, dtype=a.dtype, device=device)
+            into[start + a.shape[0]:].zero_()
+            keep.append(into)
+        into[start:start + a.shape[0]].copy_(a)
+        return into.data_ptr()
+
+    def pool_at(name, pad=0, into=None):
+        off = getattr(batch, name + "_off").astype(np.uint64) + np.uint64(at.get(name, 0))
+        return [dev(off), dev(getattr(batch, name), pad, at.get(name, 0), into)]
+    b = batch
+    ptrs = [dev(b.tid), dev(b.pos), dev(b.flag), dev(b.mapq), dev(b.lib), dev(b.l_qseq), dev(b.nm), dev(b.sm)]
+    ptrs += pool_at("cigar", into=pool) + pool_at("seq", 64) + pool_at("qual", 64)
+    torch.cuda.synchronize(device)          # the engine reads them on a stream of its own
+    return CReadBatch(b.n_reads, *ptrs), keep
+
+
+def run_device(e, case, region, cbatch, stream, *, site_list=True, n_sec_cap=1 << 20) -> str:
+    """One region of the case, its reads already on the device (device_batch), through brc_plan_device / brc_run_device /
+    brc_fetch_device_results: the raw accumulator dump.  The device path admits every read it is given."""
+    from bam_readcount_b200.engine import CRegion
+    tid, beg, end, sub, first_pos, n_slots, _ = region_geometry(case, region)
+    e.plan_device([CRegion(tid, beg, end, int(site_list), 0, sub.n_reads, 0, first_pos, n_slots)], sub.n_reads, n_sec_cap)
+    e.run_device(cbatch, None, stream.cuda_stream)
+    res = e.fetch_device_results(stream.cuda_stream)
+    _, _, seq, wb = case["contigs"][region[0]]
+    return res.dump(sub, {tid: (wb, seq)})
+
+
+def assert_anchor(json_name: str, key: str, text: str):
+    """The oracle's text hashes to what the unmodified reference binary printed (tests/golden/<json_name>, make_golden.py)."""
+    with open(os.path.join(GOLDEN, json_name)) as fh:
+        want = json.load(fh)[key]
+    assert hashlib.sha256(text.encode("latin-1")).hexdigest() == want, f"{key}: oracle differs from the reference binary"
+
+
+def cli() -> str:
+    """Builds the engine library and brc-readcount; the path of brc-readcount."""
+    from bam_readcount_b200 import build
+    build.build()
+    return build.build_cli()
+
+
+def samtools() -> str:
+    """The samtools the oracle build leaves in oracle/_ref; skips the test without it."""
+    import pytest
+    from oracle.oracle import REF_SAMTOOLS
+    if not os.path.exists(REF_SAMTOOLS):
+        pytest.skip("oracle/_ref/samtools not built")
+    return REF_SAMTOOLS
+
+
+def inflate_check(workdir: str) -> str:
+    """Compiles tests/inflate_check.cpp (the device DEFLATE core against zlib, on the CPU) into workdir; the executable's path."""
+    exe = os.path.join(workdir, "inflate_check")
+    subprocess.check_call(["g++", "-O2", "-std=c++17", "-I", os.path.join(ROOT, "bam_readcount_b200", "csrc"), "-o", exe,
+                           os.path.join(ROOT, "tests", "inflate_check.cpp"), "-lz"])
+    return exe
 
 
 def load_golden_text(name: str) -> str:

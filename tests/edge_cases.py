@@ -225,3 +225,14 @@ def all_cases():
     return [fuzz_case(3, name="fuzz_a"), fuzz_case(17, L=500, n_reads=400, name="fuzz_b"),
             fuzz_case(23, name="fuzz_plib", per_lib_safe=True), fuzz_case(29, name="fuzz_nolib", per_lib_safe=False, overhang=False, force_perlib=True),
             multi_allele_case()]
+
+
+# the fresh-fuzz seeds: cases of their own, not the ones above (tests/test_differential_fuzz.py, make_golden.py)
+FRESH_SEEDS = (101, 102, 103, 104, 105, 106)
+
+
+def fresh_fuzz_case(seed):
+    rng = np.random.default_rng(seed)
+    safe = bool(seed % 2)
+    return fuzz_case(seed, L=int(rng.integers(300, 700)), n_reads=int(rng.integers(150, 380)), name=f"fresh{seed}",
+                     per_lib_safe=safe, n_libs=int(rng.integers(1, 6)), overhang=bool(seed % 3), force_perlib=not safe)

@@ -120,7 +120,7 @@ def reference_stdout(case, flags, d, site_list):
 
 def fresh_fuzz_jobs():
     """The fuzz cases of tests/test_differential_fuzz.py, run as site lists."""
-    from test_differential_fuzz import SEEDS, _case
+    from edge_cases import FRESH_SEEDS as SEEDS, fresh_fuzz_case as _case
     jobs = []
     for seed in SEEDS:
         fc = _case(seed)

@@ -22,7 +22,6 @@ import pytest
 import bam_craft
 import cases
 from bam_readcount_b200 import bamio
-from oracle.oracle import REF_SAMTOOLS
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden")
@@ -33,10 +32,9 @@ NAMES = ["cg", "dtag", "nmtype", "rg", "rg_nolib", "trunc", "long"]
 
 @pytest.fixture(scope="module")
 def corpus(tmp_path_factory):
-    if not os.path.exists(REF_SAMTOOLS):
-        pytest.skip("oracle/_ref/samtools not built")
+    samtools = cases.samtools()
     d = str(tmp_path_factory.mktemp("craft"))
-    files = bam_craft.write_corpus(d, REF_SAMTOOLS)
+    files = bam_craft.write_corpus(d, samtools)
     return {f["name"]: dict(f, restated=None if f["bam"].endswith(".cram") else bam_craft.Restated(f["bam"])) for f in files}
 
 
@@ -130,12 +128,7 @@ RECUTS = [("level", 0), ("level", 1), ("level", 9), ("strategy", zlib.Z_FILTERED
 def test_deflate_core_on_the_recut_corpus(corpus, tmp_path):
     """The DEFLATE core of the device kernel (one lane, on the CPU) against zlib on every member of every recut file, and its
     refusal of each member cut in half."""
-    from test_bgzf_device import HARNESS
-    src = os.path.join(str(tmp_path), "h.cpp")
-    with open(src, "w") as fh:
-        fh.write(HARNESS)
-    exe = os.path.join(str(tmp_path), "h")
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-I", os.path.join(ROOT, "bam_readcount_b200", "csrc"), "-o", exe, src, "-lz"])
+    exe = cases.inflate_check(str(tmp_path))
     files = [_recut(corpus[n], how) for n in ("cg", "long") for how in RECUTS]
     nblk, bad = map(int, subprocess.check_output([exe] + files).split())
     assert bad == 0 and nblk > 100
@@ -163,12 +156,7 @@ def test_deflate_corpus_covers_every_construct(crafted):
 def test_deflate_core_on_the_crafted_members(crafted, tmp_path):
     """The DEFLATE core (one lane, on the CPU) against zlib on every crafted member, and its refusal of each member cut in half;
     bamio and the restatement read the same records from both crafted files."""
-    from test_bgzf_device import HARNESS
-    src = os.path.join(str(tmp_path), "h.cpp")
-    with open(src, "w") as fh:
-        fh.write(HARNESS)
-    exe = os.path.join(str(tmp_path), "h")
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-I", os.path.join(ROOT, "bam_readcount_b200", "csrc"), "-o", exe, src, "-lz"])
+    exe = cases.inflate_check(str(tmp_path))
     nblk, bad = map(int, subprocess.check_output([exe, crafted["deflate"]]).split())
     assert bad == 0 and nblk >= 8
     for path in (crafted["deflate"], crafted["frame"]):
@@ -273,25 +261,10 @@ def test_device_decode_equals_restatement(corpus):
 
 def _engine_text(f, host, regions, span=False, flags=None):
     """Engine text over argv regions: the reads bamio decoded, or (one region only) the file's compressed span."""
-    from bam_readcount_b200.engine import Engine
-    r = f["restated"]
-    case = _case(f, host)
-    e = Engine(lib_names=case["lib_names"], **(flags or {}))
-    try:
-        name, clen, seq, wb = case["contigs"][0]
-        e.set_reference(0, name, clen, seq, wb)
-        for (_, b1, e1) in regions:
-            tid, beg, end, sub = cases.region_reads(case, 0, b1, e1)
-            e.begin_region(tid, beg, end, False)
-            if span:
-                e.push_bam_span(bamio.bam_span(f["bam"], bamio.BaiIndex(f["bam"] + ".bai"), 0, beg - 1, end, r.rg_lib()))
-            else:
-                e.push_reads(sub)
-            e.end_region()
-        e.compute()
-        return e.format_text(-1)
-    finally:
-        e.close()
+    def push_span(e, tid, beg, end, sub):
+        e.push_bam_span(bamio.bam_span(f["bam"], bamio.BaiIndex(f["bam"] + ".bai"), 0, beg - 1, end, f["restated"].rg_lib()))
+    case = dict(_case(f, host), regions=regions)
+    return cases.run_engine(case, flags or {}, dump=False, push=push_span if span else "one").text
 
 
 @pytest.mark.gpu
@@ -314,9 +287,8 @@ def test_reads_and_span_equal_the_reference(corpus, fname, monkeypatch):
                 assert _engine_text(f, host, [reg], span=True, flags=FLAGS[fname]) == _engine_text(f, host, [reg], flags=FLAGS[fname]), (name, reg, deep)
             monkeypatch.delenv("BRC_DEEP_MIN_READS", raising=False)
         # text, raw accumulators and warning counts: engine on bamio's reads == oracle on the restatement's reads
-        etext, edump, ewarn, _ = cases.run_engine(_case(f, host), FLAGS[fname])
-        otext, odump, owarn = cases.run_oracle(_case(f, f["restated"].batch), FLAGS[fname])
-        assert (etext, edump) == (otext, odump) and (ewarn[0], ewarn[1], ewarn[3]) == owarn, name
+        cases.assert_same(cases.run_engine(_case(f, host), FLAGS[fname]), cases.run_oracle(_case(f, f["restated"].batch), FLAGS[fname]),
+                          name)
 
 
 @pytest.mark.gpu
@@ -327,7 +299,7 @@ def test_cli_reads_unwalkable_aux_as_the_restatement_does(corpus, fname):
     from bam_readcount_b200 import build
     exe = build.build_cli()
     f = corpus["trunc"]
-    want, _, _, _ = cases.run_engine(_case(f, f["restated"].batch), FLAGS[fname])
+    want = cases.run_engine(_case(f, f["restated"].batch), FLAGS[fname]).text
     args = [exe, "-w", "0"] + bam_craft.FLAG_SETS[fname] + ["-f", f["fasta"], f["bam"]] + f["regions"]
     host = subprocess.run(args, capture_output=True)
     dev = subprocess.run(args, capture_output=True, env=dict(os.environ, BRC_CLI_DEVICE_DECODE="1"))

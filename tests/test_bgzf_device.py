@@ -16,47 +16,9 @@ from bam_readcount_b200 import bamio
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden")
 
-HARNESS = r'''
-#include <cstdio>
-#include <cstring>
-#include <vector>
-#include <zlib.h>
-#include "brc_bgzf.cuh"
-int main(int argc, char **argv) {
-    int bad = 0, nblk = 0;
-    for (int a = 1; a < argc; ++a) {
-        FILE *f = fopen(argv[a], "rb"); std::vector<uint8_t> d; uint8_t buf[65536]; size_t n;
-        while ((n = fread(buf, 1, sizeof buf, f)) > 0) d.insert(d.end(), buf, buf + n);
-        fclose(f);
-        size_t o = 0; static brc::inflate::Tables T;
-        while (o + 18 <= d.size()) {
-            const uint8_t *h = &d[o]; if (h[0] != 31 || h[1] != 139) break;
-            size_t xlen = h[10] | (h[11] << 8); int bsize = -1;
-            for (size_t i = 0; i + 4 <= xlen;) { size_t sl = h[12 + i + 2] | (h[12 + i + 3] << 8); if (h[12 + i] == 'B' && h[12 + i + 1] == 'C') bsize = h[12 + i + 4] | (h[12 + i + 5] << 8); i += 4 + sl; }
-            size_t total = bsize + 1, hdr = 12 + xlen; const uint8_t *tail = h + total - 4;
-            uint32_t isize = tail[0] | (tail[1] << 8) | (tail[2] << 16) | ((uint32_t)tail[3] << 24);
-            std::vector<uint8_t> want(isize + 1), got(isize + 1);
-            z_stream zs{}; inflateInit2(&zs, -15); zs.next_in = (Bytef *)h + hdr; zs.avail_in = total - hdr - 8; zs.next_out = want.data(); zs.avail_out = isize;
-            int rc = inflate(&zs, Z_FINISH); inflateEnd(&zs);
-            int r = brc::inflate::inflate_block(brc::inflate::Lanes{0, 1}, h + hdr, total - hdr - 8, got.data(), isize, T);
-            if (r != 0 || memcmp(want.data(), got.data(), isize) || (isize && rc != Z_STREAM_END)) ++bad;
-            // a truncated stream must be refused, not over-read
-            if (isize > 100 && brc::inflate::inflate_block(brc::inflate::Lanes{0, 1}, h + hdr, (total - hdr - 8) / 2, got.data(), isize, T) == 0) ++bad;
-            ++nblk; o += total;
-        }
-    }
-    printf("%d %d\n", nblk, bad);
-    return bad != 0;
-}
-'''
-
-
 def test_deflate_core_matches_zlib_on_every_block(tmp_path):
     """The exact DEFLATE code the kernel runs (host+device source), block by block against zlib: dynamic, fixed and stored blocks."""
-    src = os.path.join(str(tmp_path), "h.cpp")
-    open(src, "w").write(HARNESS)
-    exe = os.path.join(str(tmp_path), "h")
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-I", os.path.join(ROOT, "bam_readcount_b200", "csrc"), "-o", exe, src, "-lz"])
+    exe = cases.inflate_check(str(tmp_path))
     files = [os.path.join(GOLDEN, "test.bam"), os.path.join(GOLDEN, "test_bad_rg.bam")]
     from oracle.oracle import REF_SAMTOOLS
     if os.path.exists(REF_SAMTOOLS):
@@ -123,47 +85,31 @@ def test_device_decoded_batch_equals_host_decoder():
 @pytest.mark.parametrize("flags", [dict(), dict(per_lib=True, insertion_centric=True, min_mapq=10, min_bq=15)])
 def test_region_from_compressed_span_equals_region_from_host_reads(flags):
     """brc_push_bam_span (inflate + framing + kernels, reads never on the host) == brc_push_reads of the host-decoded records."""
-    from bam_readcount_b200.engine import Engine
-    from oracle.oracle import REF_SAMTOOLS
-    if not os.path.exists(REF_SAMTOOLS):
-        pytest.skip("oracle/_ref/samtools not built")
+    samtools = cases.samtools()
     from bam_readcount_b200 import synth_cb
     tmp = tempfile.mkdtemp()
     sp = synth_cb.Spec(seed=12, contig_len=1280 * 600)
-    info = synth_cb.write_sample_bam(sp, 0, 0, 600, tmp, REF_SAMTOOLS)
+    info = synth_cb.write_sample_bam(sp, 0, 0, 600, tmp, samtools)
     hdr, host = bamio.read_bam(info["bam"])
-    libs = hdr.lib_names
     rg_lib = {rg: hdr.lib_of_rg(rg) for rg in hdr.rg_lb}
-    ref = sp.ref_host(0, 0, info["length"])
     beg, end = 100_000, 700_000
-    texts = []
-    for mode in ("host", "span"):
-        e = Engine(lib_names=libs, **flags)
-        try:
-            e.set_reference(0, "chr1", info["length"], ref, 0)
-            e.begin_region(0, beg, end, False)
-            if mode == "host":
-                e.push_reads(host.select(host.fetch(0, beg - 1, end)))
-            else:
-                e.push_bam_span(bamio.bam_span(info["bam"], bamio.BaiIndex(info["bam"] + ".bai"), 0, beg - 1, end, rg_lib))
-            e.end_region()
-            e.compute()
-            texts.append(e.format_text(-1))
-        finally:
-            e.close()
+    case = dict(name="span", contigs=[("chr1", info["length"], sp.ref_host(0, 0, info["length"]), 0)], batch=host,
+                regions=[(0, beg + 1, end)], site_list=False, lib_names=hdr.lib_names)
+
+    def push_span(e, tid, beg, end, sub):
+        e.push_bam_span(bamio.bam_span(info["bam"], bamio.BaiIndex(info["bam"] + ".bai"), 0, beg - 1, end, rg_lib))
+    texts = [cases.run_engine(case, flags, dump=False, push=push).text for push in ("one", push_span)]
     assert texts[0] == texts[1] and len(texts[0].splitlines()) == end - beg
 
 
 @pytest.mark.gpu
 def test_cli_device_decode_matches_host_decode(tmp_path):
     """brc-readcount with BRC_CLI_DEVICE_DECODE=1 (compressed spans -> GPU inflate/framing) prints what the host-decode path prints."""
-    from oracle.oracle import REF_SAMTOOLS
-    if not os.path.exists(REF_SAMTOOLS):
-        pytest.skip("oracle/_ref/samtools not built")
+    samtools = cases.samtools()
     from bam_readcount_b200 import build, synth_cb
     exe = build.build_cli()
     sp = synth_cb.Spec(seed=21, contig_len=1280 * 500)
-    info = synth_cb.write_sample_bam(sp, 0, 0, 500, str(tmp_path), REF_SAMTOOLS)
+    info = synth_cb.write_sample_bam(sp, 0, 0, 500, str(tmp_path), samtools)
     for extra in ([], ["-p", "-q", "20", "-b", "20"]):
         args = [exe, "-w", "0"] + extra + ["-f", info["fasta"], info["bam"], "chr1:5001-600000"]
         env = dict(os.environ, BRC_CLI_WINDOW="150000")

@@ -9,15 +9,12 @@ import numpy as np
 import pytest
 
 import cases
+from cases import cli as _cli
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
-def _cli():
-    from bam_readcount_b200 import build
-    build.build()
-    return build.build_cli()
 
 
 def test_cli_help_and_version_exit_code_1():
@@ -73,9 +70,7 @@ def test_cli_reproduces_reference_goldens(tmp_path, args, bam, golden):
 def test_cli_synthetic_bam_matches_oracle(tmp_path):
     """A coordinate-sorted synthetic BAM (written with the samtools the oracle build leaves in oracle/_ref) through the
     CLI, whole-contig region and a site list, against the CPU oracle."""
-    from oracle.oracle import REF_SAMTOOLS
-    if not os.path.exists(REF_SAMTOOLS):
-        pytest.skip("oracle/_ref/samtools not built")
+    REF_SAMTOOLS = cases.samtools()
     from bam_readcount_b200 import synth
     exe = _cli()
     case = cases.synthetic_case(L=40000, depth=30, seed=31, regions=((0, 1001, 38000),), site_list=False)
@@ -96,9 +91,7 @@ def test_cli_synthetic_bam_matches_oracle(tmp_path):
 def test_cli_windowed_long_region_equals_unsplit(tmp_path):
     """brc-readcount cuts long regions into windows (bounded memory); the concatenation must equal the unsplit output,
     deletions across window edges included."""
-    from oracle.oracle import REF_SAMTOOLS
-    if not os.path.exists(REF_SAMTOOLS):
-        pytest.skip("oracle/_ref/samtools not built")
+    REF_SAMTOOLS = cases.samtools()
     from bam_readcount_b200 import synth
     exe = _cli()
     case = cases.synthetic_case(L=30000, depth=30, seed=41, regions=((0, 1, 30000),), site_list=False)
@@ -164,9 +157,7 @@ def test_cli_site_list_fetch_merging_yields_samfetch_records_in_one_pass(tmp_pat
     """CPU (SURVEY.md §8 f-3): consecutive site-list lines share one forward pass over the BAM instead of one index seek
     each; every region must still receive exactly the records samfetch yields (checked against the Python decoder), and the
     fetch must seek and decode about as little as one pass over the file."""
-    from oracle.oracle import REF_SAMTOOLS
-    if not os.path.exists(REF_SAMTOOLS):
-        pytest.skip("oracle/_ref/samtools not built")
+    REF_SAMTOOLS = cases.samtools()
     exe = _cli()
     case = cases.synthetic_case(L=60000, depth=30, seed=77, regions=((0, 1, 60000),), site_list=True)
     bam, _ = _make_bam(case, str(tmp_path))
@@ -196,9 +187,7 @@ def test_cli_site_list_fetch_merging_yields_samfetch_records_in_one_pass(tmp_pat
 def test_cli_dense_site_list_matches_oracle(tmp_path):
     """A few hundred site-list lines (dense, overlapping, nested, repeated, out of order) through the merged fetch, the
     engine and the emitter, against the CPU oracle run region by region like the reference's -l loop."""
-    from oracle.oracle import REF_SAMTOOLS
-    if not os.path.exists(REF_SAMTOOLS):
-        pytest.skip("oracle/_ref/samtools not built")
+    REF_SAMTOOLS = cases.samtools()
     exe = _cli()
     regs = _site_list_regions(60000, np.random.default_rng(5))
     case = cases.synthetic_case(L=60000, depth=30, seed=77, regions=tuple((0, s, e) for s, e in regs), site_list=True)
@@ -215,9 +204,7 @@ def test_cli_dense_site_list_matches_oracle(tmp_path):
 def test_cli_fetch_merging_two_contigs_unsorted_and_past_the_end(tmp_path):
     """CPU: the merged fetch across contig changes, lines that go backwards, duplicates, a line past the contig's last read
     and an unknown contig — record sets identical to the Python decoder's samfetch."""
-    from oracle.oracle import REF_SAMTOOLS
-    if not os.path.exists(REF_SAMTOOLS):
-        pytest.skip("oracle/_ref/samtools not built")
+    REF_SAMTOOLS = cases.samtools()
     import dataclasses
     from bam_readcount_b200 import synth
     from bam_readcount_b200.batch import ReadBatch
@@ -408,9 +395,7 @@ def test_cli_cram_config_2b_matches_reference_output():
 
 def test_cli_shards_partition_the_regions(tmp_path):
     """--shard RANK/COUNT: the ranks' units are a partition of the windowed regions, in order (decode-only, no device)."""
-    from oracle.oracle import REF_SAMTOOLS
-    if not os.path.exists(REF_SAMTOOLS):
-        pytest.skip("oracle/_ref/samtools not built")
+    REF_SAMTOOLS = cases.samtools()
     from bam_readcount_b200 import synth_cb
     exe = _cli()
     sp = synth_cb.Spec(seed=3, contig_len=1280 * 400)
@@ -430,9 +415,7 @@ def test_cli_shards_partition_the_regions(tmp_path):
 
 @pytest.mark.gpu
 def test_cli_sharded_output_concatenates_to_the_unsharded_output(tmp_path):
-    from oracle.oracle import REF_SAMTOOLS
-    if not os.path.exists(REF_SAMTOOLS):
-        pytest.skip("oracle/_ref/samtools not built")
+    REF_SAMTOOLS = cases.samtools()
     from bam_readcount_b200 import synth_cb
     exe = _cli()
     sp = synth_cb.Spec(seed=8, contig_len=1280 * 300)
@@ -458,9 +441,7 @@ def test_cli_parallel_window_decode_yields_python_decoder_records(tmp_path):
     """Big fetches are decoded by several threads over position sub-ranges (ParallelFetcher) and concatenated: record count,
     position sum and quality sum per region must equal the Python decoder's samfetch, whatever the thread count and window size.
     A region under 256 kb takes the record stream instead (decode-only, no device)."""
-    from oracle.oracle import REF_SAMTOOLS
-    if not os.path.exists(REF_SAMTOOLS):
-        pytest.skip("oracle/_ref/samtools not built")
+    REF_SAMTOOLS = cases.samtools()
     from bam_readcount_b200 import synth_cb
     from bam_readcount_b200.bamio import read_bam
     exe = _cli()
@@ -545,9 +526,7 @@ def test_cli_parallel_window_decode_two_contigs_unmapped_and_edges(tmp_path):
     """CPU: the parallel window decode on a two-contig BAM with placed-but-unmapped records, a fetch that starts inside a read,
     a fetch past the last read, a site-list line long enough to be cut into windows, and a contig without reads behind it:
     per-region (count, position sum, quality sum) identical to the Python decoder's samfetch, uncut and cut into windows."""
-    from oracle.oracle import REF_SAMTOOLS
-    if not os.path.exists(REF_SAMTOOLS):
-        pytest.skip("oracle/_ref/samtools not built")
+    REF_SAMTOOLS = cases.samtools()
     import dataclasses
     from bam_readcount_b200 import synth
     from bam_readcount_b200.batch import ReadBatch

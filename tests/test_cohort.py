@@ -11,6 +11,8 @@ import numpy as np
 import pytest
 
 import cases
+from cases import cli as _cli
+from cases import samtools as _samtools
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden")
@@ -18,17 +20,6 @@ CRAM_DATA = os.path.join(ROOT, "oracle", "_ref", "test-data")
 CONTIGS = {"chrA": (24000, 11), "chrB": (16000, 12), "chrC": (12000, 13)}       # name -> (length, reference seed)
 
 
-def _cli():
-    from bam_readcount_b200 import build
-    build.build()
-    return build.build_cli()
-
-
-def _samtools():
-    from oracle.oracle import REF_SAMTOOLS
-    if not os.path.exists(REF_SAMTOOLS):
-        pytest.skip("oracle/_ref/samtools not built")
-    return REF_SAMTOOLS
 
 
 def _have_htslib(exe):

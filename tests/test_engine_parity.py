@@ -13,23 +13,16 @@ import golden_jobs
 pytestmark = pytest.mark.gpu
 
 JOBS = golden_jobs.jobs()
-
-
-def _first_diff(a: str, b: str) -> str:
-    la, lb = a.splitlines(), b.splitlines()
-    for i, (x, y) in enumerate(zip(la, lb)):
-        if x != y:
-            return f"line {i}:\n got: {x[:400]}\nwant: {y[:400]}"
-    return f"length differs: got {len(la)} lines, want {len(lb)}"
+first_diff = cases.first_diff
 
 
 @pytest.mark.parametrize("job", JOBS, ids=[j[0] for j in JOBS])
 def test_engine_text_matches_reference_golden(job):
     _, getter, flags, site_list, golden = job
     case = getter()
-    text, _, _, _ = cases.run_engine(case, flags, site_list=site_list, want_dump=False)
+    text = cases.run_engine(case, flags, site_list=site_list, dump=False).text
     want = cases.load_golden_text(golden)
-    assert text == want, _first_diff(text, want)
+    assert text == want, first_diff(text, want)
 
 
 @pytest.mark.parametrize("job", JOBS, ids=[j[0] for j in JOBS])
@@ -37,10 +30,8 @@ def test_engine_accumulators_match_oracle_bit_exact(job):
     _, getter, flags, _, _ = job
     case = getter()
     # site-list semantics for both (fresh deletion queue per region) so the raw dumps are comparable
-    _, odump, owarn = cases.run_oracle(case, flags, site_list=True)
-    _, edump, ewarn, _ = cases.run_engine(case, flags, site_list=True, want_dump=True)
-    assert edump == odump, _first_diff(edump, odump)
-    assert (ewarn[0], ewarn[1], ewarn[3]) == owarn
+    cases.assert_same(cases.run_engine(case, flags, site_list=True), cases.run_oracle(case, flags, site_list=True),
+                      fields=("dump", "warnings"))
 
 
 @pytest.mark.parametrize("job", JOBS, ids=[j[0] for j in JOBS])
@@ -51,25 +42,22 @@ def test_deep_site_kernel_matches_oracle_bit_exact(job, monkeypatch):
     monkeypatch.setenv("BRC_DEEP_MIN_READS", "1")
     _, getter, flags, site_list, golden = job
     case = getter()
-    _, odump, owarn = cases.run_oracle(case, flags, site_list=True)
-    _, edump, ewarn, _ = cases.run_engine(case, flags, site_list=True, want_dump=True)
-    assert edump == odump, _first_diff(edump, odump)
-    assert (ewarn[0], ewarn[1], ewarn[3]) == owarn
-    text, _, _, _ = cases.run_engine(case, flags, site_list=site_list, want_dump=False)
+    cases.assert_same(cases.run_engine(case, flags, site_list=True), cases.run_oracle(case, flags, site_list=True),
+                      fields=("dump", "warnings"))
+    text = cases.run_engine(case, flags, site_list=site_list, dump=False).text
     want = cases.load_golden_text(golden)
-    assert text == want, _first_diff(text, want)
+    assert text == want, first_diff(text, want)
 
 
 def test_deep_site_kernel_is_what_runs_on_a_deep_panel(monkeypatch):
     """50 000x on one site, 8 libraries: identical results with the deep-site kernel (default) and with it disabled."""
     case = cases.deep_case(n_sites=2, depth=20000, seed=9)
     fl = dict(per_lib=True, max_cnt=100000000)
-    _, d1, w1, _ = cases.run_engine(case, fl, site_list=True, want_dump=True)
+    r1 = cases.run_engine(case, fl, site_list=True)
     monkeypatch.setenv("BRC_DEEP_MIN_READS", "2147483647")
-    _, d2, w2, _ = cases.run_engine(case, fl, site_list=True, want_dump=True)
-    assert d1 == d2 and tuple(w1) == tuple(w2)
-    _, od, _ = cases.run_oracle(case, fl, site_list=True)
-    assert d1 == od
+    r2 = cases.run_engine(case, fl, site_list=True)
+    assert r1.dump == r2.dump and tuple(r1.warnings) == tuple(r2.warnings)
+    assert r1.dump == cases.run_oracle(case, fl, site_list=True).dump
 
 
 @pytest.mark.parametrize("n_libs", [12, 19])
@@ -78,13 +66,10 @@ def test_deep_site_kernel_with_more_than_eight_libraries(n_libs, monkeypatch):
     (grid.y batches of 8), each streaming the tile's reads; identical to the oracle and to pileup_kernel."""
     case = cases.deep_case(n_sites=2, depth=3000, seed=13, n_libs=n_libs)
     fl = dict(per_lib=True, max_cnt=100000000, min_bq=10)
-    _, d1, w1, _ = cases.run_engine(case, fl, site_list=True, want_dump=True)
-    _, od, ow = cases.run_oracle(case, fl, site_list=True)
-    assert d1 == od, _first_diff(d1, od)
-    assert (w1[0], w1[1], w1[3]) == ow
+    want = cases.run_oracle(case, fl, site_list=True)
+    cases.assert_same(cases.run_engine(case, fl, site_list=True), want, fields=("dump", "warnings"))
     monkeypatch.setenv("BRC_DEEP_MIN_READS", "2147483647")
-    _, d2, _, _ = cases.run_engine(case, fl, site_list=True, want_dump=True)
-    assert d2 == od
+    assert cases.run_engine(case, fl, site_list=True).dump == want.dump
 
 
 def test_exact_arithmetic_shortcuts_match_ieee_intrinsics():
@@ -126,27 +111,9 @@ def test_sharded_engine_equals_unsharded():
 
 def test_borrowed_and_copied_batches_agree():
     """brc_push_reads borrows a fully-admitted batch (zero-copy) and copies otherwise; both must give the same result."""
-    from bam_readcount_b200.engine import Engine
     case = cases.synthetic_case(L=6000, depth=30, seed=4, regions=((0, 1, 6000),))
-    name, clen, seq, wb = case["contigs"][0]
-    b = case["batch"]
-    outs = []
-    for split in (False, True):
-        eng = Engine(min_mapq=20)
-        try:
-            eng.set_reference(0, name, clen, seq, wb)
-            eng.begin_region(0, 0, 6000, False)
-            if split:   # two pushes into one region: the first is borrowed, then materialised when the second arrives
-                h = b.n_reads // 2
-                eng.push_reads(b.select(range(0, h)))
-                eng.push_reads(b.select(range(h, b.n_reads)))
-            else:
-                eng.push_reads(b)
-            eng.end_region()
-            eng.compute()
-            outs.append(eng.format_text())
-        finally:
-            eng.close()
+    # two pushes into one region: the first is borrowed, then materialised when the second arrives
+    outs = [cases.run_engine(case, dict(min_mapq=20), site_list=False, dump=False, push=push).text for push in ("one", "halves")]
     assert outs[0] == outs[1] and len(outs[0]) > 100000
 
 
@@ -156,10 +123,8 @@ def test_pipelined_push_path_many_chunks(monkeypatch):
     monkeypatch.setenv("BRC_PIPE_CHUNKS", "7")
     case = cases.synthetic_case(L=20000, depth=30, seed=13, regions=((0, 1, 20000),), site_list=False)
     for flags in (dict(), dict(per_lib=True, insertion_centric=True, min_mapq=20, min_bq=20)):
-        otext, odump, _ = cases.run_oracle(case, flags, site_list=True)
-        etext, edump, _, _ = cases.run_engine(case, flags, site_list=True)
-        assert etext == otext
-        assert edump == odump
+        cases.assert_same(cases.run_engine(case, flags, site_list=True), cases.run_oracle(case, flags, site_list=True),
+                          fields=("dump", "text"))
 
 
 def _long_read_case(seed=77, L=120000):
@@ -191,10 +156,8 @@ def _long_read_case(seed=77, L=120000):
 def test_long_reads_exact_slow_paths():
     case = _long_read_case()
     for flags in (dict(), dict(per_lib=True, min_mapq=20, min_bq=20)):
-        otext, odump, owarn = cases.run_oracle(case, flags, site_list=True)
-        etext, edump, ewarn, _ = cases.run_engine(case, flags, site_list=True)
-        assert etext == otext, _first_diff(etext, otext)
-        assert edump == odump, _first_diff(edump, odump)
+        cases.assert_same(cases.run_engine(case, flags, site_list=True), cases.run_oracle(case, flags, site_list=True),
+                          fields=("dump", "text"))
 
 
 def test_two_contigs_and_empty_region_in_one_batch():
@@ -214,10 +177,8 @@ def test_two_contigs_and_empty_region_in_one_batch():
                 lib_names=a["lib_names"])
     # make the tail of contig 1 read-free: region (0, 7990, 8000) has no reads (synth reads stop at L-153)
     for flags in (dict(insertion_centric=True), dict(per_lib=True)):
-        otext, odump, _ = cases.run_oracle(case, flags, site_list=True)
-        etext, edump, _, _ = cases.run_engine(case, flags, site_list=True)
-        assert etext == otext, _first_diff(etext, otext)
-        assert edump == odump, _first_diff(edump, odump)
+        cases.assert_same(cases.run_engine(case, flags, site_list=True), cases.run_oracle(case, flags, site_list=True),
+                          fields=("dump", "text"))
     _ = gap
 
 
@@ -250,29 +211,11 @@ def test_carried_deletion_queue_equals_one_batch():
     what the same regions print as ONE batch — the reference's never-cleared deletion queue (R:bamreadcount.cpp:650-656) travels
     with the engine — and exactly what the reference binary printed (golden edge_alleles_*)."""
     import edge_cases
-    from bam_readcount_b200.engine import Engine
     case = edge_cases.multi_allele_case()
     for fl_name, fl in case["flag_sets"].items():
-        one, _, _, _ = cases.run_engine(case, fl, site_list=False, want_dump=False)
-        e = Engine(lib_names=case["lib_names"], **fl)
-        try:
-            name, clen, seq, wb = case["contigs"][0]
-            e.set_reference(0, name, clen, seq, wb)
-            assert e.lib.brc_set_queue_carry(e.h, 1) == 0
-            parts = []
-            for (ci, b1, e1) in case["regions"]:
-                tid, beg, end, sub = cases.region_reads(case, ci, b1, e1)
-                e.reset()
-                e.begin_region(tid, beg, end, False)
-                e.push_reads(sub)
-                e.end_region()
-                e.compute()
-                parts.append(e.format_text(-1))
-            assert "".join(parts) == one, fl_name
-            # carry off again: a fresh queue per call
-            assert e.lib.brc_set_queue_carry(e.h, 0) == 0
-        finally:
-            e.close()
+        one = cases.run_engine(case, fl, site_list=False, dump=False).text
+        # run_engine_per_region turns the carry off again at the end: a fresh queue per call
+        assert "".join(r.text for r in cases.run_engine_per_region(case, fl, site_list=False)) == one, fl_name
         assert one == cases.load_golden_text(f"edge_alleles_{fl_name}.txt")
 
 
@@ -313,7 +256,7 @@ def test_two_handles_driven_from_two_threads():
     for i in range(2):
         assert len(outs[i]) == 3 and len(alone[i][0]) > 100000
         for rep in range(3):
-            assert outs[i][rep] == alone[i][0], (i, rep, _first_diff(outs[i][rep], alone[i][0]))
+            assert outs[i][rep] == alone[i][0], (i, rep, first_diff(outs[i][rep], alone[i][0]))
 
 
 def test_h2d_byte_report_counts_what_crossed_pcie(monkeypatch):

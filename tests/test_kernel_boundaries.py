@@ -11,9 +11,6 @@ GPU
   the engine against the oracle on every case and flag set (raw accumulators, text, warning counters), forced through the
   deep-site kernel, as one borrowed push and as two pushes; the reciprocal-division self-test over every hot-path numerator;
   secondary-pool growth; the site selection at scale."""
-import functools
-import hashlib
-import json
 import os
 import re
 
@@ -22,39 +19,14 @@ import pytest
 
 import boundary_cases
 import cases
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CSRC = os.path.join(ROOT, "bam_readcount_b200", "csrc")
-GOLDEN = os.path.join(ROOT, "tests", "golden")
-
-_CONST_NAMES = ("TILE", "STAGE_READS", "STAGE_QUAL", "STAGE_SEQ", "STAGE_CIGAR", "K0_READS", "K0_QUAL_CAP", "K0_SEQ_CAP", "K0_REF_CAP",
-                "FASTDIV_MAX", "DEEP_THREADS", "DEEP_ICACHE", "SEL_LAST_ROWS", "SCAN_CTA")
-
-
-@functools.lru_cache(maxsize=None)
-def kernel_constants():
-    """constexpr int NAME = <expression over earlier names>; from csrc/ (BRC_STAGE_READS from its #define)."""
-    src = "".join(open(os.path.join(CSRC, f)).read() for f in sorted(os.listdir(CSRC)) if f.endswith((".cu", ".cuh", ".h")))
-    env = {}
-    m = re.search(r"#define\s+BRC_STAGE_READS\s+(\d+)", src)
-    env["BRC_STAGE_READS"] = int(m.group(1))
-    for name in _CONST_NAMES:
-        m = re.search(r"constexpr\s+int\s+" + name + r"\s*=\s*([^;]+);", src)
-        assert m, f"{name} not found in csrc/"
-        env[name] = int(eval(m.group(1), {}, dict(env)))
-    return env
-
-
-def _first_diff(a: str, b: str) -> str:
-    la, lb = a.splitlines(), b.splitlines()
-    for i, (x, y) in enumerate(zip(la, lb)):
-        if x != y:
-            return f"line {i}:\n got: {x[:300]}\nwant: {y[:300]}"
-    return f"length differs: got {len(la)} lines, want {len(lb)}"
+from boundary_cases import initial_pool_cap, pool_case, selection_cases
+from cases import first_diff
+from kernel_model import CONST_NAMES, CSRC, k0_blocks, k1_chunks, kernel_constants, tile_ranges
+from site_filter_rule import THRESHOLDS, select_lines
 
 
 # ---------------------------------------------------------------------------------------------------------------------------
-# what the kernels decide, recomputed on the host
+# what the kernels decide, recomputed on the host (beyond kernel_model's)
 # ---------------------------------------------------------------------------------------------------------------------------
 def _reads_view(b):
     """Per read: list of (len, op char) and the decoded quality / base arrays."""
@@ -136,78 +108,6 @@ def read_facts(case, batch, site_list):
         facts.append(dict(lq=lq, clen=clen, lclip=lclip, fast=fast, hot=simple and fast and nm_ok and not sm_missing, simple=simple,
                           qoff=qoff, mmq=mmq, se=se, ops=ops))
     return facts
-
-
-def k0_blocks(batch, case):
-    """(staged, ref staged, an op past the staged reference window) per K0 block of a single-region batch."""
-    K = kernel_constants()
-    n = batch.n_reads
-    name, chrom_len, seq, wb = case["contigs"][0]
-    win_len = len(seq)
-    end = batch.ref_end()
-    out = []
-    for r0 in range(0, n, K["K0_READS"]):
-        r1 = min(n, r0 + K["K0_READS"])
-        qa, qb = int(batch.qual_off[r0]) & ~15, (int(batch.qual_off[r1]) + 15) & ~15
-        sa, sb = int(batch.seq_off[r0]) & ~15, (int(batch.seq_off[r1]) + 15) & ~15
-        staged = qb - qa <= K["K0_QUAL_CAP"] and sb - sa <= K["K0_SEQ_CAP"]
-        ra = rb = 0
-        if staged:
-            pf, pl = int(batch.pos[r0]) - wb, int(batch.pos[r1 - 1]) - wb
-            nbytes = (win_len + 1) // 2 + 16
-            ra = ((pf >> 1) if pf > 0 else 0) & ~15
-            rb = min((((pl + 1024) >> 1) + 31) & ~15, nbytes & ~15)
-            if rb <= ra or rb - ra > K["K0_REF_CAP"]:
-                ra = rb = 0
-        past = bool(rb > ra and any(((int(end[i]) - wb) >> 1) + 8 >= rb for i in range(r0, r1)))
-        out.append(dict(staged=staged, uniform=len(set(batch.l_qseq[r0:r1].tolist())) == 1, lq=int(batch.l_qseq[r0]),
-                        ref_staged=rb > ra, past=past, span=int(batch.pos[r1 - 1]) - int(batch.pos[r0])))
-    return out
-
-
-def tile_ranges(batch, first_pos, end_excl):
-    """tile_lo / tile_hi of one region (K0's atomics): first / one-past-last read overlapping each TILE-site tile."""
-    T = kernel_constants()["TILE"]
-    n_t = (end_excl - first_pos + T - 1) // T
-    lo = np.full(n_t, 2 ** 31 - 1, np.int64); hi = np.zeros(n_t, np.int64)
-    e = batch.ref_end()
-    for i in range(batch.n_reads):
-        if batch.flag[i] & 4:
-            continue
-        a, b = max(int(batch.pos[i]), first_pos), min(int(e[i]), end_excl)
-        if b <= a:
-            continue
-        for t in range((a - first_pos) // T, (b - 1 - first_pos) // T + 1):
-            lo[t] = min(lo[t], i); hi[t] = max(hi[t], i + 1)
-    return [(int(l), int(h)) if l < h else (0, 0) for l, h in zip(lo, hi)]
-
-
-def k1_chunks(batch, ranges):
-    """The producer's chunk cuts (brc_kernels.cu pileup_kernel, warp 8): per chunk (r0, r1, full size, staged, CIGAR ops window,
-    CIGAR staged)."""
-    K = kernel_constants()
-    SQ, SS, SR, SC = K["STAGE_QUAL"], K["STAGE_SEQ"], K["STAGE_READS"], K["STAGE_CIGAR"]
-    qo, so, co = (x.astype(np.int64) for x in (batch.qual_off, batch.seq_off, batch.cigar_off))
-    out = []
-    for lo, hi in ranges:
-        r0 = lo
-        while r0 < hi:
-            r1 = min(r0 + SR, hi)
-            full = r1 - r0
-            while True:
-                qa, qb = int(qo[r0]) & ~15, (int(qo[r1]) + 15) & ~15
-                sa, sb = int(so[r0]) & ~15, (int(so[r1]) + 15) & ~15
-                staged = qb - qa <= SQ and sb - sa <= SS
-                if staged or r1 - r0 == 1:
-                    break
-                fq, fs = (SQ - 32) / (qb - qa), (SS - 32) / (sb - sa)
-                n2 = int((r1 - r0) * min(fq, fs))
-                r1 = r0 + max(1, min(n2, r1 - r0 - 1))
-            ca, cb = int(co[r0]) & ~3, (int(co[r1]) + 3) & ~3
-            out.append(dict(r0=r0, r1=r1, full=full, staged=staged, cops=cb - ca, cstaged=cb - ca <= SC,
-                            lq=set(batch.l_qseq[r0:r1].tolist())))
-            r0 = r1
-    return out
 
 
 def site_sums(batch, facts, lo, hi):
@@ -383,7 +283,7 @@ CASES = boundary_cases.all_cases()
 
 def test_kernel_constants_parse():
     K = kernel_constants()
-    assert set(_CONST_NAMES) <= set(K)
+    assert set(CONST_NAMES) <= set(K)
     assert K["STAGE_QUAL"] == K["STAGE_READS"] * 152 + 32 and K["K0_QUAL_CAP"] == K["K0_READS"] * 160 + 32
 
 
@@ -407,61 +307,26 @@ JOBS = boundary_cases.jobs()
 
 @pytest.mark.parametrize("job", JOBS, ids=[j[4] for j in JOBS])
 def test_oracle_equals_reference_binary_on_boundary_cases(job):
-    with open(os.path.join(GOLDEN, "boundary_sha256.json")) as fh:
-        want = json.load(fh)
     case, fname, fl, sl, key = job
-    got, _, _ = cases.run_oracle(case, fl, site_list=sl)
-    assert hashlib.sha256(got.encode("latin-1")).hexdigest() == want[key], f"{key}: oracle differs from the reference binary"
+    cases.assert_anchor("boundary_sha256.json", key, cases.run_oracle(case, fl, site_list=sl).text)
 
 
 # ---------------------------------------------------------------------------------------------------------------------------
 # GPU
 # ---------------------------------------------------------------------------------------------------------------------------
-def _engine_two_pushes(case, flags, site_list):
-    """One region, its reads pushed in two halves: the first push is borrowed, then copied when the second arrives."""
-    from bam_readcount_b200.engine import Engine
-    e = Engine(lib_names=case["lib_names"], **flags)
-    try:
-        name, clen, seq, wb = case["contigs"][0]
-        e.set_reference(0, name, clen, seq, wb)
-        ci, b1, e1 = case["regions"][0]
-        tid, beg, end, sub = cases.region_reads(case, ci, b1, e1)
-        e.begin_region(tid, beg, end, site_list)
-        h = sub.n_reads // 2
-        e.push_reads(sub.select(np.arange(0, h)))
-        e.push_reads(sub.select(np.arange(h, sub.n_reads)))
-        e.end_region()
-        e.compute()
-        return e.format_text(-1), e.warnings()
-    finally:
-        e.close()
-
-
-@functools.lru_cache(maxsize=None)
-def _oracle(case_name, fname, sl):
-    case = {c["name"]: c for c in CASES}[case_name]
-    return cases.run_oracle(case, boundary_cases.FLAG_SETS[fname], site_list=sl)
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("job", JOBS, ids=[j[4] for j in JOBS])
 def test_engine_equals_oracle_on_boundary_cases(job, monkeypatch):
     case, fname, fl, sl, key = job
-    otext, odump, owarn = _oracle(case["name"], fname, sl)
-    etext, edump, ewarn, _ = cases.run_engine(case, fl, site_list=sl, want_dump=True)
-    assert edump == odump, _first_diff(edump, odump)
-    assert etext == otext, _first_diff(etext, otext)
-    assert (ewarn[0], ewarn[1], ewarn[3]) == owarn
+    want = cases.run_oracle_cached(case, fl, sl)
+    cases.assert_same(cases.run_engine(case, fl, site_list=sl), want)
     if len(case["regions"]) == 1 and "max_cnt" not in fl:
-        t2, w2 = _engine_two_pushes(case, fl, sl)          # the copy path (run_engine's one push is the pipelined path)
-        assert t2 == otext, _first_diff(t2, otext)
-        assert (w2[0], w2[1], w2[3]) == owarn
+        # the copy path (run_engine's one push is the pipelined path)
+        cases.assert_same(cases.run_engine(case, fl, site_list=sl, dump=False, push="halves"), want, "two pushes",
+                          fields=("text", "warnings"))
     if sl:
         monkeypatch.setenv("BRC_DEEP_MIN_READS", "1")
-        etext, edump, ewarn, _ = cases.run_engine(case, fl, site_list=sl, want_dump=True)
-        assert edump == odump, "deep-forced: " + _first_diff(edump, odump)
-        assert etext == otext, "deep-forced: " + _first_diff(etext, otext)
-        assert (ewarn[0], ewarn[1], ewarn[3]) == owarn
+        cases.assert_same(cases.run_engine(case, fl, site_list=sl), want, "deep-forced")
 
 
 def test_fastmath_selftest_bound_covers_every_hot_numerator():
@@ -487,70 +352,21 @@ def test_fastmath_selftest_covers_every_hot_numerator():
         e.close()
 
 
-@functools.lru_cache(maxsize=None)
-def pool_case():
-    """About 3000 sites at depth 60 whose reads carry random bases: every site holds four or five base classes, so the secondary
-    pool needs several times the initial capacity brc_compute gives it."""
-    c = cases.synthetic_case(L=3500, depth=60, seed=61, regions=((0, 201, 3200),), site_list=True, n_libs=8)
-    b = c["batch"]
-    rng = np.random.default_rng(61)
-    codes = np.array([1, 2, 4, 8, 15], np.uint8)
-    nib_hi, nib_lo = rng.choice(codes, b.seq.shape[0]), rng.choice(codes, b.seq.shape[0])
-    b.seq = ((nib_hi << 4) | nib_lo).astype(np.uint8)
-    return dict(c, name="pool")
-
-
-def _initial_pool_cap(case, flags, n_slots):
-    b = case["batch"]
-    n_indel = int(np.isin(b.cigar & 0xF, (1, 2)).sum())
-    rows = len(case["lib_names"]) if flags.get("per_lib") else 1
-    return rows * n_slots // 8 + 2 * n_indel + 1024
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("flags", [dict(), dict(per_lib=True)], ids=["alllib", "perlib"])
 def test_secondary_pool_grows_and_stays_exact(flags):
-    from bam_readcount_b200.engine import Engine
-    from test_site_filter import THRESHOLDS, select_lines
     case = pool_case()
-    otext, odump, _ = cases.run_oracle(case, flags, site_list=True)
+    want = cases.run_oracle(case, flags, site_list=True)
     # pipelined path (one borrowed push): its overflow falls through to the plain path, which grows the pool
-    e = Engine(lib_names=case["lib_names"], **flags)
-    try:
-        name, clen, seq, wb = case["contigs"][0]
-        e.set_reference(0, name, clen, seq, wb)
-        tid, beg, end, sub = cases.region_reads(case, *case["regions"][0])
-        e.begin_region(tid, beg, end, True)
-        e.push_reads(sub)
-        e.end_region()
-        e.compute()
-        pk = e.packed()
-        assert pk.n_sec > _initial_pool_cap(case, flags, pk.n_slots), "the pool never outgrew its initial capacity: no retry ran"
-        assert e.format_text(-1) == otext
-    finally:
-        e.close()
-    etext, edump, _, _ = cases.run_engine(case, flags, site_list=True)
-    assert edump == odump and etext == otext
-    t2, _ = _engine_two_pushes(case, flags, True)              # copy path
-    assert t2 == otext, _first_diff(t2, otext)
-    from test_site_filter import _run
+    got = cases.run_engine(case, flags, site_list=True)
+    n_slots = cases.region_geometry(case, case["regions"][0])[5]
+    assert got.n_sec > initial_pool_cap(case, flags, n_slots), "the pool never outgrew its initial capacity: no retry ran"
+    cases.assert_same(got, want, fields=("dump", "text"))
+    t2 = cases.run_engine(case, flags, site_list=True, dump=False, push="halves").text      # copy path
+    assert t2 == want.text, first_diff(t2, want.text)
     for mc, mf in THRESHOLDS:                                  # filtered path
-        text, _, _ = _run(case, flags, True, (mc, mf))
-        assert text == select_lines(otext, mc, mf), (mc, mf)
-
-
-@functools.lru_cache(maxsize=None)
-def selection_cases():
-    big = cases.synthetic_case(L=302000, depth=3, seed=71, n_libs=4,
-                               regions=((0, 1, 300000), (0, 300001, 300100), (0, 300050, 300200), (0, 300201, 300300)), site_list=False)
-    big = dict(big, name="sel_big")
-    many = cases.synthetic_case(L=14000, depth=40, seed=72, n_libs=40, regions=tuple((0, 1000 + 40 * k, 1039 + 40 * k) for k in range(300)),
-                                site_list=False)
-    b = many["batch"]
-    rng = np.random.default_rng(72)
-    b.lib = b.lib.copy()
-    b.lib[rng.random(b.n_reads) < 0.01] = 0xFFFF                # library-less reads
-    return big, dict(many, name="sel_40libs")
+        text = cases.run_engine(case, flags, True, site_filter=(mc, mf)).text
+        assert text == select_lines(want.text, mc, mf), (mc, mf)
 
 
 @pytest.mark.gpu
@@ -559,7 +375,6 @@ def test_site_selection_at_scale(which):
     """More than 1024 scan partials (> 262 144 sites) with adjacent and overlapping argv regions; and -p with 40 libraries and
     library-less reads over 300 adjacent argv regions (the LIBRARY_UNAVAILABLE count of the selection's site pass).  That the
     deletion queue survives rows >= SEL_LAST_ROWS is test_site_selection_ships_the_queue_of_high_library_rows's."""
-    from test_site_filter import THRESHOLDS, _run, select_lines
     K = kernel_constants()
     case = selection_cases()[which]
     flags = dict(per_lib=True) if which == 1 else dict()
@@ -569,26 +384,11 @@ def test_site_selection_at_scale(which):
         assert len(case["lib_names"]) > K["SEL_LAST_ROWS"]
     otext, _, owarn = cases.run_oracle(case, flags, site_list=False)
     for mc, mf in THRESHOLDS:
-        from bam_readcount_b200.engine import Engine
-        e = Engine(lib_names=case["lib_names"], **flags)
-        try:
-            name, clen, seq, wb = case["contigs"][0]
-            e.set_reference(0, name, clen, seq, wb)
-            e.set_site_filter(mc, mf)
-            for (ci, b1, e1) in case["regions"]:
-                tid, beg, end, sub = cases.region_reads(case, ci, b1, e1)
-                e.begin_region(tid, beg, end, False)
-                e.push_reads(sub)
-                e.end_region()
-            e.compute()
-            text = e.format_text(-1)
-            w = e.warnings()
-        finally:
-            e.close()
+        got = cases.run_engine(case, flags, False, site_filter=(mc, mf))
         want = select_lines(otext, mc, mf)
-        assert text == want, (mc, mf, _first_diff(text, want))
+        assert got.text == want, (mc, mf, first_diff(got.text, want))
         if which == 1:
-            assert owarn[2] > 0 and w[3] == owarn[2], (w, owarn)
+            assert owarn[2] > 0 and got.warnings[3] == owarn[2], (got.warnings, owarn)
 
 
 @pytest.mark.gpu
@@ -596,40 +396,16 @@ def test_site_selection_ships_the_queue_of_high_library_rows():
     """boundary_cases.queue_rows: deletions of library rows >= SEL_LAST_ROWS anchored at an argv region's last site, a site no lower
     row covers and whose line fails the filter.  They print only in the next region, from the never-cleared deletion queue, so the
     selection must ship that site for those rows (sel_site_kernel's global reg_last branch); rows < 32 go through shared memory."""
-    from test_site_filter import THRESHOLDS, _run, select_lines
     case = boundary_cases.queue_rows()
     flags = dict(per_lib=True)
-    otext, odump, owarn = cases.run_oracle(case, flags, site_list=False)
-    etext, _, ewarn, _ = cases.run_engine(case, flags, site_list=False, want_dump=False)
-    assert etext == otext, _first_diff(etext, otext)
-    assert (ewarn[0], ewarn[1], ewarn[3]) == owarn
+    want_all = cases.run_oracle(case, flags, site_list=False)
+    cases.assert_same(cases.run_engine(case, flags, site_list=False, dump=False), want_all, fields=("text", "warnings"))
     for a in case["probe"]["anchors"]:                          # the carried deletions do print in the next region
-        assert any(ln.startswith(f"c\t{a + 2}\t") and "\t-" in ln for ln in otext.splitlines()), a
+        assert any(ln.startswith(f"c\t{a + 2}\t") and "\t-" in ln for ln in want_all.text.splitlines()), a
     for mc, mf in THRESHOLDS:
-        text, _, _ = _run(case, flags, False, (mc, mf))
-        want = select_lines(otext, mc, mf)
-        assert text == want, (mc, mf, _first_diff(text, want))
-
-
-def _device_batch(b, device):
-    """The batch's arrays copied to the device (16 spare bytes behind the base and quality pools): a CReadBatch of device pointers
-    and the tensors that own them."""
-    import torch
-    from bam_readcount_b200.engine import CReadBatch
-    view = {np.dtype(np.uint16): np.int16, np.dtype(np.uint32): np.int32, np.dtype(np.uint64): np.int64}
-    keep = []
-
-    def dev(a, pad=0):
-        a = np.ascontiguousarray(a)
-        a = a.view(view.get(a.dtype, a.dtype))
-        if pad:
-            a = np.concatenate([a, np.zeros(pad, a.dtype)])
-        t = torch.from_numpy(a).to(device)
-        keep.append(t)
-        return t.data_ptr()
-    ptrs = [dev(b.tid), dev(b.pos), dev(b.flag), dev(b.mapq), dev(b.lib), dev(b.l_qseq), dev(b.nm), dev(b.sm), dev(b.cigar_off),
-            dev(b.cigar), dev(b.seq_off), dev(b.seq, 64), dev(b.qual_off), dev(b.qual, 64)]
-    return CReadBatch(b.n_reads, *ptrs), keep
+        text = cases.run_engine(case, flags, False, site_filter=(mc, mf)).text
+        want = select_lines(want_all.text, mc, mf)
+        assert text == want, (mc, mf, first_diff(text, want))
 
 
 @pytest.mark.gpu
@@ -637,34 +413,21 @@ def test_device_path_reports_pool_overflow_and_is_exact_when_replanned():
     """brc_plan_device with a secondary pool of 1024 records on the random-base pool case: brc_fetch_device_results must return
     BRC_E_OVERFLOW (the device path has no retry).  Re-planned with room, every raw accumulator equals the oracle's."""
     import torch
-    from bam_readcount_b200.engine import BrcError, CRegion, Engine, admitted
+    from bam_readcount_b200.engine import BrcError, admitted
     case = pool_case()
-    _, odump, _ = cases.run_oracle(case, dict(), site_list=True)
-    ci, b1, e1 = case["regions"][0]
-    tid, beg, end, sub = cases.region_reads(case, ci, b1, e1)
+    odump = cases.run_oracle(case, dict(), site_list=True).dump
+    region = case["regions"][0]
+    tid, _, _, sub = cases.region_reads(case, *region)
     assert len(admitted(sub, tid, 10_000_000)) == sub.n_reads        # the device path admits every read it is given
-    first_pos = max(beg - 1, 0)
-    n_slots = int(min(end, int(sub.ref_end().max()))) - first_pos
     dev = torch.device("cuda", 0)
-    cb, keep = _device_batch(sub, dev)
-    name, clen, seq, wb = case["contigs"][0]
-    e = Engine(lib_names=case["lib_names"])
-    try:
-        e.set_reference(tid, name, clen, seq, wb)
+    cb, keep = cases.device_batch(sub, dev)
+    with cases.open_engine(case) as e:
         s = torch.cuda.Stream(device=dev)
-        for cap in (1024, 1 << 20):
-            e.plan_device([CRegion(tid, beg, end, 1, 0, sub.n_reads, 0, first_pos, n_slots)], sub.n_reads, cap)
-            e.run_device(cb, None, s.cuda_stream)
-            if cap == 1024:
-                with pytest.raises(BrcError) as err:
-                    e.fetch_device_results(s.cuda_stream)
-                assert err.value.status == -8          # BRC_E_OVERFLOW
-            else:
-                res = e.fetch_device_results(s.cuda_stream)
-                edump = res.dump(sub, {tid: (wb, seq)})
-                assert edump == odump, _first_diff(edump, odump)
-    finally:
-        e.close()
+        with pytest.raises(BrcError) as err:
+            cases.run_device(e, case, region, cb, s, n_sec_cap=1024)
+        assert err.value.status == -8          # BRC_E_OVERFLOW
+        edump = cases.run_device(e, case, region, cb, s)
+        assert edump == odump, first_diff(edump, odump)
     del keep
 
 
@@ -675,12 +438,10 @@ def test_bgzf_record_scan_over_more_than_one_scan_level():
     import tempfile
     from bam_readcount_b200 import bamio, synth_cb
     from bam_readcount_b200.engine import Engine
-    from oracle.oracle import REF_SAMTOOLS
-    if not os.path.exists(REF_SAMTOOLS):
-        pytest.skip("oracle/_ref/samtools not built")
+    samtools = cases.samtools()
     tmp = tempfile.mkdtemp()
     sp = synth_cb.Spec(seed=31, contig_len=1280 * 1600)
-    info = synth_cb.write_sample_bam(sp, 0, 0, 1500, tmp, REF_SAMTOOLS)
+    info = synth_cb.write_sample_bam(sp, 0, 0, 1500, tmp, samtools)
     hdr, host = bamio.read_bam(info["bam"])
     rg_lib = {rg: hdr.lib_of_rg(rg) for rg in hdr.rg_lb}
     span = bamio.bam_span(info["bam"], bamio.BaiIndex(info["bam"] + ".bai"), 0, 0, info["length"], rg_lib)

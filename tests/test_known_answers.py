@@ -60,14 +60,14 @@ def test_oracle_max_count_table(d):
 @pytest.mark.parametrize("k", range(len(KNOWN)))
 def test_engine_known_answers(k):
     read, want = KNOWN[k]
-    text, _, _, _ = cases.run_engine(_case([read]), dict(), want_dump=False)
+    text = cases.run_engine(_case([read]), dict(), dump=False).text
     assert _block(text) == want
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("d", sorted(D_TABLE))
 def test_engine_max_count_table(d):
-    text, _, _, _ = cases.run_engine(_d_case(), dict(max_cnt=d), want_dump=False)
+    text = cases.run_engine(_d_case(), dict(max_cnt=d), dump=False).text
     assert [int(l.split("\t")[3]) for l in text.strip().split("\n")] == D_TABLE[d]
 
 
@@ -99,5 +99,5 @@ def test_oracle_cram_fixture_records(per_lib):
 @pytest.mark.gpu
 @pytest.mark.parametrize("per_lib", [True, False])
 def test_engine_cram_fixture_records(per_lib):
-    text, _, _, _ = cases.run_engine(_cram_case(), dict(per_lib=per_lib), want_dump=False)
+    text = cases.run_engine(_cram_case(), dict(per_lib=per_lib), dump=False).text
     assert text == cases.load_golden_text("ref_cram_twolib_perlib.txt" if per_lib else "ref_cram_twolib_alllib.txt")

@@ -1,8 +1,7 @@
 """The alternative-allele site filter (brc_set_site_filter, brc-readcount --min-alt-count / --min-alt-fraction).
 
-The rule is defined on the text: ``select_lines`` below parses bam-readcount's line grammar (with -p library blocks) and keeps a
-line iff one of its entries is an alternative allele with count >= min_alt_count and count >= min_alt_fraction * depth.  It is
-the oracle: the filtered output of the engine must equal select_lines(unfiltered output) byte for byte.
+The rule is defined on the text (tests/site_filter_rule.py): the filtered output of the engine must equal
+select_lines(unfiltered output) byte for byte.
 CPU: select_lines on the committed goldens and on hand-written lines, CLI option validation, the exported symbols.
 GPU: the engine and the C++ host, filtered, against select_lines of the reference goldens, the oracle and the unfiltered run.
 """
@@ -15,54 +14,17 @@ import pytest
 
 import cases
 import golden_jobs
+from cases import cli as _cli
+from cases import first_diff
+from site_filter_rule import THRESHOLDS, is_alt, line_entries, line_passes, select_lines
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden")
 
-_ENTRY = re.compile(r"^([=ACGTN]|[+-][^:]*):(\d+):")
-_NT16 = {"A": 1, "C": 2, "G": 4, "T": 8}
-
-
-def _line_entries(fields):
-    """(allele, count) of every allele entry of a line's fields after the depth column (library names and braces skipped)."""
-    for f in fields:
-        m = _ENTRY.match(f)
-        if m:
-            yield m.group(1), int(m.group(2))
-
-
-def is_alt(allele: str, ref_base: str) -> bool:
-    if allele[0] in "+-":
-        return True
-    if allele not in _NT16:
-        return False                          # "=" and "N"
-    return _NT16[allele] != _NT16.get(ref_base.upper(), 15)
-
-
-def line_passes(line: str, min_alt_count: int, min_alt_fraction: float, ref_lookup=None) -> bool:
-    f = line.split("\t")
-    ref = ref_lookup(f[0], int(f[1])) if ref_lookup else f[2]
-    depth = int(f[3])
-    return any(is_alt(a, ref) and c >= min_alt_count and float(c) >= min_alt_fraction * float(depth) for a, c in _line_entries(f[4:]))
-
-
-def select_lines(text: str, min_alt_count: int, min_alt_fraction: float = 0.0, ref_lookup=None) -> str:
-    """The lines of bam-readcount output `text` a site filter keeps.  ref_lookup(chrom, pos1) -> reference character; by
-    default the line's own reference column."""
-    return "".join(ln + "\n" for ln in text.splitlines() if line_passes(ln, min_alt_count, min_alt_fraction, ref_lookup))
-
-
-THRESHOLDS = [(1, 0.0), (2, 0.05), (1, 0.2), (10 ** 6, 0.0)]
-
 
 def _same(got: str, want: str) -> str:
-    """'' when equal, else the first differing line (keeps pytest from diffing megabytes of text)."""
-    if got == want:
-        return ""
-    for i, (x, y) in enumerate(zip(got.splitlines(), want.splitlines())):
-        if x != y:
-            return f"line {i}:\n got: {x[:300]}\nwant: {y[:300]}"
-    return f"length differs: got {len(got.splitlines())} lines, want {len(want.splitlines())}"
+    """'' when equal, else the first differing line."""
+    return "" if got == want else first_diff(got, want)
 
 
 # ---------------------------------------------------------------------------------------------------------------------------
@@ -85,7 +47,7 @@ def test_select_lines_on_goldens_is_a_subsequence_dropping_only_lines_without_a_
             keep = set(kept)
             for ln in lines:
                 f = ln.split("\t")
-                ok = [(a, c) for a, c in _line_entries(f[4:]) if is_alt(a, f[2]) and c >= mc and c >= mf * int(f[3])]
+                ok = [(a, c) for a, c in line_entries(f[4:]) if is_alt(a, f[2]) and c >= mc and c >= mf * int(f[3])]
                 assert (ln in keep) == bool(ok), (name, ln[:120])
         if len(lines) > 20:
             n1 = len(select_lines(text, 1).splitlines())
@@ -128,12 +90,6 @@ def test_select_lines_hand_written_reference_bases_deletions_and_library_blocks(
     assert select_lines(text, 1, ref_lookup=lambda c, p: "T") == text       # every A/G count is alternative to a T
 
 
-def _cli():
-    from bam_readcount_b200 import build
-    build.build()
-    return build.build_cli()
-
-
 def test_cli_site_filter_option_validation():
     exe = _cli()
     bam = os.path.join(GOLDEN, "test.bam")
@@ -163,26 +119,9 @@ def test_site_filter_symbols_are_exported():
 # ---------------------------------------------------------------------------------------------------------------------------
 # GPU
 # ---------------------------------------------------------------------------------------------------------------------------
-def _run(case, flags, site_list, filt=None, want_selected=False):
-    """cases.run_engine with an optional site filter: (text, selected results or None, regions, launch count)."""
-    from bam_readcount_b200.engine import Engine
-    e = Engine(lib_names=case["lib_names"], **flags)
-    try:
-        for ci, (name, clen, seq, wb) in enumerate(case["contigs"]):
-            e.set_reference(cases.case_tid(case, ci), name, clen, seq, wb)
-        if filt:
-            e.set_site_filter(*filt)
-        for (ci, b1, e1) in case["regions"]:
-            tid, beg, end, sub = cases.region_reads(case, ci, b1, e1)
-            e.begin_region(tid, beg, end, site_list)
-            e.push_reads(sub)
-            e.end_region()
-        e.compute()
-        text = e.format_text(-1)
-        sel = e.selected() if (filt and want_selected) else None
-        return text, sel, e.launch_count()
-    finally:
-        e.close()
+def _text(case, flags, site_list, filt):
+    """The engine's text with a site filter set."""
+    return cases.run_engine(case, flags, site_list, dump=False, site_filter=filt).text
 
 
 _JOBS = [j for j in golden_jobs.jobs() if j[0].startswith(("syn-", "deep-", "edge-fuzz", "testbam-"))]
@@ -195,8 +134,7 @@ def test_engine_filtered_text_equals_selected_golden(job):
     case = getter()
     want_all = cases.load_golden_text(golden)
     for mc, mf in THRESHOLDS:
-        text, _, _ = _run(case, flags, site_list, (mc, mf))
-        d = _same(text, select_lines(want_all, mc, mf))
+        d = _same(_text(case, flags, site_list, (mc, mf)), select_lines(want_all, mc, mf))
         assert not d, (mc, mf, d)
 
 
@@ -208,28 +146,14 @@ def test_device_selection_is_exact_without_carried_deletions(job):
     _, getter, flags, site_list, golden = job
     case = getter()
     want_all = cases.load_golden_text(golden)
-    from bam_readcount_b200.engine import Engine
     for mc, mf in ((1, 0.0), (2, 0.05)):
-        e = Engine(lib_names=case["lib_names"], **flags)
-        try:
-            for ci, (name, clen, seq, wb) in enumerate(case["contigs"]):
-                e.set_reference(cases.case_tid(case, ci), name, clen, seq, wb)
-            e.set_site_filter(mc, mf)
-            for (ci, b1, e1) in case["regions"]:
-                tid, beg, end, sub = cases.region_reads(case, ci, b1, e1)
-                e.begin_region(tid, beg, end, site_list)
-                e.push_reads(sub)
-                e.end_region()
-            e.compute()
-            sel = e.selected()
-            r = [p + 1 for p in sel.positions(1)]
-            kept = [int(ln.split("\t")[1]) for ln in select_lines(want_all, mc, mf).splitlines()]
-            assert r == kept, (mc, mf)
-            assert not (sel.emit == 2).any() or not site_list       # keep-all ranges only follow argv regions
-            # kept sites and their left neighbours; per argv region and library row, its last live site and that site's neighbour
-            assert sel.n_sites <= 2 * len(kept) + 2 * sel.n_rows * len(case["regions"])
-        finally:
-            e.close()
+        sel = cases.run_engine(case, flags, site_list, dump=False, site_filter=(mc, mf)).selected
+        r = [p + 1 for p in sel.positions(1)]
+        kept = [int(ln.split("\t")[1]) for ln in select_lines(want_all, mc, mf).splitlines()]
+        assert r == kept, (mc, mf)
+        assert not (sel.emit == 2).any() or not site_list       # keep-all ranges only follow argv regions
+        # kept sites and their left neighbours; per argv region and library row, its last live site and that site's neighbour
+        assert sel.n_sites <= 2 * len(kept) + 2 * sel.n_rows * len(case["regions"])
 
 
 @pytest.mark.gpu
@@ -240,10 +164,9 @@ def test_synthetic_whole_region_and_filter_off_is_unchanged():
     for flags in (dict(), dict(per_lib=True, insertion_centric=True), dict(min_mapq=20, min_bq=20)):
         want, _, _ = cases.run_oracle(case, flags, site_list=False)
         for mc, mf in THRESHOLDS:
-            text, sel, _ = _run(case, flags, False, (mc, mf), want_selected=True)
-            d = _same(text, select_lines(want, mc, mf))
+            d = _same(_text(case, flags, False, (mc, mf)), select_lines(want, mc, mf))
             assert not d, (flags, mc, mf, d)
-    fresh_text, _, fresh_launches = _run(case, dict(), False)
+    fresh = cases.run_engine(case, dict(), False, dump=False)
     from bam_readcount_b200.engine import BrcError, Engine
     name, clen, seq, wb = case["contigs"][0]
     e = Engine(lib_names=case["lib_names"])
@@ -264,8 +187,8 @@ def test_synthetic_whole_region_and_filter_off_is_unchanged():
         assert e.stage_ms(3) > 0.0
         e.clear_site_filter()
         res = step()
-        assert res is not None and e.launch_count() == fresh_launches
-        d = _same(e.format_text(-1), fresh_text)
+        assert res is not None and e.launch_count() == fresh.launches
+        d = _same(e.format_text(-1), fresh.text)
         assert not d, d
         with pytest.raises(BrcError):
             e.selected()
@@ -331,9 +254,7 @@ def test_cli_filtered_output_on_the_reference_fixture(tmp_path):
 def test_cli_filtered_output_on_a_synthetic_bam(tmp_path):
     """A few tens of kb of synthetic BAM: one argv region cut into 3777-site windows (deletions across window edges), the
     device BGZF decode path, overlapping argv regions on it and a site list."""
-    from oracle.oracle import REF_SAMTOOLS
-    if not os.path.exists(REF_SAMTOOLS):
-        pytest.skip("oracle/_ref/samtools not built")
+    samtools = cases.samtools()
     from bam_readcount_b200 import synth
     exe = _cli()
     case = cases.synthetic_case(L=40000, depth=30, seed=47, regions=((0, 1, 40000),), site_list=False)
@@ -341,8 +262,8 @@ def test_cli_filtered_output_on_a_synthetic_bam(tmp_path):
     d = str(tmp_path)
     synth.write_fasta(os.path.join(d, "ref.fa"), name, np.frombuffer(seq, dtype=np.uint8))
     synth.write_sam(os.path.join(d, "s.sam"), case["batch"], [(name, L)], n_libs=len(case["lib_names"]))
-    subprocess.check_call([REF_SAMTOOLS, "view", "-b", "-o", os.path.join(d, "s.bam"), os.path.join(d, "s.sam")])
-    subprocess.check_call([REF_SAMTOOLS, "index", os.path.join(d, "s.bam")])
+    subprocess.check_call([samtools, "view", "-b", "-o", os.path.join(d, "s.bam"), os.path.join(d, "s.sam")])
+    subprocess.check_call([samtools, "index", os.path.join(d, "s.bam")])
     base = ["-w", "0", "-f", os.path.join(d, "ref.fa"), os.path.join(d, "s.bam")]
     want, _, _ = cases.run_oracle(case, dict(per_lib=True), site_list=False)
     t = _check_cli(exe, ["-p"] + base + ["chr1:1-40000"], env={"BRC_CLI_WINDOW": "3777"})
@@ -394,8 +315,7 @@ def test_last_site_of_an_argv_region_keeps_the_deletion_from_its_left_neighbour(
     assert last[1] == "80" and any(f.startswith("-") for f in last[4:])          # the last line prints the deletion
     fractions = sorted({6 / 32, 6 / 31, 6 / 30, 0.19, 0.194, 0.195, 0.198, 0.2, 0.21} | {round(x, 3) for x in np.linspace(0.15, 0.25, 21)})
     for f in fractions:
-        text, sel, _ = _run(case, dict(), False, (1, f), want_selected=True)
-        diff = _same(text, select_lines(want, 1, f))
+        diff = _same(_text(case, dict(), False, (1, f)), select_lines(want, 1, f))
         assert not diff, (f, diff)
 
 
@@ -410,8 +330,7 @@ def test_per_library_queue_handed_to_an_overlapping_argv_region_is_the_unfiltere
     flags = dict(per_lib=True)
     want, _, _ = cases.run_oracle(case, flags, site_list=False)
     for mc, mf in THRESHOLDS + [(2, 0.0), (3, 0.0)]:
-        text, _, _ = _run(case, flags, False, (mc, mf))
-        diff = _same(text, select_lines(want, mc, mf))
+        diff = _same(_text(case, flags, False, (mc, mf)), select_lines(want, mc, mf))
         assert not diff, (mc, mf, diff)
     lines62 = [ln for ln in want.splitlines() if ln.split("\t")[1] == "62"]
     assert len(lines62) == 2 and all(sum(f.startswith("-") for f in ln.split("\t")) == 1 for ln in lines62)
@@ -431,8 +350,7 @@ def test_per_library_deletion_carried_through_a_region_that_drops_it():
     line61 = [ln for ln in want.splitlines() if ln.split("\t")[1] == "61"]
     assert len(line61) == 1 and sum(f.startswith("-") for f in line61[0].split("\t")) == 1
     for mc, mf in THRESHOLDS + [(2, 0.0), (3, 0.0)]:
-        text, _, _ = _run(case, flags, False, (mc, mf))
-        diff = _same(text, select_lines(want, mc, mf))
+        diff = _same(_text(case, flags, False, (mc, mf)), select_lines(want, mc, mf))
         assert not diff, (mc, mf, diff)
 
 
@@ -441,27 +359,20 @@ def test_device_only_reference_is_judged_by_the_printed_reference_column():
     """A contig set only on the device prints N as the reference base, so every base counts as alternative: the filtered text is
     still select_lines of the unfiltered text."""
     import torch
-    from bam_readcount_b200.engine import Engine
     case = cases.synthetic_case(L=6000, depth=30, seed=5, regions=((0, 500, 5500),), site_list=False)
     name, clen, seq, wb = case["contigs"][0]
     dev = torch.tensor(np.frombuffer(seq + b"\0" * 64, dtype=np.uint8), device="cuda")
     torch.cuda.synchronize()
     texts = []
     for filt in (None, (20, 0.5)):
-        e = Engine(lib_names=case["lib_names"])
-        try:
+        with cases.open_engine(dict(case, contigs=[])) as e:           # no host reference
             e.set_reference_device(0, name, clen, 0, dev.data_ptr(), len(seq), torch.cuda.current_stream().cuda_stream)
             torch.cuda.synchronize()
             if filt:
                 e.set_site_filter(*filt)
-            tid, beg, end, sub = cases.region_reads(case, 0, 500, 5500)
-            e.begin_region(tid, beg, end, False)
-            e.push_reads(sub)
-            e.end_region()
+            cases.push_regions(e, case, False)
             e.compute()
             texts.append(e.format_text(-1))
-        finally:
-            e.close()
     full, filtered = texts
     assert all(ln.split("\t")[2] == "N" for ln in full.splitlines()[:50])
     kept = select_lines(full, 20, 0.5)

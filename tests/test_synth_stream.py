@@ -207,19 +207,11 @@ def test_device_generator_equals_host_generator():
 
 @pytest.mark.gpu
 def test_packed_records_decode_to_the_full_width_view():
-    from bam_readcount_b200.engine import Engine
     for case, flags in ((cases.synthetic_case(L=20000, depth=40, seed=11, regions=((0, 1000, 19000),)), dict(per_lib=True)),
                         (cases.deep_case(n_sites=2, depth=3000, seed=3), dict()),           # depth > 255: every site escapes
                         (cases.deep_case(n_sites=2, depth=700, seed=4), dict(per_lib=True))):
-        e = Engine(lib_names=case["lib_names"], **flags)
-        try:
-            for ci, (name, clen, seq, wb) in enumerate(case["contigs"]):
-                e.set_reference(ci, name, clen, seq, wb)
-            for (ci, b1, e1) in case["regions"]:
-                tid, beg, end, sub = cases.region_reads(case, ci, b1, e1)
-                e.begin_region(tid, beg, end, True)
-                e.push_reads(sub)
-                e.end_region()
+        with cases.open_engine(case, flags) as e:
+            cases.push_regions(e, case, True)
             res = e.compute()
             pk = e.packed()
             ncover, npass, flg, pbase, ps = pk.widen()
@@ -229,8 +221,6 @@ def test_packed_records_decode_to_the_full_width_view():
             esc = int(((pk.words[1] & 7) == 7).sum())
             if "deep" in case["name"] and not flags:
                 assert esc > 0
-        finally:
-            e.close()
 
 
 @pytest.mark.gpu
@@ -238,21 +228,18 @@ def test_windowed_device_path_equals_whole_region():
     """A contig walked window by window on the device path (generator in HBM -> plan -> run, the bench's C4 loop) gives,
     site for site, the records of the same contig pushed as ONE region through the host path."""
     import torch
-    from bam_readcount_b200.engine import Engine
     dev = torch.device("cuda", 0)
     sp = sc.Spec(seed=4321, contig_len=1280 * 120, n_contigs=2)
     flags = dict(insertion_centric=True)
     wins = [w for w in st.wgs_windows(sp, 5) if w.contig == 1]
     hb, _ = sp.window_host(1, 0, 120)
     ref = sp.ref_host(1, 0, sp.contig_len)
-    e = Engine(**flags)
-    e.set_reference(1, "chr2", sp.contig_len, ref, 0)
-    e.begin_region(1, 0, sp.contig_len, False)
-    e.push_reads(hb)
-    e.end_region()
-    whole = e.compute()
+    case = dict(name="wgs_chr2", contigs=[("chr2", sp.contig_len, ref, 0)], tid_map={1: 0}, batch=hb, regions=[(0, 1, sp.contig_len)],
+                site_list=False, lib_names=[])
+    with cases.open_engine(case, flags) as e:
+        cases.push_regions(e, case, False, push=lambda e, *_: e.push_reads(hb))      # the whole window as generated
+        whole = e.compute()
     wdump = whole.dump(hb, {1: (0, ref)})
-    e.close()
     run = st.WindowRunner(sp, max(sp.window_reads(w.blk_lo, w.blk_hi) for w in wins), dev, flags)
     try:
         for w in wins:
@@ -277,7 +264,6 @@ def test_windowed_device_path_equals_whole_region():
 def test_site_at_50000x_eight_libraries_is_bit_exact():
     """BASELINE config 5's depth: one panel site under 50 000 reads, -p with 8 libraries, -d 100000000 — the depth at which the
     reference's own sequential-float drift exceeds 1e-6 (SURVEY.md Appendix D), so only the ordered sums match."""
-    from bam_readcount_b200.engine import Engine
     from oracle.oracle import Oracle
     sp = sc.Spec(seed=1234, mode=sc.DEEP, n_libs=8, depth=50_000, site_stride=1000, n_sites=4, contig_len=1280)
     libs = [f"lib{i}" for i in range(8)]
@@ -285,21 +271,16 @@ def test_site_at_50000x_eight_libraries_is_bit_exact():
     ref = sp.ref_host(0, 0, L)
     hb, _ = sp.window_host(0, 1, 2)
     p = sp.site_pos(1)
+    case = dict(name="deep50k", contigs=[("chr1", L, ref, 0)], batch=hb, regions=[(0, p + 1, p + 1)], site_list=True, lib_names=libs)
     for flags in (dict(per_lib=True, max_cnt=100_000_000), dict(max_cnt=100_000_000)):
         o = Oracle(lib_names=libs, **flags)
         o.region(hb, tid=0, beg=p, end=p + 1, contig="chr1", chrom_len=L, ref_seq=ref, ref_win_beg=0, site_list_mode=True)
-        e = Engine(lib_names=libs, **flags)
-        try:
-            e.set_reference(0, "chr1", L, ref, 0)
-            e.begin_region(0, p, p + 1, True)
-            e.push_reads(hb)
-            e.end_region()
+        with cases.open_engine(case, flags) as e:
+            cases.push_regions(e, case, True, push=lambda e, *_: e.push_reads(hb))   # every read of the block, as the oracle's
             res = e.compute()
             assert res.dump(hb, {0: (0, ref)}) == o.dump()
             assert e.format_text(-1) == o.text()
             assert int(res.ncover[:, 1].sum()) == 50_000
-        finally:
-            e.close()
 
 
 @pytest.mark.gpu
