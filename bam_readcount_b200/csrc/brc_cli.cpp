@@ -11,6 +11,7 @@
 //   argv regions : R:...:641-657  (bam_parse_region; a bare contig name keeps the previous beg/end, A.6)
 // With --bam-list the same per-sample run is repeated over a list of inputs in one process (DESIGN.md §11).
 #include <algorithm>
+#include <cctype>
 #include <cerrno>
 #include <cstdarg>
 #include <climits>
@@ -763,7 +764,14 @@ void usage() {
                 "                                        INPUT<TAB>OUT or INPUT<TAB>OUT<TAB>ERR (ERR defaults to OUT.log); OUT and ERR get\n"
                 "                                        exactly what `brc-readcount <options> INPUT <regions>` prints on STDOUT and\n"
                 "                                        STDERR.  Every positional argument is a region; a failed sample does not stop\n"
-                "                                        the others (exit status 1 at the end)\n\n");
+                "                                        the others (exit status 1 at the end)\n"
+                "  --vcf FILE                            (this host) write FILE (VCF, plain or bgzip) back to STDOUT with the read counts of\n"
+                "                                        each record's REF and SNV / insertion / deletion ALT alleles as FORMAT fields BRC_DP,\n"
+                "                                        BRC_AD, BRC_ADF, BRC_ADR and BRC_AF: the values the line of each record's site prints\n"
+                "                                        (STDERR is that of -l over the records' sites).  Not with -l, regions, -p,\n"
+                "                                        --min-alt-*, --shard or --bam-list\n"
+                "  --vcf-sample NAME                     (this host) the sample column that takes the values (required with several; names\n"
+                "                                        the column added to a sites-only VCF)\n\n");
 }
 
 // samtools region string "name[:beg[-end]]" as bam_parse_region (V:bam_aux.c:65-75) handles it.  Returns 0 when beg and end were
@@ -803,8 +811,205 @@ int parse_region(const BamFile &bam, const std::string &s, int &tid, int &beg, i
 // A run on one input calls the same two functions with STDOUT_FILENO and the process's stderr, so each sample of a cohort
 // prints exactly the bytes its own run prints.
 // ------------------------------------------------------------------------------------------
+// ------------------------------------------------------------------------------------------
+// --vcf FILE: the per-allele read counts of each VCF record, written back as FORMAT fields (DESIGN.md §12).  A record is
+// counted when one of its ALT alleles is an SNV, an insertion after its anchor base or a deletion after it; its site is one
+// line "CHROM L L" of a derived -l site list (L = POS, or POS + 1 for a deletion, whose entry prints on the line after the
+// anchor), and its values are what that run prints on the line: the engine answers them (brc_set_allele_queries).
+// ------------------------------------------------------------------------------------------
+const char kVcfFormat[] = ":BRC_DP:BRC_AD:BRC_ADF:BRC_ADR:BRC_AF";
+const char kVcfHeader[] =
+    "##FORMAT=<ID=BRC_DP,Number=1,Type=Integer,Description=\"brc-readcount depth of the site's line\">\n"
+    "##FORMAT=<ID=BRC_AD,Number=R,Type=Integer,Description=\"brc-readcount count of the REF and each ALT allele\">\n"
+    "##FORMAT=<ID=BRC_ADF,Number=R,Type=Integer,Description=\"brc-readcount plus-strand count of the REF and each ALT allele\">\n"
+    "##FORMAT=<ID=BRC_ADR,Number=R,Type=Integer,Description=\"brc-readcount minus-strand count of the REF and each ALT allele\">\n"
+    "##FORMAT=<ID=BRC_AF,Number=A,Type=Float,Description=\"brc-readcount BRC_AD of each ALT allele over BRC_DP\">\n";
+
+struct VcfRecord {
+    std::vector<std::string> cols;
+    bool counted = false;
+    int32_t line_pos = 0;                 // L: 1-based position of the derived site-list line
+    uint32_t ref_kind = 0;                // the REF entry: a base class of "=ACGTN"
+    std::vector<int64_t> alt_kind_len;    // per ALT: query kind | length << 8, or -1 when the ALT is not countable
+    std::vector<std::string> alt_bases;   // per ALT: an insertion's bases
+};
+struct Vcf {
+    std::string path;
+    std::vector<std::string> header;      // every line before #CHROM
+    std::string chrom_line;
+    size_t n_cols = 0;
+    int sample_col = -1;                  // column that takes the values; -1: sites-only, a FORMAT and a sample column are added
+    std::string add_sample;               // ... named so
+    std::vector<VcfRecord> rec;
+};
+
+std::vector<std::string> split(const std::string &s, char c) {
+    std::vector<std::string> out; size_t p = 0;
+    for (size_t t; (t = s.find(c, p)) != std::string::npos; p = t + 1) out.push_back(s.substr(p, t - p));
+    out.push_back(s.substr(p));
+    return out;
+}
+
+// the whole file, plain or BGZF (bgzip); false with a message
+bool read_vcf_bytes(const std::string &path, std::string &out, std::string &why) {
+    FILE *f = std::fopen(path.c_str(), "rb");
+    if (!f) { why = "cannot open " + path + ": " + std::strerror(errno); return false; }
+    uint8_t head[512]; const size_t got = std::fread(head, 1, sizeof head, f);
+    if (got < 2 || head[0] != 31 || head[1] != 139) {
+        out.assign((const char *)head, got);
+        char buf[1 << 16];
+        for (size_t n; (n = std::fread(buf, 1, sizeof buf, f)) > 0;) out.append(buf, n);
+        const bool bad = std::ferror(f);
+        std::fclose(f);
+        if (bad) why = "cannot read " + path;
+        return !bad;
+    }
+    std::fclose(f);
+    size_t hdr = 0;
+    if (!Bgzf::block_size(head, got, hdr)) { why = path + " is gzip-compressed but not BGZF: compress it with bgzip"; return false; }
+    Bgzf bz;
+    if (!bz.open(path)) { why = "cannot open " + path; return false; }
+    for (uint64_t coff = 0; bz.load_block(coff); coff = bz.next_coff) out.append((const char *)bz.block.data(), bz.block.size());
+    if (bz.error) { why = path + ": truncated or corrupt BGZF block"; return false; }
+    return true;
+}
+
+// Parses the whole VCF and applies the allele rule; false with a message (nothing may have been written yet).
+bool parse_vcf(const std::string &path, const std::string &sample, bool sample_given, Vcf &v, std::string &why) {
+    std::string text;
+    if (!read_vcf_bytes(path, text, why)) return false;
+    v.path = path;
+    auto up = [](std::string s) { for (char &c : s) c = (char)std::toupper((unsigned char)c); return s; };
+    auto acgtn = [](const std::string &s, size_t from) {
+        if (s.size() <= from) return false;
+        for (size_t i = from; i < s.size(); ++i) if (!std::strchr("ACGTN", s[i]) || !s[i]) return false;
+        return true;
+    };
+    auto kind_of = [](char c) { return (uint32_t)(std::strchr("=ACGTN", c) - "=ACGTN"); };
+    bool in_header = true;
+    size_t ln = 0;
+    for (size_t p = 0; p < text.size();) {
+        size_t e = text.find('\n', p);
+        if (e == std::string::npos) e = text.size();
+        std::string line = text.substr(p, e - p);
+        p = e + 1; ++ln;
+        const std::string at = path + ": line " + std::to_string(ln) + ": ";
+        if (in_header && line.compare(0, 2, "##") == 0) {
+            if (line.compare(0, 16, "##FORMAT=<ID=BRC") == 0 && line.size() > 16 && line[16] == '_') { why = at + "the header already declares a BRC_* FORMAT field"; return false; }
+            v.header.push_back(line);
+            continue;
+        }
+        if (in_header && line.compare(0, 6, "#CHROM") == 0) {
+            v.chrom_line = line; v.n_cols = split(line, '\t').size(); in_header = false;
+            if (v.n_cols < 8) { why = at + "the #CHROM line has fewer than 8 columns"; return false; }
+            if (v.n_cols == 9) { why = at + "a FORMAT column without sample columns"; return false; }
+            continue;
+        }
+        if (in_header) { why = at + "data before the #CHROM header line"; return false; }
+        VcfRecord r;
+        r.cols = split(line, '\t');
+        if (r.cols.size() < 8) { why = at + "fewer than 8 columns"; return false; }
+        if (r.cols.size() != v.n_cols) { why = at + std::to_string(r.cols.size()) + " columns, the #CHROM line has " + std::to_string(v.n_cols); return false; }
+        const std::string &ps = r.cols[1];
+        int64_t pos = 0;
+        bool ok = !ps.empty() && ps.size() <= 10;
+        for (char c : ps) ok = ok && c >= '0' && c <= '9';
+        if (ok) pos = std::atoll(ps.c_str());
+        if (!ok || pos < 1 || pos >= INT32_MAX) { why = at + "POS is not a positive integer below 2^31 - 1"; return false; }
+        const std::string ref = up(r.cols[3]);
+        const bool ref_ok = acgtn(ref, 0);
+        for (const std::string &a0 : split(r.cols[4], ',')) {
+            const std::string a = up(a0);
+            int64_t kl = -1; std::string bases;
+            if (ref_ok && ref.size() == 1 && a.size() == 1 && acgtn(a, 0)) kl = kind_of(a[0]);
+            else if (ref_ok && ref.size() == 1 && a.size() >= 2 && a[0] == ref[0] && acgtn(a, 1)) { kl = BRC_KIND_INS | (int64_t)(a.size() - 1) << 8; bases = a.substr(1); }
+            else if (ref_ok && ref.size() >= 2 && a.size() == 1 && a[0] == ref[0]) kl = BRC_KIND_DEL | (int64_t)(ref.size() - 1) << 8;
+            r.counted = r.counted || kl >= 0;
+            r.alt_kind_len.push_back(kl); r.alt_bases.push_back(bases);
+        }
+        if (r.counted) { r.line_pos = (int32_t)(ref.size() == 1 ? pos : pos + 1); r.ref_kind = kind_of(ref[ref.size() == 1 ? 0 : 1]); }
+        v.rec.push_back(std::move(r));
+    }
+    if (in_header) { why = path + ": no #CHROM header line"; return false; }
+    const std::vector<std::string> hc = split(v.chrom_line, '\t');
+    if (v.n_cols == 8) {
+        if (!sample_given) { why = path + " has no sample column: --vcf-sample NAME names the one added"; return false; }
+        v.add_sample = sample;
+        return true;
+    }
+    int n_match = 0;
+    for (size_t c = 9; c < hc.size(); ++c) if (hc[c] == sample) { ++n_match; v.sample_col = (int)c; }
+    if (!sample_given) {
+        if (hc.size() > 10) { why = path + " has " + std::to_string(hc.size() - 9) + " sample columns: --vcf-sample NAME is required"; return false; }
+        v.sample_col = 9;
+    } else if (n_match == 0) { why = "--vcf-sample " + sample + ": no such sample in " + path; return false; }
+    else if (n_match > 1) { why = "--vcf-sample " + sample + " is ambiguous: " + std::to_string(n_match) + " sample columns of " + path + " have that name"; return false; }
+    return true;
+}
+
+bool write_all(int fd, const std::string &s) {
+    for (size_t done = 0; done < s.size();) {
+        const ssize_t w = ::write(fd, s.data() + done, s.size() - done);
+        if (w < 0) { if (errno == EINTR) continue; return false; }
+        done += (size_t)w;
+    }
+    return true;
+}
+
+// The five values of a counted record from the answers of its queries (REF first, then each countable ALT in order).
+std::string vcf_values(const VcfRecord &r, const brc_allele_answer *ans) {
+    if (!ans) return ".:.:.:.:.";
+    const uint32_t dp = ans[0].line ? ans[0].depth : 0;
+    std::string ad, adf, adr, af;
+    auto put = [&](const brc_allele_answer *a) {
+        ad += a ? std::to_string(a->stats[BRC_S_COUNT]) : "."; adf += a ? std::to_string(a->stats[BRC_S_PLUS]) : ".";
+        adr += a ? std::to_string(a->stats[BRC_S_MINUS]) : ".";
+    };
+    put(&ans[0]);
+    size_t k = 1;
+    for (size_t i = 0; i < r.alt_kind_len.size(); ++i) {
+        const brc_allele_answer *a = r.alt_kind_len[i] >= 0 ? &ans[k++] : nullptr;
+        ad += ','; adf += ','; adr += ',';
+        put(a);
+        if (i) af += ',';
+        if (!a || dp == 0) { af += '.'; continue; }
+        char b[64]; std::snprintf(b, sizeof b, "%.6g", (double)a->stats[BRC_S_COUNT] / (double)dp);
+        af += b;
+    }
+    return std::to_string(dp) + ":" + ad + ":" + adf + ":" + adr + ":" + af;
+}
+
+// One record line with the values in the chosen sample column.
+std::string vcf_line(const Vcf &v, const VcfRecord &r, const std::string &values) {
+    std::string out;
+    const size_t n = r.cols.size();
+    for (size_t c = 0; c < n; ++c) {
+        if (c) out += '\t';
+        if (c == 8) { out += r.cols[c]; out += kVcfFormat; continue; }
+        if ((int)c != v.sample_col) { out += r.cols[c]; continue; }
+        out += r.cols[c];
+        const size_t keys = (size_t)std::count(r.cols[8].begin(), r.cols[8].end(), ':') + 1;
+        for (size_t have = (size_t)std::count(r.cols[c].begin(), r.cols[c].end(), ':') + 1; have < keys; ++have) out += ":.";
+        out += ':'; out += values;
+    }
+    if (v.sample_col < 0) { out += '\t'; out += kVcfFormat + 1; out += '\t'; out += values; }
+    out += '\n';
+    return out;
+}
+
+std::string vcf_header(const Vcf &v) {
+    std::string out;
+    for (const std::string &h : v.header) { out += h; out += '\n'; }
+    out += kVcfHeader;
+    out += v.chrom_line;
+    if (v.sample_col < 0) { out += "\tFORMAT\t"; out += v.add_sample; }
+    out += '\n';
+    return out;
+}
+
 struct Options {   // everything on the command line except the inputs: the same for every sample
     int min_mapq = 0, min_bq = 0, max_cnt = 10000000; bool per_lib = false, ic = false; long long max_warn = -1;
+    const Vcf *vcf = nullptr;     // --vcf: the parsed file
     std::string fn_pos, fn_fa, dist_arg;
     std::vector<std::string> region_args;
     int shard_rank = 0, shard_count = 1;
@@ -853,6 +1058,7 @@ struct Sample {
     RgLib rg_lib;
     std::vector<std::string> lib_names; std::vector<const char *> lib_ptrs;
     std::vector<Region> regions;
+    std::vector<int64_t> vcf_region;   // --vcf: per record, the index of its site-list region (-1: not counted, or contig not in the BAM)
     Warner warner;
     // big fetches (windows of a cut region) of a BAM are decoded by several threads, one window ahead of the engine
     // (ParallelFetcher), unless the engine decodes the file itself (BRC_CLI_DEVICE_DECODE)
@@ -941,7 +1147,7 @@ std::unique_ptr<Sample> open_sample(const Options &o, const std::string &bam_pat
     for (auto &n : s.lib_names) s.lib_ptrs.push_back(n.c_str());
     if (s.lib_ptrs.empty()) s.lib_ptrs.push_back("");
 
-    if (o.fn_pos.empty() && o.region_args.empty()) {
+    if (o.fn_pos.empty() && o.region_args.empty() && !o.vcf) {
         log.say("Whole-file mode is not supported (the reference skips its per-read pre-processing there, R:...:624); give regions or -l\n");
         return sp;
     }
@@ -953,16 +1159,24 @@ std::unique_ptr<Sample> open_sample(const Options &o, const std::string &bam_pat
     if (!s.have_fa && !o.decode_only) { log.say("A reference FASTA (-f) is required in region / site-list mode\n"); return sp; }
 
     std::vector<Region> &regions = s.regions;
-    if (!o.fn_pos.empty()) {
+    // one line "name b e" of a site list: its region, or the -l loop's message when the BAM has no such contig
+    auto site_line = [&](const std::string &name, int b, int e) {
+        auto it = bam.tid_of.find(name);
+        if (it == bam.tid_of.end()) { log.say("%s not found in bam file. Region %s %i %i skipped.\n", name.c_str(), name.c_str(), b, e); return false; }
+        regions.push_back({it->second, b - 1, e, true});
+        return true;
+    };
+    if (o.vcf) {          // the derived site list: one line per counted record, in file order
+        for (const VcfRecord &r : o.vcf->rec)
+            s.vcf_region.push_back(r.counted && site_line(r.cols[0], r.line_pos, r.line_pos) ? (int64_t)regions.size() - 1 : -1);
+    } else if (!o.fn_pos.empty()) {
         std::ifstream fp(o.fn_pos);
         if (!fp) { log.say("Failed to open region list file: %s\n", o.fn_pos.c_str()); return sp; }
         std::string line;
         while (std::getline(fp, line)) {
             std::istringstream ss(line); std::string name; int b, e;
             if (!(ss >> name >> b >> e)) continue;
-            auto it = bam.tid_of.find(name);
-            if (it == bam.tid_of.end()) { log.say("%s not found in bam file. Region %s %i %i skipped.\n", name.c_str(), name.c_str(), b, e); continue; }
-            regions.push_back({it->second, b - 1, e, true});
+            site_line(name, b, e);
         }
     } else {
         int beg = 0, end = 0x7fffffff;
@@ -1085,38 +1299,80 @@ int run_sample(const Options &o, Engines &engines, Sample &s, int out_fd, FILE *
     }
 
     std::string chrom;
-    double t_decode = 0, t_compute = 0, t_format = 0, t_ref = 0, t_results = 0, t_reset = 0;
+    double t_decode = 0, t_compute = 0, t_format = 0, t_ref = 0, t_results = 0, t_reset = 0, ms_alleles = 0;
     // BRC_CLI_DEVICE_DECODE=1: BGZF inflate + BAM framing on the GPU (per-read warning lines need host-decoded reads: counts only)
     std::vector<const char *> rg_ids; std::vector<uint16_t> rg_libs;
     for (const auto &kv : s.rg_lib) { rg_ids.push_back(kv.first.c_str()); rg_libs.push_back(kv.second); }
     int64_t warn_total[4] = {0, 0, 0, 0};
+    // --vcf: the records go out in file order, each once its region's batch is computed; the values of the records answered so far
+    const Vcf *vcf = o.vcf;
+    std::vector<int64_t> vcf_rec_of_region(regions.size(), -1);
+    for (size_t k = 0; k < s.vcf_region.size(); ++k) if (s.vcf_region[k] >= 0) vcf_rec_of_region[(size_t)s.vcf_region[k]] = (int64_t)k;
+    std::vector<std::string> vcf_vals(vcf ? vcf->rec.size() : 0);
+    size_t vcf_next = 0;
+    auto vcf_write = [&](int64_t regions_done) {     // every record not yet written whose region is done (or that has none)
+        std::string out;
+        for (; vcf_next < vcf_vals.size() && s.vcf_region[vcf_next] < regions_done; ++vcf_next)
+            out += vcf_line(*vcf, vcf->rec[vcf_next], s.vcf_region[vcf_next] < 0 ? vcf_values(vcf->rec[vcf_next], nullptr) : vcf_vals[vcf_next]);
+        return write_all(out_fd, out);
+    };
+    if (vcf && !o.decode_only && !write_all(out_fd, vcf_header(*vcf))) { std::fprintf(err, "writing the VCF: %s\n", std::strerror(errno)); return 1; }
+    int64_t batch_first = 0, batch_n = 0;            // the regions begun since the last brc_reset
     auto flush = [&]() -> int {
+        int r;
+        std::vector<brc_allele_query> q;
+        std::string q_bases;
+        if (vcf) {            // the REF entry and every countable ALT of each record of the batch
+            for (int64_t g = 0; g < batch_n; ++g) {
+                const VcfRecord &rec = vcf->rec[(size_t)vcf_rec_of_region[(size_t)(batch_first + g)]];
+                q.push_back({g, rec.line_pos - 1, rec.ref_kind, 0});
+                for (size_t i = 0; i < rec.alt_kind_len.size(); ++i)
+                    if (rec.alt_kind_len[i] >= 0) { q.push_back({g, rec.line_pos - 1, (uint32_t)rec.alt_kind_len[i], (int64_t)q_bases.size()}); q_bases += rec.alt_bases[i]; }
+            }
+            if ((r = brc_set_allele_queries(eng, q.data(), (int64_t)q.size(), q_bases.data(), (int64_t)q_bases.size())) != BRC_OK) { std::fprintf(err, "brc_set_allele_queries: %s\n", brc_last_error(eng)); return r; }
+        }
         const double c0 = now();
-        int r = brc_compute(eng);
+        r = brc_compute(eng);
         t_compute += now() - c0;
         if (r != BRC_OK) { std::fprintf(err, "brc_compute: %s\n", brc_last_error(eng)); return r; }
         brc_results res{};
         const double g0 = now();
-        if (o.site_filter) {          // only the selected sites came back: no dense view, the region table is all the loop needs
-            brc_selected_results sel{};
-            if ((r = brc_get_selected_results(eng, &sel)) != BRC_OK) { std::fprintf(err, "brc_get_selected_results: %s\n", brc_last_error(eng)); return r; }
-            res.n_regions = sel.n_regions; res.regions = sel.regions;
-        } else if ((r = brc_get_results(eng, &res)) != BRC_OK) { std::fprintf(err, "brc_get_results: %s\n", brc_last_error(eng)); return r; }
-        const double f0 = now();
-        t_results += f0 - g0;
-        const bool argv_chain = res.n_regions > 1 && !res.regions[0].site_list_mode;   // never-cleared deletion queue: one sequential pass
-        int64_t total_slots = 0;
-        for (int64_t g = 0; g < res.n_regions; ++g) total_slots += res.regions[g].n_slots;
-        const bool many_small = res.n_regions > 1 && total_slots <= (int64_t(1) << 22);  // a site list: all regions in one formatting pass
-        if (argv_chain || many_small) {
-            if (brc_write_text(eng, -1, 0, -1, lib_ptrs.data(), out_fd) < 0) { std::fprintf(err, "format: %s\n", brc_last_error(eng)); return -1; }
+        if (vcf) {
+            const brc_allele_answer *ans = nullptr; int64_t n_ans = 0;
+            if ((r = brc_get_allele_answers(eng, &ans, &n_ans)) != BRC_OK || n_ans != (int64_t)q.size()) { std::fprintf(err, "brc_get_allele_answers: %s\n", brc_last_error(eng)); return r ? r : -1; }
+            t_results += now() - g0;
+            if (o.timing) ms_alleles += brc_last_stage_ms(eng, 4);
+            const double f0 = now();
+            for (int64_t g = 0, k = 0; g < batch_n; ++g) {
+                const int64_t ri = vcf_rec_of_region[(size_t)(batch_first + g)];
+                vcf_vals[(size_t)ri] = vcf_values(vcf->rec[(size_t)ri], ans + k);
+                k += 1 + std::count_if(vcf->rec[(size_t)ri].alt_kind_len.begin(), vcf->rec[(size_t)ri].alt_kind_len.end(), [](int64_t x) { return x >= 0; });
+            }
+            if (!vcf_write(batch_first + batch_n)) { std::fprintf(err, "writing the VCF: %s\n", std::strerror(errno)); return -1; }
+            t_format += now() - f0;
         } else {
-            const int64_t WIN = 1 << 21;   // stream big regions in 2M-site windows (each formatted by several threads)
-            for (int64_t g = 0; g < res.n_regions; ++g)
-                for (int64_t first = 0; first < res.regions[g].n_slots; first += WIN)
-                    if (brc_write_text(eng, g, first, WIN, lib_ptrs.data(), out_fd) < 0) { std::fprintf(err, "format: %s\n", brc_last_error(eng)); return -1; }
+            if (o.site_filter) {          // only the selected sites came back: no dense view, the region table is all the loop needs
+                brc_selected_results sel{};
+                if ((r = brc_get_selected_results(eng, &sel)) != BRC_OK) { std::fprintf(err, "brc_get_selected_results: %s\n", brc_last_error(eng)); return r; }
+                res.n_regions = sel.n_regions; res.regions = sel.regions;
+            } else if ((r = brc_get_results(eng, &res)) != BRC_OK) { std::fprintf(err, "brc_get_results: %s\n", brc_last_error(eng)); return r; }
+            const double f0 = now();
+            t_results += f0 - g0;
+            const bool argv_chain = res.n_regions > 1 && !res.regions[0].site_list_mode;   // never-cleared deletion queue: one sequential pass
+            int64_t total_slots = 0;
+            for (int64_t g = 0; g < res.n_regions; ++g) total_slots += res.regions[g].n_slots;
+            const bool many_small = res.n_regions > 1 && total_slots <= (int64_t(1) << 22);  // a site list: all regions in one formatting pass
+            if (argv_chain || many_small) {
+                if (brc_write_text(eng, -1, 0, -1, lib_ptrs.data(), out_fd) < 0) { std::fprintf(err, "format: %s\n", brc_last_error(eng)); return -1; }
+            } else {
+                const int64_t WIN = 1 << 21;   // stream big regions in 2M-site windows (each formatted by several threads)
+                for (int64_t g = 0; g < res.n_regions; ++g)
+                    for (int64_t first = 0; first < res.regions[g].n_slots; first += WIN)
+                        if (brc_write_text(eng, g, first, WIN, lib_ptrs.data(), out_fd) < 0) { std::fprintf(err, "format: %s\n", brc_last_error(eng)); return -1; }
+            }
+            t_format += now() - f0;
         }
-        t_format += now() - f0;
+        batch_first += batch_n; batch_n = 0;
         { int64_t wc[4]; if (brc_get_warning_counts(eng, wc) == BRC_OK) for (int k = 0; k < 4; ++k) warn_total[k] += wc[k]; }
         warner.replay();
         const double r0 = now();
@@ -1150,6 +1406,7 @@ int run_sample(const Options &o, Engines &engines, Sample &s, int out_fd, FILE *
         WindowJob *job = window ? s.decoded_window(gi) : nullptr;      // nullptr: the record stream after all
         if (!o.decode_only) {
             brc_begin_region(eng, g.tid, g.beg, g.end, g.site_list ? 1 : 0);
+            ++batch_n;
             warner.begin_region(g.tid, g.beg, g.end, g.cont);
         }
         // samfetch(in, idx, ref, d.beg-1, d.end): records with tid, endpos > max(beg-1,0), pos < end, in file order
@@ -1214,6 +1471,7 @@ int run_sample(const Options &o, Engines &engines, Sample &s, int out_fd, FILE *
         // at region boundaries (the deletion queue of the argv loop is carried by the engine, brc_set_queue_carry)
         if (job || span || gi + 1 == regions.size() || pushed > 1500000) { if (flush() != BRC_OK) return 1; pushed = 0; }
     }
+    if (vcf && !o.decode_only && !vcf_write(INT64_MAX)) { std::fprintf(err, "writing the VCF: %s\n", std::strerror(errno)); return 1; }
     warner.finish(warn_total);
 #ifdef BRC_WITH_HTSLIB
     const bool decode_error = bam.bz.error || s.hts.error || s.par_decode_error;
@@ -1228,6 +1486,7 @@ int run_sample(const Options &o, Engines &engines, Sample &s, int out_fd, FILE *
     if (o.timing) std::fprintf(err, "[brc timing] reference %.3fs  decode+push %.3fs  compute %.3fs  results %.3fs  format %.3fs  reset %.3fs  | region loop %.3fs, since main() %.3fs\n",
                                t_ref, t_decode, t_compute, t_results, t_format, t_reset, now() - t_loop0, now() - t_main0);
     if (o.timing) std::fprintf(err, "[brc timing] startup (CUDA context, header, index, first window) %.3fs\n", t_loop0 - s.t0);
+    if (o.timing && vcf) std::fprintf(err, "[brc timing] allele kernels %.3f ms\n", ms_alleles);
     return decode_error ? 1 : 0;
 }
 
@@ -1360,11 +1619,12 @@ int run_cohort(const Options &o, Engines &engines, const std::string &list_path,
 int main(int argc, char **argv) {
     const double t_main0 = now();
     Options o;
-    std::string bam_list; bool shard_given = false;
+    std::string bam_list, vcf_path, vcf_sample; bool shard_given = false, vcf_sample_given = false;
     static option lo[] = {{"help", 0, 0, 'h'}, {"version", 0, 0, 'v'}, {"min-mapping-quality", 1, 0, 'q'}, {"min-base-quality", 1, 0, 'b'},
                           {"max-count", 1, 0, 'd'}, {"site-list", 1, 0, 'l'}, {"reference-fasta", 1, 0, 'f'}, {"print-individual-mapq", 1, 0, 'D'},
                           {"per-library", 0, 0, 'p'}, {"max-warnings", 1, 0, 'w'}, {"insertion-centric", 0, 0, 'i'}, {"shard", 1, 0, 1000},
-                          {"min-alt-count", 1, 0, 1001}, {"min-alt-fraction", 1, 0, 1002}, {"bam-list", 1, 0, 1003}, {0, 0, 0, 0}};
+                          {"min-alt-count", 1, 0, 1001}, {"min-alt-fraction", 1, 0, 1002}, {"bam-list", 1, 0, 1003},
+                          {"vcf", 1, 0, 1004}, {"vcf-sample", 1, 0, 1005}, {0, 0, 0, 0}};
     long min_alt_count = 0; double min_alt_fraction = -1.0;       // site filter (brc_set_site_filter); off unless one is given
     bool help = false, version = false;
     for (int c; (c = getopt_long(argc, argv, "hvq:b:d:l:f:D:pw:i", lo, nullptr)) != -1;) {
@@ -1388,6 +1648,8 @@ int main(int argc, char **argv) {
             break;
         }
         case 1003: bam_list = optarg; break;
+        case 1004: vcf_path = optarg; break;
+        case 1005: vcf_sample = optarg; vcf_sample_given = true; break;
         default: usage(); return 1;
         }
     }
@@ -1396,6 +1658,16 @@ int main(int argc, char **argv) {
     if (version) { std::printf("bam-readcount version: b200 (engine ABI %d)\n", brc_abi_version()); return 1; }   // R:...:467-470 (exit 1)
     if (help || (optind >= argc && bam_list.empty())) { usage(); return 1; }                                        // R:...:472-475
     if (!bam_list.empty() && shard_given) { std::fprintf(stderr, "--bam-list and --shard cannot be combined: shard a cohort by splitting its list\n"); return 1; }
+    Vcf vcf;
+    if (vcf_sample_given && vcf_path.empty()) { std::fprintf(stderr, "--vcf-sample needs --vcf\n"); return 1; }
+    if (!vcf_path.empty()) {
+        const char *clash = !o.fn_pos.empty() ? "-l" : optind + 1 < argc ? "positional regions" : o.per_lib ? "-p" : o.site_filter ? "--min-alt-count/--min-alt-fraction"
+                          : shard_given ? "--shard" : !bam_list.empty() ? "--bam-list" : nullptr;
+        if (clash) { std::fprintf(stderr, "--vcf cannot be combined with %s\n", clash); return 1; }
+        std::string why;
+        if (!parse_vcf(vcf_path, vcf_sample, vcf_sample_given, vcf, why)) { std::fprintf(stderr, "--vcf: %s\n", why.c_str()); return 1; }
+        o.vcf = &vcf;
+    }
     o.decode_only = std::getenv("BRC_CLI_DECODE_ONLY") != nullptr;   // test hook: exercise BGZF/BAI/region fetch without a GPU
     o.device_decode = std::getenv("BRC_CLI_DEVICE_DECODE") != nullptr && !o.decode_only;
     o.timing = std::getenv("BRC_CLI_TIMING") != nullptr;

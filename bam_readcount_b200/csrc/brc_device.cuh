@@ -25,6 +25,18 @@ constexpr uint8_t NO_BASE = 255;
 // flag bits the reference filters on (R:bamreadcount.cpp:295-310)
 constexpr uint32_t FLAG_FILTER = 4u | 256u | 512u | 1024u;
 
+// bam_nt16_canonical_table (R:bamreadcount.cpp:36-39): nibble -> index into "=ACGTN"; the text emitter prints insertion
+// bases through the same table (brc_format.cpp kCanon)
+__device__ __forceinline__ uint32_t canonical16(uint32_t nib) {
+    // packed 16 x 4-bit LUT: {0,1,2,5,3,5,5,5,4,5,5,5,5,5,5,5}
+    return (0x5555555455535210ull >> (nib * 4)) & 0xFu;
+}
+// 4-bit code of read base i of the packed bases starting at seq[off]
+__device__ __forceinline__ uint32_t seq_nib(const uint8_t *seq, uint64_t off, int i) {
+    uint32_t b = seq[off + (uint32_t)(i >> 1)];
+    return (i & 1) ? (b & 0xFu) : (b >> 4);
+}
+
 // ReadDesc.fm layout: flag[0:16) | mapq[16:24) | bits below
 constexpr uint32_t FM_SIMPLE = 1u << 24;     // CIGAR has exactly one ref-consuming op, of match type, and no I/D/N/P
 constexpr uint32_t FM_NM_ABSENT = 1u << 25;  // NM tag missing -> NM_TAG_MISSING warning per process_read
@@ -257,6 +269,86 @@ struct SelectParams {
     SecRec *c_sec;
 };
 
+#ifdef __CUDACC__   // device atomics: not for the host-only translation units
+// ---- the line a site forms (brc_format.cpp format_site), as the device sees it in the packed records ----
+// One definition for the site selection (brc_select.cu) and the allele queries (brc_alleles.cu).
+// Row r spans site s (column idx = r * n_slots + s): an escaped primary, or ncover > 0.  RS = n_rows * n_slots.
+__device__ __forceinline__ bool row_covers(const uint32_t *words, int64_t RS, int64_t idx) {
+    return (words[RS + idx] & 7u) == PB_ESCAPE || (words[idx] & 0xFFu) != 0u;
+}
+// Some row has a read without library at site s: -p abandons the site (no line, and its deletions are never queued).
+__device__ __forceinline__ bool site_abandoned(const uint32_t *words, int n_rows, int64_t NS, int64_t s) {
+    const int64_t RS = (int64_t)n_rows * NS;
+    bool ab = false;
+    for (int r = 0; r < n_rows; ++r) ab |= (words[RS + (int64_t)r * NS + s] & 8u) != 0u;
+    return ab;
+}
+// Pool pass, one secondary-pool record: what it adds to the depth of a line.  An escaped primary adds its npass to esc_np[s];
+// a deletion adds its count to dsum[s] (extra depth of the next site's line) when the same row spans the next site, where the
+// row's block prints it.  Returns true for such a deletion.  dsum and esc_np are [n_slots], zeroed before the pass.
+__device__ __forceinline__ bool pool_depth_term(const uint32_t *words, int n_rows, int64_t NS, const SecRec &rec, uint32_t *dsum,
+                                                uint32_t *esc_np) {
+    const int64_t r = (int64_t)rec.slot / NS, s = (int64_t)rec.slot - r * NS;
+    const uint32_t kind = rec.kind_len & 0xFFu;
+    if (kind >= KIND_WIDE) { atomicAdd(&esc_np[s], (uint32_t)rec.qpos); return false; }
+    if (kind != (uint32_t)KIND_DEL || s + 1 >= NS || !row_covers(words, (int64_t)n_rows * NS, r * NS + s + 1)) return false;
+    atomicAdd(&dsum[s], rec.stats[BRC_S_COUNT]);
+    return true;
+}
+// Site pass, after the pool pass: does site s form a line (a row spans it and no row abandons it), and its depth (the line's
+// 4th column): Σ npass + the escaped primaries' npass + the deletions anchored at the left neighbour, when that neighbour is in
+// the same region (`left_in_region`) and formed a line of its own.  `left` reports that last condition.
+struct SiteLine { uint64_t depth; bool live, abandoned, left; };
+__device__ __forceinline__ SiteLine site_line(const uint32_t *words, int n_rows, int64_t NS, int64_t s, bool left_in_region,
+                                              const uint32_t *dsum, const uint32_t *esc_np) {
+    const int64_t RS = (int64_t)n_rows * NS;
+    SiteLine L{esc_np[s], false, false, false};
+    bool covered = false;
+    for (int r = 0; r < n_rows; ++r) {
+        const uint32_t w0 = words[(int64_t)r * NS + s], w1 = words[RS + (int64_t)r * NS + s];
+        L.abandoned |= (w1 & 8u) != 0u;
+        if ((w1 & 7u) == PB_ESCAPE) { covered = true; continue; }      // full-width primary: a pool record (esc_np)
+        covered |= (w0 & 0xFFu) != 0u;
+        L.depth += (w0 >> 8) & 0xFFu;
+    }
+    L.left = left_in_region && !site_abandoned(words, n_rows, NS, s - 1);
+    if (L.left) L.depth += dsum[s - 1];
+    L.live = covered && !L.abandoned;
+    return L;
+}
+
+#endif
+
+// ---- allele queries (brc_alleles.cu; brc_set_allele_queries, DESIGN.md §12) ----
+constexpr uint32_t NO_SLOT = 0xFFFFFFFFu;
+struct AlleleQuery {      // one query as the kernels see it; the host sorts them by `match`
+    uint32_t match;       // slot whose pool records hold the entry: the site's own, or its left neighbour's for a deletion;
+                          // NO_SLOT when no record can (a deletion whose anchor lies outside the region, a site without a slot)
+    uint32_t kind_len;    // as brc_allele_query (base classes with length 0)
+    uint32_t site;        // slot of the queried site; NO_SLOT when the region computed none for it (no read reaches it)
+    uint32_t left;        // 1: the left neighbour is in the same region
+    int64_t bases_off;    // insertion: offset of its bases in AlleleParams::bases (indices into "=ACGTN")
+    int64_t out;          // index of its answer (the caller's order)
+};
+static_assert(sizeof(AlleleQuery) == 32, "AlleleQuery is 32 bytes");
+static_assert(sizeof(brc_allele_answer) == 64, "brc_allele_answer is 64 bytes");
+
+struct AlleleParams {
+    const uint32_t *words;  // [N_WORDS][rows*slots]
+    int32_t n_rows;
+    int64_t n_slots;
+    const SecRec *sec;
+    const int32_t *sec_count;
+    int64_t sec_cap;
+    const uint64_t *seq_off;  // the device batch: packed bases of a record's representative read (insertion alleles)
+    const uint8_t *seq;
+    const AlleleQuery *q;
+    int64_t n_q;
+    const uint8_t *bases;
+    uint32_t *dsum, *esc_np;  // [n_slots] each, zeroed before the record pass
+    brc_allele_answer *ans;   // [n_q], zeroed before the record pass
+};
+
 // launch wrappers (brc_kernels.cu)
 cudaError_t launch_init_tiles(int32_t *tile_lo, int32_t *tile_hi, int64_t n_tiles, int32_t *sec_count,
                               unsigned long long *warn, int n_dispensers, cudaStream_t s);
@@ -271,5 +363,8 @@ cudaError_t launch_fastmath_selftest(int max_b, unsigned long long *d_bad, cudaS
 constexpr int SELECT_KERNELS = 8;
 constexpr int SELECT_SCAN_CTA = 256;   // sites per scan partial (SelectParams::nb = ceil(n_slots / SELECT_SCAN_CTA))
 cudaError_t launch_select(const SelectParams &p, cudaStream_t s);
+// brc_alleles.cu: record pass, query pass (ALLELE_KERNELS launches; the scratch and answers are zeroed by the caller)
+constexpr int ALLELE_KERNELS = 2;
+cudaError_t launch_alleles(const AlleleParams &p, cudaStream_t s);
 
 }  // namespace brc

@@ -129,12 +129,12 @@ void brc_destroy(brc_engine *e) {
     cudaDeviceSynchronize();
     for (auto &r : e->refs) r.dev.release();
     DevBuf *bufs[] = {&e->d_refs, &e->d_desc, &e->d_tiles, &e->d_tile_lo, &e->d_tile_hi, &e->d_regions, &e->d_deep_tiles,
-                      &e->d_words, &e->d_sec, &e->d_sec_count, &e->d_warn, &e->d_sel, &e->d_sel_regions};
+                      &e->d_words, &e->d_sec, &e->d_sec_count, &e->d_warn, &e->d_sel, &e->d_sel_regions, &e->d_aq};
     for (auto *b : bufs) b->release();
     for (auto &b : e->d_in) b.release();
     { brc_engine::Decoded &D = e->dec; DevBuf *db[] = {&D.comp, &D.btab, &D.u, &D.meta, &D.scratch, &D.count, &D.partial, &D.cigar, &D.seq, &D.qual, &D.ins_idx, &D.ins_out};
       for (auto *b : db) b->release(); for (auto &b : D.arr) b.release(); }
-    PinBuf *pins[] = {&e->h_words, &e->h_sec, &e->h_misc, &e->h_sel};
+    PinBuf *pins[] = {&e->h_words, &e->h_sec, &e->h_misc, &e->h_sel, &e->h_ans};
     for (auto *b : pins) b->release();
     for (auto &ev : e->ev) if (ev) cudaEventDestroy(ev);
     for (auto &ev : e->pipe_ev) if (ev) cudaEventDestroy(ev);
@@ -168,11 +168,16 @@ int brc_set_reference_device(brc_engine *e, int32_t tid, const char *contig_name
     return install_ref(e, tid, contig_name, chrom_len, win_beg, win_len, nullptr, dev_ascii, (cudaStream_t)stream);
 }
 
+static void drop_allele_queries(brc_engine *e) {
+    e->queries_on = false; e->aq.clear(); e->aq_bases.clear(); e->aq_launched = false; e->answers_valid = false;
+}
+
 int brc_reset(brc_engine *e) {
     if (!e) return BRC_E_INVALID;
     e->reads.clear(); e->is_borrowed = false; e->regions.clear(); e->region_open = false; e->adm.reset(); e->n_indel_ops = 0;
     e->results_valid = false; e->planned = false; e->tiles.clear(); e->regions_dev.clear(); e->n_slots = 0; e->wide.valid = false;
     e->sparse = false; e->sel_launched = false; e->n_sel = 0;
+    drop_allele_queries(e);
     e->dec.pushed = false; e->dec.ins_reads.clear(); e->dec.ins_off.clear(); e->dec.ins_pool.clear();
     for (auto &w : e->warn_counts) w = 0;
     return BRC_OK;
@@ -219,6 +224,7 @@ int brc_begin_region(brc_engine *e, int32_t tid, int32_t beg, int32_t end, int32
     e->regions.push_back(r);
     e->region_open = true; e->adm.reset(); e->open_max_end = r.first_pos;
     e->results_valid = false; e->planned = false;
+    drop_allele_queries(e);
     return BRC_OK;
 }
 
@@ -543,7 +549,58 @@ static int fetch_selected(brc_engine *e, cudaStream_t s) {
     CU(cudaStreamSynchronize(s), "sync D2H");
     e->warn_counts[0] = (int64_t)hm[4]; e->warn_counts[1] = (int64_t)hm[5]; e->warn_counts[2] = 0;
     e->warn_counts[3] = -1;
-    e->n_sel = n; e->h_n_sec = ns; e->sparse = true;
+    e->n_sel = n; e->h_n_sec = ns; e->sparse = true; e->answers_valid = false;
+    e->results_valid = true; e->fmt_valid = false; e->wide.valid = false;
+    return BRC_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// allele queries: launch, answer fetch (kernels in brc_alleles.cu)
+// ---------------------------------------------------------------------------------------------
+// The allele kernels after the pileup kernels on stream s (ev[3], ev[4] around them); no-op without queries.
+static int launch_allele_queries(brc_engine *e, cudaStream_t s) {
+    e->aq_launched = false;
+    if (!e->queries_on) return BRC_OK;
+    const int64_t NS = e->n_slots, nq = (int64_t)e->aq.size(), nb = (int64_t)e->aq_bases.size();
+    size_t off = 0;
+    auto take = [&](size_t bytes) { const size_t o = off; off = (off + bytes + 15) & ~(size_t)15; return o; };
+    const size_t o_q = take((size_t)nq * sizeof(AlleleQuery)), o_b = take((size_t)nb), o_scr = take((size_t)NS * 8);
+    const size_t o_ans = take((size_t)nq * sizeof(brc_allele_answer));
+    CU(e->d_aq.reserve(std::max<size_t>(off, 16)), "cudaMalloc(allele queries)");
+    char *b = e->d_aq.as<char>();
+    if (nq) CU(cudaMemcpyAsync(b + o_q, e->aq.data(), (size_t)nq * sizeof(AlleleQuery), cudaMemcpyHostToDevice, s), "H2D allele queries");
+    if (nb) CU(cudaMemcpyAsync(b + o_b, e->aq_bases.data(), (size_t)nb, cudaMemcpyHostToDevice, s), "H2D insertion bases");
+    CU(cudaMemsetAsync(b + o_scr, 0, off - o_scr, s), "memset(allele scratch)");
+    AlleleParams P{};
+    P.words = e->d_words.as<uint32_t>(); P.n_rows = e->n_rows; P.n_slots = NS;
+    P.sec = e->d_sec.as<SecRec>(); P.sec_count = e->d_sec_count.as<int32_t>(); P.sec_cap = e->sec_cap;
+    P.seq_off = e->dev_reads.seq_off; P.seq = e->dev_reads.seq;
+    P.q = reinterpret_cast<const AlleleQuery *>(b + o_q); P.n_q = nq; P.bases = reinterpret_cast<const uint8_t *>(b + o_b);
+    P.dsum = reinterpret_cast<uint32_t *>(b + o_scr); P.esc_np = P.dsum + NS;
+    P.ans = reinterpret_cast<brc_allele_answer *>(b + o_ans);
+    CU(cudaEventRecord(e->ev[3], s), "event");
+    CU(launch_alleles(P, s), "launch allele queries");
+    if (nq) e->launch_count += ALLELE_KERNELS;
+    CU(cudaEventRecord(e->ev[4], s), "event");
+    e->aq_params = P;
+    e->aq_launched = true;
+    return BRC_OK;
+}
+
+// The answers, the warning words and the pool counter to the host: nothing else of the run crosses PCIe.
+static int fetch_answers(brc_engine *e, cudaStream_t s) {
+    const AlleleParams &P = e->aq_params;
+    CU(e->h_misc.reserve(64), "pin");
+    CU(e->h_ans.reserve((size_t)std::max<int64_t>(P.n_q, 1) * sizeof(brc_allele_answer)), "pin");
+    uint64_t *hm = e->h_misc.as<uint64_t>();
+    CU(cudaMemcpyAsync(hm, e->d_sec_count.p, 4, cudaMemcpyDeviceToHost, s), "D2H sec_count");
+    CU(cudaMemcpyAsync(hm + 4, e->d_warn.p, 16, cudaMemcpyDeviceToHost, s), "D2H warn");
+    if (P.n_q) CU(cudaMemcpyAsync(e->h_ans.p, P.ans, (size_t)P.n_q * sizeof(brc_allele_answer), cudaMemcpyDeviceToHost, s), "D2H allele answers");
+    CU(cudaStreamSynchronize(s), "sync D2H");
+    if ((int64_t)*e->h_misc.as<int32_t>() > e->sec_cap) return set_error(e, BRC_E_OVERFLOW, "secondary key pool overflow (re-plan with a larger n_sec_cap)");
+    e->warn_counts[0] = (int64_t)hm[4]; e->warn_counts[1] = (int64_t)hm[5]; e->warn_counts[2] = 0;
+    e->warn_counts[3] = 0;           // LIBRARY_UNAVAILABLE needs -p, which allele queries refuse
+    e->h_n_sec = 0; e->sparse = false; e->answers_valid = true;
     e->results_valid = true; e->fmt_valid = false; e->wide.valid = false;
     return BRC_OK;
 }
@@ -577,7 +634,8 @@ static int run_kernels(brc_engine *e, const int32_t *d_region_of_read, cudaStrea
     CU(launch_pileup(P1, s), "launch pileup"); if (P1.n_tiles) e->launch_count++;
     CU(launch_deep_sites(P1, s), "launch deep_sites"); if (P1.n_deep) e->launch_count++;
     CU(cudaEventRecord(e->ev[2], s), "event");
-    const int rs = launch_selection(e, s);
+    int rs = launch_selection(e, s);
+    if (rs == BRC_OK) rs = launch_allele_queries(e, s);
     if (rs != BRC_OK) return rs;
     if (check_overflow) {
         int32_t cnt = 0;
@@ -591,6 +649,7 @@ static int run_kernels(brc_engine *e, const int32_t *d_region_of_read, cudaStrea
 
 static int fetch_results(brc_engine *e, cudaStream_t s, bool slots_already_fetched = false, int64_t sec_done = 0) {
     if (e->sel_launched) return fetch_selected(e, s);
+    if (e->aq_launched) return fetch_answers(e, s);
     const int64_t rs = (int64_t)e->n_rows * e->n_slots;
     int32_t cnt = 0;
     CU(cudaMemcpyAsync(&cnt, e->d_sec_count.p, 4, cudaMemcpyDeviceToHost, s), "D2H sec_count");
@@ -609,7 +668,7 @@ static int fetch_results(brc_engine *e, cudaStream_t s, bool slots_already_fetch
     const unsigned long long *w = e->h_misc.as<unsigned long long>();
     e->warn_counts[0] = (int64_t)w[0]; e->warn_counts[1] = (int64_t)w[1]; e->warn_counts[2] = 0;
     e->warn_counts[3] = -1;          // LIBRARY_UNAVAILABLE: counted from the flag bits on demand (brc_get_warning_counts)
-    e->sparse = false;
+    e->sparse = false; e->answers_valid = false;
     e->results_valid = true; e->fmt_valid = false; e->wide.valid = false;
     return BRC_OK;
 }
@@ -748,8 +807,9 @@ static int compute_pipelined(brc_engine *e) {
     int rc = issue_h2d_chunks(e, n_chunks);
     if (rc != BRC_OK) return rc;
     e->dev_reads = reads_dev(d_in_batch(e, n));
-    // host result buffers (with a site filter only the compacted selection comes back, after the kernels: fetch_selected)
-    const bool sel = e->filter_on;
+    // host result buffers (with a site filter only the compacted selection comes back, after the kernels: fetch_selected; with
+    // allele queries only their answers: fetch_answers)
+    const bool sel = e->filter_on || e->queries_on;
     const int64_t rs1 = std::max<int64_t>(rs, 1);
     if (!sel) CU(e->h_words.reserve(rs1 * 4 * N_WORDS), "pin");
     CU(e->h_sec.reserve((size_t)e->sec_cap * sizeof(SecRec)), "pin");          // pool records leave while the kernels run
@@ -809,6 +869,7 @@ static int compute_pipelined(brc_engine *e) {
     CU(cudaEventRecord(e->ev[1], sk), "event");
     CU(cudaEventRecord(e->ev[2], sk), "event");
     rc = launch_selection(e, sk);
+    if (rc == BRC_OK) rc = launch_allele_queries(e, sk);
     if (rc != BRC_OK) return rc;
     // everything is queued: follow the kernels and ship the pool records each chunk finished (their own stream: the word copies
     // of later chunks are already queued on s_out)
@@ -904,6 +965,7 @@ int brc_get_results(brc_engine *e, brc_results *out) {
     if (!e || !out) return BRC_E_INVALID;
     if (!e->results_valid) return set_error(e, BRC_E_INVALID, "get_results: no results (call brc_compute)");
     if (e->sparse) return set_error(e, BRC_E_INVALID, "get_results: a site filter is set, there is no dense view (brc_get_selected_results)");
+    if (e->answers_valid) return set_error(e, BRC_E_INVALID, "get_results: allele queries are set, there is no dense view (brc_get_allele_answers)");
     brc::ensure_wide(e);
     const brc_engine::Wide &W = e->wide;
     out->n_regions = (int64_t)e->regions.size(); out->regions = e->regions.data(); out->n_rows = e->n_rows; out->n_slots = e->n_slots;
@@ -919,6 +981,7 @@ int brc_get_packed_results(brc_engine *e, brc_packed_results *out) {
     if (!e || !out) return BRC_E_INVALID;
     if (!e->results_valid) return set_error(e, BRC_E_INVALID, "get_packed_results: no results (call brc_compute)");
     if (e->sparse) return set_error(e, BRC_E_INVALID, "get_packed_results: a site filter is set, there is no dense view (brc_get_selected_results)");
+    if (e->answers_valid) return set_error(e, BRC_E_INVALID, "get_packed_results: allele queries are set, there is no dense view (brc_get_allele_answers)");
     out->n_regions = (int64_t)e->regions.size(); out->regions = e->regions.data(); out->n_rows = e->n_rows; out->n_slots = e->n_slots;
     out->words = e->h_words.as<uint32_t>(); out->n_sec = e->h_n_sec; out->sec = e->h_sec.as<brc_sec_record>(); out->sec_count = nullptr;
     return BRC_OK;
@@ -949,6 +1012,7 @@ int brc_plan_device(brc_engine *e, const brc_region *regions, int64_t n_regions,
     cudaSetDevice(e->cfg.device);
     e->regions.assign(regions, regions + n_regions);
     e->region_open = false; e->results_valid = false;
+    drop_allele_queries(e);
     int rc = build_geometry(e, e->regions.data(), n_regions);
     if (rc != BRC_OK) return rc;
     rc = alloc_outputs(e, n_reads_cap);
@@ -993,6 +1057,7 @@ int brc_last_launch_count(const brc_engine *e) { return e ? e->launch_count : 0;
 int brc_set_site_filter(brc_engine *e, const brc_site_filter *f) {
     if (!e) return BRC_E_INVALID;
     if (!f) { e->filter_on = false; e->filter = brc_site_filter{}; return BRC_OK; }
+    if (e->queries_on) return set_error(e, BRC_E_INVALID, "set_site_filter: allele queries are set (brc_reset drops them)");
     if (f->min_alt_count < 1 || f->reserved != 0 || !(f->min_alt_fraction >= 0.0 && f->min_alt_fraction <= 1.0))
         return set_error(e, BRC_E_INVALID, "set_site_filter: min_alt_count must be >= 1 and min_alt_fraction in [0, 1]");
     e->filter = *f; e->filter_on = true;
@@ -1006,6 +1071,54 @@ int brc_get_selected_results(brc_engine *e, brc_selected_results *out) {
     out->n_regions = (int64_t)e->regions.size(); out->regions = e->regions.data(); out->n_rows = e->n_rows; out->n_slots = e->n_slots;
     out->n_sites = e->n_sel; out->site = e->sel_site(); out->emit = e->sel_emit(); out->words = e->h_words.as<uint32_t>();
     out->n_sec = e->h_n_sec; out->sec = e->h_sec.as<brc_sec_record>();
+    return BRC_OK;
+}
+
+int brc_set_allele_queries(brc_engine *e, const brc_allele_query *q, int64_t n, const char *bases, int64_t n_bases) {
+    if (!e) return BRC_E_INVALID;
+    drop_allele_queries(e);
+    if (n < 0 || (n > 0 && !q) || n_bases < 0 || (n_bases > 0 && !bases)) return set_error(e, BRC_E_INVALID, "set_allele_queries: bad arguments");
+    if (e->region_open) return set_error(e, BRC_E_INVALID, "set_allele_queries: a region is still open");
+    if (e->n_rows != 1) return set_error(e, BRC_E_INVALID, "set_allele_queries: per-library rows are not supported");
+    if (e->filter_on) return set_error(e, BRC_E_INVALID, "set_allele_queries: a site filter is set");
+    std::vector<AlleleQuery> aq((size_t)n);
+    std::vector<uint8_t> codes;
+    for (int64_t i = 0; i < n; ++i) {
+        const brc_allele_query &x = q[i];
+        if (x.region < 0 || x.region >= (int64_t)e->regions.size()) return set_error(e, BRC_E_INVALID, "set_allele_queries: region index out of range");
+        const brc_region &r = e->regions[(size_t)x.region];
+        if (x.pos < r.beg || x.pos >= r.end) return set_error(e, BRC_E_INVALID, "set_allele_queries: position outside the region's printed sites");
+        const uint32_t kind = x.kind_len & 0xFFu, len = x.kind_len >> 8;
+        if (!(kind < 6u ? len == 0u : (kind == (uint32_t)KIND_INS || kind == (uint32_t)KIND_DEL) && len >= 1u))
+            return set_error(e, BRC_E_INVALID, "set_allele_queries: invalid kind / length");
+        AlleleQuery &a = aq[(size_t)i];
+        const int64_t o = (int64_t)x.pos - r.first_pos;
+        a.kind_len = x.kind_len; a.out = i; a.left = o > 0 ? 1u : 0u;
+        a.site = o < r.n_slots ? (uint32_t)(r.slot_base + o) : NO_SLOT;
+        a.match = a.site;
+        if (kind == (uint32_t)KIND_DEL) a.match = o > 0 && o - 1 < r.n_slots ? (uint32_t)(r.slot_base + o - 1) : NO_SLOT;
+        a.bases_off = 0;
+        if (kind == (uint32_t)KIND_INS) {
+            if (x.bases_off < 0 || x.bases_off > n_bases || (int64_t)len > n_bases - x.bases_off)
+                return set_error(e, BRC_E_INVALID, "set_allele_queries: insertion bases outside the buffer");
+            a.bases_off = (int64_t)codes.size();
+            for (uint32_t k = 0; k < len; ++k) {
+                const char *p = std::strchr("ACGTN", bases[x.bases_off + k]);
+                if (!p || !*p) return set_error(e, BRC_E_INVALID, "set_allele_queries: insertion bases must be A, C, G, T or N");
+                codes.push_back((uint8_t)(1 + (p - "ACGTN")));      // index into "=ACGTN"
+            }
+        }
+    }
+    std::stable_sort(aq.begin(), aq.end(), [](const AlleleQuery &a, const AlleleQuery &b) { return a.match < b.match; });
+    e->aq.swap(aq); e->aq_bases.swap(codes);
+    e->queries_on = true;
+    return BRC_OK;
+}
+
+int brc_get_allele_answers(brc_engine *e, const brc_allele_answer **out, int64_t *n) {
+    if (!e || !out || !n) return BRC_E_INVALID;
+    if (!e->results_valid || !e->answers_valid) return set_error(e, BRC_E_INVALID, "get_allele_answers: the last run had no allele queries");
+    *out = e->h_ans.as<brc_allele_answer>(); *n = e->aq_params.n_q;
     return BRC_OK;
 }
 
@@ -1036,7 +1149,12 @@ void brc_host_free(void *p) { if (p) { cudaFreeHost(p); cudaGetLastError(); } }
 int64_t brc_last_h2d_bytes(const brc_engine *e) { return e ? e->h2d_bytes_last : 0; }
 
 float brc_last_stage_ms(const brc_engine *e, int stage) {
-    if (!e || stage < 0 || stage > 3 || (stage == 3 && !e->sel_launched)) return 0.0f;
+    if (!e || stage < 0 || stage > 4 || (stage == 3 && !e->sel_launched)) return 0.0f;
+    if (stage == 4) {   // the allele kernels, between ev[3] and ev[4] (launch_allele_queries)
+        float ms = 0.0f;
+        if (!e->aq_launched || cudaEventSynchronize(e->ev[4]) != cudaSuccess || cudaEventElapsedTime(&ms, e->ev[3], e->ev[4]) != cudaSuccess) { cudaGetLastError(); return 0.0f; }
+        return ms;
+    }
     // events were recorded on the launching stream around K0, K1 and the selection; wait for the last one
     if (cudaEventSynchronize(e->ev[stage == 3 ? 3 : 2]) != cudaSuccess) { cudaGetLastError(); return 0.0f; }
     float ms = 0.0f;

@@ -114,7 +114,7 @@ struct brc_engine {
     std::vector<cudaEvent_t> pipe_ev;
     int64_t h2d_bytes_last = 0;      // bytes the last push path actually sent over PCIe (after the elision below)
     int skip_h2d = 0;                // borrowed batch: bit0 seq_off, bit1 qual_off arithmetic; bit2 l_qseq, bit3 sm constant -> rebuilt on the device
-    cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
+    cudaEvent_t ev[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
     std::string err;
 
     std::vector<brc::HostRef> refs;
@@ -214,6 +214,17 @@ struct brc_engine {
     const uint32_t *sel_site() const { return h_sel.as<uint32_t>(); }
     const uint8_t *sel_emit() const { return reinterpret_cast<const uint8_t *>(h_sel.as<uint32_t>() + n_sel); }
     int64_t result_cols() const { return sparse ? n_sel : n_slots; }   // columns of the host word / wide arrays
+
+    // allele queries (brc_set_allele_queries, brc_alleles.cu).  With them set, the kernels' records stay on the device and only
+    // the answers cross PCIe; there is no dense view.
+    bool queries_on = false;
+    std::vector<brc::AlleleQuery> aq;          // sorted by match slot
+    std::vector<uint8_t> aq_bases;             // insertion bases as indices into "=ACGTN"
+    brc::DevBuf d_aq;                          // queries, bases, scratch, answers
+    bool aq_launched = false;                  // the last kernel run ended with the allele kernels
+    brc::AlleleParams aq_params{};
+    brc::PinBuf h_ans;
+    bool answers_valid = false;                // the last run's results are the answers in h_ans (no records on the host)
 
     int launch_count = 0;
 };

@@ -296,6 +296,7 @@ extern "C" int brc_set_queue_carry(brc_engine *e, int on) {
 extern "C" int64_t brc_format_text(brc_engine *e, int64_t region_index, const char *const *lib_names, char *buf, int64_t cap) {
     if (!e) return BRC_E_INVALID;
     if (!e->results_valid) return brc::set_error(e, BRC_E_INVALID, "format_text: no results");
+    if (e->answers_valid) return brc::set_error(e, BRC_E_INVALID, "format_text: allele queries are set, there is no text (brc_get_allele_answers)");
     if (e->n_host_reads() == 0 && e->h_n_sec > 0 && !e->dec.pushed) return brc::set_error(e, BRC_E_INVALID, "format_text: needs the pushed reads (push path only)");
     if (region_index >= (int64_t)e->regions.size()) return BRC_E_INVALID;
     return serve(e, region_index < 0 ? -1 : region_index, -1, -1, lib_names, buf, cap);
@@ -307,6 +308,7 @@ extern "C" int64_t brc_format_window(brc_engine *e, int64_t region_index, int64_
                                      char *buf, int64_t cap) {
     if (!e || region_index < 0 || region_index >= (int64_t)e->regions.size() || first < 0 || count < 0) return BRC_E_INVALID;
     if (!e->results_valid) return brc::set_error(e, BRC_E_INVALID, "format_window: no results");
+    if (e->answers_valid) return brc::set_error(e, BRC_E_INVALID, "format_window: allele queries are set, there is no text (brc_get_allele_answers)");
     return serve(e, region_index, first, count, lib_names, buf, cap);
 }
 
@@ -315,6 +317,7 @@ extern "C" int64_t brc_format_window(brc_engine *e, int64_t region_index, int64_
 extern "C" int64_t brc_write_text(brc_engine *e, int64_t region_index, int64_t first, int64_t count, const char *const *lib_names, int fd) {
     if (!e || region_index >= (int64_t)e->regions.size() || first < 0) return BRC_E_INVALID;
     if (!e->results_valid) return brc::set_error(e, BRC_E_INVALID, "write_text: no results");
+    if (e->answers_valid) return brc::set_error(e, BRC_E_INVALID, "write_text: allele queries are set, there is no text (brc_get_allele_answers)");
     if (region_index < 0) ensure_formatted(e, -1, -1, -1, lib_names);
     else ensure_formatted(e, region_index, first, count < 0 ? (int64_t)0x7fffffff : count, lib_names);
     int64_t total = 0;

@@ -36,12 +36,6 @@ namespace brc {
 
 // seq_nt16_table (V:htslib-1.10/hts.c:73-91): ASCII -> 4-bit IUPAC code, 15 for anything else
 __constant__ uint8_t c_nt16[256];
-// bam_nt16_canonical_table (R:bamreadcount.cpp:36-39): nibble -> index into "=ACGTN"
-__device__ __forceinline__ uint32_t canonical16(uint32_t nib) {
-    // packed 16 x 4-bit LUT: {0,1,2,5,3,5,5,5,4,5,5,5,5,5,5,5}
-    return (0x5555555455535210ull >> (nib * 4)) & 0xFu;
-}
-
 // one-time, per-device set-up (constant table, opt-in shared-memory sizes, SM count) shared by every engine handle of the
 // process: callers may drive several handles from several host threads, so it is serialised and published with atomics
 static std::mutex g_init_mu;
@@ -60,10 +54,6 @@ static void build_nt16() {
 
 __device__ __forceinline__ bool is_refop(uint32_t op) { return op == 0 || op == 2 || op == 3 || op == 7 || op == 8; }
 __device__ __forceinline__ bool is_matchop(uint32_t op) { return op == 0 || op == 7 || op == 8; }
-__device__ __forceinline__ uint32_t seq_nib(const uint8_t *seq, uint64_t off, int i) {
-    uint32_t b = seq[off + (uint32_t)(i >> 1)];
-    return (i & 1) ? (b & 0xFu) : (b >> 4);
-}
 
 // ---------------------------------------------------------------------------------------------
 // init: tile read ranges + counters

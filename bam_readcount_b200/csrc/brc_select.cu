@@ -42,18 +42,6 @@ __device__ __forceinline__ uint32_t ref_code(const SelectParams &P, const SelReg
 
 __device__ __forceinline__ uint64_t umax(uint64_t a, uint64_t b) { return a > b ? a : b; }
 
-__device__ __forceinline__ bool row_covers(const SelectParams &P, int64_t idx) {
-    const int64_t RS = (int64_t)P.n_rows * P.n_slots;
-    return (P.words[RS + idx] & 7u) == PB_ESCAPE || (P.words[idx] & 0xFFu) != 0u;
-}
-
-__device__ __forceinline__ bool abandoned(const SelectParams &P, int64_t s) {
-    const int64_t RS = (int64_t)P.n_rows * P.n_slots;
-    bool ab = false;
-    for (int r = 0; r < P.n_rows; ++r) ab |= (P.words[RS + (int64_t)r * P.n_slots + s] & 8u) != 0u;
-    return ab;
-}
-
 __global__ void __launch_bounds__(SEL_CTA) sel_pool_kernel(SelectParams P) {
     const int64_t j = (int64_t)blockIdx.x * SEL_CTA + threadIdx.x;
     const int64_t n_rec = (int64_t)*P.sec_count < P.sec_cap ? (int64_t)*P.sec_count : P.sec_cap;
@@ -61,14 +49,11 @@ __global__ void __launch_bounds__(SEL_CTA) sel_pool_kernel(SelectParams P) {
     const SecRec &rec = P.sec[j];
     const int64_t slot = rec.slot, r = slot / P.n_slots, s = slot - r * P.n_slots;
     const uint32_t kind = rec.kind_len & 0xFFu, cnt = rec.stats[0];
-    if (kind == (uint32_t)KIND_DEL) {
-        // pushed here, printed in the same row's block of the next site when that row spans it (same region: sel_site_kernel)
-        if (s + 1 < P.n_slots && row_covers(P, r * P.n_slots + s + 1)) { atomicAdd(&P.dsum[s], cnt); atomicMax(&P.dbest[s], cnt); }
-        return;
-    }
+    // a deletion prints in the same row's block of the next site when that row spans it (same region: sel_site_kernel)
+    if (pool_depth_term(P.words, P.n_rows, P.n_slots, rec, P.dsum, P.esc_np)) { atomicMax(&P.dbest[s], cnt); return; }
+    if (kind == (uint32_t)KIND_DEL) return;
     if (kind == (uint32_t)KIND_INS) { atomicMax(&P.best[s], cnt); return; }
     const uint32_t bc = kind >= KIND_WIDE ? kind - KIND_WIDE : kind;
-    if (kind >= KIND_WIDE) atomicAdd(&P.esc_np[s], (uint32_t)rec.qpos);
     if (bc >= 1u && bc <= 4u && cnt > 0u) {
         const SelRegion R = P.regions[region_of(P, s)];
         if (base_is_alt(bc, ref_code(P, R, R.first_pos + (s - R.slot_base)))) atomicMax(&P.best[s], cnt);
@@ -90,18 +75,16 @@ __global__ void __launch_bounds__(SEL_CTA) sel_site_kernel(SelectParams P) {
         const int64_t o = s - R.slot_base, pos = R.first_pos + o;
         const int64_t NS = P.n_slots, RS = (int64_t)P.n_rows * NS;
         const uint32_t rc = ref_code(P, R, pos);
-        bool covered = false;
-        uint64_t depth = P.esc_np[s], best = P.best[s];
-        for (int r = 0; r < P.n_rows; ++r) {
-            const uint32_t w0 = P.words[(int64_t)r * NS + s], w1 = P.words[RS + (int64_t)r * NS + s], pc = w1 & 7u;
-            ab |= (w1 & 8u) != 0u;
-            if (pc == PB_ESCAPE) { covered = true; continue; }      // full-width primary: a pool record
-            covered |= (w0 & 0xFFu) != 0u;
-            depth += (w0 >> 8) & 0xFFu;
+        const SiteLine L = site_line(P.words, P.n_rows, NS, s, o > 0, P.dsum, P.esc_np);
+        const uint64_t depth = L.depth;
+        uint64_t best = P.best[s];
+        for (int r = 0; r < P.n_rows; ++r) {      // escaped primaries (code PB_ESCAPE, never alternative) came from the pool pass
+            const uint32_t w0 = P.words[(int64_t)r * NS + s], pc = P.words[RS + (int64_t)r * NS + s] & 7u;
             if (base_is_alt(pc, rc)) best = umax(best, (w0 >> 16) & 0xFFu);
         }
-        if (o > 0 && !abandoned(P, s - 1)) { depth += P.dsum[s - 1]; best = umax(best, P.dbest[s - 1]); }
-        live = covered && !ab;
+        if (L.left) best = umax(best, P.dbest[s - 1]);
+        ab = L.abandoned;
+        live = L.live;
         uint8_t k = 0;
         if (live) {
             k = 4;

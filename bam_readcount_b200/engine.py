@@ -86,6 +86,15 @@ class CSelectedResults(C.Structure):
                 ("sec", C.c_void_p)]
 
 
+class CAlleleQuery(C.Structure):
+    """brc_allele_query (include/brc_engine.h "allele queries")."""
+    _fields_ = [("region", C.c_int64), ("pos", C.c_int32), ("kind_len", C.c_uint32), ("bases_off", C.c_int64)]
+
+
+# brc_allele_answer: one printed line's entry, 64 bytes
+ALLELE_ANSWER = np.dtype([("stats", np.uint32, (13,)), ("depth", np.uint32), ("line", np.uint32), ("reserved", np.uint32)])
+assert ALLELE_ANSWER.itemsize == 64
+
 N_WORDS = 8
 SEC_RECORD_BYTES = 72
 
@@ -94,7 +103,7 @@ EXPORTS = [
     "brc_begin_region", "brc_push_read", "brc_push_reads", "brc_end_region", "brc_decode_bam_span", "brc_push_bam_span", "brc_fetch_decoded_batch", "brc_compute", "brc_get_results",
     "brc_get_warning_counts", "brc_format_text", "brc_format_window", "brc_write_text", "brc_set_queue_carry", "brc_plan_device", "brc_run_device", "brc_device_packed_results", "brc_get_packed_results",
     "brc_fetch_device_results", "brc_last_launch_count", "brc_last_h2d_bytes", "brc_host_alloc", "brc_host_free", "brc_last_stage_ms", "brc_selftest_fastmath",
-    "brc_set_site_filter", "brc_get_selected_results",
+    "brc_set_site_filter", "brc_get_selected_results", "brc_set_allele_queries", "brc_get_allele_answers",
 ]
 
 _lib = None
@@ -152,6 +161,8 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
     lib.brc_last_stage_ms.restype = C.c_float
     lib.brc_set_site_filter.argtypes = [C.c_void_p, C.POINTER(CSiteFilter)]
     lib.brc_get_selected_results.argtypes = [C.c_void_p, C.POINTER(CSelectedResults)]
+    lib.brc_set_allele_queries.argtypes = [C.c_void_p, C.POINTER(CAlleleQuery), C.c_int64, C.c_char_p, C.c_int64]
+    lib.brc_get_allele_answers.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int64)]
     if path is None:
         _lib = lib
     return lib
@@ -392,11 +403,13 @@ class Engine:
 
     def reset(self):
         self._check(self.lib.brc_reset(self.h))
+        self.queried = False
         self._pushed = []
         self._keep = []
 
     def begin_region(self, tid: int, beg: int, end: int, site_list_mode: bool = True):
         self._check(self.lib.brc_begin_region(self.h, tid, beg, end, int(site_list_mode)))
+        self.queried = False
 
     @staticmethod
     def c_batch(b: ReadBatch, keep: list) -> CReadBatch:
@@ -456,7 +469,7 @@ class Engine:
 
     def _results(self) -> Optional[Results]:
         """The dense results of the last run; None while a site filter is set."""
-        if getattr(self, "filtered", False):
+        if getattr(self, "filtered", False) or getattr(self, "queried", False):
             return None
         r = CResults()
         self._check(self.lib.brc_get_results(self.h, C.byref(r)))
@@ -488,6 +501,7 @@ class Engine:
         arr = (CRegion * len(regions))(*regions)
         self._plan_keep = arr
         self._check(self.lib.brc_plan_device(self.h, arr, len(regions), n_reads_cap, n_sec_cap))
+        self.queried = False
 
     def run_device(self, cbatch: CReadBatch, region_of_read_ptr: Optional[int], stream_ptr: int):
         self._check(self.lib.brc_run_device(self.h, C.byref(cbatch), region_of_read_ptr, stream_ptr))
@@ -522,6 +536,22 @@ class Engine:
         r = CSelectedResults()
         self._check(self.lib.brc_get_selected_results(self.h, C.byref(r)))
         return SelectedResults(r)
+
+    # ---- allele queries (include/brc_engine.h brc_set_allele_queries) ----------------------------------------------------
+    def set_allele_queries(self, queries: Sequence[tuple], bases: bytes = b""):
+        """Queries of the current batch, each ``(region, pos, kind_len, bases_off)``: kind_len = kind 0..5 of "=ACGTN", or
+        KIND_INS / KIND_DEL | length << 8; bases_off indexes an insertion's characters in ``bases``.  From the next compute() /
+        run_device() on, allele_answers() holds the answers and compute() returns None (no dense view); reset() drops them."""
+        arr = (CAlleleQuery * max(1, len(queries)))(*[CAlleleQuery(int(g), int(p), int(k), int(o)) for g, p, k, o in queries])
+        self.queried = False          # a refused call drops the queries
+        self._check(self.lib.brc_set_allele_queries(self.h, arr, len(queries), bytes(bases), len(bases)))
+        self.queried = True
+
+    def allele_answers(self) -> np.ndarray:
+        """The answers of the last run in query order: a structured array of ALLELE_ANSWER records."""
+        p, n = C.c_void_p(), C.c_int64()
+        self._check(self.lib.brc_get_allele_answers(self.h, C.byref(p), C.byref(n)))
+        return _np_view(p.value, n.value * ALLELE_ANSWER.itemsize, np.uint8).view(ALLELE_ANSWER).copy()
 
     def stage_ms(self, stage: int) -> float:
         return float(self.lib.brc_last_stage_ms(self.h, stage))

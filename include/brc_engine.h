@@ -329,6 +329,46 @@ typedef struct {
 } brc_selected_results;
 BRC_API int brc_get_selected_results(brc_engine *e, brc_selected_results *out);
 
+/* ---- allele queries ---------------------------------------------------------------------------
+ * "The read counts of THESE alleles at THESE sites" (a VCF's REF and ALT alleles, DESIGN.md §12), answered on the device from
+ * the packed records the kernels left in HBM: only the answers (64 B each), the warning words and the pool counter cross PCIe.
+ *
+ * One query names an entry of one printed line:
+ *   region     index of the region in brc_begin_region order since brc_reset (or in the brc_plan_device table)
+ *   pos        0-based site of that region that the text would print (beg <= pos < end)
+ *   kind_len   kind in bits [0:8): 0..5 a base entry of "=ACGTN" (length 0), BRC_KIND_INS or BRC_KIND_DEL with the indel
+ *              length (>= 1) in bits [8:32)
+ *   bases_off  BRC_KIND_INS: offset of its `length` upper-case A/C/G/T/N characters in the `bases` buffer (the "+..." entry's
+ *              characters: read bases as the text prints them, IUPAC codes read as N); ignored otherwise
+ * Its answer:
+ *   stats      the entry's 13 accumulators (floats as IEEE bits), exactly what brc_get_results holds for that key; all zeros
+ *              when the line has no such entry
+ *   depth      the line's 4th column;  line  1 when the site prints a line (0: no read spans it; stats and depth are 0)
+ * A deletion entry prints on the line after its anchor: a BRC_KIND_DEL query at `pos` is answered from the deletion of that
+ * length anchored at pos - 1, when the anchor lies in the same region (the -l loop's view; at most one deletion of a length
+ * starts at one anchor, so the length names it).
+ *
+ * Queries belong to the current batch: set them after the last brc_end_region (or brc_plan_device) and before brc_compute /
+ * brc_run_device; brc_reset, brc_begin_region and brc_plan_device drop them.  While they are set there is no dense view:
+ * brc_get_results, brc_get_packed_results and brc_format_* return BRC_E_INVALID.  brc_run_device leaves the answers on the
+ * device and brc_fetch_device_results copies them.  BRC_E_INVALID: per_lib (more than one library row), a site filter set, a
+ * region or position out of range, an unknown kind, insertion bases that are not A/C/G/T/N or lie outside `bases`. */
+typedef struct {
+    int64_t region;
+    int32_t pos;
+    uint32_t kind_len;
+    int64_t bases_off;
+} brc_allele_query;
+typedef struct {
+    uint32_t stats[BRC_N_STATS];
+    uint32_t depth;
+    uint32_t line;
+    uint32_t reserved;            /* 0 */
+} brc_allele_answer;              /* 64 B */
+BRC_API int brc_set_allele_queries(brc_engine *e, const brc_allele_query *q, int64_t n, const char *bases, int64_t n_bases);
+/* the answers of the last run, in query order (engine-owned, valid until the next run or brc_reset) */
+BRC_API int brc_get_allele_answers(brc_engine *e, const brc_allele_answer **out, int64_t *n);
+
 /* ---- device-resident path (bench "value": inputs already in HBM) -------------------------
  * brc_plan_device: fix the region geometry (host array of n_regions regions with read_lo/hi,
  * slot_base, first_pos, n_slots filled) and size the outputs.  brc_run_device: launch the
@@ -358,7 +398,7 @@ BRC_API int brc_last_launch_count(const brc_engine *e);
 BRC_API int64_t brc_last_h2d_bytes(const brc_engine *e);
 /* elapsed GPU milliseconds of the named stage of the last run, measured with CUDA events on the
  * launching stream: 0 = per-read precompute kernel, 1 = pileup kernel, 2 = whole device step (without the selection),
- * 3 = site selection + compaction (0 when no filter was set) */
+ * 3 = site selection + compaction (0 when no filter was set), 4 = allele queries (0 when none were set) */
 BRC_API float brc_last_stage_ms(const brc_engine *e, int stage);
 
 #ifdef __cplusplus
