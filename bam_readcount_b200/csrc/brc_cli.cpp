@@ -9,7 +9,8 @@
 // Mirrors, region by region, the reference's two loops:
 //   -l site list : R:...:574-608  (d.beg=beg-1, d.end=end, queues cleared per region)
 //   argv regions : R:...:641-657  (bam_parse_region; a bare contig name keeps the previous beg/end, A.6)
-// With --bam-list the same per-sample run is repeated over a list of inputs in one process (DESIGN.md §11).
+// With --bam-list the same per-sample run is repeated over a list of inputs in one process (DESIGN.md §11); --vcf-samples
+// does the same for the sample columns of one VCF (DESIGN.md §12).
 #include <algorithm>
 #include <cctype>
 #include <cerrno>
@@ -771,7 +772,12 @@ void usage() {
                 "                                        (STDERR is that of -l over the records' sites).  Not with -l, regions, -p,\n"
                 "                                        --min-alt-*, --shard or --bam-list\n"
                 "  --vcf-sample NAME                     (this host) the sample column that takes the values (required with several; names\n"
-                "                                        the column added to a sites-only VCF)\n\n");
+                "                                        the column added to a sites-only VCF)\n"
+                "  --vcf-samples FILE                    (this host) with --vcf and no positional argument: annotate several sample columns\n"
+                "                                        in one process.  Each line of FILE is NAME<TAB>INPUT or NAME<TAB>INPUT<TAB>ERR;\n"
+                "                                        NAME's column gets the values of `--vcf-sample NAME INPUT`, ERR (default: STDERR)\n"
+                "                                        that run's STDERR.  A failed sample gets '.' and does not stop the others (exit\n"
+                "                                        status 1 at the end)\n\n");
 }
 
 // samtools region string "name[:beg[-end]]" as bam_parse_region (V:bam_aux.c:65-75) handles it.  Returns 0 when beg and end were
@@ -832,15 +838,29 @@ struct VcfRecord {
     uint32_t ref_kind = 0;                // the REF entry: a base class of "=ACGTN"
     std::vector<int64_t> alt_kind_len;    // per ALT: query kind | length << 8, or -1 when the ALT is not countable
     std::vector<std::string> alt_bases;   // per ALT: an insertion's bases
+    size_t n_queries = 0;                 // counted: the REF and each countable ALT
+    size_t word_off = 0;                  // counted: where its answer words start in a sample's VcfAnswers
 };
 struct Vcf {
     std::string path;
     std::vector<std::string> header;      // every line before #CHROM
     std::string chrom_line;
     size_t n_cols = 0;
-    int sample_col = -1;                  // column that takes the values; -1: sites-only, a FORMAT and a sample column are added
-    std::string add_sample;               // ... named so
+    // the samples that take values, in the order given: each an existing column (target_of_col), or, in a sites-only VCF, a
+    // column added after an added FORMAT column
+    std::vector<std::string> samples;
+    std::vector<int> target_of_col;       // per column: the index in `samples` of the sample it holds, or -1
     std::vector<VcfRecord> rec;
+    size_t n_words = 0;                   // answer words of one sample: 1 + 3 * n_queries per counted record
+};
+
+// One sample's answers.  For each counted record, at its word_off: the depth of the record's line (0 when it prints none), then
+// count, plus and minus of the REF entry and of each countable ALT's entry.  A sample that failed has none.
+struct VcfAnswers {
+    std::vector<uint32_t> words;
+    std::vector<uint8_t> answered;        // per record: its words are set (counted, and its contig is in the sample's input)
+    bool failed = false;
+    explicit VcfAnswers(const Vcf &v) : words(v.n_words), answered(v.rec.size()) {}
 };
 
 std::vector<std::string> split(const std::string &s, char c) {
@@ -874,8 +894,9 @@ bool read_vcf_bytes(const std::string &path, std::string &out, std::string &why)
     return true;
 }
 
-// Parses the whole VCF and applies the allele rule; false with a message (nothing may have been written yet).
-bool parse_vcf(const std::string &path, const std::string &sample, bool sample_given, Vcf &v, std::string &why) {
+// Parses the whole VCF, applies the allele rule and resolves the samples that take values: `samples` as named by option `opt`,
+// or none given (the VCF's only sample column).  False with a message (nothing may have been written yet).
+bool parse_vcf(const std::string &path, const std::vector<std::string> &samples, const char *opt, Vcf &v, std::string &why) {
     std::string text;
     if (!read_vcf_bytes(path, text, why)) return false;
     v.path = path;
@@ -927,23 +948,34 @@ bool parse_vcf(const std::string &path, const std::string &sample, bool sample_g
             r.counted = r.counted || kl >= 0;
             r.alt_kind_len.push_back(kl); r.alt_bases.push_back(bases);
         }
-        if (r.counted) { r.line_pos = (int32_t)(ref.size() == 1 ? pos : pos + 1); r.ref_kind = kind_of(ref[ref.size() == 1 ? 0 : 1]); }
+        if (r.counted) {
+            r.line_pos = (int32_t)(ref.size() == 1 ? pos : pos + 1); r.ref_kind = kind_of(ref[ref.size() == 1 ? 0 : 1]);
+            r.n_queries = 1 + (size_t)std::count_if(r.alt_kind_len.begin(), r.alt_kind_len.end(), [](int64_t x) { return x >= 0; });
+            r.word_off = v.n_words; v.n_words += 1 + 3 * r.n_queries;
+        }
         v.rec.push_back(std::move(r));
     }
     if (in_header) { why = path + ": no #CHROM header line"; return false; }
     const std::vector<std::string> hc = split(v.chrom_line, '\t');
+    v.target_of_col.assign(v.n_cols, -1);
     if (v.n_cols == 8) {
-        if (!sample_given) { why = path + " has no sample column: --vcf-sample NAME names the one added"; return false; }
-        v.add_sample = sample;
+        if (samples.empty()) { why = path + " has no sample column: --vcf-sample NAME names the one added"; return false; }
+        v.samples = samples;
         return true;
     }
-    int n_match = 0;
-    for (size_t c = 9; c < hc.size(); ++c) if (hc[c] == sample) { ++n_match; v.sample_col = (int)c; }
-    if (!sample_given) {
+    if (samples.empty()) {
         if (hc.size() > 10) { why = path + " has " + std::to_string(hc.size() - 9) + " sample columns: --vcf-sample NAME is required"; return false; }
-        v.sample_col = 9;
-    } else if (n_match == 0) { why = "--vcf-sample " + sample + ": no such sample in " + path; return false; }
-    else if (n_match > 1) { why = "--vcf-sample " + sample + " is ambiguous: " + std::to_string(n_match) + " sample columns of " + path + " have that name"; return false; }
+        v.samples.assign(1, hc[9]); v.target_of_col[9] = 0;
+        return true;
+    }
+    for (size_t t = 0; t < samples.size(); ++t) {
+        int n_match = 0, col = -1;
+        for (size_t c = 9; c < hc.size(); ++c) if (hc[c] == samples[t]) { ++n_match; col = (int)c; }
+        if (n_match == 0) { why = std::string(opt) + " " + samples[t] + ": no such sample in " + path; return false; }
+        if (n_match > 1) { why = std::string(opt) + " " + samples[t] + " is ambiguous: " + std::to_string(n_match) + " sample columns of " + path + " have that name"; return false; }
+        v.target_of_col[(size_t)col] = (int)t;
+    }
+    v.samples = samples;
     return true;
 }
 
@@ -956,45 +988,51 @@ bool write_all(int fd, const std::string &s) {
     return true;
 }
 
-// The five values of a counted record from the answers of its queries (REF first, then each countable ALT in order).
-std::string vcf_values(const VcfRecord &r, const brc_allele_answer *ans) {
-    if (!ans) return ".:.:.:.:.";
-    const uint32_t dp = ans[0].line ? ans[0].depth : 0;
+// Record ri's five values in one sample from its answer words (REF first, then each countable ALT in order).  A record the
+// sample did not answer, and every record of a failed sample, gets '.' in all five.
+void vcf_values(const Vcf &v, size_t ri, const VcfAnswers &a, std::string &out) {
+    if (a.failed || !a.answered[ri]) { out += ".:.:.:.:."; return; }
+    const VcfRecord &r = v.rec[ri];
+    const uint32_t *w = a.words.data() + r.word_off;
+    const uint32_t dp = w[0];
     std::string ad, adf, adr, af;
-    auto put = [&](const brc_allele_answer *a) {
-        ad += a ? std::to_string(a->stats[BRC_S_COUNT]) : "."; adf += a ? std::to_string(a->stats[BRC_S_PLUS]) : ".";
-        adr += a ? std::to_string(a->stats[BRC_S_MINUS]) : ".";
+    auto put = [&](const uint32_t *q) {
+        ad += q ? std::to_string(q[0]) : "."; adf += q ? std::to_string(q[1]) : "."; adr += q ? std::to_string(q[2]) : ".";
     };
-    put(&ans[0]);
+    put(w + 1);
     size_t k = 1;
     for (size_t i = 0; i < r.alt_kind_len.size(); ++i) {
-        const brc_allele_answer *a = r.alt_kind_len[i] >= 0 ? &ans[k++] : nullptr;
+        const uint32_t *q = r.alt_kind_len[i] >= 0 ? w + 1 + 3 * k++ : nullptr;
         ad += ','; adf += ','; adr += ',';
-        put(a);
+        put(q);
         if (i) af += ',';
-        if (!a || dp == 0) { af += '.'; continue; }
-        char b[64]; std::snprintf(b, sizeof b, "%.6g", (double)a->stats[BRC_S_COUNT] / (double)dp);
+        if (!q || dp == 0) { af += '.'; continue; }
+        char b[64]; std::snprintf(b, sizeof b, "%.6g", (double)q[0] / (double)dp);
         af += b;
     }
-    return std::to_string(dp) + ":" + ad + ":" + adf + ":" + adr + ":" + af;
+    out += std::to_string(dp); out += ':'; out += ad; out += ':'; out += adf; out += ':'; out += adr; out += ':'; out += af;
 }
 
-// One record line with the values in the chosen sample column.
-std::string vcf_line(const Vcf &v, const VcfRecord &r, const std::string &values) {
-    std::string out;
+// Record ri's line, appended to `out`: the values of sample t from ans[t] in that sample's column.
+void vcf_line(const Vcf &v, size_t ri, const VcfAnswers *ans, std::string &out) {
+    const VcfRecord &r = v.rec[ri];
     const size_t n = r.cols.size();
     for (size_t c = 0; c < n; ++c) {
         if (c) out += '\t';
-        if (c == 8) { out += r.cols[c]; out += kVcfFormat; continue; }
-        if ((int)c != v.sample_col) { out += r.cols[c]; continue; }
         out += r.cols[c];
+        if (c == 8) { out += kVcfFormat; continue; }
+        const int t = v.target_of_col[c];
+        if (t < 0) continue;
         const size_t keys = (size_t)std::count(r.cols[8].begin(), r.cols[8].end(), ':') + 1;
         for (size_t have = (size_t)std::count(r.cols[c].begin(), r.cols[c].end(), ':') + 1; have < keys; ++have) out += ":.";
-        out += ':'; out += values;
+        out += ':';
+        vcf_values(v, ri, ans[t], out);
     }
-    if (v.sample_col < 0) { out += '\t'; out += kVcfFormat + 1; out += '\t'; out += values; }
+    if (n == 8) {
+        out += '\t'; out += kVcfFormat + 1;
+        for (size_t t = 0; t < v.samples.size(); ++t) { out += '\t'; vcf_values(v, ri, ans[t], out); }
+    }
     out += '\n';
-    return out;
 }
 
 std::string vcf_header(const Vcf &v) {
@@ -1002,14 +1040,26 @@ std::string vcf_header(const Vcf &v) {
     for (const std::string &h : v.header) { out += h; out += '\n'; }
     out += kVcfHeader;
     out += v.chrom_line;
-    if (v.sample_col < 0) { out += "\tFORMAT\t"; out += v.add_sample; }
+    if (v.n_cols == 8) { out += "\tFORMAT"; for (const std::string &s : v.samples) { out += '\t'; out += s; } }
     out += '\n';
     return out;
+}
+
+// A batch's answers into sample `a`'s words: record ri's queries are ans[0 .. n_queries) (brc_get_allele_answers' order).
+void vcf_store(const Vcf &v, size_t ri, const brc_allele_answer *ans, VcfAnswers &a) {
+    const VcfRecord &r = v.rec[ri];
+    uint32_t *w = a.words.data() + r.word_off;
+    w[0] = ans[0].line ? ans[0].depth : 0;
+    for (size_t k = 0; k < r.n_queries; ++k) {
+        w[1 + 3 * k] = ans[k].stats[BRC_S_COUNT]; w[2 + 3 * k] = ans[k].stats[BRC_S_PLUS]; w[3 + 3 * k] = ans[k].stats[BRC_S_MINUS];
+    }
+    a.answered[ri] = 1;
 }
 
 struct Options {   // everything on the command line except the inputs: the same for every sample
     int min_mapq = 0, min_bq = 0, max_cnt = 10000000; bool per_lib = false, ic = false; long long max_warn = -1;
     const Vcf *vcf = nullptr;     // --vcf: the parsed file
+    bool vcf_samples = false;     // --vcf-samples: a sample only fills its answers; the VCF is written after the last sample
     std::string fn_pos, fn_fa, dist_arg;
     std::vector<std::string> region_args;
     int shard_rank = 0, shard_count = 1;
@@ -1282,8 +1332,9 @@ struct Engines {
 };
 
 // One sample's region loop (the two loops of the reference, R:...:574-608 and 641-657): text to out_fd, messages to err.
+// With --vcf the answers go to `vcf_ans`, and a single-sample run streams the VCF to out_fd as its batches complete.
 // Returns the exit status of the run on this input alone (0 or 1), or -1 when no engine could be created.
-int run_sample(const Options &o, Engines &engines, Sample &s, int out_fd, FILE *err, double t_main0) {
+int run_sample(const Options &o, Engines &engines, Sample &s, int out_fd, FILE *err, double t_main0, VcfAnswers *vcf_ans) {
     std::fputs(s.log.held.c_str(), err);
     if (s.status != 0) return 1;
     s.warner.err = err;
@@ -1304,19 +1355,18 @@ int run_sample(const Options &o, Engines &engines, Sample &s, int out_fd, FILE *
     std::vector<const char *> rg_ids; std::vector<uint16_t> rg_libs;
     for (const auto &kv : s.rg_lib) { rg_ids.push_back(kv.first.c_str()); rg_libs.push_back(kv.second); }
     int64_t warn_total[4] = {0, 0, 0, 0};
-    // --vcf: the records go out in file order, each once its region's batch is computed; the values of the records answered so far
+    // --vcf: a single-sample run writes the records in file order, each once its region's batch is computed
     const Vcf *vcf = o.vcf;
+    const bool vcf_stream = vcf && !o.vcf_samples && !o.decode_only;
     std::vector<int64_t> vcf_rec_of_region(regions.size(), -1);
     for (size_t k = 0; k < s.vcf_region.size(); ++k) if (s.vcf_region[k] >= 0) vcf_rec_of_region[(size_t)s.vcf_region[k]] = (int64_t)k;
-    std::vector<std::string> vcf_vals(vcf ? vcf->rec.size() : 0);
     size_t vcf_next = 0;
     auto vcf_write = [&](int64_t regions_done) {     // every record not yet written whose region is done (or that has none)
         std::string out;
-        for (; vcf_next < vcf_vals.size() && s.vcf_region[vcf_next] < regions_done; ++vcf_next)
-            out += vcf_line(*vcf, vcf->rec[vcf_next], s.vcf_region[vcf_next] < 0 ? vcf_values(vcf->rec[vcf_next], nullptr) : vcf_vals[vcf_next]);
+        for (; vcf_next < s.vcf_region.size() && s.vcf_region[vcf_next] < regions_done; ++vcf_next) vcf_line(*vcf, vcf_next, vcf_ans, out);
         return write_all(out_fd, out);
     };
-    if (vcf && !o.decode_only && !write_all(out_fd, vcf_header(*vcf))) { std::fprintf(err, "writing the VCF: %s\n", std::strerror(errno)); return 1; }
+    if (vcf_stream && !write_all(out_fd, vcf_header(*vcf))) { std::fprintf(err, "writing the VCF: %s\n", std::strerror(errno)); return 1; }
     int64_t batch_first = 0, batch_n = 0;            // the regions begun since the last brc_reset
     auto flush = [&]() -> int {
         int r;
@@ -1344,11 +1394,11 @@ int run_sample(const Options &o, Engines &engines, Sample &s, int out_fd, FILE *
             if (o.timing) ms_alleles += brc_last_stage_ms(eng, 4);
             const double f0 = now();
             for (int64_t g = 0, k = 0; g < batch_n; ++g) {
-                const int64_t ri = vcf_rec_of_region[(size_t)(batch_first + g)];
-                vcf_vals[(size_t)ri] = vcf_values(vcf->rec[(size_t)ri], ans + k);
-                k += 1 + std::count_if(vcf->rec[(size_t)ri].alt_kind_len.begin(), vcf->rec[(size_t)ri].alt_kind_len.end(), [](int64_t x) { return x >= 0; });
+                const size_t ri = (size_t)vcf_rec_of_region[(size_t)(batch_first + g)];
+                vcf_store(*vcf, ri, ans + k, *vcf_ans);
+                k += (int64_t)vcf->rec[ri].n_queries;
             }
-            if (!vcf_write(batch_first + batch_n)) { std::fprintf(err, "writing the VCF: %s\n", std::strerror(errno)); return -1; }
+            if (vcf_stream && !vcf_write(batch_first + batch_n)) { std::fprintf(err, "writing the VCF: %s\n", std::strerror(errno)); return -1; }
             t_format += now() - f0;
         } else {
             if (o.site_filter) {          // only the selected sites came back: no dense view, the region table is all the loop needs
@@ -1471,7 +1521,7 @@ int run_sample(const Options &o, Engines &engines, Sample &s, int out_fd, FILE *
         // at region boundaries (the deletion queue of the argv loop is carried by the engine, brc_set_queue_carry)
         if (job || span || gi + 1 == regions.size() || pushed > 1500000) { if (flush() != BRC_OK) return 1; pushed = 0; }
     }
-    if (vcf && !o.decode_only && !vcf_write(INT64_MAX)) { std::fprintf(err, "writing the VCF: %s\n", std::strerror(errno)); return 1; }
+    if (vcf_stream && !vcf_write(INT64_MAX)) { std::fprintf(err, "writing the VCF: %s\n", std::strerror(errno)); return 1; }
     warner.finish(warn_total);
 #ifdef BRC_WITH_HTSLIB
     const bool decode_error = bam.bz.error || s.hts.error || s.par_decode_error;
@@ -1504,68 +1554,70 @@ int leave(Engines &engines, std::unique_ptr<Sample> &last, int status) {
     return status;
 }
 
-// OUT and ERR of one cohort sample.  Nothing is created or emptied until both are open: a sample that cannot have both
-// leaves no new file behind and no earlier file truncated.
-bool open_outputs(const std::string &out, const std::string &err, int &out_fd, int &err_fd, std::string &why) {
-    const std::string *path[2] = {&out, &err};
-    int fd[2] = {-1, -1}; bool made[2] = {false, false};
-    auto undo = [&](int n) { for (int j = 0; j < n; ++j) { ::close(fd[j]); if (made[j]) ::unlink(path[j]->c_str()); } };
-    for (int i = 0; i < 2; ++i) {
+// The output files of one sample (OUT and ERR of a cohort sample, the ERR of a --vcf-samples sample).  Nothing is created or
+// emptied until all are open: a sample that cannot have them all leaves no new file behind and no earlier file truncated.
+bool open_outputs(const std::vector<const std::string *> &path, std::vector<int> &fd, std::string &why) {
+    const size_t n = path.size();
+    fd.assign(n, -1); std::vector<bool> made(n, false);
+    auto undo = [&](size_t m) { for (size_t j = 0; j < m; ++j) { ::close(fd[j]); if (made[j]) ::unlink(path[j]->c_str()); } };
+    for (size_t i = 0; i < n; ++i) {
         fd[i] = ::open(path[i]->c_str(), O_WRONLY | O_CREAT | O_EXCL | O_CLOEXEC, 0666);
         if (fd[i] >= 0) made[i] = true;
         else if (errno == EEXIST) fd[i] = ::open(path[i]->c_str(), O_WRONLY | O_CLOEXEC);
         if (fd[i] < 0) { why = "cannot open " + *path[i] + ": " + std::strerror(errno); undo(i); return false; }
     }
-    for (int i = 0; i < 2; ++i)
-        if (::ftruncate(fd[i], 0) != 0) { why = "cannot truncate " + *path[i] + ": " + std::strerror(errno); undo(2); return false; }
-    out_fd = fd[0]; err_fd = fd[1];
+    for (size_t i = 0; i < n; ++i)
+        if (::ftruncate(fd[i], 0) != 0) { why = "cannot truncate " + *path[i] + ": " + std::strerror(errno); undo(n); return false; }
     return true;
 }
 
-// --bam-list FILE: a cohort in one process.  Each non-empty line of FILE is INPUT<TAB>OUT[<TAB>ERR] (ERR defaults to OUT.log);
-// OUT and ERR receive exactly what a run on INPUT alone with the same options and regions prints on STDOUT and STDERR.  A
-// sample whose own run would exit 1 is reported on this process's STDERR and the batch goes on; the exit status is 1 when any
-// sample failed.  The list is checked whole before any sample runs.
-//
-// While a sample runs, file descriptor 2 is its ERR file, so whatever a library prints there (htslib's CRAM and index messages)
-// lands in that sample's ERR in the order its own run prints it.  The next sample is opened on a worker thread while the current
-// one computes, holding its messages until its turn, unless it is a CRAM: htslib prints while it opens one, so a CRAM is opened
-// at its turn.  Its first window is decoded ahead only when the current sample does not use the process's two window jobs, so
-// page-locked window memory stays at two jobs, reused from sample to sample.
-int run_cohort(const Options &o, Engines &engines, const std::string &list_path, double t_main0) {
-    struct Entry { std::string in, out, err; };
-    std::vector<Entry> list;
-    {
-        std::ifstream f(list_path);
-        if (!f) { std::fprintf(stderr, "Failed to open sample list file: %s\n", list_path.c_str()); return 1; }
-        std::set<std::string> outputs;
-        std::string line; int ln = 0;
-        while (std::getline(f, line)) {
-            ++ln;
-            if (!line.empty() && line.back() == '\r') line.pop_back();
-            if (line.empty()) continue;
-            std::vector<std::string> fld; size_t p = 0;
-            for (size_t t; (t = line.find('\t', p)) != std::string::npos; p = t + 1) fld.push_back(line.substr(p, t - p));
-            fld.push_back(line.substr(p));
-            const bool empty_field = std::any_of(fld.begin(), fld.end(), [](const std::string &x) { return x.empty(); });
-            if ((fld.size() != 2 && fld.size() != 3) || empty_field) {
-                std::fprintf(stderr, "%s:%d: a sample line is INPUT<TAB>OUT or INPUT<TAB>OUT<TAB>ERR\n", list_path.c_str(), ln);
-                return 1;
-            }
-            Entry e{fld[0], fld[1], fld.size() == 3 ? fld[2] : fld[1] + ".log"};
-            for (const std::string *path : {&e.out, &e.err}) {
-                std::error_code ec;
-                std::filesystem::path abs = std::filesystem::absolute(*path, ec);
-                if (ec) abs = *path;
-                if (!outputs.insert(abs.lexically_normal().string()).second) {
-                    std::fprintf(stderr, "%s:%d: %s is already the output of an earlier sample\n", list_path.c_str(), ln, path->c_str());
-                    return 1;
-                }
-            }
-            list.push_back(std::move(e));
+// The lines of a sample list (--bam-list, --vcf-samples): every non-empty line, a trailing '\r' dropped, split at tabs into 2 or 3
+// non-empty fields (`shape` names them in the message), with its line number.  False with a message on stderr.
+struct ListLine { int ln; std::vector<std::string> fld; };
+bool read_list(const std::string &list_path, const char *shape, std::vector<ListLine> &out) {
+    std::ifstream f(list_path);
+    if (!f) { std::fprintf(stderr, "Failed to open sample list file: %s\n", list_path.c_str()); return false; }
+    std::string line; int ln = 0;
+    while (std::getline(f, line)) {
+        ++ln;
+        if (!line.empty() && line.back() == '\r') line.pop_back();
+        if (line.empty()) continue;
+        std::vector<std::string> fld = split(line, '\t');
+        const bool empty_field = std::any_of(fld.begin(), fld.end(), [](const std::string &x) { return x.empty(); });
+        if ((fld.size() != 2 && fld.size() != 3) || empty_field) {
+            std::fprintf(stderr, "%s:%d: a sample line is %s\n", list_path.c_str(), ln, shape);
+            return false;
         }
-        if (list.empty()) { std::fprintf(stderr, "%s lists no sample\n", list_path.c_str()); return 1; }
+        out.push_back({ln, std::move(fld)});
     }
+    if (out.empty()) { std::fprintf(stderr, "%s lists no sample\n", list_path.c_str()); return false; }
+    return true;
+}
+
+// Adds an output path to `used` (absolute and normalised); false, with a message on stderr, when an earlier sample has it.
+bool claim_output(std::set<std::string> &used, const std::string &list_path, int ln, const std::string &path) {
+    std::error_code ec;
+    std::filesystem::path abs = std::filesystem::absolute(path, ec);
+    if (ec) abs = path;
+    if (used.insert(abs.lexically_normal().string()).second) return true;
+    std::fprintf(stderr, "%s:%d: %s is already the output of an earlier sample\n", list_path.c_str(), ln, path.c_str());
+    return false;
+}
+
+// One input of a sample list and where its STDOUT and STDERR go: files, or the process's own when the path is empty.
+struct ListSample { std::string in, out, err; };
+
+// Runs the samples of a list in order, each exactly as a run on its input alone (DESIGN.md §11).  `vcf_ans` (--vcf-samples):
+// sample k's answers go to vcf_ans[k], which is marked failed when the sample fails.  A sample whose own run would exit 1, or
+// whose output files cannot be opened or written, gets one line on the process's STDERR and the list goes on.  Returns the number
+// of failed samples, or -1 when no engine could be created: the remaining samples are not run.
+//
+// While a sample with an ERR file runs, file descriptor 2 is that file, so whatever a library prints there (htslib's CRAM and
+// index messages) lands in that sample's ERR in the order its own run prints it.  The next sample is opened on a worker thread
+// while the current one computes, holding its messages until its turn, unless it is a CRAM: htslib prints while it opens one, so
+// a CRAM is opened at its turn.  Its first window is decoded ahead only when the current sample does not use the process's two
+// window jobs, so page-locked window memory stays at two jobs, reused from sample to sample.
+int run_list(const Options &o, Engines &engines, const std::vector<ListSample> &list, std::vector<VcfAnswers> *vcf_ans, double t_main0) {
     std::unique_ptr<WindowJob[]> pool(new WindowJob[2]);
     auto open_ahead = [&](size_t k, bool first_window) {
         return std::async(std::launch::async, open_sample, std::cref(o), list[k].in, now(), nullptr, pool.get(), first_window);
@@ -1573,45 +1625,94 @@ int run_cohort(const Options &o, Engines &engines, const std::string &list_path,
     if (!o.decode_only && !o.dist_refused()) engines.start_warm();
     std::future<std::unique_ptr<Sample>> ahead;                          // sample k, opened ahead of its turn
     if (!is_cram_path(list[0].in)) ahead = open_ahead(0, true);          // under the CUDA start-up
-    std::unique_ptr<Sample> cur;
     int n_failed = 0;
     for (size_t k = 0; k < list.size(); ++k) {
-        const Entry &e = list[k];
+        const ListSample &e = list[k];
         const bool next_ahead = k + 1 < list.size() && !is_cram_path(list[k + 1].in);
-        int out_fd = -1, err_fd = -1; std::string why;
-        if (!open_outputs(e.out, e.err, out_fd, err_fd, why)) {
-            if (ahead.valid()) ahead.get();
-            std::fprintf(stderr, "sample %zu (%s) failed: %s\n", k + 1, e.in.c_str(), why.c_str());
+        auto failed = [&](const char *fmt, const std::string &what) {
             ++n_failed;
+            if (vcf_ans) (*vcf_ans)[k].failed = true;
+            std::fprintf(stderr, fmt, k + 1, e.in.c_str(), what.c_str());
+        };
+        std::vector<const std::string *> paths; std::vector<int> fd; std::string why;
+        if (!e.out.empty()) paths.push_back(&e.out);
+        if (!e.err.empty()) paths.push_back(&e.err);
+        if (!open_outputs(paths, fd, why)) {
+            if (ahead.valid()) ahead.get();
+            failed("sample %zu (%s) failed: %s\n", why);
             if (next_ahead) ahead = open_ahead(k + 1, true);
             continue;
         }
-        std::fflush(stderr);
-        const int saved_fd2 = ::dup(2);
-        ::dup2(err_fd, 2);
-        cur = ahead.valid() ? ahead.get() : open_sample(o, e.in, now(), stderr, pool.get(), true);
+        const int out_fd = e.out.empty() ? STDOUT_FILENO : fd[0], err_fd = e.err.empty() ? -1 : fd.back();
+        int saved_fd2 = -1;
+        if (err_fd >= 0) { std::fflush(stderr); saved_fd2 = ::dup(2); ::dup2(err_fd, 2); }
+        std::unique_ptr<Sample> cur = ahead.valid() ? ahead.get() : open_sample(o, e.in, now(), stderr, pool.get(), true);
         if (next_ahead) ahead = open_ahead(k + 1, !cur->uses_windows());
-        const int rc = run_sample(o, engines, *cur, out_fd, stderr, t_main0);
+        const int rc = run_sample(o, engines, *cur, out_fd, stderr, t_main0, vcf_ans ? &(*vcf_ans)[k] : nullptr);
         cur.reset();                                                     // htslib's closing lines still go to this ERR
-        if (std::fflush(stderr) != 0) why = e.err + ": " + std::strerror(errno);
-        else if (std::ferror(stderr)) why = e.err + ": write error";
-        std::clearerr(stderr);
-        ::dup2(saved_fd2, 2);
-        ::close(saved_fd2);
-        if (::close(err_fd) != 0 && why.empty()) why = e.err + ": " + std::strerror(errno);
-        if (::close(out_fd) != 0 && why.empty()) why = e.out + ": " + std::strerror(errno);
+        if (err_fd >= 0) {
+            if (std::fflush(stderr) != 0) why = e.err + ": " + std::strerror(errno);
+            else if (std::ferror(stderr)) why = e.err + ": write error";
+            std::clearerr(stderr);
+            ::dup2(saved_fd2, 2);
+            ::close(saved_fd2);
+            if (::close(err_fd) != 0 && why.empty()) why = e.err + ": " + std::strerror(errno);
+        }
+        if (out_fd != STDOUT_FILENO && ::close(out_fd) != 0 && why.empty()) why = e.out + ": " + std::strerror(errno);
+        const std::string see = e.err.empty() ? "the lines above" : e.err;
         if (rc < 0) {
-            std::fprintf(stderr, "sample %zu (%s): no engine could be created (see %s); the remaining samples are not run\n", k + 1, e.in.c_str(), e.err.c_str());
-            return leave(engines, cur, 1);
+            std::fprintf(stderr, "sample %zu (%s): no engine could be created (see %s); the remaining samples are not run\n", k + 1, e.in.c_str(), see.c_str());
+            return -1;
         }
-        if (rc != 0 || !why.empty()) {
-            ++n_failed;
-            if (!why.empty()) std::fprintf(stderr, "sample %zu (%s) failed: writing %s\n", k + 1, e.in.c_str(), why.c_str());
-            else std::fprintf(stderr, "sample %zu (%s) failed: see %s\n", k + 1, e.in.c_str(), e.err.c_str());
-        }
+        if (!why.empty()) failed("sample %zu (%s) failed: writing %s\n", why);
+        else if (rc != 0) failed("sample %zu (%s) failed: see %s\n", see);
     }
+    return n_failed;
+}
+
+// --bam-list FILE: a cohort in one process.  Each non-empty line of FILE is INPUT<TAB>OUT[<TAB>ERR] (ERR defaults to OUT.log);
+// OUT and ERR receive exactly what a run on INPUT alone with the same options and regions prints on STDOUT and STDERR.  A
+// sample whose own run would exit 1 is reported on this process's STDERR and the batch goes on; the exit status is 1 when any
+// sample failed.  The list is checked whole before any sample runs.
+int run_cohort(const Options &o, Engines &engines, const std::string &list_path, double t_main0) {
+    std::vector<ListLine> lines;
+    if (!read_list(list_path, "INPUT<TAB>OUT or INPUT<TAB>OUT<TAB>ERR", lines)) return 1;
+    std::vector<ListSample> list;
+    std::set<std::string> outputs;
+    for (const ListLine &l : lines) {
+        ListSample e{l.fld[0], l.fld[1], l.fld.size() == 3 ? l.fld[2] : l.fld[1] + ".log"};
+        if (!claim_output(outputs, list_path, l.ln, e.out) || !claim_output(outputs, list_path, l.ln, e.err)) return 1;
+        list.push_back(std::move(e));
+    }
+    std::unique_ptr<Sample> none;
+    const int n_failed = run_list(o, engines, list, nullptr, t_main0);
+    if (n_failed < 0) return leave(engines, none, 1);
     if (o.timing) std::fprintf(stderr, "[brc timing] cohort: %zu samples (%d failed) in %.3fs since main()\n", list.size(), n_failed, now() - t_main0);
-    return leave(engines, cur, n_failed ? 1 : 0);
+    return leave(engines, none, n_failed ? 1 : 0);
+}
+
+// --vcf FILE --vcf-samples LIST: each non-empty line of LIST is NAME<TAB>INPUT[<TAB>ERR].  Every sample runs as the list's
+// next sample (run_list) and fills its answers; after the last one the VCF is written once, sample NAME's column holding what
+// `--vcf FILE --vcf-sample NAME INPUT` writes there, or '.' in all five fields when the sample failed.  ERR (the process's
+// STDERR without one) receives that run's STDERR.  Under BRC_CLI_DECODE_ONLY STDOUT is the samples' decode summaries in list
+// order and no VCF is written, as a single-sample run writes none.
+int run_vcf_samples(const Options &o, Engines &engines, const std::vector<ListSample> &list, double t_main0) {
+    std::vector<VcfAnswers> ans(list.size(), VcfAnswers(*o.vcf));
+    std::unique_ptr<Sample> none;
+    const int n_failed = run_list(o, engines, list, &ans, t_main0);
+    if (n_failed < 0) return leave(engines, none, 1);
+    int status = n_failed ? 1 : 0;
+    if (!o.decode_only) {
+        std::string out = vcf_header(*o.vcf);
+        bool ok = true;
+        for (size_t ri = 0; ri < o.vcf->rec.size() && ok; ++ri) {
+            vcf_line(*o.vcf, ri, ans.data(), out);
+            if (out.size() >= (size_t(1) << 22)) { ok = write_all(STDOUT_FILENO, out); out.clear(); }
+        }
+        if (!ok || !write_all(STDOUT_FILENO, out)) { std::fprintf(stderr, "writing the VCF: %s\n", std::strerror(errno)); status = 1; }
+    }
+    if (o.timing) std::fprintf(stderr, "[brc timing] vcf-samples: %zu samples (%d failed) in %.3fs since main()\n", list.size(), n_failed, now() - t_main0);
+    return leave(engines, none, status);
 }
 
 }  // namespace
@@ -1619,12 +1720,12 @@ int run_cohort(const Options &o, Engines &engines, const std::string &list_path,
 int main(int argc, char **argv) {
     const double t_main0 = now();
     Options o;
-    std::string bam_list, vcf_path, vcf_sample; bool shard_given = false, vcf_sample_given = false;
+    std::string bam_list, vcf_path, vcf_sample, vcf_samples; bool shard_given = false, vcf_sample_given = false;
     static option lo[] = {{"help", 0, 0, 'h'}, {"version", 0, 0, 'v'}, {"min-mapping-quality", 1, 0, 'q'}, {"min-base-quality", 1, 0, 'b'},
                           {"max-count", 1, 0, 'd'}, {"site-list", 1, 0, 'l'}, {"reference-fasta", 1, 0, 'f'}, {"print-individual-mapq", 1, 0, 'D'},
                           {"per-library", 0, 0, 'p'}, {"max-warnings", 1, 0, 'w'}, {"insertion-centric", 0, 0, 'i'}, {"shard", 1, 0, 1000},
                           {"min-alt-count", 1, 0, 1001}, {"min-alt-fraction", 1, 0, 1002}, {"bam-list", 1, 0, 1003},
-                          {"vcf", 1, 0, 1004}, {"vcf-sample", 1, 0, 1005}, {0, 0, 0, 0}};
+                          {"vcf", 1, 0, 1004}, {"vcf-sample", 1, 0, 1005}, {"vcf-samples", 1, 0, 1006}, {0, 0, 0, 0}};
     long min_alt_count = 0; double min_alt_fraction = -1.0;       // site filter (brc_set_site_filter); off unless one is given
     bool help = false, version = false;
     for (int c; (c = getopt_long(argc, argv, "hvq:b:d:l:f:D:pw:i", lo, nullptr)) != -1;) {
@@ -1650,23 +1751,44 @@ int main(int argc, char **argv) {
         case 1003: bam_list = optarg; break;
         case 1004: vcf_path = optarg; break;
         case 1005: vcf_sample = optarg; vcf_sample_given = true; break;
+        case 1006: vcf_samples = optarg; break;
         default: usage(); return 1;
         }
     }
     o.site_filter = min_alt_count > 0 || min_alt_fraction >= 0.0;
     o.filter.min_alt_count = (int32_t)std::max<long>(min_alt_count, 1); o.filter.min_alt_fraction = std::max(min_alt_fraction, 0.0);
     if (version) { std::printf("bam-readcount version: b200 (engine ABI %d)\n", brc_abi_version()); return 1; }   // R:...:467-470 (exit 1)
-    if (help || (optind >= argc && bam_list.empty())) { usage(); return 1; }                                        // R:...:472-475
+    if (help || (optind >= argc && bam_list.empty() && vcf_samples.empty())) { usage(); return 1; }                 // R:...:472-475
     if (!bam_list.empty() && shard_given) { std::fprintf(stderr, "--bam-list and --shard cannot be combined: shard a cohort by splitting its list\n"); return 1; }
     Vcf vcf;
     if (vcf_sample_given && vcf_path.empty()) { std::fprintf(stderr, "--vcf-sample needs --vcf\n"); return 1; }
+    if (!vcf_samples.empty()) {
+        const char *why = vcf_path.empty() ? "--vcf-samples needs --vcf" : vcf_sample_given ? "--vcf-samples cannot be combined with --vcf-sample"
+                        : optind < argc ? "--vcf-samples takes no positional argument: the inputs are in its list" : nullptr;
+        if (why) { std::fprintf(stderr, "%s\n", why); return 1; }
+    }
+    std::vector<ListSample> vcf_list;     // --vcf-samples
+    std::vector<std::string> vcf_names;
     if (!vcf_path.empty()) {
         const char *clash = !o.fn_pos.empty() ? "-l" : optind + 1 < argc ? "positional regions" : o.per_lib ? "-p" : o.site_filter ? "--min-alt-count/--min-alt-fraction"
                           : shard_given ? "--shard" : !bam_list.empty() ? "--bam-list" : nullptr;
         if (clash) { std::fprintf(stderr, "--vcf cannot be combined with %s\n", clash); return 1; }
+        if (vcf_sample_given) vcf_names.push_back(vcf_sample);
+        if (!vcf_samples.empty()) {
+            std::vector<ListLine> lines;
+            if (!read_list(vcf_samples, "NAME<TAB>INPUT or NAME<TAB>INPUT<TAB>ERR", lines)) return 1;
+            std::set<std::string> names, errs;
+            for (const ListLine &l : lines) {
+                if (!names.insert(l.fld[0]).second) { std::fprintf(stderr, "%s:%d: sample %s is listed twice\n", vcf_samples.c_str(), l.ln, l.fld[0].c_str()); return 1; }
+                if (l.fld.size() == 3 && !claim_output(errs, vcf_samples, l.ln, l.fld[2])) return 1;
+                vcf_names.push_back(l.fld[0]);
+                vcf_list.push_back({l.fld[1], "", l.fld.size() == 3 ? l.fld[2] : ""});
+            }
+        }
         std::string why;
-        if (!parse_vcf(vcf_path, vcf_sample, vcf_sample_given, vcf, why)) { std::fprintf(stderr, "--vcf: %s\n", why.c_str()); return 1; }
+        if (!parse_vcf(vcf_path, vcf_names, vcf_samples.empty() ? "--vcf-sample" : "--vcf-samples", vcf, why)) { std::fprintf(stderr, "--vcf: %s\n", why.c_str()); return 1; }
         o.vcf = &vcf;
+        o.vcf_samples = !vcf_samples.empty();
     }
     o.decode_only = std::getenv("BRC_CLI_DECODE_ONLY") != nullptr;   // test hook: exercise BGZF/BAI/region fetch without a GPU
     o.device_decode = std::getenv("BRC_CLI_DEVICE_DECODE") != nullptr && !o.decode_only;
@@ -1680,12 +1802,15 @@ int main(int argc, char **argv) {
         o.region_args.assign(argv + optind, argv + argc);          // every positional argument is a region of every sample
         return run_cohort(o, engines, bam_list, t_main0);
     }
+    if (o.vcf_samples) return run_vcf_samples(o, engines, vcf_list, t_main0);
     const std::string bam_path = argv[optind];
     o.region_args.assign(argv + optind + 1, argv + argc);
     // CUDA context creation takes a second or two: do it while the BAM header, index and FASTA index are read
     if (!o.decode_only && !o.dist_refused()) engines.start_warm();
     std::unique_ptr<WindowJob[]> pool(new WindowJob[2]);
     std::unique_ptr<Sample> s = open_sample(o, bam_path, t_main0, stderr, pool.get(), true);
-    const int rc = run_sample(o, engines, *s, STDOUT_FILENO, stderr, t_main0);
+    std::vector<VcfAnswers> vcf_ans;
+    if (o.vcf) vcf_ans.emplace_back(vcf);
+    const int rc = run_sample(o, engines, *s, STDOUT_FILENO, stderr, t_main0, vcf_ans.data());
     return leave(engines, s, rc < 0 ? 1 : rc);
 }
