@@ -71,7 +71,8 @@ static int install_ref(brc_engine *e, int32_t tid, const char *contig_name, int6
     r->tid = tid; r->name = contig_name ? contig_name : ""; r->chrom_len = chrom_len; r->win_beg = win_beg; r->win_len = win_len;
     if (host_seq) r->seq.assign(host_seq, (size_t)win_len); else r->seq.clear();
     CU(r->dev.reserve((size_t)win_len / 2 + 32), "cudaMalloc(reference)");
-    CU(cudaMemsetAsync(r->dev.p, 0xFF, (size_t)win_len / 2 + 32, s), "memset(reference)");
+    const size_t coded = (size_t)(win_len + 1) / 2;     // bytes the encode writes; the padding after them reads as code 15 (N)
+    CU(cudaMemsetAsync(r->dev.as<uint8_t>() + coded, 0xFF, (size_t)win_len / 2 + 32 - coded, s), "memset(reference)");
     CU(launch_ref_encode(dev_ascii, r->dev.as<uint8_t>(), win_len, s), "reference encode");
     std::vector<RefWin> tab(e->refs.size());
     for (size_t i = 0; i < e->refs.size(); ++i)
@@ -1134,6 +1135,19 @@ int64_t brc_selftest_fastmath(brc_engine *e, int32_t max_b) {
     cudaFree(d_bad);
     if (ce != cudaSuccess) return set_cuda_error(e, ce, "fastmath selftest");
     return (int64_t)h_bad;
+}
+
+int64_t brc_get_reference_codes(brc_engine *e, int32_t tid, uint8_t *out, int64_t cap) {
+    if (!e || (!out && cap > 0) || cap < 0) return BRC_E_INVALID;
+    const HostRef *r = nullptr;
+    for (const auto &x : e->refs) if (x.tid == tid) r = &x;
+    if (!r || !r->dev.p) return BRC_E_NO_REFERENCE;
+    cudaSetDevice(e->cfg.device);
+    const int64_t size = r->win_len / 2 + 32;
+    cudaError_t ce = cudaDeviceSynchronize();     // the encode ran on the caller's stream
+    if (ce == cudaSuccess && cap > 0) ce = cudaMemcpy(out, r->dev.p, (size_t)std::min(cap, size), cudaMemcpyDeviceToHost);
+    if (ce != cudaSuccess) return set_cuda_error(e, ce, "reference codes");
+    return size;
 }
 int brc_host_alloc(size_t bytes, void **out) {
     if (!out) return BRC_E_INVALID;

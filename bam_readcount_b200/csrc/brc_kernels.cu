@@ -77,13 +77,45 @@ cudaError_t launch_init_tiles(int32_t *tile_lo, int32_t *tile_hi, int64_t n_tile
 // ---------------------------------------------------------------------------------------------
 // reference window: ASCII -> 4-bit codes, once per brc_set_reference (part of load_reference, not of a step)
 // ---------------------------------------------------------------------------------------------
-__global__ void ref_encode_kernel(const char *ascii, uint8_t *packed, int64_t n) {
-    // two bases per byte, first base in the high nibble (the BAM sequence packing), so K0 can XOR 8 bases at a time
-    int64_t b = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-    if (2 * b >= n) return;
-    const uint32_t hi = c_nt16[(unsigned char)ascii[2 * b]];
-    const uint32_t lo = (2 * b + 1 < n) ? c_nt16[(unsigned char)ascii[2 * b + 1]] : 15u;
-    packed[b] = (uint8_t)((hi << 4) | lo);
+constexpr int REF_ENCODE_THREADS = 256;
+constexpr int REF_ENCODE_MAX_BLOCKS = 4096;
+
+// four characters (one little-endian word) -> two packed bytes
+__device__ __forceinline__ uint32_t ref_pack4(const uint8_t *tab, uint32_t c) {
+    return (uint32_t)tab[c & 255u] << 4 | tab[(c >> 8) & 255u] | (uint32_t)tab[(c >> 16) & 255u] << 12 | (uint32_t)tab[c >> 24] << 8;
+}
+
+__global__ void __launch_bounds__(REF_ENCODE_THREADS) ref_encode_kernel(const char *ascii, uint8_t *packed, int64_t n, int ascii_aligned16) {
+    // two bases per byte, first base in the high nibble (the BAM sequence packing), so K0 can XOR 8 bases at a time.
+    // One thread turns 32 characters (two 16-byte loads) into 16 packed bytes (one 16-byte store).  The code table is copied to
+    // shared memory: 32 lanes indexing the constant bank with different characters would serialise.
+    __shared__ uint8_t tab[256];
+    for (int i = threadIdx.x; i < 256; i += blockDim.x) tab[i] = c_nt16[i];
+    __syncthreads();
+    const int64_t n_groups = n / 32, nb = (n + 1) / 2;
+    const int64_t t0 = blockIdx.x * (int64_t)blockDim.x + threadIdx.x, step = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t g = t0; g < n_groups; g += step) {
+        uint32_t w[8];
+        if (ascii_aligned16) {
+            const uint4 a = __ldg(reinterpret_cast<const uint4 *>(ascii) + 2 * g), b = __ldg(reinterpret_cast<const uint4 *>(ascii) + 2 * g + 1);
+            w[0] = a.x; w[1] = a.y; w[2] = a.z; w[3] = a.w; w[4] = b.x; w[5] = b.y; w[6] = b.z; w[7] = b.w;
+        } else {
+            const uint8_t *s = reinterpret_cast<const uint8_t *>(ascii) + 32 * g;
+#pragma unroll
+            for (int k = 0; k < 8; ++k) w[k] = s[4 * k] | (uint32_t)s[4 * k + 1] << 8 | (uint32_t)s[4 * k + 2] << 16 | (uint32_t)s[4 * k + 3] << 24;
+        }
+        uint4 o;
+        o.x = ref_pack4(tab, w[0]) | ref_pack4(tab, w[1]) << 16;
+        o.y = ref_pack4(tab, w[2]) | ref_pack4(tab, w[3]) << 16;
+        o.z = ref_pack4(tab, w[4]) | ref_pack4(tab, w[5]) << 16;
+        o.w = ref_pack4(tab, w[6]) | ref_pack4(tab, w[7]) << 16;
+        reinterpret_cast<uint4 *>(packed)[g] = o;
+    }
+    for (int64_t b = 16 * n_groups + t0; b < nb; b += step) {      // the last n mod 32 characters, one packed byte per thread
+        const uint32_t hi = tab[(unsigned char)ascii[2 * b]];
+        const uint32_t lo = (2 * b + 1 < n) ? tab[(unsigned char)ascii[2 * b + 1]] : 15u;
+        packed[b] = (uint8_t)((hi << 4) | lo);
+    }
 }
 
 static cudaError_t ensure_tables() {
@@ -103,8 +135,10 @@ static cudaError_t ensure_tables() {
 cudaError_t launch_ref_encode(const char *d_ascii, uint8_t *d_code, int64_t n, cudaStream_t s) {
     cudaError_t e = ensure_tables();
     if (e != cudaSuccess || n == 0) return e;
-    const int64_t nb = (n + 1) / 2;
-    ref_encode_kernel<<<(unsigned)((nb + 255) / 256), 256, 0, s>>>(d_ascii, d_code, n);
+    if ((uintptr_t)d_code & 15) return cudaErrorInvalidValue;      // the packed window is a device allocation: 16-byte stores
+    const int64_t work = std::max<int64_t>(n / 32, 1);
+    const int64_t blocks = std::min<int64_t>((work + REF_ENCODE_THREADS - 1) / REF_ENCODE_THREADS, REF_ENCODE_MAX_BLOCKS);
+    ref_encode_kernel<<<(unsigned)blocks, REF_ENCODE_THREADS, 0, s>>>(d_ascii, d_code, n, ((uintptr_t)d_ascii & 15) == 0 ? 1 : 0);
     return cudaGetLastError();
 }
 

@@ -103,6 +103,7 @@ EXPORTS = [
     "brc_begin_region", "brc_push_read", "brc_push_reads", "brc_end_region", "brc_decode_bam_span", "brc_push_bam_span", "brc_fetch_decoded_batch", "brc_compute", "brc_get_results",
     "brc_get_warning_counts", "brc_format_text", "brc_format_window", "brc_write_text", "brc_set_queue_carry", "brc_plan_device", "brc_run_device", "brc_device_packed_results", "brc_get_packed_results",
     "brc_fetch_device_results", "brc_last_launch_count", "brc_last_h2d_bytes", "brc_host_alloc", "brc_host_free", "brc_last_stage_ms", "brc_selftest_fastmath",
+    "brc_get_reference_codes",
     "brc_set_site_filter", "brc_get_selected_results", "brc_set_allele_queries", "brc_get_allele_answers",
 ]
 
@@ -154,6 +155,8 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
     lib.brc_fetch_device_results.argtypes = [C.c_void_p, C.c_void_p]
     lib.brc_selftest_fastmath.argtypes = [C.c_void_p, C.c_int32]
     lib.brc_selftest_fastmath.restype = C.c_int64
+    lib.brc_get_reference_codes.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_int64]
+    lib.brc_get_reference_codes.restype = C.c_int64
     lib.brc_last_launch_count.argtypes = [C.c_void_p]
     lib.brc_last_h2d_bytes.argtypes = [C.c_void_p]
     lib.brc_last_h2d_bytes.restype = C.c_int64
@@ -496,6 +499,14 @@ class Engine:
     # ---- device-resident path (include/brc_engine.h "device-resident path") ---------------------------------
     def set_reference_device(self, tid: int, name: str, chrom_len: int, win_beg: int, dev_ascii_ptr: int, win_len: int, stream_ptr: int):
         self._check(self.lib.brc_set_reference_device(self.h, tid, name.encode(), chrom_len, win_beg, dev_ascii_ptr, win_len, stream_ptr))
+
+    def reference_codes(self, tid: int) -> np.ndarray:
+        """The packed reference window of contig tid as the kernels read it (brc_get_reference_codes)."""
+        n = int(self.lib.brc_get_reference_codes(self.h, tid, None, 0))
+        self._check(min(n, 0))
+        out = np.empty(n, dtype=np.uint8)
+        self._check(min(int(self.lib.brc_get_reference_codes(self.h, tid, out.ctypes.data, n)), 0))
+        return out
 
     def plan_device(self, regions: Sequence[CRegion], n_reads_cap: int, n_sec_cap: int = 0):
         arr = (CRegion * len(regions))(*regions)

@@ -16,6 +16,7 @@ shard in rank order, into two spool sets per source, and consumes them on an emi
 from __future__ import annotations
 
 import ctypes as C
+import weakref
 from dataclasses import dataclass
 from typing import List, Optional, Sequence, Tuple
 
@@ -104,37 +105,101 @@ def alias_device_bytes(ptr: int, nbytes: int, device):
     return torch.as_tensor(_CudaView(ptr, nbytes), device=device)
 
 
+def reference_length(spec: synth_cb.Spec) -> int:
+    return spec.contig_len if spec.mode == synth_cb.WGS else spec.deep_contig_len()
+
+
+class DeviceReference:
+    """One contig's reference characters in HBM, generated on one stream; every stream that reads them waits for that first."""
+
+    def __init__(self, spec: synth_cb.Spec, contig: int, stream, device):
+        import torch
+        self.length = reference_length(spec)
+        with torch.cuda.stream(stream):
+            self.ascii = torch.empty(self.length + 64, dtype=torch.uint8, device=device)
+        rc = synth_cb.load().brc_synth_ref_device(C.byref(spec.c), contig, 0, self.length, self.ascii.data_ptr(), stream.cuda_stream)
+        assert rc == 0, rc
+        self.ready = torch.cuda.Event()
+        self.ready.record(stream)
+
+    def use_on(self, stream):
+        stream.wait_event(self.ready)
+        self.ascii.record_stream(stream)          # the allocator must not hand the bytes out again before this stream has read them
+
+
+class ContigReferences:
+    """The reference characters of the contigs that the runners of one generated genome on one device are on.  A contig is
+    generated once, on the stream of the first runner that moves to it, and dropped when the last runner holding it moves on
+    or is closed.  Runners deal a contig's windows round-robin, so without sharing every runner would generate every contig
+    again.  Holders are held weakly: a runner dropped without close() stops holding its contig, which goes at the next move."""
+
+    def __init__(self):
+        self._live = {}            # contig -> (reference, WeakSet of the runners holding it)
+        self.generated = 0
+
+    def move(self, runner, old: int, new: int):
+        """`runner` leaves contig `old` for `new`; returns `new`'s reference, ready to be read on `runner.stream`."""
+        self.release(runner, old)
+        for c in [c for c, (_, holders) in self._live.items() if not holders and c != new]:
+            del self._live[c]
+        entry = self._live.get(new)
+        if entry is None:
+            entry = self._live[new] = (runner.generate_reference(new), weakref.WeakSet())
+            self.generated += 1
+        entry[0].use_on(runner.stream)
+        entry[1].add(runner)
+        return entry[0]
+
+    def release(self, runner, contig: int):
+        entry = self._live.get(contig)
+        if entry is not None:
+            entry[1].discard(runner)
+            if not entry[1]:
+                del self._live[contig]
+
+    def live(self) -> List[int]:
+        return sorted(c for c, (_, holders) in self._live.items() if holders)
+
+
+_shared_references = weakref.WeakKeyDictionary()      # spec -> {device index: ContigReferences}
+
+
+def shared_references(spec: synth_cb.Spec, device_index: int) -> ContigReferences:
+    """The ContigReferences every WindowRunner of `spec` on that device uses."""
+    return _shared_references.setdefault(spec, {}).setdefault(device_index, ContigReferences())
+
+
 class WindowRunner:
-    """One engine handle + its generator buffers: runs one window at a time on its own stream."""
+    """One engine handle + its generator buffers: runs one window at a time on its own stream.  The runners of one spec on one
+    device share the reference characters of their contigs (ContigReferences); each handle encodes them into its own window."""
 
     def __init__(self, spec: synth_cb.Spec, max_window_reads: int, device, flags: dict, lib_names: Sequence[str] = ()):
         import torch
         self.spec, self.device = spec, device
-        self.eng = Engine(device=device.index if hasattr(device, "index") and device.index is not None else 0, lib_names=lib_names, **flags)
+        index = device.index if hasattr(device, "index") and device.index is not None else 0
+        self.eng = Engine(device=index, lib_names=lib_names, **flags)
         self.dw = synth_cb.DeviceWindow(spec, max_window_reads, device)
         self.stream = torch.cuda.Stream(device=device)
         self.done = torch.cuda.Event()            # kernels of the current window finished
         self.sent = torch.cuda.Event()            # its records left the handle (gather) — safe to re-plan
-        self.ref_ascii = None
+        self.refs = shared_references(spec, index)
         self.cur_contig = -1
         self.window: Optional[Window] = None
         self.n_sec_host = None                    # pinned int32[1]: the window's record count
         self.busy = False
 
     def close(self):
+        self.refs.release(self, self.cur_contig)
         self.eng.close()
 
+    def generate_reference(self, contig: int) -> DeviceReference:
+        return DeviceReference(self.spec, contig, self.stream, self.device)
+
     def _ensure_reference(self, contig: int):
-        import torch
         if contig == self.cur_contig:
             return
-        L = self.spec.contig_len if self.spec.mode == synth_cb.WGS else self.spec.deep_contig_len()
-        if self.ref_ascii is None or self.ref_ascii.numel() < L + 64:
-            self.ref_ascii = torch.empty(L + 64, dtype=torch.uint8, device=self.device)
-        sp = self.stream.cuda_stream
-        rc = synth_cb.load().brc_synth_ref_device(C.byref(self.spec.c), contig, 0, L, self.ref_ascii.data_ptr(), sp)
-        assert rc == 0, rc
-        self.eng.set_reference_device(contig, f"chr{contig + 1}", L, 0, self.ref_ascii.data_ptr(), L, sp)
+        ref = self.refs.move(self, self.cur_contig, contig)
+        self.eng.set_reference_device(contig, f"chr{contig + 1}", ref.length, 0, ref.ascii.data_ptr(), ref.length, self.stream.cuda_stream)
         self.cur_contig = contig
 
     def launch(self, w: Window, sec_cap: int = 0, resident=None):

@@ -385,6 +385,10 @@ BRC_API int brc_fetch_device_results(brc_engine *e, void *stream);
 /* Self-test of the kernels' exact-arithmetic shortcuts (reciprocal division, float<->double bit casts)
  * against the IEEE intrinsics for every divisor 1..max_b; returns the number of mismatches (0 = ok). */
 BRC_API int64_t brc_selftest_fastmath(brc_engine *e, int32_t max_b);
+/* The packed reference window of contig `tid` as the kernels read it: seq_nt16 codes, two per byte, first base in the high
+ * nibble, then 0xFF padding (win_len / 2 + 32 bytes in all).  Waits for the device, copies min(cap, that size) bytes to `out`
+ * and returns the full size, or a negative status (BRC_E_NO_REFERENCE when the contig has none). */
+BRC_API int64_t brc_get_reference_codes(brc_engine *e, int32_t tid, uint8_t *out, int64_t cap);
 /* kernels launched by the last brc_run_device/brc_compute (for bench.py's gpu_launches) */
 /* Page-locked host memory for batches handed to brc_push_reads (a borrowed batch is DMA'd straight out of the caller's arrays:
  * from pageable memory the copies are staged and synchronous).  cudaHostAlloc / cudaFreeHost behind plain pointers, so that a host
