@@ -27,6 +27,14 @@ const HostRef *find_ref(const brc_engine *e, int32_t tid) {
     for (const auto &r : e->refs) if (r.tid == tid) return &r;
     return nullptr;
 }
+int check_view(brc_engine *e, const char *who, unsigned kinds) {
+    static const char *const held[] = {"", "dense results", "a site filter's selected sites", "allele answers"};
+    static const char *const view[] = {"", "brc_get_results", "brc_get_selected_results", "brc_get_allele_answers"};
+    const int k = e->results_kind();
+    if (k == BRC_RESULTS_NONE) return set_error(e, BRC_E_INVALID, std::string(who) + ": no results (call brc_compute)");
+    if (kinds >> k & 1u) return BRC_OK;
+    return set_error(e, BRC_E_INVALID, std::string(who) + ": the last run produced " + held[k] + " (" + view[k] + ")");
+}
 }  // namespace brc
 
 #define CU(call, what) do { cudaError_t ce_ = (call); if (ce_ != cudaSuccess) return set_cuda_error(e, ce_, what); } while (0)
@@ -169,15 +177,16 @@ int brc_set_reference_device(brc_engine *e, int32_t tid, const char *contig_name
     return install_ref(e, tid, contig_name, chrom_len, win_beg, win_len, nullptr, dev_ascii, (cudaStream_t)stream);
 }
 
+// The queries belong to the batch being dropped, and so do answers they produced.
 static void drop_allele_queries(brc_engine *e) {
-    e->queries_on = false; e->aq.clear(); e->aq_bases.clear(); e->aq_launched = false; e->answers_valid = false;
+    e->queries_on = false; e->aq.clear(); e->aq_bases.clear();
+    if (e->last.kind == BRC_RESULTS_ANSWERS) e->last = {};
 }
 
 int brc_reset(brc_engine *e) {
     if (!e) return BRC_E_INVALID;
     e->reads.clear(); e->is_borrowed = false; e->regions.clear(); e->region_open = false; e->adm.reset(); e->n_indel_ops = 0;
-    e->results_valid = false; e->planned = false; e->tiles.clear(); e->regions_dev.clear(); e->n_slots = 0; e->wide.valid = false;
-    e->sparse = false; e->sel_launched = false; e->n_sel = 0;
+    e->last = {}; e->planned = false; e->tiles.clear(); e->regions_dev.clear(); e->n_slots = 0; e->n_sel = 0;
     drop_allele_queries(e);
     e->dec.pushed = false; e->dec.ins_reads.clear(); e->dec.ins_off.clear(); e->dec.ins_pool.clear();
     for (auto &w : e->warn_counts) w = 0;
@@ -224,7 +233,7 @@ int brc_begin_region(brc_engine *e, int32_t tid, int32_t beg, int32_t end, int32
     r.n_slots = 0;
     e->regions.push_back(r);
     e->region_open = true; e->adm.reset(); e->open_max_end = r.first_pos;
-    e->results_valid = false; e->planned = false;
+    e->last.on_host = false; e->planned = false;
     drop_allele_queries(e);
     return BRC_OK;
 }
@@ -480,10 +489,8 @@ static void plan_selection(brc_engine *e) {
     }
 }
 
-// The selection kernels after the pileup kernels on stream s (ev[3] after them); no-op without a filter.
+// The selection kernels after the pileup kernels on stream s (ev[3] after them).
 static int launch_selection(brc_engine *e, cudaStream_t s) {
-    e->sel_launched = false;
-    if (!e->filter_on) return BRC_OK;
     const int64_t NS = e->n_slots, rows = e->n_rows, R = (int64_t)e->sel_regions.size();
     const int64_t nb = std::max<int64_t>(1, (NS + SELECT_SCAN_CTA - 1) / SELECT_SCAN_CTA);
     size_t off = 0;
@@ -517,51 +524,14 @@ static int launch_selection(brc_engine *e, cudaStream_t s) {
     CU(cudaEventRecord(e->ev[3], s), "event");
     e->sel_params = P;
     e->sel_filter = e->filter;
-    e->sel_launched = true;
-    return BRC_OK;
-}
-
-// The compact selection to the host: the counts first, then exactly the shipped bytes.
-static int fetch_selected(brc_engine *e, cudaStream_t s) {
-    const SelectParams &P = e->sel_params;
-    int32_t cnt = 0;
-    CU(e->h_misc.reserve(64), "pin");
-    uint64_t *hm = e->h_misc.as<uint64_t>();
-    hm[0] = hm[1] = hm[2] = 0;
-    CU(cudaMemcpyAsync(&cnt, e->d_sec_count.p, 4, cudaMemcpyDeviceToHost, s), "D2H sec_count");
-    if (P.n_slots > 0) {
-        CU(cudaMemcpyAsync(hm, P.idx + P.n_slots, 8, cudaMemcpyDeviceToHost, s), "D2H selected sites");
-        CU(cudaMemcpyAsync(hm + 1, P.counters, 16, cudaMemcpyDeviceToHost, s), "D2H selection counters");
-    }
-    CU(cudaStreamSynchronize(s), "sync");
-    if ((int64_t)cnt > e->sec_cap) return set_error(e, BRC_E_OVERFLOW, "secondary key pool overflow (re-plan with a larger n_sec_cap)");
-    const int64_t n = (int64_t)hm[0], ns = (int64_t)hm[1];
-    e->sel_abandoned = (int64_t)hm[2];
-    const size_t wbytes = (size_t)n * e->n_rows * 4 * N_WORDS;
-    CU(e->h_words.reserve(std::max<size_t>(wbytes, 4)), "pin"); CU(e->h_sec.reserve((size_t)std::max<int64_t>(ns, 1) * sizeof(SecRec)), "pin");
-    CU(e->h_sel.reserve((size_t)std::max<int64_t>(n, 1) * 5), "pin");
-    if (n) {
-        CU(cudaMemcpyAsync(e->h_words.p, P.c_words, wbytes, cudaMemcpyDeviceToHost, s), "D2H selected words");
-        CU(cudaMemcpyAsync(e->h_sel.p, P.c_site, (size_t)n * 4, cudaMemcpyDeviceToHost, s), "D2H selected site ids");
-        CU(cudaMemcpyAsync(e->h_sel.as<uint32_t>() + n, P.c_emit, (size_t)n, cudaMemcpyDeviceToHost, s), "D2H selected emit bytes");
-    }
-    if (ns) CU(cudaMemcpyAsync(e->h_sec.p, P.c_sec, (size_t)ns * sizeof(SecRec), cudaMemcpyDeviceToHost, s), "D2H selected records");
-    CU(cudaMemcpyAsync(hm + 4, e->d_warn.p, 16, cudaMemcpyDeviceToHost, s), "D2H warn");
-    CU(cudaStreamSynchronize(s), "sync D2H");
-    e->warn_counts[0] = (int64_t)hm[4]; e->warn_counts[1] = (int64_t)hm[5]; e->warn_counts[2] = 0;
-    e->warn_counts[3] = -1;
-    e->n_sel = n; e->h_n_sec = ns; e->sparse = true; e->answers_valid = false;
-    e->results_valid = true; e->fmt_valid = false; e->wide.valid = false;
     return BRC_OK;
 }
 
 // ---------------------------------------------------------------------------------------------
 // allele queries: launch, answer fetch (kernels in brc_alleles.cu)
 // ---------------------------------------------------------------------------------------------
-// The allele kernels after the pileup kernels on stream s (ev[3], ev[4] around them); no-op without queries.
+// The allele kernels after the pileup kernels on stream s (ev[3], ev[4] around them).
 static int launch_allele_queries(brc_engine *e, cudaStream_t s) {
-    e->aq_launched = false;
-    if (!e->queries_on) return BRC_OK;
     const int64_t NS = e->n_slots, nq = (int64_t)e->aq.size(), nb = (int64_t)e->aq_bases.size();
     size_t off = 0;
     auto take = [&](size_t bytes) { const size_t o = off; off = (off + bytes + 15) & ~(size_t)15; return o; };
@@ -584,25 +554,6 @@ static int launch_allele_queries(brc_engine *e, cudaStream_t s) {
     if (nq) e->launch_count += ALLELE_KERNELS;
     CU(cudaEventRecord(e->ev[4], s), "event");
     e->aq_params = P;
-    e->aq_launched = true;
-    return BRC_OK;
-}
-
-// The answers, the warning words and the pool counter to the host: nothing else of the run crosses PCIe.
-static int fetch_answers(brc_engine *e, cudaStream_t s) {
-    const AlleleParams &P = e->aq_params;
-    CU(e->h_misc.reserve(64), "pin");
-    CU(e->h_ans.reserve((size_t)std::max<int64_t>(P.n_q, 1) * sizeof(brc_allele_answer)), "pin");
-    uint64_t *hm = e->h_misc.as<uint64_t>();
-    CU(cudaMemcpyAsync(hm, e->d_sec_count.p, 4, cudaMemcpyDeviceToHost, s), "D2H sec_count");
-    CU(cudaMemcpyAsync(hm + 4, e->d_warn.p, 16, cudaMemcpyDeviceToHost, s), "D2H warn");
-    if (P.n_q) CU(cudaMemcpyAsync(e->h_ans.p, P.ans, (size_t)P.n_q * sizeof(brc_allele_answer), cudaMemcpyDeviceToHost, s), "D2H allele answers");
-    CU(cudaStreamSynchronize(s), "sync D2H");
-    if ((int64_t)*e->h_misc.as<int32_t>() > e->sec_cap) return set_error(e, BRC_E_OVERFLOW, "secondary key pool overflow (re-plan with a larger n_sec_cap)");
-    e->warn_counts[0] = (int64_t)hm[4]; e->warn_counts[1] = (int64_t)hm[5]; e->warn_counts[2] = 0;
-    e->warn_counts[3] = 0;           // LIBRARY_UNAVAILABLE needs -p, which allele queries refuse
-    e->h_n_sec = 0; e->sparse = false; e->answers_valid = true;
-    e->results_valid = true; e->fmt_valid = false; e->wide.valid = false;
     return BRC_OK;
 }
 
@@ -622,8 +573,18 @@ static void make_params(brc_engine *e, const int32_t *d_region_of_read, Precompu
     P1.work_counter = P1.res.warn + WARN_WORDS;                 // pileup launch k of a run takes dispenser k
 }
 
-// K(init) + K0 + K1 on stream s.  Returns BRC_E_OVERFLOW (after syncing) if the secondary pool was too small.
-static int run_kernels(brc_engine *e, const int32_t *d_region_of_read, cudaStream_t s, bool check_overflow) {
+// The stream tail after the pileup kernels, shared by run_kernels and compute_pipelined: ev[2], then the selection (with a site
+// filter) or the allele kernels (with queries).  Fixes the kind of results the run produces.
+static int launch_tail(brc_engine *e, cudaStream_t s) {
+    e->last = {e->filter_on ? BRC_RESULTS_SELECTED : e->queries_on ? BRC_RESULTS_ANSWERS : BRC_RESULTS_DENSE, false};
+    CU(cudaEventRecord(e->ev[2], s), "event");
+    if (e->filter_on) return launch_selection(e, s);
+    if (e->queries_on) return launch_allele_queries(e, s);
+    return BRC_OK;
+}
+
+// K(init) + K0 + K1 and the tail on stream s.  Launches only: fetch_results brings the results to the host.
+static int run_kernels(brc_engine *e, const int32_t *d_region_of_read, cudaStream_t s) {
     PrecomputeParams P0; PileupParams P1;
     make_params(e, d_region_of_read, P0, P1);
 
@@ -634,43 +595,62 @@ static int run_kernels(brc_engine *e, const int32_t *d_region_of_read, cudaStrea
     CU(cudaEventRecord(e->ev[1], s), "event");
     CU(launch_pileup(P1, s), "launch pileup"); if (P1.n_tiles) e->launch_count++;
     CU(launch_deep_sites(P1, s), "launch deep_sites"); if (P1.n_deep) e->launch_count++;
-    CU(cudaEventRecord(e->ev[2], s), "event");
-    int rs = launch_selection(e, s);
-    if (rs == BRC_OK) rs = launch_allele_queries(e, s);
-    if (rs != BRC_OK) return rs;
-    if (check_overflow) {
-        int32_t cnt = 0;
-        CU(cudaMemcpyAsync(&cnt, P1.res.sec_count, 4, cudaMemcpyDeviceToHost, s), "D2H sec_count");
-        CU(cudaStreamSynchronize(s), "sync kernels");
-        e->h_n_sec = cnt;
-        if ((int64_t)cnt > e->sec_cap) return BRC_E_OVERFLOW;
-    }
-    return BRC_OK;
+    return launch_tail(e, s);
 }
 
-static int fetch_results(brc_engine *e, cudaStream_t s, bool slots_already_fetched = false, int64_t sec_done = 0) {
-    if (e->sel_launched) return fetch_selected(e, s);
-    if (e->aq_launched) return fetch_answers(e, s);
-    const int64_t rs = (int64_t)e->n_rows * e->n_slots;
-    int32_t cnt = 0;
-    CU(cudaMemcpyAsync(&cnt, e->d_sec_count.p, 4, cudaMemcpyDeviceToHost, s), "D2H sec_count");
-    CU(cudaStreamSynchronize(s), "sync");
-    if ((int64_t)cnt > e->sec_cap) return set_error(e, BRC_E_OVERFLOW, "secondary key pool overflow (re-plan with a larger n_sec_cap)");
-    e->h_n_sec = cnt;
-    const int64_t rs1 = std::max<int64_t>(rs, 1), ns1 = std::max<int64_t>(cnt, 1);
-    CU(e->h_words.reserve(rs1 * 4 * N_WORDS), "pin"); CU(e->h_sec.reserve((size_t)ns1 * sizeof(SecRec)), "pin");
+// The last run's results to the host, on every path.  The pool counter crosses once, in a first round trip together with the
+// selection's two counts (the sizes of its compact outputs) or with all an allele run ships (warning words and answers).  When
+// the pool overflowed, BRC_E_OVERFLOW and nothing else: the caller grows the pool or reports it.  Then exactly the bytes of the
+// run's kind.  sec_done >= 0: compute_pipelined's chunks have already copied every dense word and pool records [0, sec_done).
+static int fetch_results(brc_engine *e, cudaStream_t s, int64_t sec_done = -1) {
+    const int kind = e->last.kind;
+    const SelectParams &S = e->sel_params;
+    const AlleleParams &A = e->aq_params;
     CU(e->h_misc.reserve(64), "pin");
-    if (rs && !slots_already_fetched) CU(cudaMemcpyAsync(e->h_words.p, e->d_words.p, rs * 4 * N_WORDS, cudaMemcpyDeviceToHost, s), "D2H words");
-    if (cnt > sec_done)      // records [0, sec_done) were copied while the kernels ran (compute_pipelined)
-        CU(cudaMemcpyAsync((char *)e->h_sec.p + (size_t)sec_done * sizeof(SecRec), (char *)e->d_sec.p + (size_t)sec_done * sizeof(SecRec),
-                           (size_t)(cnt - sec_done) * sizeof(SecRec), cudaMemcpyDeviceToHost, s), "D2H sec");
-    CU(cudaMemcpyAsync(e->h_misc.p, e->d_warn.p, 16, cudaMemcpyDeviceToHost, s), "D2H warn");
-    CU(cudaStreamSynchronize(s), "sync D2H");
-    const unsigned long long *w = e->h_misc.as<unsigned long long>();
-    e->warn_counts[0] = (int64_t)w[0]; e->warn_counts[1] = (int64_t)w[1]; e->warn_counts[2] = 0;
-    e->warn_counts[3] = -1;          // LIBRARY_UNAVAILABLE: counted from the flag bits on demand (brc_get_warning_counts)
-    e->sparse = false; e->answers_valid = false;
-    e->results_valid = true; e->fmt_valid = false; e->wide.valid = false;
+    uint64_t *hm = e->h_misc.as<uint64_t>();   // [0] pool counter, [1] selected sites, [2] their records, [3] abandoned sites, [4..5] warnings
+    hm[0] = hm[1] = hm[2] = hm[3] = 0;
+    CU(cudaMemcpyAsync(hm, e->d_sec_count.p, 4, cudaMemcpyDeviceToHost, s), "D2H sec_count");
+    if (kind == BRC_RESULTS_SELECTED && S.n_slots > 0) {
+        CU(cudaMemcpyAsync(hm + 1, S.idx + S.n_slots, 8, cudaMemcpyDeviceToHost, s), "D2H selected sites");
+        CU(cudaMemcpyAsync(hm + 2, S.counters, 16, cudaMemcpyDeviceToHost, s), "D2H selection counters");
+    }
+    if (kind == BRC_RESULTS_ANSWERS) {
+        CU(e->h_ans.reserve((size_t)std::max<int64_t>(A.n_q, 1) * sizeof(brc_allele_answer)), "pin");
+        CU(cudaMemcpyAsync(hm + 4, e->d_warn.p, 16, cudaMemcpyDeviceToHost, s), "D2H warn");
+        if (A.n_q) CU(cudaMemcpyAsync(e->h_ans.p, A.ans, (size_t)A.n_q * sizeof(brc_allele_answer), cudaMemcpyDeviceToHost, s), "D2H allele answers");
+    }
+    CU(cudaStreamSynchronize(s), "sync");
+    const int64_t cnt = *e->h_misc.as<int32_t>();
+    if (cnt > e->sec_cap) { e->h_n_sec = cnt; return BRC_E_OVERFLOW; }   // the retry loop grows the pool past it
+    e->h_n_sec = 0;
+    if (kind != BRC_RESULTS_ANSWERS) {
+        const bool sel = kind == BRC_RESULTS_SELECTED;
+        const int64_t n = sel ? (int64_t)hm[1] : e->n_slots, ns = sel ? (int64_t)hm[2] : cnt, done = std::max<int64_t>(sec_done, 0);
+        const size_t wbytes = (size_t)n * e->n_rows * 4 * N_WORDS;
+        CU(e->h_words.reserve(std::max<size_t>(wbytes, 4 * N_WORDS)), "pin");
+        CU(e->h_sec.reserve((size_t)std::max<int64_t>(ns, 1) * sizeof(SecRec)), "pin");
+        if (sel) {
+            CU(e->h_sel.reserve((size_t)std::max<int64_t>(n, 1) * 5), "pin");
+            if (n) {
+                CU(cudaMemcpyAsync(e->h_words.p, S.c_words, wbytes, cudaMemcpyDeviceToHost, s), "D2H selected words");
+                CU(cudaMemcpyAsync(e->h_sel.p, S.c_site, (size_t)n * 4, cudaMemcpyDeviceToHost, s), "D2H selected site ids");
+                CU(cudaMemcpyAsync(e->h_sel.as<uint32_t>() + n, S.c_emit, (size_t)n, cudaMemcpyDeviceToHost, s), "D2H selected emit bytes");
+            }
+        } else if (n && sec_done < 0) {
+            CU(cudaMemcpyAsync(e->h_words.p, e->d_words.p, wbytes, cudaMemcpyDeviceToHost, s), "D2H words");
+        }
+        if (ns > done)
+            CU(cudaMemcpyAsync(e->h_sec.as<SecRec>() + done, (sel ? S.c_sec : e->d_sec.as<SecRec>()) + done, (size_t)(ns - done) * sizeof(SecRec),
+                               cudaMemcpyDeviceToHost, s), "D2H sec");
+        CU(cudaMemcpyAsync(hm + 4, e->d_warn.p, 16, cudaMemcpyDeviceToHost, s), "D2H warn");
+        CU(cudaStreamSynchronize(s), "sync D2H");
+        e->h_n_sec = ns;
+        if (sel) { e->n_sel = n; e->sel_abandoned = (int64_t)hm[3]; }
+    }
+    e->warn_counts[0] = (int64_t)hm[4]; e->warn_counts[1] = (int64_t)hm[5]; e->warn_counts[2] = 0;
+    // LIBRARY_UNAVAILABLE: counted from the flag bits on demand (brc_get_warning_counts); it needs -p, which allele queries refuse
+    e->warn_counts[3] = kind == BRC_RESULTS_ANSWERS ? 0 : -1;
+    e->last.on_host = true; e->wide.valid = false; e->fmt_valid = false;   // the views expanded from earlier results are stale
     return BRC_OK;
 }
 
@@ -681,13 +661,12 @@ static int compute_batch(brc_engine *e, int64_t cap, const int32_t *d_region_of_
     if (rc != BRC_OK) return rc;
     for (int attempt = 0; attempt < 8; ++attempt) {
         rc = alloc_sec(e, cap);
-        if (rc != BRC_OK) return rc;
-        rc = run_kernels(e, d_region_of_read, s, true);
-        if (rc != BRC_E_OVERFLOW) break;
+        if (rc == BRC_OK) rc = run_kernels(e, d_region_of_read, s);
+        if (rc == BRC_OK) rc = fetch_results(e, s);
+        if (rc != BRC_E_OVERFLOW) return rc;
         cap = std::max<int64_t>(cap * 2, e->h_n_sec + 1024);
     }
-    if (rc != BRC_OK) return rc == BRC_E_OVERFLOW ? set_error(e, rc, "secondary key pool overflow") : rc;
-    return fetch_results(e, s);
+    return set_error(e, BRC_E_OVERFLOW, "secondary key pool overflow");
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -808,8 +787,8 @@ static int compute_pipelined(brc_engine *e) {
     int rc = issue_h2d_chunks(e, n_chunks);
     if (rc != BRC_OK) return rc;
     e->dev_reads = reads_dev(d_in_batch(e, n));
-    // host result buffers (with a site filter only the compacted selection comes back, after the kernels: fetch_selected; with
-    // allele queries only their answers: fetch_answers)
+    // host result buffers (with a site filter only the compacted selection comes back, and with allele queries only their
+    // answers, after the kernels: fetch_results)
     const bool sel = e->filter_on || e->queries_on;
     const int64_t rs1 = std::max<int64_t>(rs, 1);
     if (!sel) CU(e->h_words.reserve(rs1 * 4 * N_WORDS), "pin");
@@ -868,9 +847,7 @@ static int compute_pipelined(brc_engine *e) {
         }
     }
     CU(cudaEventRecord(e->ev[1], sk), "event");
-    CU(cudaEventRecord(e->ev[2], sk), "event");
-    rc = launch_selection(e, sk);
-    if (rc == BRC_OK) rc = launch_allele_queries(e, sk);
+    rc = launch_tail(e, sk);
     if (rc != BRC_OK) return rc;
     // everything is queued: follow the kernels and ship the pool records each chunk finished (their own stream: the word copies
     // of later chunks are already queued on s_out)
@@ -885,14 +862,9 @@ static int compute_pipelined(brc_engine *e) {
         }
     }
     CU(cudaStreamSynchronize(e->s_in), "sync H2D");
-    CU(cudaStreamSynchronize(sk), "sync kernels");
     CU(cudaStreamSynchronize(e->s_out), "sync D2H");
-    int32_t cnt = 0;
-    CU(cudaMemcpy(&cnt, e->d_sec_count.p, 4, cudaMemcpyDeviceToHost), "D2H sec_count");
-    e->h_n_sec = cnt;
     CU(cudaStreamSynchronize(e->s_sec), "sync D2H sec");
-    if ((int64_t)cnt > e->sec_cap) return BRC_E_OVERFLOW;
-    return fetch_results(e, sk, true, sec_done);
+    return fetch_results(e, sk, sec_done);
 }
 
 extern "C" {
@@ -964,9 +936,7 @@ int brc_compute(brc_engine *e) {
 
 int brc_get_results(brc_engine *e, brc_results *out) {
     if (!e || !out) return BRC_E_INVALID;
-    if (!e->results_valid) return set_error(e, BRC_E_INVALID, "get_results: no results (call brc_compute)");
-    if (e->sparse) return set_error(e, BRC_E_INVALID, "get_results: a site filter is set, there is no dense view (brc_get_selected_results)");
-    if (e->answers_valid) return set_error(e, BRC_E_INVALID, "get_results: allele queries are set, there is no dense view (brc_get_allele_answers)");
+    if (int rc = check_view(e, "get_results", 1u << BRC_RESULTS_DENSE)) return rc;
     brc::ensure_wide(e);
     const brc_engine::Wide &W = e->wide;
     out->n_regions = (int64_t)e->regions.size(); out->regions = e->regions.data(); out->n_rows = e->n_rows; out->n_slots = e->n_slots;
@@ -980,9 +950,7 @@ int brc_get_results(brc_engine *e, brc_results *out) {
 
 int brc_get_packed_results(brc_engine *e, brc_packed_results *out) {
     if (!e || !out) return BRC_E_INVALID;
-    if (!e->results_valid) return set_error(e, BRC_E_INVALID, "get_packed_results: no results (call brc_compute)");
-    if (e->sparse) return set_error(e, BRC_E_INVALID, "get_packed_results: a site filter is set, there is no dense view (brc_get_selected_results)");
-    if (e->answers_valid) return set_error(e, BRC_E_INVALID, "get_packed_results: allele queries are set, there is no dense view (brc_get_allele_answers)");
+    if (int rc = check_view(e, "get_packed_results", 1u << BRC_RESULTS_DENSE)) return rc;
     out->n_regions = (int64_t)e->regions.size(); out->regions = e->regions.data(); out->n_rows = e->n_rows; out->n_slots = e->n_slots;
     out->words = e->h_words.as<uint32_t>(); out->n_sec = e->h_n_sec; out->sec = e->h_sec.as<brc_sec_record>(); out->sec_count = nullptr;
     return BRC_OK;
@@ -990,10 +958,10 @@ int brc_get_packed_results(brc_engine *e, brc_packed_results *out) {
 
 int brc_get_warning_counts(brc_engine *e, int64_t out[4]) {
     if (!e || !out) return BRC_E_INVALID;
-    if (e->results_valid && e->warn_counts[3] < 0) {
+    if (e->last.on_host && e->warn_counts[3] < 0) {
         // LIBRARY_UNAVAILABLE fires once per abandoned site callback (R:bamreadcount.cpp:281-284)
         int64_t lu = 0;
-        if (e->cfg.per_lib && e->sparse) lu = e->sel_abandoned;   // counted by the selection's site pass
+        if (e->cfg.per_lib && e->selected()) lu = e->sel_abandoned;   // counted by the selection's site pass
         else if (e->cfg.per_lib) {
             const uint32_t *w1 = e->h_words.as<uint32_t>() + (int64_t)e->n_rows * e->n_slots;
             for (int64_t sidx = 0; sidx < e->n_slots; ++sidx) {
@@ -1012,7 +980,7 @@ int brc_plan_device(brc_engine *e, const brc_region *regions, int64_t n_regions,
     if (!e || !regions || n_regions <= 0) return BRC_E_INVALID;
     cudaSetDevice(e->cfg.device);
     e->regions.assign(regions, regions + n_regions);
-    e->region_open = false; e->results_valid = false;
+    e->region_open = false; e->last.on_host = false;
     drop_allele_queries(e);
     int rc = build_geometry(e, e->regions.data(), n_regions);
     if (rc != BRC_OK) return rc;
@@ -1034,9 +1002,9 @@ int brc_run_device(brc_engine *e, const brc_read_batch *b, const int32_t *dev_re
     cudaSetDevice(e->cfg.device);
     e->dev_reads = reads_dev(*b);
     if ((size_t)std::max<int64_t>(b->n_reads, 1) * sizeof(ReadDesc) > e->d_desc.cap) return set_error(e, BRC_E_INVALID, "run_device: batch larger than planned n_reads_cap");
-    e->results_valid = false;
+    e->last.on_host = false;
     plan_selection(e);
-    return run_kernels(e, dev_region_of_read, (cudaStream_t)stream, false);
+    return run_kernels(e, dev_region_of_read, (cudaStream_t)stream);
 }
 
 int brc_device_packed_results(brc_engine *e, brc_packed_results *out) {
@@ -1050,10 +1018,13 @@ int brc_device_packed_results(brc_engine *e, brc_packed_results *out) {
 int brc_fetch_device_results(brc_engine *e, void *stream) {
     if (!e || !e->planned) return BRC_E_INVALID;
     cudaSetDevice(e->cfg.device);
-    return fetch_results(e, (cudaStream_t)stream);
+    const int rc = fetch_results(e, (cudaStream_t)stream);
+    return rc == BRC_E_OVERFLOW ? set_error(e, rc, "secondary key pool overflow (re-plan with a larger n_sec_cap)") : rc;
 }
 
 int brc_last_launch_count(const brc_engine *e) { return e ? e->launch_count : 0; }
+
+int brc_last_results_kind(const brc_engine *e) { return e ? e->results_kind() : BRC_RESULTS_NONE; }
 
 int brc_set_site_filter(brc_engine *e, const brc_site_filter *f) {
     if (!e) return BRC_E_INVALID;
@@ -1067,8 +1038,7 @@ int brc_set_site_filter(brc_engine *e, const brc_site_filter *f) {
 
 int brc_get_selected_results(brc_engine *e, brc_selected_results *out) {
     if (!e || !out) return BRC_E_INVALID;
-    if (!e->results_valid) return set_error(e, BRC_E_INVALID, "get_selected_results: no results (call brc_compute)");
-    if (!e->sparse) return set_error(e, BRC_E_INVALID, "get_selected_results: the last run had no site filter (brc_get_packed_results)");
+    if (int rc = check_view(e, "get_selected_results", 1u << BRC_RESULTS_SELECTED)) return rc;
     out->n_regions = (int64_t)e->regions.size(); out->regions = e->regions.data(); out->n_rows = e->n_rows; out->n_slots = e->n_slots;
     out->n_sites = e->n_sel; out->site = e->sel_site(); out->emit = e->sel_emit(); out->words = e->h_words.as<uint32_t>();
     out->n_sec = e->h_n_sec; out->sec = e->h_sec.as<brc_sec_record>();
@@ -1118,7 +1088,7 @@ int brc_set_allele_queries(brc_engine *e, const brc_allele_query *q, int64_t n, 
 
 int brc_get_allele_answers(brc_engine *e, const brc_allele_answer **out, int64_t *n) {
     if (!e || !out || !n) return BRC_E_INVALID;
-    if (!e->results_valid || !e->answers_valid) return set_error(e, BRC_E_INVALID, "get_allele_answers: the last run had no allele queries");
+    if (int rc = check_view(e, "get_allele_answers", 1u << BRC_RESULTS_ANSWERS)) return rc;
     *out = e->h_ans.as<brc_allele_answer>(); *n = e->aq_params.n_q;
     return BRC_OK;
 }
@@ -1163,10 +1133,10 @@ void brc_host_free(void *p) { if (p) { cudaFreeHost(p); cudaGetLastError(); } }
 int64_t brc_last_h2d_bytes(const brc_engine *e) { return e ? e->h2d_bytes_last : 0; }
 
 float brc_last_stage_ms(const brc_engine *e, int stage) {
-    if (!e || stage < 0 || stage > 4 || (stage == 3 && !e->sel_launched)) return 0.0f;
+    if (!e || stage < 0 || stage > 4 || (stage == 3 && e->last.kind != BRC_RESULTS_SELECTED)) return 0.0f;
     if (stage == 4) {   // the allele kernels, between ev[3] and ev[4] (launch_allele_queries)
         float ms = 0.0f;
-        if (!e->aq_launched || cudaEventSynchronize(e->ev[4]) != cudaSuccess || cudaEventElapsedTime(&ms, e->ev[3], e->ev[4]) != cudaSuccess) { cudaGetLastError(); return 0.0f; }
+        if (e->last.kind != BRC_RESULTS_ANSWERS || cudaEventSynchronize(e->ev[4]) != cudaSuccess || cudaEventElapsedTime(&ms, e->ev[3], e->ev[4]) != cudaSuccess) { cudaGetLastError(); return 0.0f; }
         return ms;
     }
     // events were recorded on the launching stream around K0, K1 and the selection; wait for the last one

@@ -152,7 +152,10 @@ struct brc_engine {
     // host results: the PACKED records as they come off the device (pinned) ...
     brc::PinBuf h_words, h_sec, h_misc;
     int64_t h_n_sec = 0;
-    bool results_valid = false;
+    // The last run: the kind of results its launch produces (BRC_RESULTS_*, fixed where its kernels are queued) and whether they
+    // have reached the host.  filter_on and queries_on below are requests for the next run.
+    struct LastRun { int kind = BRC_RESULTS_NONE; bool on_host = false; } last;
+    int results_kind() const { return last.on_host ? last.kind : BRC_RESULTS_NONE; }   // the kind the host holds (brc_last_results_kind)
     // ... and the full-width view brc_get_results / the text emitter read, expanded from them on first use (ensure_wide)
     struct Wide {
         std::vector<uint32_t> ncover, npass, pstats, sec_stats;
@@ -203,17 +206,16 @@ struct brc_engine {
     brc_site_filter filter{};
     std::vector<brc::SelRegion> sel_regions;   // the selection's region table of the current batch
     brc::DevBuf d_sel, d_sel_regions;          // scratch + compact outputs; region table
-    bool sel_launched = false;                 // the last kernel run ended with the selection
-    brc::SelectParams sel_params{};            // ... on these buffers
+    brc::SelectParams sel_params{};            // the last selection ran on these buffers
     brc_site_filter sel_filter{};              // the filter the selection ran with
-    // host results are SPARSE: n_sel shipped sites (ids ascending, emit bytes in h_sel), their words in h_words as
+    // SELECTED host results: n_sel shipped sites (ids ascending, emit bytes in h_sel), their words in h_words as
     // [N_WORDS][rows*n_sel], their pool records in h_sec with slot = row * n_sel + compact index
-    bool sparse = false;
     int64_t n_sel = 0, sel_abandoned = 0;
     brc::PinBuf h_sel;
     const uint32_t *sel_site() const { return h_sel.as<uint32_t>(); }
     const uint8_t *sel_emit() const { return reinterpret_cast<const uint8_t *>(h_sel.as<uint32_t>() + n_sel); }
-    int64_t result_cols() const { return sparse ? n_sel : n_slots; }   // columns of the host word / wide arrays
+    bool selected() const { return last.kind == BRC_RESULTS_SELECTED; }   // the last run is SELECTED: n_sel columns
+    int64_t result_cols() const { return selected() ? n_sel : n_slots; }   // columns of the host word / wide arrays
 
     // allele queries (brc_set_allele_queries, brc_alleles.cu).  With them set, the kernels' records stay on the device and only
     // the answers cross PCIe; there is no dense view.
@@ -221,10 +223,8 @@ struct brc_engine {
     std::vector<brc::AlleleQuery> aq;          // sorted by match slot
     std::vector<uint8_t> aq_bases;             // insertion bases as indices into "=ACGTN"
     brc::DevBuf d_aq;                          // queries, bases, scratch, answers
-    bool aq_launched = false;                  // the last kernel run ended with the allele kernels
-    brc::AlleleParams aq_params{};
-    brc::PinBuf h_ans;
-    bool answers_valid = false;                // the last run's results are the answers in h_ans (no records on the host)
+    brc::AlleleParams aq_params{};             // the last allele kernels ran on these buffers
+    brc::PinBuf h_ans;                         // ANSWERS host results (no records on the host)
 
     int launch_count = 0;
 };
@@ -233,6 +233,9 @@ namespace brc {
 int set_error(brc_engine *e, int status, const std::string &msg);
 int set_cuda_error(brc_engine *e, cudaError_t ce, const char *what);
 const HostRef *find_ref(const brc_engine *e, int32_t tid);
+// The guard of every result view: BRC_OK when the host holds results of a kind in `kinds` (a mask of 1 << BRC_RESULTS_*);
+// otherwise BRC_E_INVALID, with a message naming `who` and the getter that serves what the host holds.
+int check_view(brc_engine *e, const char *who, unsigned kinds);
 int fetch_insertion_reads(brc_engine *e, cudaStream_t s);   // brc_bgzf.cu
 void ensure_wide(brc_engine *e);   // expand the packed host records into e->wide (multi-threaded; no-op when already done)
 }  // namespace brc

@@ -72,7 +72,7 @@ struct View {   // raw result arrays of one engine
     View(const brc_engine *en, int64_t g) : e(en), rg(&en->regions[(size_t)g]), ref(brc::find_ref(en, rg->tid)) {
         const brc_engine::Wide &W = e->wide;            // full-width view of the packed device records (brc::ensure_wide)
         rows = e->n_rows; NS = e->result_cols(); RS = (int64_t)rows * NS; SC = (int64_t)W.sec_next.size();
-        if (e->sparse) { csite = e->sel_site(); cemit = e->sel_emit(); n_sel = e->n_sel; }
+        if (e->selected()) { csite = e->sel_site(); cemit = e->sel_emit(); n_sel = e->n_sel; }
         ncover = W.ncover.data(); npass = W.npass.data(); pstats = W.pstats.data(); sstats = W.sec_stats.data();
         flags = W.flags.data(); pbase = W.pbase.data(); skind = W.sec_kind.data();
         shead = W.sec_head.data(); snext = W.sec_next.data(); slen = W.sec_len.data(); sqpos = W.sec_qpos.data();
@@ -231,7 +231,7 @@ bool format_many_site_list_regions(const brc_engine *e, const char *const *lib_n
         std::string &dst = parts_out[base + (size_t)t];
         int64_t slots = 0;
         for (size_t g = cut[(size_t)t]; g < cut[(size_t)t + 1]; ++g) slots += e->regions[g].n_slots;
-        if (!e->sparse) dst.reserve((size_t)slots * 200);
+        if (!e->selected()) dst.reserve((size_t)slots * 200);
         for (size_t g = cut[(size_t)t]; g < cut[(size_t)t + 1]; ++g) {
             const View V(e, (int64_t)g);
             format_range(V, 0, V.rg->n_slots, lib_names, st, dst, false);
@@ -283,6 +283,9 @@ int64_t serve(brc_engine *e, int64_t k0, int64_t k1, int64_t k2, const char *con
     return n;
 }
 
+// the text is formed from dense or selected records; allele answers have none
+constexpr unsigned kTextKinds = 1u << BRC_RESULTS_DENSE | 1u << BRC_RESULTS_SELECTED;
+
 }  // namespace
 
 extern "C" int brc_set_queue_carry(brc_engine *e, int on) {
@@ -295,8 +298,7 @@ extern "C" int brc_set_queue_carry(brc_engine *e, int on) {
 
 extern "C" int64_t brc_format_text(brc_engine *e, int64_t region_index, const char *const *lib_names, char *buf, int64_t cap) {
     if (!e) return BRC_E_INVALID;
-    if (!e->results_valid) return brc::set_error(e, BRC_E_INVALID, "format_text: no results");
-    if (e->answers_valid) return brc::set_error(e, BRC_E_INVALID, "format_text: allele queries are set, there is no text (brc_get_allele_answers)");
+    if (int rc = brc::check_view(e, "format_text", kTextKinds)) return rc;
     if (e->n_host_reads() == 0 && e->h_n_sec > 0 && !e->dec.pushed) return brc::set_error(e, BRC_E_INVALID, "format_text: needs the pushed reads (push path only)");
     if (region_index >= (int64_t)e->regions.size()) return BRC_E_INVALID;
     return serve(e, region_index < 0 ? -1 : region_index, -1, -1, lib_names, buf, cap);
@@ -307,8 +309,7 @@ extern "C" int64_t brc_format_text(brc_engine *e, int64_t region_index, const ch
 extern "C" int64_t brc_format_window(brc_engine *e, int64_t region_index, int64_t first, int64_t count, const char *const *lib_names,
                                      char *buf, int64_t cap) {
     if (!e || region_index < 0 || region_index >= (int64_t)e->regions.size() || first < 0 || count < 0) return BRC_E_INVALID;
-    if (!e->results_valid) return brc::set_error(e, BRC_E_INVALID, "format_window: no results");
-    if (e->answers_valid) return brc::set_error(e, BRC_E_INVALID, "format_window: allele queries are set, there is no text (brc_get_allele_answers)");
+    if (int rc = brc::check_view(e, "format_window", kTextKinds)) return rc;
     return serve(e, region_index, first, count, lib_names, buf, cap);
 }
 
@@ -316,8 +317,7 @@ extern "C" int64_t brc_format_window(brc_engine *e, int64_t region_index, int64_
 // otherwise the window [first, first+count) of that region (count < 0 = to the region's end).  Returns bytes written.
 extern "C" int64_t brc_write_text(brc_engine *e, int64_t region_index, int64_t first, int64_t count, const char *const *lib_names, int fd) {
     if (!e || region_index >= (int64_t)e->regions.size() || first < 0) return BRC_E_INVALID;
-    if (!e->results_valid) return brc::set_error(e, BRC_E_INVALID, "write_text: no results");
-    if (e->answers_valid) return brc::set_error(e, BRC_E_INVALID, "write_text: allele queries are set, there is no text (brc_get_allele_answers)");
+    if (int rc = brc::check_view(e, "write_text", kTextKinds)) return rc;
     if (region_index < 0) ensure_formatted(e, -1, -1, -1, lib_names);
     else ensure_formatted(e, region_index, first, count < 0 ? (int64_t)0x7fffffff : count, lib_names);
     int64_t total = 0;

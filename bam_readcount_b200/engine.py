@@ -97,6 +97,8 @@ assert ALLELE_ANSWER.itemsize == 64
 
 N_WORDS = 8
 SEC_RECORD_BYTES = 72
+# brc_last_results_kind: which view the host holds of the last run
+RESULTS_NONE, RESULTS_DENSE, RESULTS_SELECTED, RESULTS_ANSWERS = 0, 1, 2, 3
 
 EXPORTS = [
     "brc_abi_version", "brc_create", "brc_destroy", "brc_last_error", "brc_strerror", "brc_set_reference", "brc_set_reference_device", "brc_reset",
@@ -104,7 +106,7 @@ EXPORTS = [
     "brc_get_warning_counts", "brc_format_text", "brc_format_window", "brc_write_text", "brc_set_queue_carry", "brc_plan_device", "brc_run_device", "brc_device_packed_results", "brc_get_packed_results",
     "brc_fetch_device_results", "brc_last_launch_count", "brc_last_h2d_bytes", "brc_host_alloc", "brc_host_free", "brc_last_stage_ms", "brc_selftest_fastmath",
     "brc_get_reference_codes",
-    "brc_set_site_filter", "brc_get_selected_results", "brc_set_allele_queries", "brc_get_allele_answers",
+    "brc_set_site_filter", "brc_get_selected_results", "brc_set_allele_queries", "brc_get_allele_answers", "brc_last_results_kind",
 ]
 
 _lib = None
@@ -166,6 +168,7 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
     lib.brc_get_selected_results.argtypes = [C.c_void_p, C.POINTER(CSelectedResults)]
     lib.brc_set_allele_queries.argtypes = [C.c_void_p, C.POINTER(CAlleleQuery), C.c_int64, C.c_char_p, C.c_int64]
     lib.brc_get_allele_answers.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int64)]
+    lib.brc_last_results_kind.argtypes = [C.c_void_p]
     if path is None:
         _lib = lib
     return lib
@@ -338,8 +341,8 @@ class PackedResults:
 
 
 class SelectedResults:
-    """Host copy of a filtered run's sparse results (brc_get_selected_results): the shipped sites' global slot ids (ascending),
-    their emit bytes (1 = the line passes, 2 = shipped for the deletion queue, 0 = context), packed words
+    """Host copy of the sparse results of a run with a site filter (brc_get_selected_results): the shipped sites' global slot
+    ids (ascending), their emit bytes (1 = the line passes, 2 = shipped for the deletion queue, 0 = context), packed words
     [N_WORDS][rows][n_sites] and secondary records (slot = row * n_sites + index into ``site``)."""
 
     def __init__(self, r: CSelectedResults):
@@ -406,13 +409,11 @@ class Engine:
 
     def reset(self):
         self._check(self.lib.brc_reset(self.h))
-        self.queried = False
         self._pushed = []
         self._keep = []
 
     def begin_region(self, tid: int, beg: int, end: int, site_list_mode: bool = True):
         self._check(self.lib.brc_begin_region(self.h, tid, beg, end, int(site_list_mode)))
-        self.queried = False
 
     @staticmethod
     def c_batch(b: ReadBatch, keep: list) -> CReadBatch:
@@ -470,9 +471,13 @@ class Engine:
         self._check(self.lib.brc_compute(self.h))
         return self._results()
 
+    def results_kind(self) -> int:
+        """Which view the host holds of the last run (brc_last_results_kind): RESULTS_NONE, _DENSE, _SELECTED or _ANSWERS."""
+        return int(self.lib.brc_last_results_kind(self.h))
+
     def _results(self) -> Optional[Results]:
-        """The dense results of the last run; None while a site filter is set."""
-        if getattr(self, "filtered", False) or getattr(self, "queried", False):
+        """The dense results of the last run; None when it produced selected sites (a site filter) or allele answers."""
+        if self.results_kind() != RESULTS_DENSE:
             return None
         r = CResults()
         self._check(self.lib.brc_get_results(self.h, C.byref(r)))
@@ -512,7 +517,6 @@ class Engine:
         arr = (CRegion * len(regions))(*regions)
         self._plan_keep = arr
         self._check(self.lib.brc_plan_device(self.h, arr, len(regions), n_reads_cap, n_sec_cap))
-        self.queried = False
 
     def run_device(self, cbatch: CReadBatch, region_of_read_ptr: Optional[int], stream_ptr: int):
         self._check(self.lib.brc_run_device(self.h, C.byref(cbatch), region_of_read_ptr, stream_ptr))
@@ -537,11 +541,9 @@ class Engine:
         compute() on); while set, compute() returns None (no dense view) and selected() is the sparse result."""
         f = CSiteFilter(int(min_alt_count), 0, float(min_alt_fraction))
         self._check(self.lib.brc_set_site_filter(self.h, C.byref(f)))
-        self.filtered = True
 
     def clear_site_filter(self):
         self._check(self.lib.brc_set_site_filter(self.h, None))
-        self.filtered = False
 
     def selected(self) -> SelectedResults:
         r = CSelectedResults()
@@ -554,9 +556,7 @@ class Engine:
         KIND_INS / KIND_DEL | length << 8; bases_off indexes an insertion's characters in ``bases``.  From the next compute() /
         run_device() on, allele_answers() holds the answers and compute() returns None (no dense view); reset() drops them."""
         arr = (CAlleleQuery * max(1, len(queries)))(*[CAlleleQuery(int(g), int(p), int(k), int(o)) for g, p, k, o in queries])
-        self.queried = False          # a refused call drops the queries
         self._check(self.lib.brc_set_allele_queries(self.h, arr, len(queries), bytes(bases), len(bases)))
-        self.queried = True
 
     def allele_answers(self) -> np.ndarray:
         """The answers of the last run in query order: a structured array of ALLELE_ANSWER records."""

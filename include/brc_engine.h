@@ -397,6 +397,12 @@ BRC_API int brc_host_alloc(size_t bytes, void **out);
 BRC_API void brc_host_free(void *p);
 
 BRC_API int brc_last_launch_count(const brc_engine *e);
+/* which view the host holds of the last run: BRC_RESULTS_DENSE (brc_get_results, brc_get_packed_results), BRC_RESULTS_SELECTED
+ * (brc_get_selected_results: a site filter was set when it was launched), BRC_RESULTS_ANSWERS (brc_get_allele_answers: allele
+ * queries were set), or BRC_RESULTS_NONE (nothing fetched since the last brc_reset, brc_begin_region, brc_plan_device or
+ * brc_run_device; brc_set_allele_queries drops earlier answers) */
+enum { BRC_RESULTS_NONE = 0, BRC_RESULTS_DENSE = 1, BRC_RESULTS_SELECTED = 2, BRC_RESULTS_ANSWERS = 3 };
+BRC_API int brc_last_results_kind(const brc_engine *e);
 /* bytes the last brc_compute() of pushed host reads copied host->device (regular offset arrays and constant columns of
  * fixed-length reads are rebuilt on the device and do not count) */
 BRC_API int64_t brc_last_h2d_bytes(const brc_engine *e);

@@ -167,27 +167,40 @@ def test_synthetic_whole_region_and_filter_off_is_unchanged():
             d = _same(_text(case, flags, False, (mc, mf)), select_lines(want, mc, mf))
             assert not d, (flags, mc, mf, d)
     fresh = cases.run_engine(case, dict(), False, dump=False)
-    from bam_readcount_b200.engine import BrcError, Engine
+    import ctypes as C
+    from bam_readcount_b200.engine import RESULTS_DENSE, RESULTS_NONE, RESULTS_SELECTED, BrcError, CResults, Engine
     name, clen, seq, wb = case["contigs"][0]
     e = Engine(lib_names=case["lib_names"])
     try:
         e.set_reference(0, name, clen, seq, wb)
+        assert e.results_kind() == RESULTS_NONE
 
         def step():
             e.reset()
+            assert e.results_kind() == RESULTS_NONE
             tid, beg, end, sub = cases.region_reads(case, 0, 1, 40000)
             e.begin_region(tid, beg, end, False)
             e.push_reads(sub)
             e.end_region()
+            assert e.results_kind() == RESULTS_NONE
             return e.compute()
         e.set_site_filter(2, 0.05)
-        assert step() is None
+        assert step() is None and e.results_kind() == RESULTS_SELECTED
         with pytest.raises(BrcError):
             e.packed()
+        assert e.results_kind() == RESULTS_SELECTED
         assert e.stage_ms(3) > 0.0
+        filtered_text, n_sites = e.format_text(-1), e.selected().n_sites
+        assert n_sites > 0
+        # the filter is a request for the next run: clearing it leaves the last run's selected view, and still no dense view
         e.clear_site_filter()
+        assert e.results_kind() == RESULTS_SELECTED and e.selected().n_sites == n_sites and e.format_text(-1) == filtered_text
+        with pytest.raises(BrcError):
+            e.packed()
+        assert e.lib.brc_get_results(e.h, C.byref(CResults())) != 0
+        assert e.results_kind() == RESULTS_SELECTED
         res = step()
-        assert res is not None and e.launch_count() == fresh.launches
+        assert res is not None and e.results_kind() == RESULTS_DENSE and e.launch_count() == fresh.launches
         d = _same(e.format_text(-1), fresh.text)
         assert not d, d
         with pytest.raises(BrcError):
@@ -196,6 +209,7 @@ def test_synthetic_whole_region_and_filter_off_is_unchanged():
             e.set_site_filter(0)
         with pytest.raises(BrcError):
             e.set_site_filter(1, 1.5)
+        assert e.results_kind() == RESULTS_DENSE
     finally:
         e.close()
 

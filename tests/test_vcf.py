@@ -135,19 +135,23 @@ def test_answers_device_path():
 
 def test_refusals_and_reset():
     import ctypes as C
-    from bam_readcount_b200.engine import BrcError, CPackedResults, CResults
+    from bam_readcount_b200.engine import RESULTS_ANSWERS, RESULTS_DENSE, RESULTS_NONE, BrcError, CPackedResults, CResults
     case = cases.synthetic_case(L=6000, depth=20, seed=15, regions=[(0, 500, 1500)], n_libs=2)   # prints sites [499, 1500)
     with cases.open_engine(case, dict(per_lib=True)) as e:
         cases.push_regions(e, case, True)
+        assert e.results_kind() == RESULTS_NONE
         with pytest.raises(BrcError):
             e.set_allele_queries([(0, 600, 1, 0)])
+        assert e.results_kind() == RESULTS_NONE
     with cases.open_engine(case) as e:
         cases.push_regions(e, case, True)
         e.compute()
+        assert e.results_kind() == RESULTS_DENSE
         plain_text, plain_launches = e.format_text(-1), e.launch_count()
     with cases.open_engine(case) as e:
         e.set_site_filter(1, 0.0)
         cases.push_regions(e, case, True)
+        assert e.results_kind() == RESULTS_NONE
         with pytest.raises(BrcError):
             e.set_allele_queries([(0, 600, 1, 0)])
         e.clear_site_filter()
@@ -156,18 +160,33 @@ def test_refusals_and_reset():
                            ([(0, 600, KIND_INS | 2 << 8, 1)], b"AC")):
             with pytest.raises(BrcError):
                 e.set_allele_queries(bad, bases)
+            assert e.results_kind() == RESULTS_NONE
         e.set_allele_queries([(0, 499, 1, 0), (0, 1499, KIND_INS | 2 << 8, 0)], b"AC")
         with pytest.raises(BrcError):
             e.set_site_filter(1, 0.0)
+        assert e.results_kind() == RESULTS_NONE
         assert e.lib.brc_compute(e.h) == 0
+        assert e.results_kind() == RESULTS_ANSWERS
         assert e.lib.brc_get_results(e.h, C.byref(CResults())) != 0
         assert e.lib.brc_get_packed_results(e.h, C.byref(CPackedResults())) != 0
         assert e.lib.brc_format_text(e.h, -1, e._names_arr, None, 0) < 0
+        with pytest.raises(BrcError):
+            e.selected()
+        assert e.results_kind() == RESULTS_ANSWERS
         assert len(e.allele_answers()) == 2 and e.stage_ms(4) > 0.0
+        e.set_allele_queries([(0, 499, 1, 0)])                  # queries of a next run drop the answers of the last one
+        assert e.results_kind() == RESULTS_NONE and e.stage_ms(4) == 0.0
+        with pytest.raises(BrcError):
+            e.allele_answers()
+        assert e.lib.brc_compute(e.h) == 0
+        assert e.results_kind() == RESULTS_ANSWERS and len(e.allele_answers()) == 1
         e.reset()
+        assert e.results_kind() == RESULTS_NONE
         assert e.stage_ms(4) == 0.0
         cases.push_regions(e, case, True)
+        assert e.results_kind() == RESULTS_NONE
         e.compute()
+        assert e.results_kind() == RESULTS_DENSE
         assert e.format_text(-1) == plain_text and e.launch_count() == plain_launches
 
 
