@@ -777,7 +777,10 @@ void usage() {
                 "                                        in one process.  Each line of FILE is NAME<TAB>INPUT or NAME<TAB>INPUT<TAB>ERR;\n"
                 "                                        NAME's column gets the values of `--vcf-sample NAME INPUT`, ERR (default: STDERR)\n"
                 "                                        that run's STDERR.  A failed sample gets '.' and does not stop the others (exit\n"
-                "                                        status 1 at the end)\n\n");
+                "                                        status 1 at the end)\n"
+                "  --vcf-complex                         (this host) with --vcf: also count MNP and complex records (an A/C/G/T/N ALT\n"
+                "                                        that no printed entry answers) by each read's bases between the two reference\n"
+                "                                        bases flanking REF, matched exactly against REF and each ALT\n\n");
 }
 
 // samtools region string "name[:beg[-end]]" as bam_parse_region (V:bam_aux.c:65-75) handles it.  Returns 0 when beg and end were
@@ -822,6 +825,9 @@ int parse_region(const BamFile &bam, const std::string &s, int &tid, int &beg, i
 // counted when one of its ALT alleles is an SNV, an insertion after its anchor base or a deletion after it; its site is one
 // line "CHROM L L" of a derived -l site list (L = POS, or POS + 1 for a deletion, whose entry prints on the line after the
 // anchor), and its values are what that run prints on the line: the engine answers them (brc_set_allele_queries).
+// With --vcf-complex a record with an A/C/G/T/N ALT that no entry answers (an MNP, a complex substitution, an indel without
+// its anchor base) is counted by the complex rule instead: its site is the line "CHROM POS POS", and the engine matches each
+// read's bases between the two flanks of REF against REF and its ALTs (brc_set_complex_queries).
 // ------------------------------------------------------------------------------------------
 const char kVcfFormat[] = ":BRC_DP:BRC_AD:BRC_ADF:BRC_ADR:BRC_AF";
 const char kVcfHeader[] =
@@ -837,7 +843,9 @@ struct VcfRecord {
     int32_t line_pos = 0;                 // L: 1-based position of the derived site-list line
     uint32_t ref_kind = 0;                // the REF entry: a base class of "=ACGTN"
     std::vector<int64_t> alt_kind_len;    // per ALT: query kind | length << 8, or -1 when the ALT is not countable
-    std::vector<std::string> alt_bases;   // per ALT: an insertion's bases
+    std::vector<std::string> alt_bases;   // per ALT: an insertion's bases; a complex record: the ALT as upper-case letters
+    bool complex = false;                 // counted by the complex rule (--vcf-complex): alt_kind_len 0 for each A/C/G/T/N ALT
+    std::string ref;                      // a complex record: REF as upper-case letters
     size_t n_queries = 0;                 // counted: the REF and each countable ALT
     size_t word_off = 0;                  // counted: where its answer words start in a sample's VcfAnswers
 };
@@ -896,7 +904,8 @@ bool read_vcf_bytes(const std::string &path, std::string &out, std::string &why)
 
 // Parses the whole VCF, applies the allele rule and resolves the samples that take values: `samples` as named by option `opt`,
 // or none given (the VCF's only sample column).  False with a message (nothing may have been written yet).
-bool parse_vcf(const std::string &path, const std::vector<std::string> &samples, const char *opt, Vcf &v, std::string &why) {
+bool parse_vcf(const std::string &path, const std::vector<std::string> &samples, const char *opt, bool complex_on, Vcf &v,
+               std::string &why) {
     std::string text;
     if (!read_vcf_bytes(path, text, why)) return false;
     v.path = path;
@@ -939,17 +948,27 @@ bool parse_vcf(const std::string &path, const std::vector<std::string> &samples,
         if (!ok || pos < 1 || pos >= INT32_MAX) { why = at + "POS is not a positive integer below 2^31 - 1"; return false; }
         const std::string ref = up(r.cols[3]);
         const bool ref_ok = acgtn(ref, 0);
+        std::vector<std::string> alts;
         for (const std::string &a0 : split(r.cols[4], ',')) {
             const std::string a = up(a0);
+            alts.push_back(a);
             int64_t kl = -1; std::string bases;
             if (ref_ok && ref.size() == 1 && a.size() == 1 && acgtn(a, 0)) kl = kind_of(a[0]);
             else if (ref_ok && ref.size() == 1 && a.size() >= 2 && a[0] == ref[0] && acgtn(a, 1)) { kl = BRC_KIND_INS | (int64_t)(a.size() - 1) << 8; bases = a.substr(1); }
             else if (ref_ok && ref.size() >= 2 && a.size() == 1 && a[0] == ref[0]) kl = BRC_KIND_DEL | (int64_t)(ref.size() - 1) << 8;
             r.counted = r.counted || kl >= 0;
+            r.complex = r.complex || (complex_on && pos >= 2 && ref_ok && kl < 0 && acgtn(a, 0));
             r.alt_kind_len.push_back(kl); r.alt_bases.push_back(bases);
         }
+        if (r.complex) {      // the whole record by the complex rule: the REF and every A/C/G/T/N ALT
+            r.counted = true; r.line_pos = (int32_t)pos; r.ref = ref;
+            for (size_t i = 0; i < alts.size(); ++i) {
+                r.alt_kind_len[i] = acgtn(alts[i], 0) ? 0 : -1;
+                r.alt_bases[i] = r.alt_kind_len[i] >= 0 ? alts[i] : "";
+            }
+        }
         if (r.counted) {
-            r.line_pos = (int32_t)(ref.size() == 1 ? pos : pos + 1); r.ref_kind = kind_of(ref[ref.size() == 1 ? 0 : 1]);
+            if (!r.complex) { r.line_pos = (int32_t)(ref.size() == 1 ? pos : pos + 1); r.ref_kind = kind_of(ref[ref.size() == 1 ? 0 : 1]); }
             r.n_queries = 1 + (size_t)std::count_if(r.alt_kind_len.begin(), r.alt_kind_len.end(), [](int64_t x) { return x >= 0; });
             r.word_off = v.n_words; v.n_words += 1 + 3 * r.n_queries;
         }
@@ -1055,11 +1074,20 @@ void vcf_store(const Vcf &v, size_t ri, const brc_allele_answer *ans, VcfAnswers
     }
     a.answered[ri] = 1;
 }
+// A complex record's answer (brc_get_complex_answers): the reads that count, then per allele (REF first) count, plus, minus.
+void vcf_store_complex(const Vcf &v, size_t ri, uint32_t depth, const brc_complex_count *c, VcfAnswers &a) {
+    const VcfRecord &r = v.rec[ri];
+    uint32_t *w = a.words.data() + r.word_off;
+    w[0] = depth;
+    for (size_t k = 0; k < r.n_queries; ++k) { w[1 + 3 * k] = c[k].count; w[2 + 3 * k] = c[k].plus; w[3 + 3 * k] = c[k].count - c[k].plus; }
+    a.answered[ri] = 1;
+}
 
 struct Options {   // everything on the command line except the inputs: the same for every sample
     int min_mapq = 0, min_bq = 0, max_cnt = 10000000; bool per_lib = false, ic = false; long long max_warn = -1;
     const Vcf *vcf = nullptr;     // --vcf: the parsed file
     bool vcf_samples = false;     // --vcf-samples: a sample only fills its answers; the VCF is written after the last sample
+    bool vcf_complex = false;     // --vcf-complex: MNP and complex records are counted too (DESIGN.md §12)
     std::string fn_pos, fn_fa, dist_arg;
     std::vector<std::string> region_args;
     int shard_rank = 0, shard_count = 1;
@@ -1350,7 +1378,7 @@ int run_sample(const Options &o, Engines &engines, Sample &s, int out_fd, FILE *
     }
 
     std::string chrom;
-    double t_decode = 0, t_compute = 0, t_format = 0, t_ref = 0, t_results = 0, t_reset = 0, ms_alleles = 0;
+    double t_decode = 0, t_compute = 0, t_format = 0, t_ref = 0, t_results = 0, t_reset = 0, ms_alleles = 0, ms_complex = 0;
     // BRC_CLI_DEVICE_DECODE=1: BGZF inflate + BAM framing on the GPU (per-read warning lines need host-decoded reads: counts only)
     std::vector<const char *> rg_ids; std::vector<uint16_t> rg_libs;
     for (const auto &kv : s.rg_lib) { rg_ids.push_back(kv.first.c_str()); rg_libs.push_back(kv.second); }
@@ -1372,14 +1400,23 @@ int run_sample(const Options &o, Engines &engines, Sample &s, int out_fd, FILE *
         int r;
         std::vector<brc_allele_query> q;
         std::string q_bases;
+        std::vector<brc_complex_query> cq; std::vector<brc_complex_allele> ca; std::string c_bases;
         if (vcf) {            // the REF entry and every countable ALT of each record of the batch
             for (int64_t g = 0; g < batch_n; ++g) {
                 const VcfRecord &rec = vcf->rec[(size_t)vcf_rec_of_region[(size_t)(batch_first + g)]];
+                if (rec.complex) {      // the REF and every A/C/G/T/N ALT, matched against the reads' bases between the flanks
+                    cq.push_back({g, rec.line_pos - 1, (int32_t)rec.ref.size(), (int32_t)rec.n_queries, 0});
+                    ca.push_back({(int64_t)c_bases.size(), (int32_t)rec.ref.size(), 0}); c_bases += rec.ref;
+                    for (size_t i = 0; i < rec.alt_kind_len.size(); ++i)
+                        if (rec.alt_kind_len[i] >= 0) { ca.push_back({(int64_t)c_bases.size(), (int32_t)rec.alt_bases[i].size(), 0}); c_bases += rec.alt_bases[i]; }
+                    continue;
+                }
                 q.push_back({g, rec.line_pos - 1, rec.ref_kind, 0});
                 for (size_t i = 0; i < rec.alt_kind_len.size(); ++i)
                     if (rec.alt_kind_len[i] >= 0) { q.push_back({g, rec.line_pos - 1, (uint32_t)rec.alt_kind_len[i], (int64_t)q_bases.size()}); q_bases += rec.alt_bases[i]; }
             }
             if ((r = brc_set_allele_queries(eng, q.data(), (int64_t)q.size(), q_bases.data(), (int64_t)q_bases.size())) != BRC_OK) { std::fprintf(err, "brc_set_allele_queries: %s\n", brc_last_error(eng)); return r; }
+            if (!cq.empty() && (r = brc_set_complex_queries(eng, cq.data(), (int64_t)cq.size(), ca.data(), (int64_t)ca.size(), c_bases.data(), (int64_t)c_bases.size())) != BRC_OK) { std::fprintf(err, "brc_set_complex_queries: %s\n", brc_last_error(eng)); return r; }
         }
         const double c0 = now();
         r = brc_compute(eng);
@@ -1390,13 +1427,17 @@ int run_sample(const Options &o, Engines &engines, Sample &s, int out_fd, FILE *
         if (vcf) {
             const brc_allele_answer *ans = nullptr; int64_t n_ans = 0;
             if ((r = brc_get_allele_answers(eng, &ans, &n_ans)) != BRC_OK || n_ans != (int64_t)q.size()) { std::fprintf(err, "brc_get_allele_answers: %s\n", brc_last_error(eng)); return r ? r : -1; }
+            const uint32_t *c_depth = nullptr; const brc_complex_count *c_cnt = nullptr; int64_t n_c = 0, n_ca = 0;
+            if (!cq.empty() && ((r = brc_get_complex_answers(eng, &c_depth, &c_cnt, &n_c, &n_ca)) != BRC_OK || n_c != (int64_t)cq.size() || n_ca != (int64_t)ca.size())) { std::fprintf(err, "brc_get_complex_answers: %s\n", brc_last_error(eng)); return r ? r : -1; }
             t_results += now() - g0;
-            if (o.timing) ms_alleles += brc_last_stage_ms(eng, 4);
+            if (o.timing) { ms_alleles += brc_last_stage_ms(eng, 4); ms_complex += brc_last_stage_ms(eng, 5); }
             const double f0 = now();
-            for (int64_t g = 0, k = 0; g < batch_n; ++g) {
+            for (int64_t g = 0, k = 0, c = 0, a = 0; g < batch_n; ++g) {
                 const size_t ri = (size_t)vcf_rec_of_region[(size_t)(batch_first + g)];
+                const VcfRecord &rec = vcf->rec[ri];
+                if (rec.complex) { vcf_store_complex(*vcf, ri, c_depth[c++], c_cnt + a, *vcf_ans); a += (int64_t)rec.n_queries; continue; }
                 vcf_store(*vcf, ri, ans + k, *vcf_ans);
-                k += (int64_t)vcf->rec[ri].n_queries;
+                k += (int64_t)rec.n_queries;
             }
             if (vcf_stream && !vcf_write(batch_first + batch_n)) { std::fprintf(err, "writing the VCF: %s\n", std::strerror(errno)); return -1; }
             t_format += now() - f0;
@@ -1537,6 +1578,7 @@ int run_sample(const Options &o, Engines &engines, Sample &s, int out_fd, FILE *
                                t_ref, t_decode, t_compute, t_results, t_format, t_reset, now() - t_loop0, now() - t_main0);
     if (o.timing) std::fprintf(err, "[brc timing] startup (CUDA context, header, index, first window) %.3fs\n", t_loop0 - s.t0);
     if (o.timing && vcf) std::fprintf(err, "[brc timing] allele kernels %.3f ms\n", ms_alleles);
+    if (o.timing && o.vcf_complex) std::fprintf(err, "[brc timing] complex kernel %.3f ms\n", ms_complex);
     return decode_error ? 1 : 0;
 }
 
@@ -1725,7 +1767,8 @@ int main(int argc, char **argv) {
                           {"max-count", 1, 0, 'd'}, {"site-list", 1, 0, 'l'}, {"reference-fasta", 1, 0, 'f'}, {"print-individual-mapq", 1, 0, 'D'},
                           {"per-library", 0, 0, 'p'}, {"max-warnings", 1, 0, 'w'}, {"insertion-centric", 0, 0, 'i'}, {"shard", 1, 0, 1000},
                           {"min-alt-count", 1, 0, 1001}, {"min-alt-fraction", 1, 0, 1002}, {"bam-list", 1, 0, 1003},
-                          {"vcf", 1, 0, 1004}, {"vcf-sample", 1, 0, 1005}, {"vcf-samples", 1, 0, 1006}, {0, 0, 0, 0}};
+                          {"vcf", 1, 0, 1004}, {"vcf-sample", 1, 0, 1005}, {"vcf-samples", 1, 0, 1006},
+                          {"vcf-complex", 0, 0, 1007}, {0, 0, 0, 0}};
     long min_alt_count = 0; double min_alt_fraction = -1.0;       // site filter (brc_set_site_filter); off unless one is given
     bool help = false, version = false;
     for (int c; (c = getopt_long(argc, argv, "hvq:b:d:l:f:D:pw:i", lo, nullptr)) != -1;) {
@@ -1752,6 +1795,7 @@ int main(int argc, char **argv) {
         case 1004: vcf_path = optarg; break;
         case 1005: vcf_sample = optarg; vcf_sample_given = true; break;
         case 1006: vcf_samples = optarg; break;
+        case 1007: o.vcf_complex = true; break;
         default: usage(); return 1;
         }
     }
@@ -1762,6 +1806,7 @@ int main(int argc, char **argv) {
     if (!bam_list.empty() && shard_given) { std::fprintf(stderr, "--bam-list and --shard cannot be combined: shard a cohort by splitting its list\n"); return 1; }
     Vcf vcf;
     if (vcf_sample_given && vcf_path.empty()) { std::fprintf(stderr, "--vcf-sample needs --vcf\n"); return 1; }
+    if (o.vcf_complex && vcf_path.empty()) { std::fprintf(stderr, "--vcf-complex needs --vcf\n"); return 1; }
     if (!vcf_samples.empty()) {
         const char *why = vcf_path.empty() ? "--vcf-samples needs --vcf" : vcf_sample_given ? "--vcf-samples cannot be combined with --vcf-sample"
                         : optind < argc ? "--vcf-samples takes no positional argument: the inputs are in its list" : nullptr;
@@ -1786,7 +1831,7 @@ int main(int argc, char **argv) {
             }
         }
         std::string why;
-        if (!parse_vcf(vcf_path, vcf_names, vcf_samples.empty() ? "--vcf-sample" : "--vcf-samples", vcf, why)) { std::fprintf(stderr, "--vcf: %s\n", why.c_str()); return 1; }
+        if (!parse_vcf(vcf_path, vcf_names, vcf_samples.empty() ? "--vcf-sample" : "--vcf-samples", o.vcf_complex, vcf, why)) { std::fprintf(stderr, "--vcf: %s\n", why.c_str()); return 1; }
         o.vcf = &vcf;
         o.vcf_samples = !vcf_samples.empty();
     }

@@ -349,6 +349,33 @@ struct AlleleParams {
     brc_allele_answer *ans;   // [n_q], zeroed before the record pass
 };
 
+// ---- complex-record queries (brc_complex.cu; brc_set_complex_queries, DESIGN.md §12) ----
+struct ComplexQuery {     // one query as the kernel sees it, resolved against the batch's geometry when it is launched
+    int64_t tile;         // the tile holding `pos`; -1 when no read can span (no slot there, or the right flank past the contig)
+    int32_t pos;          // first span base
+    int32_t ref_len;
+    int64_t allele0;      // its alleles are ComplexParams::alleles[allele0, allele0 + n_alleles), its answers the same counts
+    int32_t n_alleles;
+    int32_t reserved;
+};
+static_assert(sizeof(ComplexQuery) == 32, "ComplexQuery is 32 bytes");
+
+struct ComplexParams {
+    const ReadDesc *desc;
+    const int32_t *tile_lo, *tile_hi;
+    const uint64_t *cigar_off; const uint32_t *cigar;
+    const uint64_t *seq_off; const uint8_t *seq;
+    const uint64_t *qual_off; const uint8_t *qual;
+    int32_t min_bq;
+    const ComplexQuery *q;
+    int64_t n_q;
+    const brc_complex_allele *alleles;   // bases_off indexes `bases`
+    int64_t n_alleles;
+    const uint8_t *bases;                // allele bases as indices into "=ACGTN"
+    uint32_t *depth;                     // [n_q]
+    brc_complex_count *counts;           // [n_alleles]
+};
+
 // launch wrappers (brc_kernels.cu)
 cudaError_t launch_init_tiles(int32_t *tile_lo, int32_t *tile_hi, int64_t n_tiles, int32_t *sec_count,
                               unsigned long long *warn, int n_dispensers, cudaStream_t s);
@@ -366,5 +393,8 @@ cudaError_t launch_select(const SelectParams &p, cudaStream_t s);
 // brc_alleles.cu: record pass, query pass (ALLELE_KERNELS launches; the scratch and answers are zeroed by the caller)
 constexpr int ALLELE_KERNELS = 2;
 cudaError_t launch_alleles(const AlleleParams &p, cudaStream_t s);
+// brc_complex.cu: one warp per complex query (COMPLEX_KERNELS launch)
+constexpr int COMPLEX_KERNELS = 1;
+cudaError_t launch_complex(const ComplexParams &p, cudaStream_t s);
 
 }  // namespace brc

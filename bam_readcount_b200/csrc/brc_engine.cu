@@ -28,8 +28,8 @@ const HostRef *find_ref(const brc_engine *e, int32_t tid) {
     return nullptr;
 }
 int check_view(brc_engine *e, const char *who, unsigned kinds) {
-    static const char *const held[] = {"", "dense results", "a site filter's selected sites", "allele answers"};
-    static const char *const view[] = {"", "brc_get_results", "brc_get_selected_results", "brc_get_allele_answers"};
+    static const char *const held[] = {"", "dense results", "a site filter's selected sites", "query answers"};
+    static const char *const view[] = {"", "brc_get_results", "brc_get_selected_results", "brc_get_allele_answers, brc_get_complex_answers"};
     const int k = e->results_kind();
     if (k == BRC_RESULTS_NONE) return set_error(e, BRC_E_INVALID, std::string(who) + ": no results (call brc_compute)");
     if (kinds >> k & 1u) return BRC_OK;
@@ -138,12 +138,12 @@ void brc_destroy(brc_engine *e) {
     cudaDeviceSynchronize();
     for (auto &r : e->refs) r.dev.release();
     DevBuf *bufs[] = {&e->d_refs, &e->d_desc, &e->d_tiles, &e->d_tile_lo, &e->d_tile_hi, &e->d_regions, &e->d_deep_tiles,
-                      &e->d_words, &e->d_sec, &e->d_sec_count, &e->d_warn, &e->d_sel, &e->d_sel_regions, &e->d_aq};
+                      &e->d_words, &e->d_sec, &e->d_sec_count, &e->d_warn, &e->d_sel, &e->d_sel_regions, &e->d_aq, &e->d_cq};
     for (auto *b : bufs) b->release();
     for (auto &b : e->d_in) b.release();
     { brc_engine::Decoded &D = e->dec; DevBuf *db[] = {&D.comp, &D.btab, &D.u, &D.meta, &D.scratch, &D.count, &D.partial, &D.cigar, &D.seq, &D.qual, &D.ins_idx, &D.ins_out};
       for (auto *b : db) b->release(); for (auto &b : D.arr) b.release(); }
-    PinBuf *pins[] = {&e->h_words, &e->h_sec, &e->h_misc, &e->h_sel, &e->h_ans};
+    PinBuf *pins[] = {&e->h_words, &e->h_sec, &e->h_misc, &e->h_sel, &e->h_ans, &e->h_cans};
     for (auto *b : pins) b->release();
     for (auto &ev : e->ev) if (ev) cudaEventDestroy(ev);
     for (auto &ev : e->pipe_ev) if (ev) cudaEventDestroy(ev);
@@ -177,9 +177,11 @@ int brc_set_reference_device(brc_engine *e, int32_t tid, const char *contig_name
     return install_ref(e, tid, contig_name, chrom_len, win_beg, win_len, nullptr, dev_ascii, (cudaStream_t)stream);
 }
 
-// The queries belong to the batch being dropped, and so do answers they produced.
-static void drop_allele_queries(brc_engine *e) {
-    e->queries_on = false; e->aq.clear(); e->aq_bases.clear();
+// The queries belong to the batch being dropped, and so do answers they produced: the allele queries, the complex-record
+// queries, or (the default) both.
+static void drop_queries(brc_engine *e, bool allele = true, bool complex = true) {
+    if (allele) { e->queries_on = false; e->aq.clear(); e->aq_bases.clear(); }
+    if (complex) { e->complex_on = false; e->cq.clear(); e->ca.clear(); e->cq_bases.clear(); }
     if (e->last.kind == BRC_RESULTS_ANSWERS) e->last = {};
 }
 
@@ -187,7 +189,7 @@ int brc_reset(brc_engine *e) {
     if (!e) return BRC_E_INVALID;
     e->reads.clear(); e->is_borrowed = false; e->regions.clear(); e->region_open = false; e->adm.reset(); e->n_indel_ops = 0;
     e->last = {}; e->planned = false; e->tiles.clear(); e->regions_dev.clear(); e->n_slots = 0; e->n_sel = 0;
-    drop_allele_queries(e);
+    drop_queries(e);
     e->dec.pushed = false; e->dec.ins_reads.clear(); e->dec.ins_off.clear(); e->dec.ins_pool.clear();
     for (auto &w : e->warn_counts) w = 0;
     return BRC_OK;
@@ -234,7 +236,7 @@ int brc_begin_region(brc_engine *e, int32_t tid, int32_t beg, int32_t end, int32
     e->regions.push_back(r);
     e->region_open = true; e->adm.reset(); e->open_max_end = r.first_pos;
     e->last.on_host = false; e->planned = false;
-    drop_allele_queries(e);
+    drop_queries(e);
     return BRC_OK;
 }
 
@@ -532,6 +534,12 @@ static int launch_selection(brc_engine *e, cudaStream_t s) {
 // ---------------------------------------------------------------------------------------------
 // The allele kernels after the pileup kernels on stream s (ev[3], ev[4] around them).
 static int launch_allele_queries(brc_engine *e, cudaStream_t s) {
+    if (!e->queries_on) {             // complex-record queries only
+        e->aq_params = AlleleParams{};
+        CU(cudaEventRecord(e->ev[3], s), "event");
+        CU(cudaEventRecord(e->ev[4], s), "event");
+        return BRC_OK;
+    }
     const int64_t NS = e->n_slots, nq = (int64_t)e->aq.size(), nb = (int64_t)e->aq_bases.size();
     size_t off = 0;
     auto take = [&](size_t bytes) { const size_t o = off; off = (off + bytes + 15) & ~(size_t)15; return o; };
@@ -557,6 +565,48 @@ static int launch_allele_queries(brc_engine *e, cudaStream_t s) {
     return BRC_OK;
 }
 
+// The complex-record kernel after the allele kernels on stream s (ev[6], ev[5] around it: its uploads are not timed).  Each query is resolved against the batch's
+// geometry here: the tile holding its first span base, or none when no read can span it.
+static int launch_complex_queries(brc_engine *e, cudaStream_t s) {
+    e->cq_params = ComplexParams{};
+    if (!e->complex_on) return BRC_OK;
+    const int64_t nq = (int64_t)e->cq.size(), na = (int64_t)e->ca.size(), nb = (int64_t)e->cq_bases.size();
+    std::vector<ComplexQuery> q((size_t)nq);
+    for (int64_t i = 0, a0 = 0; i < nq; ++i) {
+        const brc_complex_query &x = e->cq[(size_t)i];
+        const brc_region &r = e->regions[(size_t)x.region];
+        const HostRef *ref = find_ref(e, r.tid);
+        const int64_t o = (int64_t)x.pos - r.first_pos;
+        ComplexQuery &c = q[(size_t)i];
+        c.pos = x.pos; c.ref_len = x.ref_len; c.allele0 = a0; c.n_alleles = x.n_alleles; c.reserved = 0;
+        c.tile = o < r.n_slots && ref && (int64_t)x.pos + x.ref_len < ref->chrom_len ? e->regions_dev[(size_t)x.region].tile_base + o / TILE : -1;
+        a0 += x.n_alleles;
+    }
+    size_t off = 0;
+    auto take = [&](size_t bytes) { const size_t o = off; off = (off + bytes + 15) & ~(size_t)15; return o; };
+    const size_t o_q = take((size_t)nq * sizeof(ComplexQuery)), o_a = take((size_t)na * sizeof(brc_complex_allele)), o_b = take((size_t)nb);
+    const size_t o_d = take((size_t)nq * 4), o_c = take((size_t)na * sizeof(brc_complex_count));
+    CU(e->d_cq.reserve(std::max<size_t>(off, 16)), "cudaMalloc(complex queries)");
+    char *b = e->d_cq.as<char>();
+    // pageable sources: staged before the calls return
+    if (nq) CU(cudaMemcpyAsync(b + o_q, q.data(), (size_t)nq * sizeof(ComplexQuery), cudaMemcpyHostToDevice, s), "H2D complex queries");
+    if (na) CU(cudaMemcpyAsync(b + o_a, e->ca.data(), (size_t)na * sizeof(brc_complex_allele), cudaMemcpyHostToDevice, s), "H2D complex alleles");
+    if (nb) CU(cudaMemcpyAsync(b + o_b, e->cq_bases.data(), (size_t)nb, cudaMemcpyHostToDevice, s), "H2D complex allele bases");
+    ComplexParams P{};
+    P.desc = e->d_desc.as<ReadDesc>(); P.tile_lo = e->d_tile_lo.as<int32_t>(); P.tile_hi = e->d_tile_hi.as<int32_t>();
+    P.cigar_off = e->dev_reads.cigar_off; P.cigar = e->dev_reads.cigar; P.seq_off = e->dev_reads.seq_off; P.seq = e->dev_reads.seq;
+    P.qual_off = e->dev_reads.qual_off; P.qual = e->dev_reads.qual; P.min_bq = e->cfg.min_bq;
+    P.q = reinterpret_cast<const ComplexQuery *>(b + o_q); P.n_q = nq;
+    P.alleles = reinterpret_cast<const brc_complex_allele *>(b + o_a); P.n_alleles = na; P.bases = reinterpret_cast<const uint8_t *>(b + o_b);
+    P.depth = reinterpret_cast<uint32_t *>(b + o_d); P.counts = reinterpret_cast<brc_complex_count *>(b + o_c);
+    CU(cudaEventRecord(e->ev[6], s), "event");
+    CU(launch_complex(P, s), "launch complex queries");
+    if (nq) e->launch_count += COMPLEX_KERNELS;
+    CU(cudaEventRecord(e->ev[5], s), "event");
+    e->cq_params = P;
+    return BRC_OK;
+}
+
 static void make_params(brc_engine *e, const int32_t *d_region_of_read, PrecomputeParams &P0, PileupParams &P1) {
     P0 = PrecomputeParams{};
     P0.reads = e->dev_reads; P0.regions = e->d_regions.as<RegionDev>(); P0.n_regions = (int64_t)e->regions_dev.size();
@@ -574,13 +624,14 @@ static void make_params(brc_engine *e, const int32_t *d_region_of_read, Precompu
 }
 
 // The stream tail after the pileup kernels, shared by run_kernels and compute_pipelined: ev[2], then the selection (with a site
-// filter) or the allele kernels (with queries).  Fixes the kind of results the run produces.
+// filter) or the allele kernels and the complex-record kernel (with queries).  Fixes the kind of results the run produces.
 static int launch_tail(brc_engine *e, cudaStream_t s) {
-    e->last = {e->filter_on ? BRC_RESULTS_SELECTED : e->queries_on ? BRC_RESULTS_ANSWERS : BRC_RESULTS_DENSE, false};
+    e->last = {e->filter_on ? BRC_RESULTS_SELECTED : e->answers_on() ? BRC_RESULTS_ANSWERS : BRC_RESULTS_DENSE, false};
     CU(cudaEventRecord(e->ev[2], s), "event");
     if (e->filter_on) return launch_selection(e, s);
-    if (e->queries_on) return launch_allele_queries(e, s);
-    return BRC_OK;
+    if (!e->answers_on()) return BRC_OK;
+    const int rc = launch_allele_queries(e, s);
+    return rc != BRC_OK ? rc : launch_complex_queries(e, s);
 }
 
 // K(init) + K0 + K1 and the tail on stream s.  Launches only: fetch_results brings the results to the host.
@@ -606,6 +657,7 @@ static int fetch_results(brc_engine *e, cudaStream_t s, int64_t sec_done = -1) {
     const int kind = e->last.kind;
     const SelectParams &S = e->sel_params;
     const AlleleParams &A = e->aq_params;
+    const ComplexParams &X = e->cq_params;
     CU(e->h_misc.reserve(64), "pin");
     uint64_t *hm = e->h_misc.as<uint64_t>();   // [0] pool counter, [1] selected sites, [2] their records, [3] abandoned sites, [4..5] warnings
     hm[0] = hm[1] = hm[2] = hm[3] = 0;
@@ -618,6 +670,12 @@ static int fetch_results(brc_engine *e, cudaStream_t s, int64_t sec_done = -1) {
         CU(e->h_ans.reserve((size_t)std::max<int64_t>(A.n_q, 1) * sizeof(brc_allele_answer)), "pin");
         CU(cudaMemcpyAsync(hm + 4, e->d_warn.p, 16, cudaMemcpyDeviceToHost, s), "D2H warn");
         if (A.n_q) CU(cudaMemcpyAsync(e->h_ans.p, A.ans, (size_t)A.n_q * sizeof(brc_allele_answer), cudaMemcpyDeviceToHost, s), "D2H allele answers");
+        if (X.n_q) {
+            e->cans_counts = ((size_t)X.n_q * 4 + 15) & ~(size_t)15;
+            CU(e->h_cans.reserve(e->cans_counts + (size_t)X.n_alleles * sizeof(brc_complex_count)), "pin");
+            CU(cudaMemcpyAsync(e->h_cans.p, X.depth, (size_t)X.n_q * 4, cudaMemcpyDeviceToHost, s), "D2H complex depths");
+            CU(cudaMemcpyAsync(e->h_cans.as<char>() + e->cans_counts, X.counts, (size_t)X.n_alleles * sizeof(brc_complex_count), cudaMemcpyDeviceToHost, s), "D2H complex counts");
+        }
     }
     CU(cudaStreamSynchronize(s), "sync");
     const int64_t cnt = *e->h_misc.as<int32_t>();
@@ -789,7 +847,7 @@ static int compute_pipelined(brc_engine *e) {
     e->dev_reads = reads_dev(d_in_batch(e, n));
     // host result buffers (with a site filter only the compacted selection comes back, and with allele queries only their
     // answers, after the kernels: fetch_results)
-    const bool sel = e->filter_on || e->queries_on;
+    const bool sel = e->filter_on || e->answers_on();
     const int64_t rs1 = std::max<int64_t>(rs, 1);
     if (!sel) CU(e->h_words.reserve(rs1 * 4 * N_WORDS), "pin");
     CU(e->h_sec.reserve((size_t)e->sec_cap * sizeof(SecRec)), "pin");          // pool records leave while the kernels run
@@ -981,7 +1039,7 @@ int brc_plan_device(brc_engine *e, const brc_region *regions, int64_t n_regions,
     cudaSetDevice(e->cfg.device);
     e->regions.assign(regions, regions + n_regions);
     e->region_open = false; e->last.on_host = false;
-    drop_allele_queries(e);
+    drop_queries(e);
     int rc = build_geometry(e, e->regions.data(), n_regions);
     if (rc != BRC_OK) return rc;
     rc = alloc_outputs(e, n_reads_cap);
@@ -1029,7 +1087,7 @@ int brc_last_results_kind(const brc_engine *e) { return e ? e->results_kind() : 
 int brc_set_site_filter(brc_engine *e, const brc_site_filter *f) {
     if (!e) return BRC_E_INVALID;
     if (!f) { e->filter_on = false; e->filter = brc_site_filter{}; return BRC_OK; }
-    if (e->queries_on) return set_error(e, BRC_E_INVALID, "set_site_filter: allele queries are set (brc_reset drops them)");
+    if (e->answers_on()) return set_error(e, BRC_E_INVALID, "set_site_filter: allele or complex queries are set (brc_reset drops them)");
     if (f->min_alt_count < 1 || f->reserved != 0 || !(f->min_alt_fraction >= 0.0 && f->min_alt_fraction <= 1.0))
         return set_error(e, BRC_E_INVALID, "set_site_filter: min_alt_count must be >= 1 and min_alt_fraction in [0, 1]");
     e->filter = *f; e->filter_on = true;
@@ -1047,7 +1105,7 @@ int brc_get_selected_results(brc_engine *e, brc_selected_results *out) {
 
 int brc_set_allele_queries(brc_engine *e, const brc_allele_query *q, int64_t n, const char *bases, int64_t n_bases) {
     if (!e) return BRC_E_INVALID;
-    drop_allele_queries(e);
+    drop_queries(e, true, false);
     if (n < 0 || (n > 0 && !q) || n_bases < 0 || (n_bases > 0 && !bases)) return set_error(e, BRC_E_INVALID, "set_allele_queries: bad arguments");
     if (e->region_open) return set_error(e, BRC_E_INVALID, "set_allele_queries: a region is still open");
     if (e->n_rows != 1) return set_error(e, BRC_E_INVALID, "set_allele_queries: per-library rows are not supported");
@@ -1093,6 +1151,53 @@ int brc_get_allele_answers(brc_engine *e, const brc_allele_answer **out, int64_t
     return BRC_OK;
 }
 
+int brc_set_complex_queries(brc_engine *e, const brc_complex_query *q, int64_t n, const brc_complex_allele *a, int64_t n_alleles,
+                            const char *bases, int64_t n_bases) {
+    if (!e) return BRC_E_INVALID;
+    drop_queries(e, false, true);
+    if (n < 0 || (n > 0 && !q) || n_alleles < 0 || (n_alleles > 0 && !a) || n_bases < 0 || (n_bases > 0 && !bases))
+        return set_error(e, BRC_E_INVALID, "set_complex_queries: bad arguments");
+    if (e->region_open) return set_error(e, BRC_E_INVALID, "set_complex_queries: a region is still open");
+    if (e->n_rows != 1) return set_error(e, BRC_E_INVALID, "set_complex_queries: per-library rows are not supported");
+    if (e->filter_on) return set_error(e, BRC_E_INVALID, "set_complex_queries: a site filter is set");
+    int64_t total = 0;
+    for (int64_t i = 0; i < n; ++i) {
+        const brc_complex_query &x = q[i];
+        if (x.region < 0 || x.region >= (int64_t)e->regions.size()) return set_error(e, BRC_E_INVALID, "set_complex_queries: region index out of range");
+        const brc_region &r = e->regions[(size_t)x.region];
+        if (x.pos < 1 || x.pos < r.beg || x.pos >= r.end) return set_error(e, BRC_E_INVALID, "set_complex_queries: position outside the region's printed sites or below 1");
+        if (x.ref_len < 1 || x.n_alleles < 1) return set_error(e, BRC_E_INVALID, "set_complex_queries: ref_len and n_alleles must be >= 1");
+        total += x.n_alleles;
+    }
+    if (total != n_alleles) return set_error(e, BRC_E_INVALID, "set_complex_queries: the queries' n_alleles do not add up to n_alleles");
+    std::vector<brc_complex_allele> ca(a, a + n_alleles);
+    std::vector<uint8_t> codes;
+    for (brc_complex_allele &x : ca) {
+        if (x.len < 1 || x.bases_off < 0 || x.bases_off > n_bases || (int64_t)x.len > n_bases - x.bases_off)
+            return set_error(e, BRC_E_INVALID, "set_complex_queries: allele bases outside the buffer");
+        const int64_t at = (int64_t)codes.size();
+        for (int32_t k = 0; k < x.len; ++k) {
+            const char *p = std::strchr("ACGTN", bases[x.bases_off + k]);
+            if (!p || !*p) return set_error(e, BRC_E_INVALID, "set_complex_queries: allele bases must be A, C, G, T or N");
+            codes.push_back((uint8_t)(1 + (p - "ACGTN")));      // index into "=ACGTN"
+        }
+        x.bases_off = at; x.reserved = 0;
+    }
+    e->cq.assign(q, q + n); e->ca.swap(ca); e->cq_bases.swap(codes);
+    e->complex_on = true;
+    return BRC_OK;
+}
+
+int brc_get_complex_answers(brc_engine *e, const uint32_t **depth, const brc_complex_count **counts, int64_t *n, int64_t *n_alleles) {
+    if (!e || !depth || !counts || !n || !n_alleles) return BRC_E_INVALID;
+    if (int rc = check_view(e, "get_complex_answers", 1u << BRC_RESULTS_ANSWERS)) return rc;
+    const ComplexParams &X = e->cq_params;
+    *depth = e->h_cans.as<uint32_t>();
+    *counts = reinterpret_cast<const brc_complex_count *>(e->h_cans.as<char>() + e->cans_counts);
+    *n = X.n_q; *n_alleles = X.n_alleles;
+    return BRC_OK;
+}
+
 int64_t brc_selftest_fastmath(brc_engine *e, int32_t max_b) {
     if (!e || max_b < 1) return BRC_E_INVALID;
     cudaSetDevice(e->cfg.device);
@@ -1133,7 +1238,12 @@ void brc_host_free(void *p) { if (p) { cudaFreeHost(p); cudaGetLastError(); } }
 int64_t brc_last_h2d_bytes(const brc_engine *e) { return e ? e->h2d_bytes_last : 0; }
 
 float brc_last_stage_ms(const brc_engine *e, int stage) {
-    if (!e || stage < 0 || stage > 4 || (stage == 3 && e->last.kind != BRC_RESULTS_SELECTED)) return 0.0f;
+    if (!e || stage < 0 || stage > 5 || (stage == 3 && e->last.kind != BRC_RESULTS_SELECTED)) return 0.0f;
+    if (stage == 5) {   // the complex-record kernel, between ev[6] and ev[5] (launch_complex_queries)
+        float ms = 0.0f;
+        if (e->last.kind != BRC_RESULTS_ANSWERS || !e->cq_params.depth || cudaEventSynchronize(e->ev[5]) != cudaSuccess || cudaEventElapsedTime(&ms, e->ev[6], e->ev[5]) != cudaSuccess) { cudaGetLastError(); return 0.0f; }
+        return ms;
+    }
     if (stage == 4) {   // the allele kernels, between ev[3] and ev[4] (launch_allele_queries)
         float ms = 0.0f;
         if (e->last.kind != BRC_RESULTS_ANSWERS || cudaEventSynchronize(e->ev[4]) != cudaSuccess || cudaEventElapsedTime(&ms, e->ev[3], e->ev[4]) != cudaSuccess) { cudaGetLastError(); return 0.0f; }

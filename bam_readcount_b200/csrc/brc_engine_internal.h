@@ -114,7 +114,7 @@ struct brc_engine {
     std::vector<cudaEvent_t> pipe_ev;
     int64_t h2d_bytes_last = 0;      // bytes the last push path actually sent over PCIe (after the elision below)
     int skip_h2d = 0;                // borrowed batch: bit0 seq_off, bit1 qual_off arithmetic; bit2 l_qseq, bit3 sm constant -> rebuilt on the device
-    cudaEvent_t ev[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
+    cudaEvent_t ev[7] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};   // see brc_last_stage_ms
     std::string err;
 
     std::vector<brc::HostRef> refs;
@@ -225,6 +225,18 @@ struct brc_engine {
     brc::DevBuf d_aq;                          // queries, bases, scratch, answers
     brc::AlleleParams aq_params{};             // the last allele kernels ran on these buffers
     brc::PinBuf h_ans;                         // ANSWERS host results (no records on the host)
+
+    // complex-record queries (brc_set_complex_queries, brc_complex.cu): the same lifecycle and results kind as the allele
+    // queries; both may be set for one batch, and the complex kernel runs after the allele kernels.
+    bool complex_on = false;
+    std::vector<brc_complex_query> cq;         // as the caller gave them
+    std::vector<brc_complex_allele> ca;        // bases_off rebased into cq_bases
+    std::vector<uint8_t> cq_bases;             // allele bases as indices into "=ACGTN"
+    brc::DevBuf d_cq;                          // queries, alleles, bases, answers
+    brc::ComplexParams cq_params{};            // the last complex kernel ran on these buffers (n_q = 0: it did not run)
+    brc::PinBuf h_cans;                        // its answers on the host: depth[n_q], then counts[n_alleles] at cans_counts
+    size_t cans_counts = 0;
+    bool answers_on() const { return queries_on || complex_on; }   // the next run produces BRC_RESULTS_ANSWERS
 
     int launch_count = 0;
 };

@@ -9,7 +9,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
-from typing import List, Optional, Sequence
+from typing import List, Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -95,6 +95,19 @@ class CAlleleQuery(C.Structure):
 ALLELE_ANSWER = np.dtype([("stats", np.uint32, (13,)), ("depth", np.uint32), ("line", np.uint32), ("reserved", np.uint32)])
 assert ALLELE_ANSWER.itemsize == 64
 
+class CComplexQuery(C.Structure):
+    """brc_complex_query (include/brc_engine.h "complex-record queries")."""
+    _fields_ = [("region", C.c_int64), ("pos", C.c_int32), ("ref_len", C.c_int32), ("n_alleles", C.c_int32), ("reserved", C.c_int32)]
+
+
+class CComplexAllele(C.Structure):
+    """brc_complex_allele: `len` A/C/G/T/N characters at bases[bases_off]."""
+    _fields_ = [("bases_off", C.c_int64), ("len", C.c_int32), ("reserved", C.c_int32)]
+
+
+# brc_complex_count: the reads whose allele string equals one allele, and how many of them are on the forward strand
+COMPLEX_COUNT = np.dtype([("count", np.uint32), ("plus", np.uint32)])
+
 N_WORDS = 8
 SEC_RECORD_BYTES = 72
 # brc_last_results_kind: which view the host holds of the last run
@@ -107,6 +120,7 @@ EXPORTS = [
     "brc_fetch_device_results", "brc_last_launch_count", "brc_last_h2d_bytes", "brc_host_alloc", "brc_host_free", "brc_last_stage_ms", "brc_selftest_fastmath",
     "brc_get_reference_codes",
     "brc_set_site_filter", "brc_get_selected_results", "brc_set_allele_queries", "brc_get_allele_answers", "brc_last_results_kind",
+    "brc_set_complex_queries", "brc_get_complex_answers",
 ]
 
 _lib = None
@@ -169,6 +183,10 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
     lib.brc_set_allele_queries.argtypes = [C.c_void_p, C.POINTER(CAlleleQuery), C.c_int64, C.c_char_p, C.c_int64]
     lib.brc_get_allele_answers.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int64)]
     lib.brc_last_results_kind.argtypes = [C.c_void_p]
+    lib.brc_set_complex_queries.argtypes = [C.c_void_p, C.POINTER(CComplexQuery), C.c_int64, C.POINTER(CComplexAllele), C.c_int64,
+                                            C.c_char_p, C.c_int64]
+    lib.brc_get_complex_answers.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_int64),
+                                            C.POINTER(C.c_int64)]
     if path is None:
         _lib = lib
     return lib
@@ -563,6 +581,29 @@ class Engine:
         p, n = C.c_void_p(), C.c_int64()
         self._check(self.lib.brc_get_allele_answers(self.h, C.byref(p), C.byref(n)))
         return _np_view(p.value, n.value * ALLELE_ANSWER.itemsize, np.uint8).view(ALLELE_ANSWER).copy()
+
+    # ---- complex-record queries (include/brc_engine.h brc_set_complex_queries) ----------------------------------------------
+    def set_complex_queries(self, queries: Sequence[tuple]):
+        """Complex-record queries of the current batch, each ``(region, pos, ref_len, alleles)``: pos the 0-based first span base,
+        alleles a sequence of A/C/G/T/N strings (the REF and the ALTs to count).  Same lifecycle as set_allele_queries, with
+        which it may be combined; complex_answers() holds the answers."""
+        qs, al, buf = [], [], b""
+        for g, p, n, alleles in queries:
+            qs.append(CComplexQuery(int(g), int(p), int(n), len(alleles), 0))
+            for a in alleles:
+                a = a.encode() if isinstance(a, str) else bytes(a)
+                al.append(CComplexAllele(len(buf), len(a), 0))
+                buf += a
+        qa = (CComplexQuery * max(1, len(qs)))(*qs)
+        aa = (CComplexAllele * max(1, len(al)))(*al)
+        self._check(self.lib.brc_set_complex_queries(self.h, qa, len(qs), aa, len(al), buf, len(buf)))
+
+    def complex_answers(self) -> Tuple[np.ndarray, np.ndarray]:
+        """The answers of the last run: (depth per query, COMPLEX_COUNT per allele in query order)."""
+        d, c, n, na = C.c_void_p(), C.c_void_p(), C.c_int64(), C.c_int64()
+        self._check(self.lib.brc_get_complex_answers(self.h, C.byref(d), C.byref(c), C.byref(n), C.byref(na)))
+        return (_np_view(d.value, n.value, np.uint32).copy(),
+                _np_view(c.value, na.value * COMPLEX_COUNT.itemsize, np.uint8).view(COMPLEX_COUNT).copy())
 
     def stage_ms(self, stage: int) -> float:
         return float(self.lib.brc_last_stage_ms(self.h, stage))

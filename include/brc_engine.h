@@ -369,6 +369,30 @@ BRC_API int brc_set_allele_queries(brc_engine *e, const brc_allele_query *q, int
 /* the answers of the last run, in query order (engine-owned, valid until the next run or brc_reset) */
 BRC_API int brc_get_allele_answers(brc_engine *e, const brc_allele_answer **out, int64_t *n);
 
+/* ---- complex-record queries (DESIGN.md §12 "MNP and complex records") ----------------------
+ * A query counts the reads of one record whose span is reference positions [pos, pos + ref_len) by their bases between the
+ * two flanks pos - 1 and pos + ref_len:
+ *   region     as brc_allele_query;  pos  0-based first span base, a site of that region (beg <= pos < end), >= 1
+ *   ref_len    >= 1;  n_alleles  >= 1: its alleles are the next n_alleles entries of `a`, in query order
+ * An allele is >= 1 upper-case A/C/G/T/N characters at bases[bases_off .. bases_off + len).
+ * A read counts when it is not dropped by -q or the flag filter, both flanks are aligned to read bases by M, = or X ops, and
+ * every read base strictly between them (inserted bases included) has quality >= -b.  Its string S is those bases, IUPAC
+ * codes read as N.  Answers: depth[i] = the reads that count for query i; counts[j] = those whose S equals allele j exactly,
+ * and how many of them are on the forward strand.  A right flank past the contig's end gives 0.  -i has no effect.
+ * Same lifecycle as the allele queries, and both may be set for one batch (each is answered as it would be alone); the
+ * results are BRC_RESULTS_ANSWERS.  BRC_E_INVALID: per_lib, a site filter set, a region or position out of range, pos < 1,
+ * ref_len < 1, n_alleles < 1, allele counts that do not add up to n_alleles, allele bases that are not A/C/G/T/N or lie
+ * outside `bases`. */
+typedef struct { int64_t region; int32_t pos; int32_t ref_len; int32_t n_alleles; int32_t reserved; } brc_complex_query;
+typedef struct { int64_t bases_off; int32_t len; int32_t reserved; } brc_complex_allele;
+BRC_API int brc_set_complex_queries(brc_engine *e, const brc_complex_query *q, int64_t n, const brc_complex_allele *a,
+                                    int64_t n_alleles, const char *bases, int64_t n_bases);
+typedef struct { uint32_t count, plus; } brc_complex_count;        /* minus = count - plus */
+/* the answers of the last run: depth[n] in query order, counts[n_alleles] in allele order (engine-owned, valid until the next
+ * run or brc_reset) */
+BRC_API int brc_get_complex_answers(brc_engine *e, const uint32_t **depth, const brc_complex_count **counts, int64_t *n,
+                                    int64_t *n_alleles);
+
 /* ---- device-resident path (bench "value": inputs already in HBM) -------------------------
  * brc_plan_device: fix the region geometry (host array of n_regions regions with read_lo/hi,
  * slot_base, first_pos, n_slots filled) and size the outputs.  brc_run_device: launch the
@@ -398,9 +422,10 @@ BRC_API void brc_host_free(void *p);
 
 BRC_API int brc_last_launch_count(const brc_engine *e);
 /* which view the host holds of the last run: BRC_RESULTS_DENSE (brc_get_results, brc_get_packed_results), BRC_RESULTS_SELECTED
- * (brc_get_selected_results: a site filter was set when it was launched), BRC_RESULTS_ANSWERS (brc_get_allele_answers: allele
- * queries were set), or BRC_RESULTS_NONE (nothing fetched since the last brc_reset, brc_begin_region, brc_plan_device or
- * brc_run_device; brc_set_allele_queries drops earlier answers) */
+ * (brc_get_selected_results: a site filter was set when it was launched), BRC_RESULTS_ANSWERS (brc_get_allele_answers and
+ * brc_get_complex_answers: allele or complex queries were set), or BRC_RESULTS_NONE (nothing fetched since the last brc_reset,
+ * brc_begin_region, brc_plan_device or brc_run_device; brc_set_allele_queries and brc_set_complex_queries drop earlier
+ * answers) */
 enum { BRC_RESULTS_NONE = 0, BRC_RESULTS_DENSE = 1, BRC_RESULTS_SELECTED = 2, BRC_RESULTS_ANSWERS = 3 };
 BRC_API int brc_last_results_kind(const brc_engine *e);
 /* bytes the last brc_compute() of pushed host reads copied host->device (regular offset arrays and constant columns of
@@ -408,7 +433,8 @@ BRC_API int brc_last_results_kind(const brc_engine *e);
 BRC_API int64_t brc_last_h2d_bytes(const brc_engine *e);
 /* elapsed GPU milliseconds of the named stage of the last run, measured with CUDA events on the
  * launching stream: 0 = per-read precompute kernel, 1 = pileup kernel, 2 = whole device step (without the selection),
- * 3 = site selection + compaction (0 when no filter was set), 4 = allele queries (0 when none were set) */
+ * 3 = site selection + compaction (0 when no filter was set), 4 = allele queries (0 when none were set), 5 = the complex-record
+ * kernel, without the upload of its queries (0 when none were set) */
 BRC_API float brc_last_stage_ms(const brc_engine *e, int stage);
 
 #ifdef __cplusplus
