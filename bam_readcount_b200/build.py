@@ -10,7 +10,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libbrc_engine.so")
 SOURCES = ["brc_kernels.cu", "brc_engine.cu", "brc_bgzf.cu", "brc_select.cu", "brc_alleles.cu", "brc_complex.cu", "brc_format.cpp"]
-HEADERS = ["brc_device.cuh", "brc_engine_internal.h", "brc_fmt_num.h", "brc_aux.cuh", "brc_bgzf.cuh", "brc_scan.cuh", "brc_complex.cuh", os.path.join("..", "..", "include", "brc_engine.h")]
+HEADERS = ["brc_device.cuh", "brc_engine_internal.h", "brc_reads.h", "brc_fmt_num.h", "brc_aux.cuh", "brc_bgzf.cuh", "brc_scan.cuh", "brc_complex.cuh", os.path.join("..", "..", "include", "brc_engine.h")]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
@@ -87,16 +87,19 @@ def build_synth(force: bool = False) -> str:
 
 
 CLI = os.path.join(HERE, "brc-readcount")
+CLI_SOURCES = ["brc_cli.cpp", "brc_cli_input.cpp", "brc_cli_vcf.cpp"]
+CLI_HEADERS = ["brc_cli_input.h", "brc_cli_vcf.h", "brc_cli_warn.h", "brc_reads.h", "brc_aux.cuh", os.path.join("..", "..", "include", "brc_engine.h")]
 
 
 def build_cli(force: bool = False) -> str:
     """The C++ host binary (same CLI / STDOUT as bam-readcount) on top of libbrc_engine.so."""
-    src = os.path.join(CSRC, "brc_cli.cpp")
+    srcs = [os.path.join(CSRC, f) for f in CLI_SOURCES]
     hts_a = os.path.join(HERE, "third_party", "htslib", "libhts.a")
-    newest = max([os.path.getmtime(src), os.path.getmtime(os.path.join(CSRC, "brc_aux.cuh")), os.path.getmtime(LIB)] + ([os.path.getmtime(hts_a)] if os.path.exists(hts_a) else []))
+    deps = srcs + [os.path.join(CSRC, f) for f in CLI_HEADERS] + [LIB] + ([hts_a] if os.path.exists(hts_a) else [])
+    newest = max(os.path.getmtime(f) for f in deps)
     if not force and os.path.exists(CLI) and os.path.getmtime(CLI) >= newest:
         return CLI
-    cmd = ["g++", "-O2", "-std=c++17", "-Wall", "-o", CLI, src, "-I", os.path.join(HERE, "..", "include"),
+    cmd = ["g++", "-O2", "-std=c++17", "-Wall", "-o", CLI] + srcs + ["-I", os.path.join(HERE, "..", "include"),
            "-L", HERE, "-lbrc_engine"]
     hts = os.path.join(HERE, "third_party", "htslib")          # tools/build_htslib.sh: htslib 1.10 as vendored with the reference (CRAM only)
     if os.path.exists(os.path.join(hts, "libhts.a")):

@@ -268,12 +268,8 @@ int brc_push_read(brc_engine *e, int32_t tid, int32_t pos, uint16_t flag, uint8_
     if (tid != rg.tid) return BRC_OK;   // another contig's read can never span a site of this region
 
     HostReads &H = e->reads;
-    H.pos.push_back(pos); H.flag.push_back(flag); H.mapq.push_back(mapq); H.lib.push_back(lib); H.l_qseq.push_back(l_qseq);
-    H.nm.push_back(nm); H.sm.push_back(sm); H.region.push_back((int32_t)(e->regions.size() - 1));
-    H.cigar.insert(H.cigar.end(), cigar, cigar + n_cigar); H.cigar_off.push_back(H.cigar.size());
-    const size_t sb = (size_t)(l_qseq + 1) / 2;
-    H.seq.insert(H.seq.end(), seq, seq + sb); H.seq_off.push_back(H.seq.size());
-    H.qual.insert(H.qual.end(), qual, qual + l_qseq); H.qual_off.push_back(H.qual.size());
+    H.append(pos, flag, mapq, lib, l_qseq, nm, sm, n_cigar, cigar, seq, qual);
+    H.region.push_back((int32_t)(e->regions.size() - 1));
     e->n_indel_ops += indel_ops;
     if (end > e->open_max_end) e->open_max_end = end;
     rg.read_hi = H.n();

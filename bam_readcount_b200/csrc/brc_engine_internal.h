@@ -5,13 +5,13 @@
 #include <deque>
 #include <queue>
 #include <string>
-#include <thread>
 #include <vector>
 
 #include <cuda_runtime.h>
 
 #include "../../include/brc_engine.h"
 #include "brc_device.cuh"
+#include "brc_reads.h"
 
 namespace brc {
 
@@ -50,25 +50,9 @@ struct HostRef {
     DevBuf dev;            // device copy
 };
 
-struct HostReads {         // staging SoA of admitted reads, all regions, file order
-    std::vector<int32_t> pos, l_qseq, nm, sm, region;
-    std::vector<uint16_t> flag, lib;
-    std::vector<uint8_t> mapq;
-    std::vector<uint64_t> cigar_off{0}, seq_off{0}, qual_off{0};
-    std::vector<uint32_t> cigar;
-    std::vector<uint8_t> seq, qual;
-    int64_t n() const { return (int64_t)pos.size(); }
-    brc_read_batch batch() const {   // the staged reads as a batch (tid NULL: every staged read is on its region's contig)
-        brc_read_batch b{};
-        b.n_reads = n(); b.pos = pos.data(); b.flag = flag.data(); b.mapq = mapq.data(); b.lib = lib.data(); b.l_qseq = l_qseq.data();
-        b.nm = nm.data(); b.sm = sm.data(); b.cigar_off = cigar_off.data(); b.cigar = cigar.data(); b.seq_off = seq_off.data();
-        b.seq = seq.data(); b.qual_off = qual_off.data(); b.qual = qual.data();
-        return b;
-    }
-    void clear() {
-        pos.clear(); l_qseq.clear(); nm.clear(); sm.clear(); region.clear(); flag.clear(); lib.clear(); mapq.clear();
-        cigar_off.assign(1, 0); seq_off.assign(1, 0); qual_off.assign(1, 0); cigar.clear(); seq.clear(); qual.clear();
-    }
+struct HostReads : ReadArrays {   // staging SoA of admitted reads, all regions, file order, and the region of each
+    std::vector<int32_t> region;
+    void clear() { ReadArrays::clear(); region.clear(); }
 };
 
 // pileup-buffer admission state of the open region (bam_plp_push, V:htslib-1.10/sam.c:4484-4531)
@@ -90,19 +74,6 @@ struct EmitState {
     void clear() { for (auto &d : q) d.clear(); std::fill(q_exists.begin(), q_exists.end(), 0); }
     bool pending() const { for (auto &d : q) if (!d.empty()) return true; return false; }
 };
-
-// Worker threads for n items: one more per `grain` items, at most `cap` and the core count.
-inline int worker_count(int64_t n, int64_t grain, int cap) {
-    const unsigned hw = std::thread::hardware_concurrency();
-    return (int)std::max<int64_t>(1, std::min<int64_t>({(int64_t)(hw ? hw : 1), (int64_t)cap, n / grain + 1}));
-}
-// Runs work(t) for t in [0, nt): t >= 1 on threads of their own, t = 0 on the calling thread; returns when all are done.
-template <class F> void fan_out(int nt, const F &work) {
-    std::vector<std::thread> th;
-    for (int t = 1; t < nt; ++t) th.emplace_back(work, t);
-    if (nt > 0) work(0);
-    for (auto &x : th) x.join();
-}
 
 }  // namespace brc
 
