@@ -1220,6 +1220,21 @@ int64_t brc_get_reference_codes(brc_engine *e, int32_t tid, uint8_t *out, int64_
     if (ce != cudaSuccess) return set_cuda_error(e, ce, "reference codes");
     return size;
 }
+int64_t brc_get_read_descriptors(brc_engine *e, void *desc, int64_t desc_cap, int32_t *tile_lo, int32_t *tile_hi, int64_t tile_cap,
+                                 int64_t *n_tiles) {
+    if (!e || !n_tiles || desc_cap < 0 || tile_cap < 0 || (!desc && desc_cap > 0) || ((!tile_lo || !tile_hi) && tile_cap > 0)) return BRC_E_INVALID;
+    if (e->last.kind == BRC_RESULTS_NONE) return set_error(e, BRC_E_INVALID, "get_read_descriptors: no run since the last reset");
+    cudaSetDevice(e->cfg.device);
+    const int64_t n = e->dev_reads.n_reads, nt = (int64_t)e->tiles.size();
+    *n_tiles = nt;
+    cudaError_t ce = cudaDeviceSynchronize();     // K0 ran on the caller's stream
+    if (ce == cudaSuccess && std::min(desc_cap, n) > 0)
+        ce = cudaMemcpy(desc, e->d_desc.p, (size_t)std::min(desc_cap, n) * sizeof(ReadDesc), cudaMemcpyDeviceToHost);
+    if (ce == cudaSuccess && std::min(tile_cap, nt) > 0) ce = cudaMemcpy(tile_lo, e->d_tile_lo.p, (size_t)std::min(tile_cap, nt) * 4, cudaMemcpyDeviceToHost);
+    if (ce == cudaSuccess && std::min(tile_cap, nt) > 0) ce = cudaMemcpy(tile_hi, e->d_tile_hi.p, (size_t)std::min(tile_cap, nt) * 4, cudaMemcpyDeviceToHost);
+    if (ce != cudaSuccess) return set_cuda_error(e, ce, "read descriptors");
+    return n;
+}
 int brc_host_alloc(size_t bytes, void **out) {
     if (!out) return BRC_E_INVALID;
     *out = nullptr;

@@ -238,24 +238,31 @@ __device__ __forceinline__ uint32_t nib8(const uint8_t *base, int64_t t) {
     if (t & 1) x = (x << 4) | ((__byte_perm(w0, w1, sh + 4u) >> 4) & 0xFu);
     return x;
 }
-// same, from shared memory with 32-bit addressing (addr = byte address of symbol 0)
-__device__ __forceinline__ uint32_t nib8_smem(uint32_t addr, int t) {
-    const uint32_t a = addr + (uint32_t)(t >> 1);
-    const uint32_t sh = a & 3u, aw = a - sh;
-    uint32_t w0, w1;
-    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(w0) : "r"(aw));
-    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(w1) : "r"(aw + 4u));
-    const uint32_t sel = (sh + 3u) | ((sh + 2u) << 4) | ((sh + 1u) << 8) | (sh << 12);
-    uint32_t x = __byte_perm(w0, w1, sel);
-    if (t & 1) x = (x << 4) | ((__byte_perm(w0, w1, sh + 4u) >> 4) & 0xFu);
-    return x;
-}
 __device__ __forceinline__ uint32_t lds_u8(uint32_t addr) {
     uint32_t v;
     asm volatile("ld.shared.u8 %0, [%1];" : "=r"(v) : "r"(addr));
     return v;
 }
-__device__ __forceinline__ uint32_t nib_nonzero(uint32_t v) { return (v | (v >> 1) | (v >> 2) | (v >> 3)) & 0x11111111u; }
+__device__ __forceinline__ uint32_t lds_u32(uint32_t addr) {
+    uint32_t v;
+    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(addr));
+    return v;
+}
+// 16 consecutive 4-bit symbols starting at symbol index t, symbol t in bits 63:60.  Shared memory: the three aligned words
+// holding bytes t/2 .. t/2 + 8, byte-swapped to big-endian and funnel-shifted (reads up to 11 bytes past byte t/2).
+__device__ __forceinline__ uint64_t nib16_smem(uint32_t addr, int t) {
+    const uint32_t a = addr + (uint32_t)(t >> 1);
+    const uint32_t aw = a & ~3u, s = ((a & 3u) << 3) | ((uint32_t)(t & 1) << 2);
+    const uint32_t b0 = __byte_perm(lds_u32(aw), 0u, 0x0123u), b1 = __byte_perm(lds_u32(aw + 4u), 0u, 0x0123u);
+    const uint32_t b2 = __byte_perm(lds_u32(aw + 8u), 0u, 0x0123u);
+    return (uint64_t)__funnelshift_l(b1, b0, s) << 32 | __funnelshift_l(b2, b1, s);
+}
+// global memory (a read too long for the stage, a reference op outside the staged window): two nib8, the second only when any of
+// its symbols is below `nv`, so no load reaches further past the last valid symbol than nib8 does
+__device__ __forceinline__ uint64_t nib16(const uint8_t *base, int64_t t, int nv) {
+    return (uint64_t)nib8(base, t) << 32 | (nv > 8 ? nib8(base, t + 8) : 0u);
+}
+__device__ __forceinline__ uint64_t nib_nonzero(uint64_t v) { return (v | (v >> 1) | (v >> 2) | (v >> 3)) & 0x1111111111111111ull; }
 
 constexpr int K0_READS = 128;
 constexpr int K0_SEQ_CAP = K0_READS * 80 + 32;
@@ -326,7 +333,7 @@ __global__ void __launch_bounds__(K0_READS) read_precompute_kernel(PrecomputePar
     const uint8_t *refc = reinterpret_cast<const uint8_t *>(rw.seq);   // packed 4-bit codes (launch_ref_encode)
 
     // --- fetch_func CIGAR/reference walk (R:...:133-199) + bam_cigar2rlen + SIMPLE detection ---
-    // Flattened into ONE loop whose iterations are either "fetch the next CIGAR op" or "compare 8 bases of the
+    // Flattened into ONE loop whose iterations are either "fetch the next CIGAR op" or "compare 16 bases of the
     // current M op", so the 32 reads of a warp stay converged whatever their CIGAR shapes are.
     uint32_t sum_mmq = 0;
     int left_clip = 0, clipped_length = l_qseq, right_clip = l_qseq;
@@ -378,19 +385,19 @@ __global__ void __launch_bounds__(K0_READS) read_precompute_kernel(PrecomputePar
             continue;
         }
         if (j < jend) {
-            // 8 bases per step: XOR of the packed read nibbles with the packed reference codes
-            const uint32_t X = staged ? nib8_smem(seq_sa, read_position + j) : nib8(seq, read_position + j);
-            const uint32_t Y = ref_staged ? nib8_smem(ref_sa, (int)(wrel + j)) : nib8(refc, wrel + j);
-            const uint32_t x = X ^ Y;
+            // 16 bases per step: XOR of the packed read nibbles with the packed reference codes
+            const int nv = jend - j;
+            const uint64_t X = staged ? nib16_smem(seq_sa, read_position + j) : nib16(seq, read_position + j, nv);
+            const uint64_t Y = ref_staged ? nib16_smem(ref_sa, (int)(wrel + j)) : nib16(refc, wrel + j, nv);
+            const uint64_t x = X ^ Y;
             if (x != 0u) {
-                const int nv = jend - j;
-                const uint32_t keep = nv >= 8 ? 0xFFFFFFFFu : ~(0xFFFFFFFFu >> (4 * nv));
+                const uint64_t keep = nv >= 16 ? ~0ull : ~(~0ull >> (4 * nv));
                 // mismatch iff read != ref && ref != 15 && read != 0   (R:...:152)
-                uint32_t m = nib_nonzero(x) & ~((Y & (Y >> 1) & (Y >> 2) & (Y >> 3)) & 0x11111111u) & nib_nonzero(X) & keep;
+                uint64_t m = nib_nonzero(x) & ~((Y & (Y >> 1) & (Y >> 2) & (Y >> 3)) & 0x1111111111111111ull) & nib_nonzero(X) & keep;
                 while (m) {
-                    const int k8 = __clz(m) >> 2;          // flag of symbol i sits at bit 28-4i
-                    m &= ~(0x10000000u >> (4 * k8));
-                    const int cur = read_position + j + k8;
+                    const int k16 = __clzll(m) >> 2;       // flag of symbol i sits at bit 60-4i
+                    m &= ~(0x1000000000000000ull >> (4 * k16));
+                    const int cur = read_position + j + k16;
                     const int q = staged ? (int)lds_u8(qual_sa + (uint32_t)cur) : (int)qual[cur];
                     if (last_mm_pos != -1) {
                         if (last_mm_pos + 1 != cur) { sum_mmq += (uint32_t)last_mm_qual; last_mm_qual = q; }
@@ -399,7 +406,7 @@ __global__ void __launch_bounds__(K0_READS) read_precompute_kernel(PrecomputePar
                     } else { last_mm_pos = cur; last_mm_qual = q; }
                 }
             }
-            j += 8;
+            j += 16;
             continue;
         }
         // M op finished.  Site-list mode skips positions beyond chrom_len (R:...:144-148) but position == chrom_len still reads the NUL.
@@ -411,13 +418,26 @@ __global__ void __launch_bounds__(K0_READS) read_precompute_kernel(PrecomputePar
     if (n_refops != 1) simple = false;
 
     // --- Q2 run / effective 3' end (R:...:202-238) ---
-    int tpi, q2_pos = -1, kk, inc;
+    // q2_pos = (index of the first quality byte != 2 from the 3' end) - 1, or -1 when there is none.  Scanned 4 bytes per step
+    // in the aligned words holding the read's qualities; bytes of the first and last word outside [0, l_qseq) are masked off.
+    int tpi, q2_pos = -1;
     const bool reverse = (flag & 16u) != 0;
-    if (reverse) { kk = tpi = 0; inc = 1; if (tpi < left_clip) tpi = left_clip; }
-    else { kk = tpi = l_qseq - 1; inc = -1; if (tpi > right_clip) tpi = right_clip; }
-    while (kk >= 0 && kk < l_qseq) {
-        if ((staged ? lds_u8(qual_sa + (uint32_t)kk) : (uint32_t)qual[kk]) != 2u) { q2_pos = kk - 1; break; }
-        kk += inc;
+    if (reverse) { tpi = 0; if (tpi < left_clip) tpi = left_clip; }
+    else { tpi = l_qseq - 1; if (tpi > right_clip) tpi = right_clip; }
+    if (l_qseq > 0) {
+        const int lead = (int)((staged ? qual_sa : (uint32_t)reinterpret_cast<uintptr_t>(qual)) & 3u);   // byte 0's place in its word
+        const int wl = (l_qseq - 1 + lead) >> 2;                                                         // last word
+        const uint32_t first_mask = ~0u << (8 * lead), last_mask = ~0u >> (8 * (3 - ((l_qseq - 1 + lead) & 3)));
+        const int winc = reverse ? 1 : -1;
+        for (int w = reverse ? 0 : wl; w >= 0 && w <= wl; w += winc) {
+            const uint32_t v = (staged ? lds_u32(qual_sa - (uint32_t)lead + 4u * (uint32_t)w)
+                                       : *reinterpret_cast<const uint32_t *>(qual - lead + 4 * w)) ^ 0x02020202u;
+            // bit 7 of each byte: that byte != 2
+            uint32_t ne = (((v & 0x7F7F7F7Fu) + 0x7F7F7F7Fu) | v) & 0x80808080u;
+            if (w == 0) ne &= first_mask;
+            if (w == wl) ne &= last_mask;
+            if (ne) { q2_pos = 4 * w + ((reverse ? __ffs(ne) - 1 : 31 - __clz(ne)) >> 3) - lead - 1; break; }
+        }
     }
     if (reverse) { if (tpi < q2_pos) tpi = q2_pos; }
     else { if (tpi > q2_pos && q2_pos != -1) tpi = q2_pos; }

@@ -219,9 +219,9 @@ __device__ __forceinline__ uint32_t seq4(uint32_t c) {
     return ((nib & 0x0F0F0F0Fu) << 4) | ((nib >> 4) & 0x0F0F0F0Fu);
 }
 
-// quality group g (query positions 8g .. 8g+7) of a read: 8 quality bytes (little-endian) and 8 base codes (2 bits each), the
-// substitutions applied.  The values make_body computes, position for position.
-__device__ __forceinline__ void fill_group(const Hdr &h, int64_t start, uint64_t subs, int g, const uint64_t *win, int64_t w_lo,
+// quality group g (query positions 8g .. 8g+7) of a read: 8 quality bytes (little-endian) and 8 base codes (2 bits each), before
+// the substitutions.  The values make_body computes, position for position.
+__device__ __forceinline__ void fill_group(const Hdr &h, int64_t start, int g, const uint64_t *win, int64_t w_lo,
                                            uint64_t seed, uint64_t unit, uint64_t &qual8, uint32_t &codes) {
     const int q0 = 8 * g;
     const uint64_t hq = sub_stream(h.rk, 8 + (uint64_t)g);
@@ -250,13 +250,6 @@ __device__ __forceinline__ void fill_group(const Hdr &h, int64_t start, uint64_t
             const uint32_t b = ro >= 0 ? (uint32_t)(bases >> (2 * (ro - ro0))) & 3u : (uint32_t)(hb >> (2 * (q & 31))) & 3u;
             c |= b << (2 * k);
         }
-    }
-    for (int k = 0; k < (int)(subs >> 60); ++k) {
-        const uint32_t e = (uint32_t)(subs >> (10 * k)), p = e & 0xFFu;
-        if ((int)(p >> 3) != g) continue;
-        const int sh = 2 * (int)(p & 7u);
-        const uint32_t b = (c >> sh) & 3u;
-        c ^= (b ^ ((b + ((e >> 8) & 3u)) & 3u)) << sh;
     }
     codes = c;
 }
@@ -294,17 +287,15 @@ __global__ void __launch_bounds__(1024) synth_scan_kernel(unsigned long long *v,
     for (int64_t i = lo; i < hi; ++i) { const unsigned long long y = v[i]; v[i] = acc; acc += y; }
 }
 
-// One CTA = one block of 256 reads.  Each read's header is hashed once and kept in shared memory; its metadata and substitution
-// list are made by one thread, its bases and qualities by all: the CTA's 256 x 19 quality groups are spread over the 256 threads,
-// consecutive lanes on consecutive groups of a read, the reference bases taken from words staged once per CTA.  The rows are staged
-// in shared memory and leave with 16-byte stores.
+// One CTA = one block of 256 reads.  Each read's header is hashed once and kept in shared memory for the sort; after it, thread t
+// owns row t: its metadata, its substitution list and its 19 quality groups, the header, start and list held in registers and the
+// reference bases taken from words staged once per CTA.  The substitutions are patched into the row once, after its groups.  The
+// rows are staged in shared memory and leave with 16-byte stores.
 __global__ void __launch_bounds__(BR) synth_fill_kernel(DevArgs A) {
     extern __shared__ __align__(16) uint8_t smem[];
     uint8_t *seq_s = smem, *qual_s = smem + BR * SB;                                          // 19200 + 38400 bytes
-    Hdr *hs = reinterpret_cast<Hdr *>(smem + BR * (SB + RL));                                 // headers: by j, then by row
-    int64_t *start_s = reinterpret_cast<int64_t *>(hs + BR);
-    uint64_t *subs_s = reinterpret_cast<uint64_t *>(start_s + BR);
-    uint64_t *win = subs_s + BR;                                                              // NWIN reference words from w_lo
+    Hdr *hs = reinterpret_cast<Hdr *>(smem + BR * (SB + RL));                                 // headers by j (the sort's lookup)
+    uint64_t *win = reinterpret_cast<uint64_t *>(hs + BR);                                    // NWIN reference words from w_lo
     uint32_t *xs = reinterpret_cast<uint32_t *>(win + NWIN);                                  // sort exchange / scan totals
     __shared__ int64_t w_lo_s;
     const int t = threadIdx.x;
@@ -334,10 +325,9 @@ __global__ void __launch_bounds__(BR) synth_fill_kernel(DevArgs A) {
     const int nc = s.valid ? n_cigar_of(s.h.kind) : 0;
     const unsigned long long coff = A.blk_cig[b] + cta_exclusive_scan((uint32_t)nc, xs, t);   // its barrier: every header read by j
     const brc_synth_out &O = A.O;
+    uint64_t subs = 0;
     if (s.valid) {
-        uint64_t subs;
         const int32_t nm = sub_list(s.h, subs);
-        hs[t] = s.h; start_s[t] = s.start; subs_s[t] = subs;
         if (O.tid) O.tid[i] = A.contig;
         O.pos[i] = (int32_t)s.start; O.flag[i] = (uint16_t)(s.h.reverse ? 16 : 0); O.mapq[i] = (uint8_t)s.h.mapq; O.lib[i] = (uint16_t)s.lib;
         O.l_qseq[i] = RL; O.nm[i] = nm; O.sm[i] = TAG_ABSENT;
@@ -347,21 +337,28 @@ __global__ void __launch_bounds__(BR) synth_fill_kernel(DevArgs A) {
         if (O.region_of_read) O.region_of_read[i] = s.region;
         if (i == A.n_reads - 1) { O.cigar_off[i + 1] = coff + nc; O.seq_off[i + 1] = (uint64_t)(i + 1) * SB; O.qual_off[i + 1] = (uint64_t)(i + 1) * RL; }
     }
-    __syncthreads();
-    // bases and qualities: item it = quality group g of row r
+    // bases and qualities: thread t builds row t (its own read) group by group, then patches in the read's substitutions
     const int rows = (int)imin64(BR, A.n_reads - b * BR);
+    if (t < rows) {
+        uint16_t *qd = reinterpret_cast<uint16_t *>(qual_s + t * RL);                          // rows and groups start at even bytes
+        uint8_t *sd = seq_s + t * SB;
 #pragma unroll 2
-    for (int it = t; it < rows * NG; it += BR) {
-        const int r = it / NG, g = it - r * NG;
-        uint64_t qv; uint32_t codes;
-        fill_group(hs[r], start_s[r], subs_s[r], g, win, w_lo, seed, unit, qv, codes);
-        const int nq = g == NG - 1 ? RL - 8 * (NG - 1) : 8;
-        uint16_t *qd = reinterpret_cast<uint16_t *>(qual_s + r * RL + 8 * g);                  // rows and groups start at even bytes
-        uint8_t *sd = seq_s + r * SB + 4 * g;
-        const uint32_t sq = seq4(codes);
-        for (int k = 0; k < nq / 2; ++k) {
-            qd[k] = (uint16_t)(qv >> (16 * k));
-            sd[k] = (uint8_t)(sq >> (8 * k));
+        for (int g = 0; g < NG; ++g) {
+            uint64_t qv; uint32_t codes;
+            fill_group(s.h, s.start, g, win, w_lo, seed, unit, qv, codes);
+            const int nq = g == NG - 1 ? RL - 8 * (NG - 1) : 8;
+            const uint32_t sq = seq4(codes);
+            for (int k = 0; k < nq / 2; ++k) {
+                qd[4 * g + k] = (uint16_t)(qv >> (16 * k));
+                sd[4 * g + k] = (uint8_t)(sq >> (8 * k));
+            }
+        }
+        // distinct positions: each substitution shifts the base the group left there
+        for (int k = 0; k < (int)(subs >> 60); ++k) {
+            const uint32_t e = (uint32_t)(subs >> (10 * k)), p = e & 0xFFu;
+            const uint32_t byte = sd[p >> 1], sh = (p & 1u) ? 0u : 4u;
+            const uint32_t code = __ffs((byte >> sh) & 15u) - 1;
+            sd[p >> 1] = (uint8_t)((byte & ~(15u << sh)) | (1u << ((code + ((e >> 8) & 3u)) & 3u)) << sh);
         }
     }
     __syncthreads();
@@ -527,7 +524,7 @@ int brc_synth_fill_device(const brc_synth_spec *S, int32_t contig, int64_t lo, i
     if (O->n_reads != n) return BRC_E_INVALID;
     if (n == 0) return BRC_OK;
     const int64_t nblk = (n + BR - 1) / BR;
-    const int smem = BR * (SB + RL) + BR * (int)(sizeof(Hdr) + 2 * sizeof(uint64_t)) + NWIN * (int)sizeof(uint64_t) + BR * 4;
+    const int smem = BR * (SB + RL) + BR * (int)sizeof(Hdr) + NWIN * (int)sizeof(uint64_t) + BR * 4;
     if (cudaFuncSetAttribute(synth_fill_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) return BRC_E_CUDA;
     DevArgs A; A.S = *S; A.contig = contig; A.blk_lo = lo; A.n_reads = n; A.O = *O; A.blk_cig = reinterpret_cast<unsigned long long *>(scratch_dev);
     cudaStream_t s = (cudaStream_t)stream;

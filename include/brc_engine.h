@@ -413,6 +413,12 @@ BRC_API int64_t brc_selftest_fastmath(brc_engine *e, int32_t max_b);
  * nibble, then 0xFF padding (win_len / 2 + 32 bytes in all).  Waits for the device, copies min(cap, that size) bytes to `out`
  * and returns the full size, or a negative status (BRC_E_NO_REFERENCE when the contig has none). */
 BRC_API int64_t brc_get_reference_codes(brc_engine *e, int32_t tid, uint8_t *out, int64_t cap);
+/* The per-read work of the last brc_run_device/brc_compute as the pileup kernels read it (debug view): the read descriptors K0
+ * wrote (80 bytes each, brc_device.cuh ReadDesc) and the first / one-past-last read index of every tile.  Waits for the device,
+ * copies min(desc_cap, n_reads) descriptors to `desc` and min(tile_cap, n_tiles) entries to `tile_lo` / `tile_hi`, stores n_tiles
+ * in *n_tiles and returns n_reads, or a negative status (BRC_E_INVALID before any run). */
+BRC_API int64_t brc_get_read_descriptors(brc_engine *e, void *desc, int64_t desc_cap, int32_t *tile_lo, int32_t *tile_hi, int64_t tile_cap,
+                                         int64_t *n_tiles);
 /* kernels launched by the last brc_run_device/brc_compute (for bench.py's gpu_launches) */
 /* Page-locked host memory for batches handed to brc_push_reads (a borrowed batch is DMA'd straight out of the caller's arrays:
  * from pageable memory the copies are staged and synchronous).  cudaHostAlloc / cudaFreeHost behind plain pointers, so that a host
