@@ -188,6 +188,17 @@ static int64_t read_endpos(const orc_reads *R, int64_t i) {
     return (int64_t)R->pos[i] + 1;
 }
 
+/* fetch_values and read_endpos of reads [lo, hi), one reference (tests: the read descriptors of the engine's K0).
+ * out_zm: 5 int32 per read in orc_zm order; out_end: one int64 per read. */
+void orc_read_values(const orc_ref *ref, const orc_reads *R, int64_t lo, int64_t hi, int ref_len_check, int32_t *out_zm,
+                     int64_t *out_end) {
+    for (int64_t i = lo; i < hi; ++i) {
+        orc_zm z = fetch_values(R, i, ref, ref_len_check);
+        memcpy(out_zm + 5 * (i - lo), &z, sizeof z);
+        out_end[i - lo] = read_endpos(R, i);
+    }
+}
+
 /* ---- live list node + incremental CIGAR cursor (V:htslib-1.10/sam.c:3904-3918) ---------- */
 typedef struct { int64_t read; int64_t beg, end; int k, y; int64_t x; orc_zm zm; } orc_node;
 typedef struct { int qpos, indel, is_del, is_refskip; } orc_plp;

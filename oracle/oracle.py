@@ -8,7 +8,7 @@ from __future__ import annotations
 import ctypes as C
 import os
 import subprocess
-from typing import List, Optional, Sequence, Tuple
+from typing import List, NamedTuple, Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -73,7 +73,43 @@ def _load():
         _lib.orc_region.restype = C.c_int64
         _lib.orc_region.argtypes = [C.c_void_p, C.POINTER(_Config), C.POINTER(_Ref), C.POINTER(_Reads), C.c_int64,
                                     C.c_int64, C.c_int32, C.c_int64, C.c_int64, C.c_int]
+        _lib.orc_read_values.restype = None
+        _lib.orc_read_values.argtypes = [C.POINTER(_Ref), C.POINTER(_Reads), C.c_int64, C.c_int64, C.c_int, C.c_void_p,
+                                         C.c_void_p]
     return _lib
+
+
+def _c_reads(b):
+    """The batch as orc_reads, and the arrays its pointers point into (keep them alive while it is used)."""
+    keep = [np.ascontiguousarray(a) for a in (b.tid, b.pos, b.flag, b.mapq, b.lib, b.l_qseq, b.nm, b.sm, b.cigar_off,
+                                               b.cigar, b.seq_off, b.seq, b.qual_off, b.qual)]
+    return _Reads(b.n_reads, *[a.ctypes.data for a in keep]), keep
+
+
+class ReadValues(NamedTuple):
+    """fetch_func's per-read values (R:bamreadcount.cpp:114-253) and bam_endpos (V:htslib-1.10/sam.c:507-513)."""
+    mmq: np.ndarray            # sum_of_mismatch_qualities, int32
+    clipped_length: np.ndarray
+    left_clip: np.ndarray
+    tpi: np.ndarray            # three_prime_index
+    q2_pos: np.ndarray
+    endpos: np.ndarray         # int64; pos + 1 for unmapped reads and reads without CIGAR
+
+
+def read_values(batch, contig, site_list_mode: bool, lo: int = 0, hi: Optional[int] = None) -> ReadValues:
+    """fetch_values / read_endpos of reads [lo, hi) of ``batch`` against ``contig`` = (name, chrom_len, window bytes,
+    win_beg); ``site_list_mode`` is the reference's ref_len check (-l)."""
+    lib = _load()
+    hi = batch.n_reads if hi is None else hi
+    name, chrom_len, seq, win_beg = contig
+    reads, keep = _c_reads(batch)
+    ref = _Ref(0, name.encode(), chrom_len, win_beg, len(seq), seq)
+    zm = np.zeros((max(hi - lo, 0), 5), np.int32)
+    end = np.zeros(max(hi - lo, 0), np.int64)
+    if hi > lo:
+        lib.orc_read_values(C.byref(ref), C.byref(reads), lo, hi, int(site_list_mode), zm.ctypes.data, end.ctypes.data)
+    del keep
+    return ReadValues(*(zm[:, k].copy() for k in range(5)), end)
 
 
 class Oracle:
@@ -102,10 +138,7 @@ class Oracle:
         """Run one region: ``beg`` is the reference's d.beg (0-based first printed site), ``end`` its d.end.
         ``batch`` holds (from read_lo to read_hi) the records fetched for [beg-1, end) in file order."""
         b = batch
-        keep = [np.ascontiguousarray(a) for a in (b.tid, b.pos, b.flag, b.mapq, b.lib, b.l_qseq, b.nm, b.sm, b.cigar_off,
-                                                   b.cigar, b.seq_off, b.seq, b.qual_off, b.qual)]
-        ptrs = [a.ctypes.data for a in keep]
-        reads = _Reads(b.n_reads, *ptrs)
+        reads, keep = _c_reads(b)
         ref = _Ref(tid, contig.encode(), chrom_len, ref_win_beg, len(ref_seq), ref_seq)
         hi = b.n_reads if read_hi is None else read_hi
         n = self.lib.orc_region(self.ctx, C.byref(self.cfg), C.byref(ref), C.byref(reads), read_lo, hi, tid, beg, end,

@@ -21,7 +21,8 @@ import boundary_cases
 import cases
 from boundary_cases import initial_pool_cap, pool_case, selection_cases
 from cases import first_diff
-from kernel_model import CONST_NAMES, CSRC, k0_blocks, k1_chunks, kernel_constants, tile_ranges
+from kernel_model import (CONST_NAMES, CSRC, FM_FASTDIV, FM_HOT, FM_SIMPLE, cigar_shape, k0_blocks, k0_descriptors, k1_chunks,
+                          kernel_constants, tile_ranges)
 from site_filter_rule import THRESHOLDS, select_lines
 
 
@@ -38,76 +39,16 @@ def _reads_view(b):
     return out
 
 
-def read_facts(case, batch, site_list):
-    """fetch_func's per-read values as K0 forms them (brc_kernels.cu read_precompute_kernel)."""
-    K = kernel_constants()
-    name, clen_chrom, seq, wb = case["contigs"][0]
-    ref = np.frombuffer(case.get("full_ref", seq), np.uint8)
-    from bam_readcount_b200.batch import _NT16
-    refc = _NT16[ref]
-    cig = _reads_view(batch)
-    so = batch.seq_off.astype(np.int64)
-    qo = batch.qual_off.astype(np.int64)
-    facts = []
-    for i, ops in enumerate(cig):
-        lq = int(batch.l_qseq[i])
-        pk = batch.seq[so[i]:so[i + 1]]
-        nib = np.empty(pk.shape[0] * 2, np.uint8); nib[0::2] = pk >> 4; nib[1::2] = pk & 15
-        qual = batch.qual[qo[i]:qo[i + 1]]
-        refops = [o for _, o in ops if o in "MDN=X"]
-        simple = len(refops) == 1 and refops[0] in "M=X" and not any(o in "IP" for _, o in ops)
-        lclip, clen = 0, lq
-        refpos, rp, walking = int(batch.pos[i]), 0, True
-        mm = []                       # (read offset, quality) of mismatches
-        for k, (l, o) in enumerate(ops):
-            if not walking:
-                break
-            if o == "M":
-                jn, hit = l, False
-                if refpos + l > clen_chrom:
-                    if site_list and refpos > clen_chrom:
-                        jn = 0
-                    else:
-                        jn, hit = max(0, clen_chrom - refpos), True
-                for j in range(jn):
-                    r, q = int(refc[refpos + j]), int(nib[rp + j])
-                    if r != q and r != 15 and q != 0:
-                        mm.append((rp + j, int(qual[rp + j])))
-                if hit:
-                    walking = False
-                else:
-                    refpos += l; rp += l
-            elif o in "DN":
-                refpos += l
-            elif o == "I":
-                rp += l
-            elif o == "S":
-                rp += l; clen -= l
-                if k == 0:
-                    lclip += l
-        mmq, last_p, last_q = 0, -1, 0
-        for p, q in mm:
-            if last_p != -1 and last_p + 1 != p:
-                mmq += last_q; last_q = q
-            elif last_p != -1:
-                last_q = max(last_q, q)
-            else:
-                last_q = q
-            last_p = p
-        mmq += last_q
-        fast = 1 <= lq <= K["FASTDIV_MAX"] and 1 <= clen <= K["FASTDIV_MAX"]
-        nm_ok = int(batch.nm[i]) != -2 ** 31
-        sm_missing = bool(batch.flag[i] & 2) and int(batch.sm[i]) == -2 ** 31
-        qoff = 0
-        for l, o in ops:
-            if o in "MDN=X":
-                break
-            if o == "S":
-                qoff += l
-        se = (int(batch.sm[i]) if not sm_missing else 0) if batch.flag[i] & 2 else int(batch.mapq[i])
-        facts.append(dict(lq=lq, clen=clen, lclip=lclip, fast=fast, hot=simple and fast and nm_ok and not sm_missing, simple=simple,
-                          qoff=qoff, mmq=mmq, se=se, ops=ops))
-    return facts
+def read_model(case, batch, site_list):
+    """Per read, the descriptor K0 writes for it (kernel_model.k0_descriptors, the model tests/test_k0_descriptors.py holds the
+    device to) as the targets below read it, with its CIGAR as (len, op char) pairs and its qoff."""
+    contig = case["contigs"][0]
+    region = dict(ref=0, site_list=site_list, first_pos=0, n_slots=0, read_lo=0, read_hi=batch.n_reads)
+    d, _, _ = k0_descriptors(batch, [region], [contig], {})
+    _, qoff = cigar_shape(batch)
+    return [dict(lq=int(batch.l_qseq[i]), clen=int(d["clen"][i]), lclip=int(d["lclip"][i]), fast=bool(d["fm"][i] & FM_FASTDIV),
+                 hot=bool(d["fm"][i] & FM_HOT), simple=bool(d["fm"][i] & FM_SIMPLE), qoff=int(qoff[i]), mmq=int(d["mmq"][i]),
+                 se=int(d["se"][i]), ops=ops) for i, ops in enumerate(_reads_view(batch))]
 
 
 def site_sums(batch, facts, lo, hi):
@@ -140,7 +81,7 @@ def check_targets(case):
     tid, beg, end, batch = cases.region_reads(case, ci, b1, e1)
     if batch.n_reads != case["batch"].n_reads:      # site-list cases: per-read facts over every read of the case
         batch = case["batch"]
-    facts = read_facts(case, batch, case["site_list"])
+    facts = read_model(case, batch, case["site_list"])
     first_pos = max(beg, 0)
     for target in case["targets"]:
         if target == "k0_qual_cap":
