@@ -45,6 +45,21 @@ constexpr uint32_t FM_FASTDIV = 1u << 27;    // 1 <= l_qseq, clipped_length <= F
 constexpr uint32_t FM_HOT = 1u << 28;        // SIMPLE && FASTDIV && no missing-tag warnings: the hot loop's straight-line path
 constexpr uint32_t FM_DEAD = 1u << 29;       // fails -q or the flag filter (R:bamreadcount.cpp:288-310): only counts as a spanning read
 constexpr int FASTDIV_MAX = 2048;
+// Exact quotient tables of the FM_FASTDIV event terms (brc_kernels.cu, one copy per device).  Row d (1 <= d <= FASTDIV_MAX) holds,
+// at column QTAB_MID + j for -QTAB_MID <= j < QTAB_MID:
+//   Q[d][QTAB_MID + j] = RN(|j| / d)                          (float)
+//   P[d][QTAB_MID + j] = 1 - (double)RN(|2 j - d| / d)        (double, exact)
+// so an event reads d3p at j = qpos - three_prime_index and the Q2 term at j = qpos - q2_pos in row l_qseq, and 1 - posf at
+// j = qpos - left_clip in row clipped_length: the read's row and offset are folded into one base index, the event adds qpos.
+// Every such j lies in (-QTAB_MID, QTAB_MID) since 0 <= qpos, left_clip, three_prime_index < l_qseq <= FASTDIV_MAX, except the
+// Q2 column of a read without a Q2 position (q2_pos = -1), whose value is never used and whose j = l_qseq can reach QTAB_MID:
+// row QTAB_ROWS - 1 is there to keep that load inside the allocation.  The row of l_qseq is found from ReadDesc::fl without a
+// conversion: the bits of fl + 2^23 are 0x4B000000 + l_qseq, and shifted left by QTAB_SHIFT only l_qseq << QTAB_SHIFT remains.
+constexpr int QTAB_SHIFT = 12;
+constexpr int QTAB_MID = FASTDIV_MAX;
+constexpr int QTAB_ROWS = FASTDIV_MAX + 2;
+constexpr int64_t QTAB_ENTRIES = (int64_t)QTAB_ROWS << QTAB_SHIFT;
+static_assert(2 * QTAB_MID == 1 << QTAB_SHIFT, "a quotient-table row spans j in [-QTAB_MID, QTAB_MID)");
 
 struct __align__(16) ReadDesc {
     // q0
@@ -182,6 +197,9 @@ struct PileupParams {
     int32_t deep_min_reads;
     // tile dispenser of THIS launch (ResultsDev::warn + WARN_WORDS + k, zeroed by init_tiles_kernel)
     unsigned long long *work_counter;
+    // the device's quotient tables (QTAB_* above), filled in by launch_pileup for the kernels that read them (brc_kernels.cu USE_QTAB)
+    const float *qtab_q;
+    const double *qtab_p;
 };
 constexpr int WARN_WORDS = 4;          // ResultsDev::warn: [0] SM missing, [1] NM missing, [2..3] spare; followed by one tile
                                        // dispenser per pileup launch of a run
@@ -386,6 +404,8 @@ cudaError_t launch_deep_sites(const PileupParams &p, cudaStream_t s);   // no-op
 cudaError_t launch_fill_offsets(uint64_t *off, int64_t n, uint64_t base, uint64_t stride, cudaStream_t s);   // off[i] = base + i * stride
 cudaError_t launch_fill_i32(int32_t *dst, int64_t n, int32_t v, cudaStream_t s);
 cudaError_t launch_fastmath_selftest(int max_b, unsigned long long *d_bad, cudaStream_t s);
+// the current device's quotient tables (QTAB_*), built on first use
+cudaError_t quotient_tables(const float **q, const double **p);
 // brc_select.cu: pool pass, site pass, ship flags, scan, compaction of sites and pool records (SELECT_KERNELS launches)
 constexpr int SELECT_KERNELS = 8;
 constexpr int SELECT_SCAN_CTA = 256;   // sites per scan partial (SelectParams::nb = ceil(n_slots / SELECT_SCAN_CTA))

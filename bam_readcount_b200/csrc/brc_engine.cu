@@ -1208,6 +1208,18 @@ int64_t brc_selftest_fastmath(brc_engine *e, int32_t max_b) {
     return (int64_t)h_bad;
 }
 
+int64_t brc_get_quotient_rows(brc_engine *e, int32_t d_lo, int32_t d_hi, float *q, double *p) {
+    if (!e || !q || !p || d_lo < 1 || d_hi < d_lo || d_hi > FASTDIV_MAX) return BRC_E_INVALID;
+    cudaSetDevice(e->cfg.device);
+    const float *dq = nullptr; const double *dp = nullptr;
+    cudaError_t ce = quotient_tables(&dq, &dp);
+    const int64_t first = (int64_t)d_lo << QTAB_SHIFT, n = (int64_t)(d_hi - d_lo + 1) << QTAB_SHIFT;
+    if (ce == cudaSuccess) ce = cudaMemcpy(q, dq + first, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost);
+    if (ce == cudaSuccess) ce = cudaMemcpy(p, dp + first, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost);
+    if (ce != cudaSuccess) return set_cuda_error(e, ce, "quotient rows");
+    return n;
+}
+
 int64_t brc_get_reference_codes(brc_engine *e, int32_t tid, uint8_t *out, int64_t cap) {
     if (!e || (!out && cap > 0) || cap < 0) return BRC_E_INVALID;
     const HostRef *r = nullptr;

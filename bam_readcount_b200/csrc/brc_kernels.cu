@@ -22,9 +22,10 @@
 // feeding a 2-stage shared-memory ring, eight consumer warps).
 //
 // Float arithmetic uses explicit round-to-nearest intrinsics and the library is built with
-// --fmad=false: results must match the reference's x86-64 SSE arithmetic bit for bit.  The two
-// shortcuts of the hot loop (reciprocal division for small integers, float<->double by bit
-// casts) are exact and checked against the IEEE intrinsics by brc_selftest_fastmath.
+// --fmad=false: results must match the reference's x86-64 SSE arithmetic bit for bit.  The hot
+// loop reads its quotients from exact per-device tables (brc_device.cuh QTAB_*) and rounds to
+// float32 precision in double without conversions; both are checked against the IEEE intrinsics
+// by brc_selftest_fastmath.
 #include <algorithm>
 #include <atomic>
 #include <mutex>
@@ -129,6 +130,45 @@ static cudaError_t ensure_tables() {
         if (e != cudaSuccess) return e;
         if (dev < 64) uploaded[dev].store(true, std::memory_order_release);
     }
+    return cudaSuccess;
+}
+
+// the quotient tables of brc_device.cuh (QTAB_*): one thread per entry, with the IEEE intrinsics the tables stand in for
+__global__ void qtab_build_kernel(float *q, double *p) {
+    const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    if (i >= QTAB_ENTRIES) return;
+    const int d = (int)(i >> QTAB_SHIFT), j = (int)(i & ((1 << QTAB_SHIFT) - 1)) - QTAB_MID;
+    if (d == 0) { q[i] = 0.0f; p[i] = 0.0; return; }    // never read: l_qseq and clipped_length are >= 1
+    q[i] = __fdiv_rn((float)abs(j), (float)d);
+    p[i] = __dsub_rn(1.0, (double)__fdiv_rn((float)abs(2 * j - d), (float)d));
+}
+
+static float *g_qtab_q[64];
+static double *g_qtab_p[64];
+static std::atomic<bool> g_qtab_ready[64];
+cudaError_t quotient_tables(const float **q, const double **p) {
+    int dev = 0; cudaGetDevice(&dev);
+    if (dev >= 64) return cudaErrorInvalidDevice;
+    if (!g_qtab_ready[dev].load(std::memory_order_acquire)) {
+        std::lock_guard<std::mutex> lk(g_init_mu);
+        if (!g_qtab_ready[dev].load(std::memory_order_relaxed)) {
+            // built on a stream of its own and waited for: every engine stream of the process may use the tables afterwards
+            float *dq = nullptr; double *dp = nullptr; cudaStream_t s = nullptr;
+            cudaError_t e = cudaMalloc(&dq, QTAB_ENTRIES * sizeof(float));
+            if (e == cudaSuccess) e = cudaMalloc(&dp, QTAB_ENTRIES * sizeof(double));
+            if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking);
+            if (e == cudaSuccess) {
+                qtab_build_kernel<<<(unsigned)((QTAB_ENTRIES + 255) / 256), 256, 0, s>>>(dq, dp);
+                e = cudaGetLastError();
+                if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+            }
+            if (s) cudaStreamDestroy(s);
+            if (e != cudaSuccess) { cudaFree(dq); cudaFree(dp); return e; }
+            g_qtab_q[dev] = dq; g_qtab_p[dev] = dp;
+            g_qtab_ready[dev].store(true, std::memory_order_release);
+        }
+    }
+    *q = g_qtab_q[dev]; *p = g_qtab_p[dev];
     return cudaSuccess;
 }
 
@@ -561,9 +601,34 @@ __device__ __forceinline__ float div_small(float a, float b, float rcp) {
 
 // One (site, read) event's contributions — the body of BasicStat::process_read (R:BasicStat.cpp:28-107).
 struct Terms { float q2term, d3pterm, posf; double posterm; };   // posterm == 1.0 - (double)posf
-__device__ __forceinline__ Terms event_terms(bool fast, int qpos, int q2pos, int tpi, int lclip, int clen, float fl, float fclen,
-                                             float rcp_l, float rcp_c) {
+// Which kernels read the quotient tables (brc_device.cuh QTAB_*) for an FM_FASTDIV event, and which divide with div_small.  The
+// per-library pileup_kernel sits at its 72-register cap, where the table path costs it one more spilled value in the per-read
+// loop, and the deep-site kernel is not an issue-bound walk: both keep the reciprocal divisions.  -DBRC_NO_QTAB builds every
+// kernel with the divisions (the tests compare a run of the table path against that build).
+#ifdef BRC_NO_QTAB
+constexpr bool USE_QTAB = false;
+#else
+constexpr bool USE_QTAB = true;
+#endif
+// l_qseq << QTAB_SHIFT from fl = (float)l_qseq
+__device__ __forceinline__ uint32_t qtab_row(float fl) { return __float_as_uint(__fadd_rn(fl, 8388608.0f)) << QTAB_SHIFT; }
+// The terms of an FM_FASTDIV read (1 <= l_qseq, clipped_length <= FASTDIV_MAX) from the tables.  The Q2 term is only accumulated
+// when the read has a Q2 position: without one the value here is not used.  posf is 1 - posterm, exactly (both are exact in
+// double); only the events that are not the site's primary base class use it.
+__device__ __forceinline__ Terms table_terms(const float *qt, const double *pt, int qpos, int q2pos, int tpi, int lclip, int clen, float fl) {
     Terms t;
+    const uint32_t lrow = qtab_row(fl) + (uint32_t)(QTAB_MID + qpos);
+    t.d3pterm = __ldg(qt + (lrow - (uint32_t)tpi));
+    t.q2term = __ldg(qt + (lrow - (uint32_t)q2pos));
+    t.posterm = __ldg(pt + (((uint32_t)clen << QTAB_SHIFT) + (uint32_t)(QTAB_MID + qpos) - (uint32_t)lclip));
+    t.posf = __double2float_rn(__dsub_rn(1.0, t.posterm));
+    return t;
+}
+template <bool QTAB>
+__device__ __forceinline__ Terms event_terms(const float *qt, const double *pt, bool fast, int qpos, int q2pos, int tpi, int lclip,
+                                             int clen, float fl, float fclen, float rcp_l, float rcp_c) {
+    Terms t;
+    if (fast && QTAB) return table_terms(qt, pt, qpos, q2pos, tpi, lclip, clen, fl);
     const float a_3p = (float)abs(qpos - tpi);
     if (fast) {
         t.d3pterm = div_small(a_3p, fl, rcp_l);
@@ -588,7 +653,9 @@ __device__ __forceinline__ Terms event_terms(bool fast, int qpos, int q2pos, int
 // event_terms for an FM_HOT read, from its staged descriptor words q1 (mmq,clen,lclip,tpi), q2 (q2,nmfrac,se,fl) and
 // q4 (rcp_l,rcp_clen,fclen,inc).  The Q2 term only counts when the read has a Q2 position, which for most forward reads IS the
 // effective 3' end (R:...:229-238); it is not tested here, a read without one never adds the term.
-__device__ __forceinline__ Terms hot_terms(const int4 &q1, const int4 &q2, const int4 &q4, int qpos) {
+template <bool QTAB>
+__device__ __forceinline__ Terms hot_terms(const PileupParams &P, const int4 &q1, const int4 &q2, const int4 &q4, int qpos) {
+    if (QTAB) return table_terms(P.qtab_q, P.qtab_p, qpos, q2.x, q1.w, q1.z, q1.y, __int_as_float(q2.w));
     Terms t;
     const float fl = __int_as_float(q2.w), rcp_l = __int_as_float(q4.x);
     t.d3pterm = div_small((float)abs(qpos - q1.w), fl, rcp_l);
@@ -717,7 +784,7 @@ __device__ __forceinline__ int32_t sec_append(const Pool &R, uint32_t slot, int3
 // one event of BasicStat::process_read into a pool record (slow, exact IEEE path)
 __device__ __forceinline__ void sec_accumulate(const ReadDesc *desc, SecRec &r, int32_t read, int qpos, uint32_t bq, bool is_indel) {
     const ReadDesc d = desc[read];
-    const Terms t = event_terms(false, qpos, d.q2, d.tpi, d.lclip, d.clen, d.fl, d.fclen, 0.f, 0.f);
+    const Terms t = event_terms<false>(nullptr, nullptr, false, qpos, d.q2, d.tpi, d.lclip, d.clen, d.fl, d.fclen, 0.f, 0.f);
     uint32_t w[N_STATS];
     const bool has_q2 = event_words(w, d.fm, d.se, d.nmfrac, d.mmq, d.clen, d.q2, is_indel ? 0u : bq, t);
     stats_add([&](int k) -> uint32_t & { return r.stats[k]; }, w, has_q2);
@@ -839,7 +906,7 @@ __device__ __forceinline__ void off_primary_event(const PileupParams &P, uint32_
     const int4 q1 = lds128(da + 16u);                            // mmq,clen,lclip,tpi
     const int4 q2 = lds128(da + 32u);                            // q2,nmfrac,se,fl
     const int4 q4 = lds128(da + 64u);                            // rcp_l, rcp_clen, fclen
-    const Terms t = event_terms(fast, qpos, q2.x, q1.w, q1.z, q1.y, __int_as_float(q2.w), __int_as_float(q4.z),
+    const Terms t = event_terms<USE_QTAB && !PER_LIB>(P.qtab_q, P.qtab_p, fast, qpos, q2.x, q1.w, q1.z, q1.y, __int_as_float(q2.w), __int_as_float(q4.z),
                                 __int_as_float(q4.x), __int_as_float(q4.y));
     uint32_t w[N_STATS];
     const bool has_q2 = event_words(w, fm, q2.z, __int_as_float(q2.y), q1.x, q1.y, q2.x, bq, t);
@@ -889,7 +956,7 @@ __device__ __forceinline__ void hot_pair(const PileupParams &P, uint32_t (*sacc)
     const int4 q1a = lds128(da + 16u), q1b = lds128(db + 16u);    // mmq,clen,lclip,tpi
     const int4 q2a = lds128(da + 32u), q2b = lds128(db + 32u);    // q2,nmfrac,se,fl
     const int4 q4a = lds128(da + 64u), q4b = lds128(db + 64u);    // rcp_l, rcp_clen, fclen, inc
-    const Terms t_a = hot_terms(q1a, q2a, q4a, qpos_a), t_b = hot_terms(q1b, q2b, q4b, qpos_b);
+    const Terms t_a = hot_terms<USE_QTAB && !PER_LIB>(P, q1a, q2a, q4a, qpos_a), t_b = hot_terms<USE_QTAB && !PER_LIB>(P, q1b, q2b, q4b, qpos_b);
     acc_primary(S.acc, pk3, pkmb, prim_a, fm_a, bq_a, q1a, q2a, q4a, t_a);
     acc_primary(S.acc, pk3, pkmb, prim_b, fm_b, bq_b, q1b, q2b, q4b, t_b);
 
@@ -983,7 +1050,7 @@ __device__ __forceinline__ void process_chunk(const PileupParams &P, const Stage
                 const int4 q1 = lds128(da + 16u);                // mmq,clen,lclip,tpi
                 const int4 q2 = lds128(da + 32u);                // q2,nmfrac,se,fl
                 const int4 q4 = lds128(da + 64u);                // rcp_l, rcp_clen, fclen, inc
-                acc_primary(S.acc, pk3, pkmb, true, fm, bq, q1, q2, q4, hot_terms(q1, q2, q4, qpos));
+                acc_primary(S.acc, pk3, pkmb, true, fm, bq, q1, q2, q4, hot_terms<USE_QTAB && !PER_LIB>(P, q1, q2, q4, qpos));
                 continue;
             }
         } else {
@@ -1024,7 +1091,7 @@ __device__ __forceinline__ void process_chunk(const PileupParams &P, const Stage
         const int4 q1 = lds128(da + 16u);                        // mmq,clen,lclip,tpi
         const int4 q2 = lds128(da + 32u);                        // q2,nmfrac,se,fl
         const int4 q4 = lds128(da + 64u);                        // rcp_l, rcp_clen, fclen, inc
-        const Terms t = event_terms((fm & FM_FASTDIV) != 0, qpos, q2.x, q1.w, q1.z, q1.y, __int_as_float(q2.w), __int_as_float(q4.z),
+        const Terms t = event_terms<USE_QTAB && !PER_LIB>(P.qtab_q, P.qtab_p, (fm & FM_FASTDIV) != 0, qpos, q2.x, q1.w, q1.z, q1.y, __int_as_float(q2.w), __int_as_float(q4.z),
                                     __int_as_float(q4.x), __int_as_float(q4.y));
         acc_primary(S.acc, pk3, pkmb, true, fm, bq, q1, q2, q4, t);
     }
@@ -1250,8 +1317,11 @@ cudaError_t launch_pileup(const PileupParams &p, cudaStream_t s) {
     const int64_t slots = std::max<int64_t>((int64_t)sms * BRC_K1_CTAS_PER_SM - reserve, sms);
     const unsigned grid = (unsigned)std::min<int64_t>(n_work, slots);
     const size_t smem = sizeof(PileupSmem);
-    if (p.per_lib) pileup_kernel<true><<<grid, K1_THREADS, smem, s>>>(p);
-    else pileup_kernel<false><<<grid, K1_THREADS, smem, s>>>(p);
+    PileupParams q = p;
+    if (USE_QTAB && !p.per_lib)
+        if (cudaError_t e = quotient_tables(&q.qtab_q, &q.qtab_p)) return e;
+    if (p.per_lib) pileup_kernel<true><<<grid, K1_THREADS, smem, s>>>(q);
+    else pileup_kernel<false><<<grid, K1_THREADS, smem, s>>>(q);
     return cudaGetLastError();
 }
 
@@ -1453,7 +1523,7 @@ __global__ void __launch_bounds__(DEEP_THREADS, 2) deep_site_kernel(PileupParams
             const uint32_t nw = (indel != 0 ? 1u : 0u) + (base_part ? 1u : 0u);   // process_read calls that warn
             warn_nm += nw * ((fm >> 25) & 1u); warn_sm += nw * ((fm >> 26) & 1u);
             const uint32_t base = base_class(bytev[sg], qpos);
-            const Terms t = event_terms((fm & FM_FASTDIV) != 0, qpos, d.q2, d.tpi, d.lclip, d.clen, d.fl, d.fclen, d.rcp_l, d.rcp_clen);
+            const Terms t = event_terms<false>(nullptr, nullptr, (fm & FM_FASTDIV) != 0, qpos, d.q2, d.tpi, d.lclip, d.clen, d.fl, d.fclen, d.rcp_l, d.rcp_clen);
             // phase 2 adds every word: for a read without a Q2 position the Q2 words are 0, and + 0.0f leaves the sum unchanged
             event_words(w[sg], fm, d.se, d.nmfrac, d.mmq, d.clen, d.q2, bq, t);
             emeta[sg] = base | (indel != 0 ? 8u : 0u) | (base_part ? 16u : 0u) | (bq << 8);
@@ -1633,13 +1703,23 @@ cudaError_t launch_deep_sites(const PileupParams &p, cudaStream_t s) {
 }
 
 // ---------------------------------------------------------------------------------------------
-// self-test: div_small / round_to_f32_precision / f32_to_f64_nonneg against the IEEE intrinsics
+// self-test: div_small / round_to_f32_precision / f32_to_f64_nonneg and the quotient tables against the IEEE intrinsics
 // ---------------------------------------------------------------------------------------------
-__global__ void fastmath_selftest_kernel(int max_b, unsigned long long *bad) {
+__global__ void fastmath_selftest_kernel(int max_b, unsigned long long *bad, const float *qt, const double *pt) {
     const int b = blockIdx.x + 1;
     if (b > max_b) return;
     const float fb = (float)b, rcp = __frcp_rn(fb);
     unsigned long long nbad = 0;
+    // every entry of row b of both tables (brc_device.cuh: column QTAB_MID + j); rows exist up to FASTDIV_MAX
+    for (int c = threadIdx.x; b <= FASTDIV_MAX && c < 1 << QTAB_SHIFT; c += blockDim.x) {
+        const int j = c - QTAB_MID;
+        const int64_t i = ((int64_t)b << QTAB_SHIFT) + c;
+        if (__float_as_uint(qt[i]) != __float_as_uint(__fdiv_rn((float)abs(j), fb))) nbad++;
+        const double want = __dsub_rn(1.0, (double)__fdiv_rn((float)abs(2 * j - b), fb));
+        if (__double_as_longlong(pt[i]) != __double_as_longlong(want)) nbad++;
+        // posf as fast_terms recovers it from the P entry
+        if (__float_as_uint(__double2float_rn(__dsub_rn(1.0, pt[i]))) != __float_as_uint(__fdiv_rn((float)abs(2 * j - b), fb))) nbad++;
+    }
     // every numerator the hot path can form for any divisor: |2 (qpos - left_clip) - clipped_length| reaches 2 (l_qseq - 1) when a
     // soft clip after a hard clip counts as a right clip (5H100S10M: 190..208 over 10)
     for (int a = threadIdx.x; a <= 2 * FASTDIV_MAX + 2; a += blockDim.x) {
@@ -1661,7 +1741,9 @@ __global__ void fastmath_selftest_kernel(int max_b, unsigned long long *bad) {
 }
 
 cudaError_t launch_fastmath_selftest(int max_b, unsigned long long *d_bad, cudaStream_t s) {
-    fastmath_selftest_kernel<<<max_b, 128, 0, s>>>(max_b, d_bad);
+    const float *qt = nullptr; const double *pt = nullptr;
+    if (cudaError_t e = quotient_tables(&qt, &pt)) return e;
+    fastmath_selftest_kernel<<<max_b, 128, 0, s>>>(max_b, d_bad, qt, pt);
     return cudaGetLastError();
 }
 

@@ -118,7 +118,7 @@ EXPORTS = [
     "brc_begin_region", "brc_push_read", "brc_push_reads", "brc_end_region", "brc_decode_bam_span", "brc_push_bam_span", "brc_fetch_decoded_batch", "brc_compute", "brc_get_results",
     "brc_get_warning_counts", "brc_format_text", "brc_format_window", "brc_write_text", "brc_set_queue_carry", "brc_plan_device", "brc_run_device", "brc_device_packed_results", "brc_get_packed_results",
     "brc_fetch_device_results", "brc_last_launch_count", "brc_last_h2d_bytes", "brc_host_alloc", "brc_host_free", "brc_last_stage_ms", "brc_selftest_fastmath",
-    "brc_get_reference_codes", "brc_get_read_descriptors",
+    "brc_get_reference_codes", "brc_get_read_descriptors", "brc_get_quotient_rows",
     "brc_set_site_filter", "brc_get_selected_results", "brc_set_allele_queries", "brc_get_allele_answers", "brc_last_results_kind",
     "brc_set_complex_queries", "brc_get_complex_answers",
 ]
@@ -175,6 +175,8 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
     lib.brc_get_reference_codes.restype = C.c_int64
     lib.brc_get_read_descriptors.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.POINTER(C.c_int64)]
     lib.brc_get_read_descriptors.restype = C.c_int64
+    lib.brc_get_quotient_rows.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
+    lib.brc_get_quotient_rows.restype = C.c_int64
     lib.brc_last_launch_count.argtypes = [C.c_void_p]
     lib.brc_last_h2d_bytes.argtypes = [C.c_void_p]
     lib.brc_last_h2d_bytes.restype = C.c_int64
@@ -545,6 +547,14 @@ class Engine:
         self._check(min(int(self.lib.brc_get_read_descriptors(self.h, desc.ctypes.data, n, lo.ctypes.data, hi.ctypes.data, nt.value,
                                                               C.byref(nt))), 0))
         return desc, lo, hi
+
+    def quotient_rows(self, d_lo: int, d_hi: int):
+        """(q, p): rows d_lo..d_hi of the device's quotient tables (brc_get_quotient_rows), each a (rows, 4096) array, float32 and
+        float64."""
+        q = np.empty((d_hi - d_lo + 1, 4096), dtype=np.float32)
+        p = np.empty(q.shape, dtype=np.float64)
+        self._check(min(int(self.lib.brc_get_quotient_rows(self.h, d_lo, d_hi, q.ctypes.data, p.ctypes.data)), 0))
+        return q, p
 
     def plan_device(self, regions: Sequence[CRegion], n_reads_cap: int, n_sec_cap: int = 0):
         arr = (CRegion * len(regions))(*regions)

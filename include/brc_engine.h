@@ -406,9 +406,14 @@ BRC_API int brc_plan_device(brc_engine *e, const brc_region *regions, int64_t n_
 BRC_API int brc_run_device(brc_engine *e, const brc_read_batch *dev_batch, const int32_t *dev_region_of_read, void *stream);
 BRC_API int brc_device_packed_results(brc_engine *e, brc_packed_results *out);
 BRC_API int brc_fetch_device_results(brc_engine *e, void *stream);
-/* Self-test of the kernels' exact-arithmetic shortcuts (reciprocal division, float<->double bit casts)
+/* Self-test of the kernels' exact-arithmetic shortcuts (reciprocal division, float<->double bit casts, the quotient tables)
  * against the IEEE intrinsics for every divisor 1..max_b; returns the number of mismatches (0 = ok). */
 BRC_API int64_t brc_selftest_fastmath(brc_engine *e, int32_t max_b);
+/* Rows d_lo..d_hi (1 <= d_lo <= d_hi <= 2048) of the device's quotient tables, which the pileup kernels read in place of divisions
+ * (brc_device.cuh QTAB_*): 4096 entries per row, entry c of row d being, with j = c - 2048,
+ *   q: RN((float)|j| / (float)d)    p: 1.0 - (double)RN((float)|2 j - d| / (float)d).
+ * Copies (d_hi - d_lo + 1) * 4096 floats to `q` and as many doubles to `p`; returns that count or a negative status. */
+BRC_API int64_t brc_get_quotient_rows(brc_engine *e, int32_t d_lo, int32_t d_hi, float *q, double *p);
 /* The packed reference window of contig `tid` as the kernels read it: seq_nt16 codes, two per byte, first base in the high
  * nibble, then 0xFF padding (win_len / 2 + 32 bytes in all).  Waits for the device, copies min(cap, that size) bytes to `out`
  * and returns the full size, or a negative status (BRC_E_NO_REFERENCE when the contig has none). */
