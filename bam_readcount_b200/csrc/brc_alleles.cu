@@ -60,12 +60,7 @@ __global__ void __launch_bounds__(ALLELE_CTA) allele_query_kernel(AlleleParams P
     const int64_t NS = P.n_slots, s = Q.site;
     const uint32_t w1 = P.words[NS + s];
     if (kind >= 6u || (w1 & 7u) != kind) return;   // not the primary held in the words (pool records came from the record pass)
-    const uint32_t w0 = P.words[s], w2 = P.words[2 * NS + s], w3 = P.words[3 * NS + s];
-    const uint32_t count = (w0 >> 16) & 0xFFu, plus = w0 >> 24;
-    A.stats[BRC_S_COUNT] = count; A.stats[BRC_S_MAPQ] = w1 >> 16; A.stats[BRC_S_BASEQ] = w2 & 0xFFFFu; A.stats[BRC_S_SE_MAPQ] = w2 >> 16;
-    A.stats[BRC_S_PLUS] = plus; A.stats[BRC_S_MINUS] = count - plus; A.stats[BRC_S_POS_FRAC] = P.words[4 * NS + s];
-    A.stats[BRC_S_NM_FRAC] = P.words[5 * NS + s]; A.stats[BRC_S_MMQS] = w3 >> 16; A.stats[BRC_S_NQ2] = (w1 >> 8) & 0xFFu;
-    A.stats[BRC_S_Q2_DIST] = P.words[6 * NS + s]; A.stats[BRC_S_CLIP_LEN] = w3 & 0xFFFFu; A.stats[BRC_S_3P_DIST] = P.words[7 * NS + s];
+    unpack_primary(P.words, NS, s, A.stats);   // one library row: RS = NS
 }
 
 }  // namespace

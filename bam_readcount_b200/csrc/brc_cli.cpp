@@ -62,6 +62,13 @@ void usage() {
                 "                                        the reference base, an insertion or a deletion) has a count of at least N\n"
                 "  --min-alt-fraction F                  (this host) ... and of at least F times the site's depth (0 <= F <= 1; without\n"
                 "                                        --min-alt-count the count must be at least 1).  Printed lines are unchanged\n"
+                "  --alt-min NAME=V                      (this host) ... and that allele's field NAME, as the line prints it, is at least V\n"
+                "                                        (V: digits with at most two decimals; NAME: count, avg_mapping_quality,\n"
+                "                                        avg_basequality, avg_se_mapping_quality, num_plus_strand, num_minus_strand,\n"
+                "                                        avg_pos_as_fraction, avg_num_mismatches_as_fraction, avg_sum_mismatch_qualities,\n"
+                "                                        num_q2_containing_reads, avg_distance_to_q2_start_in_q2_reads, avg_clipped_length,\n"
+                "                                        avg_distance_to_effective_3p_end).  Repeatable; alone it means count >= 1\n"
+                "  --alt-max NAME=V                      (this host) ... and at most V\n"
                 "  --bam-list FILE                       (this host) run many samples in one process.  Each line of FILE is\n"
                 "                                        INPUT<TAB>OUT or INPUT<TAB>OUT<TAB>ERR (ERR defaults to OUT.log); OUT and ERR get\n"
                 "                                        exactly what `brc-readcount <options> INPUT <regions>` prints on STDOUT and\n"
@@ -71,7 +78,7 @@ void usage() {
                 "                                        each record's REF and SNV / insertion / deletion ALT alleles as FORMAT fields BRC_DP,\n"
                 "                                        BRC_AD, BRC_ADF, BRC_ADR and BRC_AF: the values the line of each record's site prints\n"
                 "                                        (STDERR is that of -l over the records' sites).  Not with -l, regions, -p,\n"
-                "                                        --min-alt-*, --shard or --bam-list\n"
+                "                                        --min-alt-*, --alt-min/--alt-max, --shard or --bam-list\n"
                 "  --vcf-sample NAME                     (this host) the sample column that takes the values (required with several; names\n"
                 "                                        the column added to a sites-only VCF)\n"
                 "  --vcf-samples FILE                    (this host) with --vcf and no positional argument: annotate several sample columns\n"
@@ -93,9 +100,35 @@ struct Options {   // everything on the command line except the inputs: the same
     std::vector<std::string> region_args;
     int shard_rank = 0, shard_count = 1;
     bool site_filter = false; brc_site_filter filter{};
+    bool has_bounds = false; brc_entry_bounds bounds{};   // --alt-min / --alt-max (brc_set_site_filter_bounds)
     bool decode_only = false, device_decode = false, timing = false;
     bool dist_refused() const { return dist_arg == "1" || dist_arg == "true"; }
 };
+
+// the allele entry's 13 numbers by bam-readcount's column names, in print order (BRC_S_*)
+const char *const kEntryFields[BRC_N_STATS] = {
+    "count", "avg_mapping_quality", "avg_basequality", "avg_se_mapping_quality", "num_plus_strand", "num_minus_strand",
+    "avg_pos_as_fraction", "avg_num_mismatches_as_fraction", "avg_sum_mismatch_qualities", "num_q2_containing_reads",
+    "avg_distance_to_q2_start_in_q2_reads", "avg_clipped_length", "avg_distance_to_effective_3p_end"};
+
+// --alt-min / --alt-max NAME=V: V is ^[0-9]+(\.[0-9]{1,2})?$, kept exactly as hundredths.  False (message on stderr) when malformed.
+bool parse_bound(const char *opt, const char *arg, uint32_t &set, int64_t *val) {
+    const char *eq = std::strchr(arg, '=');
+    if (!eq) { std::fprintf(stderr, "%s wants NAME=V, got '%s'\n", opt, arg); return false; }
+    const std::string name(arg, (size_t)(eq - arg));
+    int k = 0;
+    while (k < BRC_N_STATS && name != kEntryFields[k]) ++k;
+    if (k == BRC_N_STATS) { std::fprintf(stderr, "%s: unknown field '%s' (NAME=V with NAME one of the allele entry's column names)\n", opt, name.c_str()); return false; }
+    const char *v = eq + 1, *p = v;
+    int64_t h = 0; int ip = 0, fp = -1;
+    for (; *p >= '0' && *p <= '9'; ++p, ++ip) if (ip < 15) h = h * 10 + (*p - '0');
+    if (*p == '.') for (fp = 0, ++p; *p >= '0' && *p <= '9'; ++p) { if (++fp <= 2) h = h * 10 + (*p - '0'); }
+    if (ip == 0 || ip > 15 || *p || fp == 0 || fp > 2) { std::fprintf(stderr, "%s %s: V wants digits with at most two decimals\n", opt, name.c_str()); return false; }
+    for (int f = fp < 0 ? 0 : fp; f < 2; ++f) h *= 10;
+    if ((set >> k) & 1u) { std::fprintf(stderr, "%s %s is given twice\n", opt, name.c_str()); return false; }
+    set |= 1u << k; val[k] = h;
+    return true;
+}
 
 double now() { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
 
@@ -358,7 +391,9 @@ struct Engines {
         brc_engine *eng = nullptr;
         const int rc = warm_rc != BRC_OK ? warm_rc : brc_create(&c, &eng);
         if (rc != BRC_OK) { std::fprintf(err, "brc_create: %s\n", brc_strerror(rc)); return nullptr; }
-        if (o.site_filter && brc_set_site_filter(eng, &o.filter) != BRC_OK) { std::fprintf(err, "brc_set_site_filter: %s\n", brc_last_error(eng)); brc_destroy(eng); return nullptr; }
+        if (o.site_filter && brc_set_site_filter_bounds(eng, &o.filter, o.has_bounds ? &o.bounds : nullptr) != BRC_OK) {
+            std::fprintf(err, "brc_set_site_filter: %s\n", brc_last_error(eng)); brc_destroy(eng); return nullptr;
+        }
         Handle &h = handles[key]; h.eng = eng;
         return &h;
     }
@@ -800,7 +835,7 @@ int main(int argc, char **argv) {
                           {"per-library", 0, 0, 'p'}, {"max-warnings", 1, 0, 'w'}, {"insertion-centric", 0, 0, 'i'}, {"shard", 1, 0, 1000},
                           {"min-alt-count", 1, 0, 1001}, {"min-alt-fraction", 1, 0, 1002}, {"bam-list", 1, 0, 1003},
                           {"vcf", 1, 0, 1004}, {"vcf-sample", 1, 0, 1005}, {"vcf-samples", 1, 0, 1006},
-                          {"vcf-complex", 0, 0, 1007}, {0, 0, 0, 0}};
+                          {"vcf-complex", 0, 0, 1007}, {"alt-min", 1, 0, 1008}, {"alt-max", 1, 0, 1009}, {0, 0, 0, 0}};
     long min_alt_count = 0; double min_alt_fraction = -1.0;       // site filter (brc_set_site_filter); off unless one is given
     bool help = false, version = false;
     for (int c; (c = getopt_long(argc, argv, "hvq:b:d:l:f:D:pw:i", lo, nullptr)) != -1;) {
@@ -828,10 +863,17 @@ int main(int argc, char **argv) {
         case 1005: vcf_sample = optarg; vcf_sample_given = true; break;
         case 1006: vcf_samples = optarg; break;
         case 1007: o.vcf_complex = true; break;
+        case 1008: if (!parse_bound("--alt-min", optarg, o.bounds.lo_set, o.bounds.lo)) return 1; break;
+        case 1009: if (!parse_bound("--alt-max", optarg, o.bounds.hi_set, o.bounds.hi)) return 1; break;
         default: usage(); return 1;
         }
     }
-    o.site_filter = min_alt_count > 0 || min_alt_fraction >= 0.0;
+    for (int k = 0; k < BRC_N_STATS; ++k)
+        if (((o.bounds.lo_set & o.bounds.hi_set) >> k & 1u) && o.bounds.lo[k] > o.bounds.hi[k]) {
+            std::fprintf(stderr, "--alt-min %s is larger than --alt-max %s\n", kEntryFields[k], kEntryFields[k]); return 1;
+        }
+    o.has_bounds = (o.bounds.lo_set | o.bounds.hi_set) != 0;
+    o.site_filter = min_alt_count > 0 || min_alt_fraction >= 0.0 || o.has_bounds;
     o.filter.min_alt_count = (int32_t)std::max<long>(min_alt_count, 1); o.filter.min_alt_fraction = std::max(min_alt_fraction, 0.0);
     if (version) { std::printf("bam-readcount version: b200 (engine ABI %d)\n", brc_abi_version()); return 1; }   // R:...:467-470 (exit 1)
     if (help || (optind >= argc && bam_list.empty() && vcf_samples.empty())) { usage(); return 1; }                 // R:...:472-475
@@ -847,7 +889,7 @@ int main(int argc, char **argv) {
     std::vector<ListSample> vcf_list;     // --vcf-samples
     std::vector<std::string> vcf_names;
     if (!vcf_path.empty()) {
-        const char *clash = !o.fn_pos.empty() ? "-l" : optind + 1 < argc ? "positional regions" : o.per_lib ? "-p" : o.site_filter ? "--min-alt-count/--min-alt-fraction"
+        const char *clash = !o.fn_pos.empty() ? "-l" : optind + 1 < argc ? "positional regions" : o.per_lib ? "-p" : o.has_bounds ? "--alt-min/--alt-max" : o.site_filter ? "--min-alt-count/--min-alt-fraction"
                           : shard_given ? "--shard" : !bam_list.empty() ? "--bam-list" : nullptr;
         if (clash) { std::fprintf(stderr, "--vcf cannot be combined with %s\n", clash); return 1; }
         if (vcf_sample_given) vcf_names.push_back(vcf_sample);

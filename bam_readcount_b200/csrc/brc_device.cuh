@@ -13,6 +13,7 @@
 #include <cuda_runtime.h>
 
 #include "../../include/brc_engine.h"
+#include "brc_fmt_num.h"
 
 namespace brc {
 
@@ -244,6 +245,64 @@ __host__ __device__ inline bool site_passes(uint64_t best_alt, uint64_t depth, i
     return best_alt >= (uint64_t)min_alt_count && (double)best_alt >= min_alt_fraction * (double)depth;
 }
 
+// Entry bounds (brc_set_site_filter_bounds): the entry that makes a line pass must satisfy every bound that is set, on its fields
+// as the line prints them, in hundredths.  Evaluated by the device selection (pool records and the packed primaries) and by the
+// host emitter (lines it forms itself), like site_passes.
+using EntryBounds = brc_entry_bounds;
+constexpr uint32_t BOUNDS_MASK = (1u << N_STATS) - 1u;
+
+// The float32 quotient put_stat (brc_format.cpp) prints for a sum over a count.  Both evaluators round it once to nearest:
+// __fdiv_rn is the IEEE division on the device whatever -prec-div says, the library is built with --fmad=false so nothing is
+// contracted around it, and the host's `/` on floats is the IEEE division.  The u32 sums are converted to float with
+// round-to-nearest on both sides too (__uint2float_rn, the host conversion).
+__host__ __device__ inline float stat_u2f(uint32_t v) {
+#ifdef __CUDA_ARCH__
+    return __uint2float_rn(v);
+#else
+    return (float)v;
+#endif
+}
+__host__ __device__ inline float stat_bits(uint32_t v) { float f; std::memcpy(&f, &v, 4); return f; }
+__host__ __device__ inline float stat_quot(float num, uint32_t den) {
+#ifdef __CUDA_ARCH__
+    return __fdiv_rn(num, __uint2float_rn(den));
+#else
+    return num / (float)den;
+#endif
+}
+// a printed average in hundredths (put_f2's digits, signed); no average of the engine's sums reaches 2^54, which saturates
+__host__ __device__ inline int64_t printed_hundredths(float q) {
+    const uint64_t h = f2_hundredths(q);
+    if (h > (uint64_t)INT64_MAX) return INT64_MAX;
+    return q < 0.0f ? -(int64_t)h : (int64_t)h;
+}
+// Field k (BRC_S_*) of an entry as put_stat prints it, in hundredths.
+__host__ __device__ inline int64_t entry_field(const uint32_t v[N_STATS], int k, bool is_indel) {
+    const uint32_t n = v[BRC_S_COUNT];
+    if (n == 0) return 0;                                     // the all-zero entry
+    switch (k) {
+    case BRC_S_COUNT: case BRC_S_PLUS: case BRC_S_MINUS: case BRC_S_NQ2: return (int64_t)v[k] * 100;
+    case BRC_S_BASEQ: return is_indel ? 0 : printed_hundredths(stat_quot(stat_u2f(v[k]), n));
+    case BRC_S_MAPQ: case BRC_S_SE_MAPQ: case BRC_S_MMQS: case BRC_S_CLIP_LEN: return printed_hundredths(stat_quot(stat_u2f(v[k]), n));
+    case BRC_S_Q2_DIST: return v[BRC_S_NQ2] ? printed_hundredths(stat_quot(stat_bits(v[k]), v[BRC_S_NQ2])) : 0;
+    default: return printed_hundredths(stat_quot(stat_bits(v[k]), n));   // POS_FRAC, NM_FRAC, 3P_DIST: float sums
+    }
+}
+// Every bound that is set holds on the entry; only the fields with a bound are evaluated.
+__host__ __device__ inline bool entry_within(const uint32_t v[N_STATS], bool is_indel, const EntryBounds &B) {
+    const uint32_t set = B.lo_set | B.hi_set;
+    if (!set) return true;
+#ifdef __CUDA_ARCH__
+#pragma unroll
+#endif
+    for (int k = 0; k < N_STATS; ++k) {
+        if (!((set >> k) & 1u)) continue;
+        const int64_t x = entry_field(v, k, is_indel);
+        if ((((B.lo_set >> k) & 1u) && x < B.lo[k]) || (((B.hi_set >> k) & 1u) && x > B.hi[k])) return false;
+    }
+    return true;
+}
+
 struct SelRegion {         // one region as the selection kernels see it
     int64_t slot_base;
     int32_t n_slots;
@@ -267,6 +326,7 @@ struct SelectParams {
     const RefWin *refs;
     int32_t min_alt_count;
     double min_alt_fraction;
+    EntryBounds bounds;     // no bit set: no bounds
     // per-site scratch, [n_slots] each (best .. esc_np and reg_last, counters zeroed before the pool pass)
     uint32_t *best;         // largest alternative count of the site's pool records
     uint32_t *dsum;         // deletion counts anchored here that print at the next site (extra depth there)
@@ -293,6 +353,17 @@ struct SelectParams {
 // Row r spans site s (column idx = r * n_slots + s): an escaped primary, or ncover > 0.  RS = n_rows * n_slots.
 __device__ __forceinline__ bool row_covers(const uint32_t *words, int64_t RS, int64_t idx) {
     return (words[RS + idx] & 7u) == PB_ESCAPE || (words[idx] & 0xFFu) != 0u;
+}
+// The 13 accumulators of the primary held in the packed words of column idx (word w at words[w * RS + idx]; layout above).
+__device__ __forceinline__ void unpack_primary(const uint32_t *words, int64_t RS, int64_t idx, uint32_t v[N_STATS]) {
+    uint32_t w[N_WORDS];
+#pragma unroll
+    for (int k = 0; k < N_WORDS; ++k) w[k] = words[k * RS + idx];
+    const uint32_t count = (w[0] >> 16) & 0xFFu, plus = w[0] >> 24;
+    v[BRC_S_COUNT] = count; v[BRC_S_MAPQ] = w[1] >> 16; v[BRC_S_BASEQ] = w[2] & 0xFFFFu; v[BRC_S_SE_MAPQ] = w[2] >> 16;
+    v[BRC_S_PLUS] = plus; v[BRC_S_MINUS] = count - plus; v[BRC_S_POS_FRAC] = w[4]; v[BRC_S_NM_FRAC] = w[5];
+    v[BRC_S_MMQS] = w[3] >> 16; v[BRC_S_NQ2] = (w[1] >> 8) & 0xFFu; v[BRC_S_Q2_DIST] = w[6]; v[BRC_S_CLIP_LEN] = w[3] & 0xFFFFu;
+    v[BRC_S_3P_DIST] = w[7];
 }
 // Some row has a read without library at site s: -p abandons the site (no line, and its deletions are never queued).
 __device__ __forceinline__ bool site_abandoned(const uint32_t *words, int n_rows, int64_t NS, int64_t s) {

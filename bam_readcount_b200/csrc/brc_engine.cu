@@ -510,6 +510,7 @@ static int launch_selection(brc_engine *e, cudaStream_t s) {
     P.sec = e->d_sec.as<SecRec>(); P.sec_count = e->d_sec_count.as<int32_t>(); P.sec_cap = e->sec_cap;
     P.regions = e->d_sel_regions.as<SelRegion>(); P.n_regions = R; P.refs = e->d_refs.as<RefWin>();
     P.min_alt_count = e->filter.min_alt_count; P.min_alt_fraction = e->filter.min_alt_fraction;
+    P.bounds = e->bounds;
     P.best = reinterpret_cast<uint32_t *>(b + o_best); P.dsum = P.best + NS; P.dbest = P.dsum + NS; P.esc_np = P.dbest + NS;
     P.reg_last = reinterpret_cast<uint32_t *>(b + o_last); P.counters = reinterpret_cast<unsigned long long *>(b + o_cnt);
     P.keep = reinterpret_cast<uint8_t *>(b + o_keep); P.emit = reinterpret_cast<uint8_t *>(b + o_emit);
@@ -522,6 +523,7 @@ static int launch_selection(brc_engine *e, cudaStream_t s) {
     CU(cudaEventRecord(e->ev[3], s), "event");
     e->sel_params = P;
     e->sel_filter = e->filter;
+    e->sel_bounds = e->bounds;
     return BRC_OK;
 }
 
@@ -1082,11 +1084,26 @@ int brc_last_results_kind(const brc_engine *e) { return e ? e->results_kind() : 
 
 int brc_set_site_filter(brc_engine *e, const brc_site_filter *f) {
     if (!e) return BRC_E_INVALID;
-    if (!f) { e->filter_on = false; e->filter = brc_site_filter{}; return BRC_OK; }
+    if (!f) { e->filter_on = false; e->filter = brc_site_filter{}; e->bounds = brc_entry_bounds{}; return BRC_OK; }
     if (e->answers_on()) return set_error(e, BRC_E_INVALID, "set_site_filter: allele or complex queries are set (brc_reset drops them)");
     if (f->min_alt_count < 1 || f->reserved != 0 || !(f->min_alt_fraction >= 0.0 && f->min_alt_fraction <= 1.0))
         return set_error(e, BRC_E_INVALID, "set_site_filter: min_alt_count must be >= 1 and min_alt_fraction in [0, 1]");
-    e->filter = *f; e->filter_on = true;
+    e->filter = *f; e->filter_on = true; e->bounds = brc_entry_bounds{};
+    return BRC_OK;
+}
+
+int brc_set_site_filter_bounds(brc_engine *e, const brc_site_filter *f, const brc_entry_bounds *b) {
+    if (!e) return BRC_E_INVALID;
+    if (!b) return brc_set_site_filter(e, f);
+    if (!f) return set_error(e, BRC_E_INVALID, "set_site_filter_bounds: bounds need a filter");
+    if ((b->lo_set | b->hi_set) & ~BOUNDS_MASK) return set_error(e, BRC_E_INVALID, "set_site_filter_bounds: a mask bit past BRC_S_3P_DIST");
+    for (int k = 0; k < N_STATS; ++k) {
+        const bool lo = (b->lo_set >> k) & 1u, hi = (b->hi_set >> k) & 1u;
+        if ((lo && b->lo[k] < 0) || (hi && b->hi[k] < 0)) return set_error(e, BRC_E_INVALID, "set_site_filter_bounds: a negative bound");
+        if (lo && hi && b->lo[k] > b->hi[k]) return set_error(e, BRC_E_INVALID, "set_site_filter_bounds: lo > hi on one field");
+    }
+    if (int rc = brc_set_site_filter(e, f)) return rc;
+    e->bounds = *b;
     return BRC_OK;
 }
 

@@ -175,10 +175,12 @@ struct brc_engine {
     // the device to the sites that print a passing line plus their context, and only those cross PCIe.
     bool filter_on = false;
     brc_site_filter filter{};
+    brc_entry_bounds bounds{};                 // brc_set_site_filter_bounds; no bit set: none
     std::vector<brc::SelRegion> sel_regions;   // the selection's region table of the current batch
     brc::DevBuf d_sel, d_sel_regions;          // scratch + compact outputs; region table
     brc::SelectParams sel_params{};            // the last selection ran on these buffers
-    brc_site_filter sel_filter{};              // the filter the selection ran with
+    brc_site_filter sel_filter{};              // the filter and entry bounds the selection ran with
+    brc_entry_bounds sel_bounds{};
     // SELECTED host results: n_sel shipped sites (ids ascending, emit bytes in h_sel), their words in h_words as
     // [N_WORDS][rows*n_sel], their pool records in h_sec with slot = row * n_sel + compact index
     int64_t n_sel = 0, sel_abandoned = 0;

@@ -90,7 +90,8 @@ inline uint32_t nt16(char c) {
 
 // One site: pileup_func's print section.  emit=false only replays the deletion pushes (used to seed a thread's first site).
 // `slot` is the site's column in the result arrays (dense: rg.slot_base + s; sparse: its index among the shipped sites).  With
-// a site filter the line is printed only when the filter's rule holds on it (brc::site_passes, the device selection's rule).
+// a site filter the line is printed only when the filter's rule holds on it (brc::site_passes and brc::entry_within, the device
+// selection's rule).
 void format_site(const View &V, int32_t s, int64_t slot, const char *const *lib_names, EmitState &st, std::string &out, Scratch &W, bool emit) {
     const brc_region &rg = *V.rg;
     const int rows = V.rows; const int64_t NS = V.NS;
@@ -104,6 +105,7 @@ void format_site(const View &V, int32_t s, int64_t slot, const char *const *lib_
     if (emit && V.ref && pos < V.ref->chrom_len && pos >= V.ref->win_beg && pos < V.ref->win_beg + (int64_t)V.ref->seq.size()) rb = V.ref->seq[(size_t)(pos - V.ref->win_beg)];   // a device-only reference window (brc_set_reference_device) has no characters here
     const bool gate = emit && V.csite;
     const uint32_t rcode = gate ? nt16(rb) : 15u;
+    const brc::EntryBounds &bounds = V.e->sel_bounds;   // an entry counts toward best_alt only within them
     uint64_t best_alt = 0;
     for (int r = 0; r < rows; ++r) {
         const int64_t idx = r * NS + slot;
@@ -131,11 +133,13 @@ void format_site(const View &V, int32_t s, int64_t slot, const char *const *lib_
             W.indels.push_back(std::move(in));
         }
         if (emit) for (int j = 0; j < 6; ++j) { rec += '\t'; rec += kNt[j]; rec += ':'; put_stat(rec, have[j] ? &base[j] : nullptr, false); }
-        if (gate) for (int j = 1; j <= 4; ++j) if (have[j] && brc::base_is_alt((uint32_t)j, rcode)) best_alt = std::max<uint64_t>(best_alt, base[j].v[BRC_S_COUNT]);
+        if (gate) for (int j = 1; j <= 4; ++j) if (have[j] && brc::base_is_alt((uint32_t)j, rcode) && brc::entry_within(base[j].v, false, bounds)) best_alt = std::max<uint64_t>(best_alt, base[j].v[BRC_S_COUNT]);
         if (W.indels.size() > 1) std::sort(W.indels.begin(), W.indels.end(), [](const Indel &a, const Indel &b) { return a.allele < b.allele; });
         for (auto &in : W.indels) {
             if (in.allele[0] == '-') { st.q[(size_t)r].push_back(make_qent(rg.tid, pos + 1, in.st, in.allele)); st.q_exists[(size_t)r] = 1; }
-            else if (emit) { rec += '\t'; rec += in.allele; rec += ':'; put_stat(rec, &in.st, true); best_alt = std::max<uint64_t>(best_alt, in.st.v[BRC_S_COUNT]); }
+            else if (emit) { rec += '\t'; rec += in.allele; rec += ':'; put_stat(rec, &in.st, true);
+                if (gate && brc::entry_within(in.st.v, true, bounds)) best_alt = std::max<uint64_t>(best_alt, in.st.v[BRC_S_COUNT]);
+            }
         }
         if (emit && st.q_exists[(size_t)r]) {          // IndelQueue::process(tid, pos, record)
             auto &q = st.q[(size_t)r];
@@ -143,7 +147,7 @@ void format_site(const View &V, int32_t s, int64_t slot, const char *const *lib_
             while (!q.empty() && q.front().tid == rg.tid && q.front().pos == pos) {
                 rec += '\t'; rec += q.front().allele; rec += ':'; put_stat(rec, qstat(q.front()), true);
                 extra_depth += q.front().st[BRC_S_COUNT];
-                best_alt = std::max<uint64_t>(best_alt, q.front().st[BRC_S_COUNT]);
+                if (gate && brc::entry_within(q.front().st, true, bounds)) best_alt = std::max<uint64_t>(best_alt, q.front().st[BRC_S_COUNT]);
                 q.pop_front();
             }
         }

@@ -3,8 +3,10 @@
 // Runs on the launch stream after the pileup kernels, over the packed records they left in HBM, and leaves behind only what
 // the text emitter needs for the lines that pass the filter:
 //   sel_pool_kernel    one thread per secondary-pool record: largest alternative count per site, the depth and largest count a
-//                      site's deletions add to the next site's line, the npass of escaped primaries
-//   sel_site_kernel    one thread per site: depth, largest alternative count, the rule; keep bits
+//                      site's deletions add to the next site's line, the npass of escaped primaries (counts only of entries
+//                      within the entry bounds)
+//   sel_site_kernel    one thread per site: depth, largest alternative count (the packed primaries judged by the entry bounds
+//                      too), the rule; keep bits
 //   sel_flag_kernel    one thread per site: the emit byte (1 passes; 2 keep-all range, or the last live site of an argv region
 //                      that a library row covers); shipped = emit byte set, or the left neighbour of a site with one (the
 //                      emitter replays its deletion pushes, so the line and its depth are whole)
@@ -50,17 +52,23 @@ __global__ void __launch_bounds__(SEL_CTA) sel_pool_kernel(SelectParams P) {
     const int64_t slot = rec.slot, r = slot / P.n_slots, s = slot - r * P.n_slots;
     const uint32_t kind = rec.kind_len & 0xFFu, cnt = rec.stats[0];
     // a deletion prints in the same row's block of the next site when that row spans it (same region: sel_site_kernel)
-    if (pool_depth_term(P.words, P.n_rows, P.n_slots, rec, P.dsum, P.esc_np)) { atomicMax(&P.dbest[s], cnt); return; }
+    // an entry counts only when it satisfies the entry bounds (none set: every entry does)
+    if (pool_depth_term(P.words, P.n_rows, P.n_slots, rec, P.dsum, P.esc_np)) {
+        if (entry_within(rec.stats, true, P.bounds)) atomicMax(&P.dbest[s], cnt);
+        return;
+    }
     if (kind == (uint32_t)KIND_DEL) return;
-    if (kind == (uint32_t)KIND_INS) { atomicMax(&P.best[s], cnt); return; }
+    if (kind == (uint32_t)KIND_INS) { if (entry_within(rec.stats, true, P.bounds)) atomicMax(&P.best[s], cnt); return; }
     const uint32_t bc = kind >= KIND_WIDE ? kind - KIND_WIDE : kind;
     if (bc >= 1u && bc <= 4u && cnt > 0u) {
         const SelRegion R = P.regions[region_of(P, s)];
-        if (base_is_alt(bc, ref_code(P, R, R.first_pos + (s - R.slot_base)))) atomicMax(&P.best[s], cnt);
+        if (base_is_alt(bc, ref_code(P, R, R.first_pos + (s - R.slot_base))) && entry_within(rec.stats, false, P.bounds))
+            atomicMax(&P.best[s], cnt);
     }
 }
 
-__global__ void __launch_bounds__(SEL_CTA) sel_site_kernel(SelectParams P) {
+// 5 CTAs per SM: 48 registers, no spills with the entry bounds
+__global__ void __launch_bounds__(SEL_CTA, 5) sel_site_kernel(SelectParams P) {
     __shared__ int64_t s_g0;
     __shared__ unsigned int s_last[SEL_LAST_ROWS];
     const int64_t s = (int64_t)blockIdx.x * SEL_CTA + threadIdx.x;
@@ -78,9 +86,17 @@ __global__ void __launch_bounds__(SEL_CTA) sel_site_kernel(SelectParams P) {
         const SiteLine L = site_line(P.words, P.n_rows, NS, s, o > 0, P.dsum, P.esc_np);
         const uint64_t depth = L.depth;
         uint64_t best = P.best[s];
+        const bool bounded = (P.bounds.lo_set | P.bounds.hi_set) != 0u;
         for (int r = 0; r < P.n_rows; ++r) {      // escaped primaries (code PB_ESCAPE, never alternative) came from the pool pass
-            const uint32_t w0 = P.words[(int64_t)r * NS + s], pc = P.words[RS + (int64_t)r * NS + s] & 7u;
-            if (base_is_alt(pc, rc)) best = umax(best, (w0 >> 16) & 0xFFu);
+            const int64_t idx = (int64_t)r * NS + s;
+            const uint32_t cnt = (P.words[idx] >> 16) & 0xFFu, pc = P.words[RS + idx] & 7u;
+            if (!base_is_alt(pc, rc) || cnt <= best) continue;
+            if (bounded) {                        // the entry bounds on the primary's 13 values
+                uint32_t v[N_STATS];
+                unpack_primary(P.words, RS, idx, v);
+                if (!entry_within(v, false, P.bounds)) continue;
+            }
+            best = cnt;
         }
         if (L.left) best = umax(best, P.dbest[s - 1]);
         ab = L.abandoned;

@@ -9,6 +9,8 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+from decimal import Decimal
+from fractions import Fraction
 from typing import List, Optional, Sequence, Tuple
 
 import numpy as np
@@ -79,6 +81,54 @@ class CSiteFilter(C.Structure):
     _fields_ = [("min_alt_count", C.c_int32), ("reserved", C.c_int32), ("min_alt_fraction", C.c_double)]
 
 
+class CEntryBounds(C.Structure):
+    """brc_entry_bounds: bounds in hundredths of the printed fields, indexed by BRC_S_* (include/brc_engine.h)."""
+    _fields_ = [("lo_set", C.c_uint32), ("hi_set", C.c_uint32), ("lo", C.c_int64 * 13), ("hi", C.c_int64 * 13)]
+
+
+# the 13 numbers of an allele entry, by bam-readcount's column names, in print order (BRC_S_*)
+ENTRY_FIELDS = ("count", "avg_mapping_quality", "avg_basequality", "avg_se_mapping_quality", "num_plus_strand", "num_minus_strand",
+                "avg_pos_as_fraction", "avg_num_mismatches_as_fraction", "avg_sum_mismatch_qualities", "num_q2_containing_reads",
+                "avg_distance_to_q2_start_in_q2_reads", "avg_clipped_length", "avg_distance_to_effective_3p_end")
+
+
+def hundredths(v) -> int:
+    """A bound in hundredths, exactly: from an int, a decimal string, a Decimal or a Fraction (a float by its shortest decimal
+    repr, never by a binary product).  At most two decimals, not negative."""
+    if isinstance(v, bool):
+        raise ValueError(f"bound {v!r}: not a number")
+    if isinstance(v, float):
+        v = repr(v)
+    if isinstance(v, str):
+        try:
+            v = Decimal(v.strip())
+        except ArithmeticError:
+            raise ValueError(f"bound {v!r}: not a decimal number") from None
+        if not v.is_finite():
+            raise ValueError(f"bound {v!r}: not finite")
+    x = Fraction(v) * 100
+    if x.denominator != 1 or x < 0:
+        raise ValueError(f"bound {v!r}: wants a number >= 0 with at most two decimals")
+    return int(x)
+
+
+def entry_bounds(bounds: dict) -> CEntryBounds:
+    """{field name: (lo, hi)} with either side None, in the printed units -> brc_entry_bounds."""
+    b = CEntryBounds()
+    for name, lohi in bounds.items():
+        if name not in ENTRY_FIELDS:
+            raise ValueError(f"unknown entry field {name!r} (one of {', '.join(ENTRY_FIELDS)})")
+        k = ENTRY_FIELDS.index(name)
+        lo, hi = lohi
+        if lo is not None:
+            b.lo_set |= 1 << k
+            b.lo[k] = hundredths(lo)
+        if hi is not None:
+            b.hi_set |= 1 << k
+            b.hi[k] = hundredths(hi)
+    return b
+
+
 class CSelectedResults(C.Structure):
     """brc_selected_results: the sites a site filter shipped (include/brc_engine.h)."""
     _fields_ = [("n_regions", C.c_int64), ("regions", C.POINTER(CRegion)), ("n_rows", C.c_int32), ("n_slots", C.c_int64),
@@ -119,7 +169,7 @@ EXPORTS = [
     "brc_get_warning_counts", "brc_format_text", "brc_format_window", "brc_write_text", "brc_set_queue_carry", "brc_plan_device", "brc_run_device", "brc_device_packed_results", "brc_get_packed_results",
     "brc_fetch_device_results", "brc_last_launch_count", "brc_last_h2d_bytes", "brc_host_alloc", "brc_host_free", "brc_last_stage_ms", "brc_selftest_fastmath",
     "brc_get_reference_codes", "brc_get_read_descriptors", "brc_get_quotient_rows",
-    "brc_set_site_filter", "brc_get_selected_results", "brc_set_allele_queries", "brc_get_allele_answers", "brc_last_results_kind",
+    "brc_set_site_filter", "brc_set_site_filter_bounds", "brc_get_selected_results", "brc_set_allele_queries", "brc_get_allele_answers", "brc_last_results_kind",
     "brc_set_complex_queries", "brc_get_complex_answers",
 ]
 
@@ -183,6 +233,7 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
     lib.brc_last_stage_ms.argtypes = [C.c_void_p, C.c_int]
     lib.brc_last_stage_ms.restype = C.c_float
     lib.brc_set_site_filter.argtypes = [C.c_void_p, C.POINTER(CSiteFilter)]
+    lib.brc_set_site_filter_bounds.argtypes = [C.c_void_p, C.POINTER(CSiteFilter), C.POINTER(CEntryBounds)]
     lib.brc_get_selected_results.argtypes = [C.c_void_p, C.POINTER(CSelectedResults)]
     lib.brc_set_allele_queries.argtypes = [C.c_void_p, C.POINTER(CAlleleQuery), C.c_int64, C.c_char_p, C.c_int64]
     lib.brc_get_allele_answers.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int64)]
@@ -579,11 +630,16 @@ class Engine:
         return PackedResults(r)
 
     # ---- alternative-allele site filter (include/brc_engine.h brc_set_site_filter) ----------------------------------------
-    def set_site_filter(self, min_alt_count: int, min_alt_fraction: float = 0.0):
+    def set_site_filter(self, min_alt_count: int, min_alt_fraction: float = 0.0, *, bounds: Optional[dict] = None):
         """Print only lines with an alternative allele of count >= min_alt_count and >= min_alt_fraction * depth (from the next
-        compute() on); while set, compute() returns None (no dense view) and selected() is the sparse result."""
+        compute() on); while set, compute() returns None (no dense view) and selected() is the sparse result.  bounds: {field
+        name (ENTRY_FIELDS): (lo, hi)}, either side None, in the units the line prints: that allele entry must also satisfy
+        lo <= field <= hi (brc_set_site_filter_bounds)."""
         f = CSiteFilter(int(min_alt_count), 0, float(min_alt_fraction))
-        self._check(self.lib.brc_set_site_filter(self.h, C.byref(f)))
+        if bounds is None:
+            self._check(self.lib.brc_set_site_filter(self.h, C.byref(f)))
+        else:
+            self._check(self.lib.brc_set_site_filter_bounds(self.h, C.byref(f), C.byref(entry_bounds(bounds))))
 
     def clear_site_filter(self):
         self._check(self.lib.brc_set_site_filter(self.h, None))

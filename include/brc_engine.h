@@ -308,6 +308,20 @@ typedef struct {
 /* f == NULL turns the filter off (the unfiltered path, exactly as without this call); takes effect at the next brc_compute /
  * brc_run_device.  Out-of-range values: BRC_E_INVALID. */
 BRC_API int brc_set_site_filter(brc_engine *e, const brc_site_filter *f);
+/* Bounds on an alternative allele's statistics, for filters in the style of false-positive filters (one-strand alleles,
+ * read-end alleles, low base quality ...).  With bounds, the entry that makes a line pass must also satisfy every bound that
+ * is set: lo[k] <= value (bit k of lo_set) and value <= hi[k] (bit k of hi_set), k = BRC_S_*.  The value is the field as the
+ * line prints it, in hundredths: an integer field (count, strand counts, Q2 reads) times 100; an average the two decimals the
+ * line prints (so avg_basequality of an indel entry is 0, as is the Q2 distance of an entry without Q2 reads).  A deletion is
+ * judged on the line where it prints (p+1). */
+typedef struct {
+    uint32_t lo_set, hi_set;      /* bit k: lo[k] / hi[k] is a bound; bits 13..31 are 0 */
+    int64_t lo[BRC_N_STATS];      /* hundredths, >= 0 */
+    int64_t hi[BRC_N_STATS];      /* hundredths, >= 0, and >= lo[k] when both are set */
+} brc_entry_bounds;
+/* brc_set_site_filter with bounds.  b == NULL is exactly brc_set_site_filter(e, f); f == NULL with bounds, a mask bit past
+ * bit 12, a negative bound or lo > hi on one field: BRC_E_INVALID.  brc_set_site_filter clears the bounds. */
+BRC_API int brc_set_site_filter_bounds(brc_engine *e, const brc_site_filter *f, const brc_entry_bounds *b);
 /* Sparse host view of a filtered run: the shipped sites (global slot ids, ascending) with their emit byte
  *   1: the line passes the filter   2: shipped for the deletion queue (a range whose lines may carry deletions queued by an
  *      earlier region, or the last site of an argv region that forms a line and that a library row covers); the emitter forms
