@@ -10,7 +10,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libbrc_engine.so")
 SOURCES = ["brc_kernels.cu", "brc_engine.cu", "brc_bgzf.cu", "brc_select.cu", "brc_alleles.cu", "brc_complex.cu", "brc_format.cpp"]
-HEADERS = ["brc_device.cuh", "brc_engine_internal.h", "brc_reads.h", "brc_fmt_num.h", "brc_aux.cuh", "brc_bgzf.cuh", "brc_scan.cuh", "brc_complex.cuh", os.path.join("..", "..", "include", "brc_engine.h")]
+HEADERS = ["brc_device.cuh", "brc_engine_internal.h", "brc_reads.h", "brc_fmt_num.h", "brc_aux.cuh", "brc_seq.cuh", "brc_bgzf.cuh", "brc_scan.cuh", "brc_complex.cuh", os.path.join("..", "..", "include", "brc_engine.h")]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
@@ -74,8 +74,8 @@ SYNTH_LIB = os.path.join(HERE, "libbrc_synth.so")
 def build_synth(force: bool = False) -> str:
     """The counter-based workload generator (include/brc_synth.h): device kernels + the identical host implementation."""
     src = os.path.join(CSRC, "brc_synth.cu")
-    hdr = os.path.join(HERE, "..", "include", "brc_synth.h")
-    if not force and os.path.exists(SYNTH_LIB) and os.path.getmtime(SYNTH_LIB) >= max(os.path.getmtime(src), os.path.getmtime(hdr)):
+    deps = [src, os.path.join(CSRC, "brc_seq.cuh"), os.path.join(HERE, "..", "include", "brc_synth.h")]
+    if not force and os.path.exists(SYNTH_LIB) and os.path.getmtime(SYNTH_LIB) >= max(os.path.getmtime(f) for f in deps):
         return SYNTH_LIB
     flags = [f for f in NVCC_FLAGS if f != "--fmad=false"]
     cmd = [nvcc_path()] + flags + ["-I", os.path.join(HERE, "..", "include"), "-o", SYNTH_LIB, src]
@@ -88,7 +88,7 @@ def build_synth(force: bool = False) -> str:
 
 CLI = os.path.join(HERE, "brc-readcount")
 CLI_SOURCES = ["brc_cli.cpp", "brc_cli_input.cpp", "brc_cli_vcf.cpp"]
-CLI_HEADERS = ["brc_cli_input.h", "brc_cli_vcf.h", "brc_cli_warn.h", "brc_reads.h", "brc_aux.cuh", os.path.join("..", "..", "include", "brc_engine.h")]
+CLI_HEADERS = ["brc_cli_input.h", "brc_cli_vcf.h", "brc_cli_warn.h", "brc_reads.h", "brc_aux.cuh", "brc_seq.cuh", os.path.join("..", "..", "include", "brc_engine.h")]
 
 
 def build_cli(force: bool = False) -> str:

@@ -107,7 +107,7 @@ __global__ void bam_extract_kernel(ExtractArgs A) {
     A.sz[i] = n_cigar; A.sz[A.n_reads + i] = (uint32_t)((l_seq + 1) / 2); A.sz[2 * A.n_reads + i] = (uint32_t)l_seq;
     if (!(flag & 4u)) {
         int64_t rl = 0;
-        for (uint32_t k = 0; k < n_cigar; ++k) { const uint32_t c = ld_u32(d + ax.cig_o + 4 * k), op = c & 15u; if (op == 0 || op == 2 || op == 3 || op == 7 || op == 8) rl += c >> 4; }
+        for (uint32_t k = 0; k < n_cigar; ++k) { const uint32_t c = ld_u32(d + ax.cig_o + 4 * k); if (cigar_consumes_ref(c & 15u)) rl += c >> 4; }
         const unsigned long long end = (unsigned long long)((int64_t)pos + (n_cigar ? rl : 1));
         atomicMax(A.max_end, end);
     }

@@ -17,6 +17,7 @@
 #include "../../include/brc_engine.h"
 #include "brc_aux.cuh"
 #include "brc_reads.h"
+#include "brc_seq.cuh"
 
 namespace brc::cli {
 
@@ -97,9 +98,6 @@ struct Rec {   // one decoded alignment (the bam1_t fields the path reads)
     const uint32_t *cigar; const uint8_t *seq, *qual; std::string rg; bool has_rg;
 };
 
-// CIGAR operations that consume the reference: M, D, N, = and X
-inline bool cigar_ref_op(uint32_t op) { return op == 0 || op == 2 || op == 3 || op == 7 || op == 8; }
-
 inline bool read_record(Bgzf &bz, Rec &r) {
     int32_t bs;
     if (!bz.read(&bs, 4)) return false;                                   // EOF (clean unless bz.error)
@@ -123,11 +121,7 @@ inline bool read_record(Bgzf &bz, Rec &r) {
 }
 
 inline int64_t rec_endpos(const Rec &r) {   // bam_endpos
-    if (!(r.flag & 4) && r.n_cigar > 0) {
-        int64_t l = 0;
-        for (uint32_t k = 0; k < r.n_cigar; ++k) if (cigar_ref_op(r.cigar[k] & 0xF)) l += r.cigar[k] >> 4;
-        return r.pos + l;
-    }
+    if (!(r.flag & 4) && r.n_cigar > 0) return r.pos + brc::cigar_span(r.cigar, r.n_cigar).rlen;
     return (int64_t)r.pos + 1;
 }
 

@@ -62,10 +62,10 @@ bool parse_vcf(const std::string &path, const std::vector<std::string> &samples,
     auto up = [](std::string s) { for (char &c : s) c = (char)std::toupper((unsigned char)c); return s; };
     auto acgtn = [](const std::string &s, size_t from) {
         if (s.size() <= from) return false;
-        for (size_t i = from; i < s.size(); ++i) if (!std::strchr("ACGTN", s[i]) || !s[i]) return false;
+        for (size_t i = from; i < s.size(); ++i) if (!std::strchr(canonical_nt + 1, s[i]) || !s[i]) return false;
         return true;
     };
-    auto kind_of = [](char c) { return (uint32_t)(std::strchr("=ACGTN", c) - "=ACGTN"); };
+    auto kind_of = [](char c) { return (uint32_t)(std::strchr(canonical_nt, c) - canonical_nt); };
     bool in_header = true;
     size_t ln = 0;
     for (size_t p = 0; p < text.size();) {

@@ -66,21 +66,20 @@ struct Warner {
     // stateless resolve_cigar2 (V:htslib-1.10/sam.c:3964-4041): qpos / is_del / indel of `site` in a read
     static bool resolve(const Cand &c, int64_t site, int &qpos, int &indel) {
         int64_t x = c.pos; int y = 0; size_t k = 0; uint32_t op = 0; int len = 0; const size_t n = c.cigar.size();
-        auto matchop = [](uint32_t o) { return o == 0 || o == 7 || o == 8; };
         for (; k < n; ++k) {
             op = c.cigar[k] & 0xF; len = (int)(c.cigar[k] >> 4);
-            if (cigar_ref_op(op)) { if (site < x + len) break; x += len; if (matchop(op)) y += len; }
+            if (cigar_consumes_ref(op)) { if (site < x + len) break; x += len; if (cigar_is_match(op)) y += len; }
             else if (op == 1 || op == 4) y += len;
         }
         indel = 0;
         if (k >= n) return false;
-        const bool is_del = !matchop(op);
+        const bool is_del = !cigar_is_match(op);
         qpos = is_del ? y : y + (int)(site - x);
         if (x + len - 1 == site && k + 1 < n) {
             const uint32_t op2 = c.cigar[k + 1] & 0xF; const int l2 = (int)(c.cigar[k + 1] >> 4);
             if (op2 == 2) indel = -l2;
             else if (op2 == 1) indel = l2;
-            else if (op2 == 6) { int l3 = 0; for (size_t m = k + 2; m < n; ++m) { const uint32_t o3 = c.cigar[m] & 0xF; if (o3 == 1) l3 += (int)(c.cigar[m] >> 4); else if (cigar_ref_op(o3)) break; } if (l3 > 0) indel = l3; }
+            else if (op2 == 6) { int l3 = 0; for (size_t m = k + 2; m < n; ++m) { const uint32_t o3 = c.cigar[m] & 0xF; if (o3 == 1) l3 += (int)(c.cigar[m] >> 4); else if (cigar_consumes_ref(o3)) break; } if (l3 > 0) indel = l3; }
         }
         return !is_del;
     }

@@ -10,11 +10,7 @@
 #pragma once
 #include <cstdint>
 
-#if defined(__CUDACC__)
-#define BRC_CX_HD __host__ __device__ __forceinline__
-#else
-#define BRC_CX_HD inline
-#endif
+#include "brc_seq.cuh"
 
 namespace brc {
 
@@ -22,7 +18,7 @@ struct Flanks { int32_t ql, qr; };     // query positions of the left and right 
 
 // cig: the read's n_cigar BAM CIGAR words (op in bits [0:4), length in [4:32)); pos: its leftmost reference position;
 // left = p - 1, right = p + n (left < right).
-BRC_CX_HD Flanks resolve_flanks(const uint32_t *cig, uint32_t n_cigar, int64_t pos, int64_t left, int64_t right) {
+BRC_SEQ_HD Flanks resolve_flanks(const uint32_t *cig, uint32_t n_cigar, int64_t pos, int64_t left, int64_t right) {
     Flanks f{-1, -1};
     int64_t rp = pos;
     int64_t qp = 0;
@@ -30,7 +26,7 @@ BRC_CX_HD Flanks resolve_flanks(const uint32_t *cig, uint32_t n_cigar, int64_t p
     for (uint32_t k = 0; k < n_cigar; ++k) {
         const uint32_t c = cig[k], op = c & 0xFu;
         const int64_t len = (int64_t)(c >> 4);
-        if (op == 0u || op == 7u || op == 8u) {             // M = X: reference and query advance together
+        if (cigar_is_match(op)) {                           // M = X: reference and query advance together
             if (ql < 0 && left >= rp && left < rp + len) ql = (int32_t)(qp + (left - rp));
             if (right >= rp && right < rp + len) {
                 if (ql >= 0) { f.ql = ql; f.qr = (int32_t)(qp + (right - rp)); }

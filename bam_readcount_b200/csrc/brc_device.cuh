@@ -14,6 +14,7 @@
 
 #include "../../include/brc_engine.h"
 #include "brc_fmt_num.h"
+#include "brc_seq.cuh"
 
 namespace brc {
 
@@ -25,18 +26,6 @@ constexpr uint8_t NO_BASE = 255;
 
 // flag bits the reference filters on (R:bamreadcount.cpp:295-310)
 constexpr uint32_t FLAG_FILTER = 4u | 256u | 512u | 1024u;
-
-// bam_nt16_canonical_table (R:bamreadcount.cpp:36-39): nibble -> index into "=ACGTN"; the text emitter prints insertion
-// bases through the same table (brc_format.cpp kCanon)
-__device__ __forceinline__ uint32_t canonical16(uint32_t nib) {
-    // packed 16 x 4-bit LUT: {0,1,2,5,3,5,5,5,4,5,5,5,5,5,5,5}
-    return (0x5555555455535210ull >> (nib * 4)) & 0xFu;
-}
-// 4-bit code of read base i of the packed bases starting at seq[off]
-__device__ __forceinline__ uint32_t seq_nib(const uint8_t *seq, uint64_t off, int i) {
-    uint32_t b = seq[off + (uint32_t)(i >> 1)];
-    return (i & 1) ? (b & 0xFu) : (b >> 4);
-}
 
 // ReadDesc.fm layout: flag[0:16) | mapq[16:24) | bits below
 constexpr uint32_t FM_SIMPLE = 1u << 24;     // CIGAR has exactly one ref-consuming op, of match type, and no I/D/N/P
@@ -347,17 +336,19 @@ struct SelectParams {
     SecRec *c_sec;
 };
 
-#ifdef __CUDACC__   // device atomics: not for the host-only translation units
-// ---- the line a site forms (brc_format.cpp format_site), as the device sees it in the packed records ----
-// One definition for the site selection (brc_select.cu) and the allele queries (brc_alleles.cu).
+// ---- the line a site forms (brc_format.cpp format_site), as the packed records hold it ----
+// One definition for the site selection (brc_select.cu), the allele queries (brc_alleles.cu) and the engine host (ensure_wide,
+// brc_get_warning_counts).
 // Row r spans site s (column idx = r * n_slots + s): an escaped primary, or ncover > 0.  RS = n_rows * n_slots.
-__device__ __forceinline__ bool row_covers(const uint32_t *words, int64_t RS, int64_t idx) {
+__host__ __device__ __forceinline__ bool row_covers(const uint32_t *words, int64_t RS, int64_t idx) {
     return (words[RS + idx] & 7u) == PB_ESCAPE || (words[idx] & 0xFFu) != 0u;
 }
 // The 13 accumulators of the primary held in the packed words of column idx (word w at words[w * RS + idx]; layout above).
-__device__ __forceinline__ void unpack_primary(const uint32_t *words, int64_t RS, int64_t idx, uint32_t v[N_STATS]) {
+__host__ __device__ __forceinline__ void unpack_primary(const uint32_t *words, int64_t RS, int64_t idx, uint32_t v[N_STATS]) {
     uint32_t w[N_WORDS];
+#ifdef __CUDA_ARCH__
 #pragma unroll
+#endif
     for (int k = 0; k < N_WORDS; ++k) w[k] = words[k * RS + idx];
     const uint32_t count = (w[0] >> 16) & 0xFFu, plus = w[0] >> 24;
     v[BRC_S_COUNT] = count; v[BRC_S_MAPQ] = w[1] >> 16; v[BRC_S_BASEQ] = w[2] & 0xFFFFu; v[BRC_S_SE_MAPQ] = w[2] >> 16;
@@ -366,12 +357,13 @@ __device__ __forceinline__ void unpack_primary(const uint32_t *words, int64_t RS
     v[BRC_S_3P_DIST] = w[7];
 }
 // Some row has a read without library at site s: -p abandons the site (no line, and its deletions are never queued).
-__device__ __forceinline__ bool site_abandoned(const uint32_t *words, int n_rows, int64_t NS, int64_t s) {
+__host__ __device__ __forceinline__ bool site_abandoned(const uint32_t *words, int n_rows, int64_t NS, int64_t s) {
     const int64_t RS = (int64_t)n_rows * NS;
     bool ab = false;
     for (int r = 0; r < n_rows; ++r) ab |= (words[RS + (int64_t)r * NS + s] & 8u) != 0u;
     return ab;
 }
+#ifdef __CUDACC__   // device atomics: not for the host-only translation units
 // Pool pass, one secondary-pool record: what it adds to the depth of a line.  An escaped primary adds its npass to esc_np[s];
 // a deletion adds its count to dsum[s] (extra depth of the next site's line) when the same row spans the next site, where the
 // row's block prints it.  Returns true for such a deletion.  dsum and esc_np are [n_slots], zeroed before the pass.

@@ -39,17 +39,6 @@ int check_view(brc_engine *e, const char *who, unsigned kinds) {
 
 #define CU(call, what) do { cudaError_t ce_ = (call); if (ce_ != cudaSuccess) return set_cuda_error(e, ce_, what); } while (0)
 
-// bam_cigar2rlen: reference length of a CIGAR; with n_indel, also counts its I and D ops there
-static inline int64_t cigar_rlen(const uint32_t *cig, uint64_t n, int64_t *n_indel = nullptr) {
-    int64_t l = 0;
-    for (uint64_t k = 0; k < n; ++k) {
-        const uint32_t op = cig[k] & 0xF;
-        if (op == 0 || op == 2 || op == 3 || op == 7 || op == 8) l += cig[k] >> 4;
-        if (n_indel && (op == 1 || op == 2)) ++*n_indel;
-    }
-    return l;
-}
-
 // The kernels' view of a batch whose arrays are in device memory.
 static ReadsDev reads_dev(const brc_read_batch &b) {
     ReadsDev R;
@@ -218,7 +207,7 @@ static void materialize_borrowed(brc_engine *e) {
         A.max_tid = A.it_tid = e->regions.back().tid; A.max_pos = A.it_pos = H.pos[n - 1];
         for (size_t i = 0; i < n; ++i) {
             const uint64_t nc = H.cigar_off[i + 1] - H.cigar_off[i];
-            const int64_t end = nc ? (int64_t)H.pos[i] + cigar_rlen(H.cigar.data() + H.cigar_off[i], nc) : (int64_t)H.pos[i] + 1;
+            const int64_t end = nc ? (int64_t)H.pos[i] + cigar_span(H.cigar.data() + H.cigar_off[i], nc).rlen : (int64_t)H.pos[i] + 1;
             if (end >= A.it_pos) A.live_ends.push(end);
         }
     }
@@ -252,8 +241,8 @@ int brc_push_read(brc_engine *e, int32_t tid, int32_t pos, uint16_t flag, uint8_
     // pileup buffer refuses; bam_plp_push (V:htslib-1.10/sam.c:4484-4531):
     if (tid < 0 || (flag & 4)) return BRC_OK;                                   // :4488-4490
     if (e->cfg.per_lib && lib != BRC_LIB_NONE && (int)lib >= e->n_rows) return set_error(e, BRC_E_BAD_LIBRARY, "push_read: library id >= n_libs");
-    int64_t indel_ops = 0;
-    const int64_t end = n_cigar > 0 ? (int64_t)pos + cigar_rlen(cigar, n_cigar, &indel_ops) : (int64_t)pos + 1;  // bam_endpos
+    const CigarSpan span = cigar_span(cigar, n_cigar);
+    const int64_t end = n_cigar > 0 ? (int64_t)pos + span.rlen : (int64_t)pos + 1;  // bam_endpos
     if (A.it_tid == tid && A.it_pos == pos) {                                   // :4491 maxcnt rule
         while (!A.live_ends.empty() && A.live_ends.top() < A.it_pos) A.live_ends.pop();   // retired while draining positions < it_pos
         if ((int64_t)A.live_ends.size() + 1 > (int64_t)e->cfg.max_cnt) return BRC_OK;
@@ -270,7 +259,7 @@ int brc_push_read(brc_engine *e, int32_t tid, int32_t pos, uint16_t flag, uint8_
     HostReads &H = e->reads;
     H.append(pos, flag, mapq, lib, l_qseq, nm, sm, n_cigar, cigar, seq, qual);
     H.region.push_back((int32_t)(e->regions.size() - 1));
-    e->n_indel_ops += indel_ops;
+    e->n_indel_ops += span.n_indel;
     if (end > e->open_max_end) e->open_max_end = end;
     rg.read_hi = H.n();
     return BRC_OK;
@@ -301,16 +290,12 @@ static BatchScan scan_batch(const brc_read_batch *b, int32_t rtid, int per_lib, 
             if ((b->tid && b->tid[i] != rtid) || (b->flag[i] & 4)) { r.ok = false; break; }
             if (i > 0 && b->pos[i] < b->pos[i - 1]) { r.ok = false; break; }
             if (per_lib && b->lib && b->lib[i] != BRC_LIB_NONE && (int)b->lib[i] >= n_rows) { r.ok = false; break; }
-            // cigar_rlen written out: calling it here made the C3 push path (e2e leg) about 2.5 ms per window slower
-            // (22.7 -> 25.2 ms, H100 80GB HBM3 at 400 W), although its inner loop compiles the same
+            // the running I/D total goes through cigar_span by value: counting it through a pointer here made the C3 push path
+            // (e2e leg) about 2.5 ms per window slower (22.7 -> 25.2 ms, H100 80GB HBM3 at 400 W)
             const uint64_t c0 = b->cigar_off[i], c1 = b->cigar_off[i + 1];
-            int64_t l = 0;
-            for (uint64_t k = c0; k < c1; ++k) {
-                const uint32_t op = b->cigar[k] & 0xF;
-                if (op == 0 || op == 2 || op == 3 || op == 7 || op == 8) l += b->cigar[k] >> 4;
-                if (op == 1 || op == 2) ++r.indel_ops;
-            }
-            const int64_t end = c1 > c0 ? (int64_t)b->pos[i] + l : (int64_t)b->pos[i] + 1;
+            const CigarSpan span = cigar_span(b->cigar + c0, c1 > c0 ? c1 - c0 : 0, r.indel_ops);
+            r.indel_ops = span.n_indel;
+            const int64_t end = c1 > c0 ? (int64_t)b->pos[i] + span.rlen : (int64_t)b->pos[i] + 1;
             if (end <= (int64_t)b->pos[i] && i > 0 && b->pos[i] == b->pos[i - 1]) { r.ok = false; break; }  // zero-span read: exact linking rule lives in brc_push_read
             if (end > r.max_end) r.max_end = end;
         }
@@ -742,15 +727,13 @@ void ensure_wide(brc_engine *e) {
         const int64_t lo = rs * t / nt, hi = rs * (t + 1) / nt;
         uint32_t *ps = W.pstats.data();
         for (int64_t i = lo; i < hi; ++i) {
-            const uint32_t w0 = words[i], w1 = words[rs + i], w2 = words[2 * rs + i], w3 = words[3 * rs + i];
-            const uint32_t count = (w0 >> 16) & 0xFFu, plus = w0 >> 24, pc = w1 & 7u;
+            const uint32_t w0 = words[i], w1 = words[rs + i], pc = w1 & 7u;
             W.ncover[(size_t)i] = w0 & 0xFFu; W.npass[(size_t)i] = (w0 >> 8) & 0xFFu;
             W.flags[(size_t)i] = (uint8_t)((w1 >> 3) & 1u); W.pbase[(size_t)i] = (uint8_t)(pc < 6u ? pc : BRC_NO_BASE);
             W.sec_head[(size_t)i] = -1;
-            ps[BRC_S_COUNT * rs + i] = count; ps[BRC_S_MAPQ * rs + i] = w1 >> 16; ps[BRC_S_BASEQ * rs + i] = w2 & 0xFFFFu; ps[BRC_S_SE_MAPQ * rs + i] = w2 >> 16;
-            ps[BRC_S_PLUS * rs + i] = plus; ps[BRC_S_MINUS * rs + i] = count - plus; ps[BRC_S_POS_FRAC * rs + i] = words[4 * rs + i]; ps[BRC_S_NM_FRAC * rs + i] = words[5 * rs + i];
-            ps[BRC_S_MMQS * rs + i] = w3 >> 16; ps[BRC_S_NQ2 * rs + i] = (w1 >> 8) & 0xFFu; ps[BRC_S_Q2_DIST * rs + i] = words[6 * rs + i]; ps[BRC_S_CLIP_LEN * rs + i] = w3 & 0xFFFFu;
-            ps[BRC_S_3P_DIST * rs + i] = words[7 * rs + i];
+            uint32_t v[N_STATS];
+            unpack_primary(words, rs, i, v);
+            for (int k = 0; k < N_STATS; ++k) ps[k * rs + i] = v[k];
         }
     });
     // secondary records: keys are chained per slot (order is immaterial to every consumer); escaped primaries fill their slot
@@ -1019,12 +1002,8 @@ int brc_get_warning_counts(brc_engine *e, int64_t out[4]) {
         int64_t lu = 0;
         if (e->cfg.per_lib && e->selected()) lu = e->sel_abandoned;   // counted by the selection's site pass
         else if (e->cfg.per_lib) {
-            const uint32_t *w1 = e->h_words.as<uint32_t>() + (int64_t)e->n_rows * e->n_slots;
-            for (int64_t sidx = 0; sidx < e->n_slots; ++sidx) {
-                bool ab = false;
-                for (int r = 0; r < e->n_rows && !ab; ++r) ab = (w1[(int64_t)r * e->n_slots + sidx] & 8u) != 0;
-                lu += ab;
-            }
+            const uint32_t *words = e->h_words.as<uint32_t>();
+            for (int64_t s = 0; s < e->n_slots; ++s) lu += site_abandoned(words, e->n_rows, e->n_slots, s);
         }
         e->warn_counts[3] = lu;
     }
@@ -1145,9 +1124,9 @@ int brc_set_allele_queries(brc_engine *e, const brc_allele_query *q, int64_t n, 
                 return set_error(e, BRC_E_INVALID, "set_allele_queries: insertion bases outside the buffer");
             a.bases_off = (int64_t)codes.size();
             for (uint32_t k = 0; k < len; ++k) {
-                const char *p = std::strchr("ACGTN", bases[x.bases_off + k]);
+                const char *p = std::strchr(canonical_nt + 1, bases[x.bases_off + k]);
                 if (!p || !*p) return set_error(e, BRC_E_INVALID, "set_allele_queries: insertion bases must be A, C, G, T or N");
-                codes.push_back((uint8_t)(1 + (p - "ACGTN")));      // index into "=ACGTN"
+                codes.push_back((uint8_t)(p - canonical_nt));
             }
         }
     }
@@ -1190,9 +1169,9 @@ int brc_set_complex_queries(brc_engine *e, const brc_complex_query *q, int64_t n
             return set_error(e, BRC_E_INVALID, "set_complex_queries: allele bases outside the buffer");
         const int64_t at = (int64_t)codes.size();
         for (int32_t k = 0; k < x.len; ++k) {
-            const char *p = std::strchr("ACGTN", bases[x.bases_off + k]);
+            const char *p = std::strchr(canonical_nt + 1, bases[x.bases_off + k]);
             if (!p || !*p) return set_error(e, BRC_E_INVALID, "set_complex_queries: allele bases must be A, C, G, T or N");
-            codes.push_back((uint8_t)(1 + (p - "ACGTN")));      // index into "=ACGTN"
+            codes.push_back((uint8_t)(p - canonical_nt));
         }
         x.bases_off = at; x.reserved = 0;
     }

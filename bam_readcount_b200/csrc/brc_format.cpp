@@ -30,6 +30,7 @@ inline float f32(uint32_t u) { float f; std::memcpy(&f, &u, 4); return f; }
 
 using brc::put_u;
 using brc::put_f2;
+using brc::canonical_nt;
 
 // operator<<(std::ostream&, const BasicStat&)
 void put_stat(std::string &o, const Stat *s, bool is_indel) {
@@ -59,9 +60,6 @@ inline QEnt make_qent(int32_t tid, int64_t pos, const Stat &st, const std::strin
 }
 inline const Stat *qstat(const QEnt &q) { return reinterpret_cast<const Stat *>(q.st); }
 
-const char kNt[] = "=ACGTN";
-const uint8_t kCanon[16] = {0, 1, 2, 5, 3, 5, 5, 5, 4, 5, 5, 5, 5, 5, 5, 5};
-
 struct View {   // raw result arrays of one engine
     const brc_engine *e; const brc_region *rg; const brc::HostRef *ref;
     int rows; int64_t NS, RS, SC;
@@ -83,8 +81,9 @@ struct View {   // raw result arrays of one engine
 struct Indel { std::string allele; Stat st; };
 struct Scratch { std::string rec; std::vector<Indel> indels; };
 
-// seq_nt16 code of a reference character (1/2/4/8 for one base; 15 for N, IUPAC codes and anything else)
-inline uint32_t nt16(char c) {
+// The site filter's code of a reference character as the line prints it: 1/2/4/8 for A/C/G/T (either case), 15 for N, IUPAC
+// codes and anything else.  Not seq_nt16 (brc_seq.cuh), which also maps the digits '0'..'3' to 1/2/4/8 (DESIGN.md §10).
+inline uint32_t printed_base_code(char c) {
     switch (c) { case 'A': case 'a': return 1; case 'C': case 'c': return 2; case 'G': case 'g': return 4; case 'T': case 't': return 8; default: return 15; }
 }
 
@@ -104,7 +103,7 @@ void format_site(const View &V, int32_t s, int64_t slot, const char *const *lib_
     char rb = 'N';
     if (emit && V.ref && pos < V.ref->chrom_len && pos >= V.ref->win_beg && pos < V.ref->win_beg + (int64_t)V.ref->seq.size()) rb = V.ref->seq[(size_t)(pos - V.ref->win_beg)];   // a device-only reference window (brc_set_reference_device) has no characters here
     const bool gate = emit && V.csite;
-    const uint32_t rcode = gate ? nt16(rb) : 15u;
+    const uint32_t rcode = gate ? printed_base_code(rb) : 15u;
     const brc::EntryBounds &bounds = V.e->sel_bounds;   // an entry counts toward best_alt only within them
     uint64_t best_alt = 0;
     for (int r = 0; r < rows; ++r) {
@@ -121,7 +120,7 @@ void format_site(const View &V, int32_t s, int64_t slot, const char *const *lib_
             if (V.skind[j] == BRC_KIND_INS) {          // "+" + canonicalised read bases qpos+1..qpos+len  (R:...:324-330)
                 in.allele = "+";
                 const uint8_t *sq = V.e->host_read_seq(V.sread[j]);
-                for (int k = 1; k <= V.slen[j]; ++k) { int i = V.sqpos[j] + k; uint8_t b = sq ? sq[i >> 1] : (uint8_t)0xFF; in.allele += kNt[kCanon[(i & 1) ? (b & 15) : (b >> 4)]]; }
+                for (int k = 1; k <= V.slen[j]; ++k) in.allele += canonical_nt[brc::canonical16(sq ? brc::seq_nib(sq, 0, V.sqpos[j] + k) : 15u)];
             } else {                                   // "-" + raw reference characters pos+1..pos+len (R:...:331-339)
                 in.allele = "-";
                 for (int k = 1; k <= V.slen[j]; ++k) {
@@ -132,7 +131,7 @@ void format_site(const View &V, int32_t s, int64_t slot, const char *const *lib_
             }
             W.indels.push_back(std::move(in));
         }
-        if (emit) for (int j = 0; j < 6; ++j) { rec += '\t'; rec += kNt[j]; rec += ':'; put_stat(rec, have[j] ? &base[j] : nullptr, false); }
+        if (emit) for (int j = 0; j < 6; ++j) { rec += '\t'; rec += canonical_nt[j]; rec += ':'; put_stat(rec, have[j] ? &base[j] : nullptr, false); }
         if (gate) for (int j = 1; j <= 4; ++j) if (have[j] && brc::base_is_alt((uint32_t)j, rcode) && brc::entry_within(base[j].v, false, bounds)) best_alt = std::max<uint64_t>(best_alt, base[j].v[BRC_S_COUNT]);
         if (W.indels.size() > 1) std::sort(W.indels.begin(), W.indels.end(), [](const Indel &a, const Indel &b) { return a.allele < b.allele; });
         for (auto &in : W.indels) {

@@ -35,26 +35,11 @@
 
 namespace brc {
 
-// seq_nt16_table (V:htslib-1.10/hts.c:73-91): ASCII -> 4-bit IUPAC code, 15 for anything else
-__constant__ uint8_t c_nt16[256];
-// one-time, per-device set-up (constant table, opt-in shared-memory sizes, SM count) shared by every engine handle of the
+// seq_nt16_table (brc_seq.cuh), read by ref_encode_kernel
+__constant__ uint8_t c_nt16[256] = BRC_SEQ_NT16_TABLE;
+// one-time, per-device set-up (quotient tables, opt-in shared-memory sizes, SM count) shared by every engine handle of the
 // process: callers may drive several handles from several host threads, so it is serialised and published with atomics
 static std::mutex g_init_mu;
-static uint8_t h_nt16[256];
-static bool h_nt16_ready = false;          // guarded by g_init_mu
-static void build_nt16() {
-    for (int i = 0; i < 256; ++i) h_nt16[i] = 15;
-    const char *s = "=ACMGRSVTWYHKDBN";
-    for (int i = 0; i < 16; ++i) {
-        h_nt16[(unsigned char)s[i]] = (uint8_t)i;
-        if (s[i] >= 'A' && s[i] <= 'Z') h_nt16[(unsigned char)(s[i] + 32)] = (uint8_t)i;
-    }
-    h_nt16['0'] = 1; h_nt16['1'] = 2; h_nt16['2'] = 4; h_nt16['3'] = 8;
-    h_nt16_ready = true;
-}
-
-__device__ __forceinline__ bool is_refop(uint32_t op) { return op == 0 || op == 2 || op == 3 || op == 7 || op == 8; }
-__device__ __forceinline__ bool is_matchop(uint32_t op) { return op == 0 || op == 7 || op == 8; }
 
 // ---------------------------------------------------------------------------------------------
 // init: tile read ranges + counters
@@ -119,20 +104,6 @@ __global__ void __launch_bounds__(REF_ENCODE_THREADS) ref_encode_kernel(const ch
     }
 }
 
-static cudaError_t ensure_tables() {
-    static std::atomic<bool> uploaded[64];
-    int dev = 0; cudaGetDevice(&dev);
-    if (dev < 64 && uploaded[dev].load(std::memory_order_acquire)) return cudaSuccess;
-    std::lock_guard<std::mutex> lk(g_init_mu);
-    if (!h_nt16_ready) build_nt16();
-    if (dev >= 64 || !uploaded[dev].load(std::memory_order_relaxed)) {
-        cudaError_t e = cudaMemcpyToSymbol(c_nt16, h_nt16, 256);
-        if (e != cudaSuccess) return e;
-        if (dev < 64) uploaded[dev].store(true, std::memory_order_release);
-    }
-    return cudaSuccess;
-}
-
 // the quotient tables of brc_device.cuh (QTAB_*): one thread per entry, with the IEEE intrinsics the tables stand in for
 __global__ void qtab_build_kernel(float *q, double *p) {
     const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
@@ -173,8 +144,7 @@ cudaError_t quotient_tables(const float **q, const double **p) {
 }
 
 cudaError_t launch_ref_encode(const char *d_ascii, uint8_t *d_code, int64_t n, cudaStream_t s) {
-    cudaError_t e = ensure_tables();
-    if (e != cudaSuccess || n == 0) return e;
+    if (n == 0) return cudaSuccess;
     if ((uintptr_t)d_code & 15) return cudaErrorInvalidValue;      // the packed window is a device allocation: 16-byte stores
     const int64_t work = std::max<int64_t>(n / 32, 1);
     const int64_t blocks = std::min<int64_t>((work + REF_ENCODE_THREADS - 1) / REF_ENCODE_THREADS, REF_ENCODE_MAX_BLOCKS);
@@ -395,7 +365,7 @@ __global__ void __launch_bounds__(K0_READS) read_precompute_kernel(PrecomputePar
             const uint32_t c = cig[k];
             const int op_length = (int)(c >> 4);
             const uint32_t op = c & 0xFu;
-            if (is_refop(op)) { rlen += op_length; n_refops++; seen_ref = true; if (!is_matchop(op)) simple = false; }
+            if (cigar_consumes_ref(op)) { rlen += op_length; n_refops++; seen_ref = true; if (!cigar_is_match(op)) simple = false; }
             else if (op == 1 || op == 6) simple = false;
             else if (op == 4 && !seen_ref) qoff += op_length;
             if (walking) {
@@ -540,8 +510,6 @@ __global__ void __launch_bounds__(K0_READS) read_precompute_kernel(PrecomputePar
 }
 
 cudaError_t launch_precompute(const PrecomputeParams &p, cudaStream_t s) {
-    cudaError_t e = ensure_tables();
-    if (e != cudaSuccess) return e;
     const int64_t n = p.read_end - p.read_begin;
     if (n <= 0) return cudaSuccess;
     read_precompute_kernel<<<(unsigned)((n + K0_READS - 1) / K0_READS), K0_READS, 0, s>>>(p);
@@ -718,14 +686,14 @@ __device__ __noinline__ int3 resolve_general(const uint32_t *cig, uint32_t n_cig
     int64_t x = pos; int y = 0; uint32_t k = 0; uint32_t op = 0; int len = 0;
     for (; k < n_cigar; ++k) {
         const uint32_t c = cig[k]; op = c & 0xFu; len = (int)(c >> 4);
-        if (is_refop(op)) {
+        if (cigar_consumes_ref(op)) {
             if ((int64_t)site < x + len) break;
-            x += len; if (is_matchop(op)) y += len;
+            x += len; if (cigar_is_match(op)) y += len;
         } else if (op == 1 || op == 4) y += len;
     }
     int3 out = make_int3(0, 0, 0);
     if (k >= n_cigar) { out.z = 1; return out; }  // cannot happen for pos <= site < end
-    if (is_matchop(op)) out.x = y + (int)(site - x); else { out.z = 1; out.x = y; }
+    if (cigar_is_match(op)) out.x = y + (int)(site - x); else { out.z = 1; out.x = y; }
     if (x + len - 1 == site && k + 1 < n_cigar) {
         const uint32_t c2 = cig[k + 1]; const uint32_t op2 = c2 & 0xFu; const int l2 = (int)(c2 >> 4);
         if (op2 == 2) out.y = -l2;
@@ -735,7 +703,7 @@ __device__ __noinline__ int3 resolve_general(const uint32_t *cig, uint32_t n_cig
             for (uint32_t m = k + 2; m < n_cigar; ++m) {
                 const uint32_t c3 = cig[m]; const uint32_t op3 = c3 & 0xFu;
                 if (op3 == 1) l3 += (int)(c3 >> 4);
-                else if (op3 == 2 || op3 == 0 || op3 == 3 || op3 == 7 || op3 == 8) break;
+                else if (cigar_consumes_ref(op3)) break;
             }
             if (l3 > 0) out.y = l3;
         }

@@ -38,8 +38,7 @@ __device__ __forceinline__ uint32_t ref_code(const SelectParams &P, const SelReg
     const RefWin w = P.refs[R.tid_slot];
     const int64_t i = pos - w.win_beg;
     if (i < 0 || i >= w.win_len || pos >= w.chrom_len) return 15u;
-    const uint32_t b = (uint8_t)w.seq[i >> 1];
-    return (i & 1) ? (b & 15u) : (b >> 4);
+    return seq_nib(reinterpret_cast<const uint8_t *>(w.seq), (uint64_t)(i >> 1), (int)(i & 1));   // i may pass 2^31: byte in off
 }
 
 __device__ __forceinline__ uint64_t umax(uint64_t a, uint64_t b) { return a > b ? a : b; }

@@ -14,6 +14,7 @@
 #include <cuda_runtime.h>
 
 #include "../../include/brc_synth.h"
+#include "brc_seq.cuh"
 
 #define HD __host__ __device__ __forceinline__
 
@@ -555,7 +556,7 @@ int brc_synth_write_sam(const brc_synth_spec *S, int32_t contig, int64_t lo, int
     if (!fh) return BRC_E_INVALID;
     std::fprintf(fh, "@HD\tVN:1.6\tSO:coordinate\n@SQ\tSN:%s\tLN:%lld\n", contig_name, (long long)declared_len);
     for (int i = 0; i < S->n_libs; ++i) std::fprintf(fh, "@RG\tID:rg%d\tSM:s\tLB:lib%d\n", i, i);
-    const char *ops = "MIDNSHP=XB", *dec = "=ACMGRSVTWYHKDBN";
+    const char *ops = "MIDNSHP=XB";
     std::string line;
     char tmp[64];
     const int64_t base_index = S->mode == BRC_SYNTH_DEEP ? lo * (int64_t)S->depth : lo * BR;
@@ -567,7 +568,7 @@ int brc_synth_write_sam(const brc_synth_spec *S, int32_t contig, int64_t lo, int
         for (uint64_t k = co[(size_t)i]; k < co[(size_t)i + 1]; ++k) { std::snprintf(tmp, sizeof tmp, "%u%c", cig[k] >> 4, ops[cig[k] & 15]); line += tmp; }
         line += "\t*\t0\t0\t";
         const uint8_t *sq = seq.data() + so[(size_t)i];
-        for (int q = 0; q < RL; ++q) line += dec[(q & 1) ? (sq[q >> 1] & 15) : (sq[q >> 1] >> 4)];
+        for (int q = 0; q < RL; ++q) line += brc::seq_nt16_str[brc::seq_nib(sq, 0, q)];
         line += '\t';
         const uint8_t *ql = qual.data() + qo[(size_t)i];
         for (int q = 0; q < RL; ++q) line += (char)(ql[q] + 33);
