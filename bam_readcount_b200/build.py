@@ -9,8 +9,8 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libbrc_engine.so")
-SOURCES = ["brc_kernels.cu", "brc_engine.cu", "brc_bgzf.cu", "brc_select.cu", "brc_alleles.cu", "brc_complex.cu", "brc_format.cpp"]
-HEADERS = ["brc_device.cuh", "brc_engine_internal.h", "brc_reads.h", "brc_fmt_num.h", "brc_aux.cuh", "brc_seq.cuh", "brc_bgzf.cuh", "brc_scan.cuh", "brc_complex.cuh", os.path.join("..", "..", "include", "brc_engine.h")]
+SOURCES = ["brc_kernels.cu", "brc_engine.cu", "brc_bgzf.cu", "brc_select.cu", "brc_alleles.cu", "brc_complex.cu", "brc_deflate.cu", "brc_format.cpp"]
+HEADERS = ["brc_device.cuh", "brc_engine_internal.h", "brc_reads.h", "brc_fmt_num.h", "brc_aux.cuh", "brc_seq.cuh", "brc_bgzf.cuh", "brc_scan.cuh", "brc_complex.cuh", "brc_deflate.cuh", os.path.join("..", "..", "include", "brc_engine.h")]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",

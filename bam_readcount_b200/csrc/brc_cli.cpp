@@ -88,7 +88,9 @@ void usage() {
                 "                                        status 1 at the end)\n"
                 "  --vcf-complex                         (this host) with --vcf: also count MNP and complex records (an A/C/G/T/N ALT\n"
                 "                                        that no printed entry answers) by each read's bases between the two reference\n"
-                "                                        bases flanking REF, matched exactly against REF and each ALT\n\n");
+                "                                        bases flanking REF, matched exactly against REF and each ALT\n"
+                "  --bgzf                                (this host) write STDOUT, the VCF and every --bam-list OUT file as BGZF (bgzip's\n"
+                "                                        format, compressed on the GPU); STDERR and ERR files stay plain\n\n");
 }
 
 struct Options {   // everything on the command line except the inputs: the same for every sample
@@ -102,7 +104,45 @@ struct Options {   // everything on the command line except the inputs: the same
     bool site_filter = false; brc_site_filter filter{};
     bool has_bounds = false; brc_entry_bounds bounds{};   // --alt-min / --alt-max (brc_set_site_filter_bounds)
     bool decode_only = false, device_decode = false, timing = false;
+    bool bgzf = false;            // --bgzf: every output destination gets a BGZF writer (not under BRC_CLI_DECODE_ONLY: no device)
+    int device = 0;               // BRC_DEVICE: the device of the engines and of the BGZF writers
     bool dist_refused() const { return dist_arg == "1" || dist_arg == "true"; }
+};
+
+// One output destination (STDOUT, a --bam-list OUT file): plain writes to fd, or with --bgzf a BGZF writer on fd.  Every write of
+// text or VCF lines goes through here.
+struct Out {
+    int fd = STDOUT_FILENO;
+    brc_bgzf_writer *bgzf = nullptr;
+    bool failed = false;          // a BGZF write failed and the caller reported it
+    // --bgzf: the writer is opened with the destination, on the engines' device; false with the reason in `why`
+    bool open(const Options &o, int f, std::string &why) {
+        fd = f;
+        if (!o.bgzf || o.decode_only) return true;
+        int rc = brc_set_device(o.device);
+        if (rc == BRC_OK) rc = brc_bgzf_open(fd, &bgzf);
+        if (rc != BRC_OK) why = std::string("--bgzf: ") + brc_strerror(rc);
+        return rc == BRC_OK;
+    }
+    bool write(const std::string &s) {
+        if (!bgzf) return write_all(fd, s);
+        failed = failed || brc_bgzf_write(bgzf, s.data(), s.size()) != BRC_OK;
+        return !failed;
+    }
+    int64_t text(brc_engine *eng, int64_t g, int64_t first, int64_t count, const char *const *libs) {
+        if (!bgzf) return brc_write_text(eng, g, first, count, libs, fd);
+        const int64_t n = brc_write_text_bgzf(eng, g, first, count, libs, bgzf);
+        failed = failed || n < 0;
+        return n;
+    }
+    // the rest of the BGZF stream and its EOF member; false (errno set when a write failed) on failure.  fd stays open.
+    bool close() {
+        if (!bgzf) return true;
+        const int rc = brc_bgzf_close(bgzf);
+        bgzf = nullptr;
+        if (rc != BRC_OK && rc != BRC_E_IO) errno = EIO;
+        return rc == BRC_OK;
+    }
 };
 
 // the allele entry's 13 numbers by bam-readcount's column names, in print order (BRC_S_*)
@@ -455,9 +495,9 @@ struct DecodeSummary {
 };
 
 // One sample's run on an engine handle, the sink of its region loop.  Regions are pushed as they come and computed in batches
-// (flush): text to out_fd, or, with --vcf, the answers to vcf_ans.  Messages go to err.
+// (flush): text to out, or, with --vcf, the answers to vcf_ans.  Messages go to err.
 struct Run {
-    const Options &o; Sample &s; Engines::Handle &h; brc_engine *eng; int out_fd; FILE *err;
+    const Options &o; Sample &s; Engines::Handle &h; brc_engine *eng; Out &out; FILE *err;
     const Vcf *vcf; VcfAnswers *vcf_ans;
     const bool vcf_stream;        // --vcf: a single-sample run writes the records in file order, each once its region's batch is computed
     std::vector<int64_t> vcf_rec_of_region; size_t vcf_next = 0;
@@ -468,8 +508,8 @@ struct Run {
     int64_t warn_total[4] = {0, 0, 0, 0};
     double t_decode = 0, t_compute = 0, t_format = 0, t_ref = 0, t_results = 0, t_reset = 0, ms_alleles = 0, ms_complex = 0, d1 = 0;
 
-    Run(const Options &opt, Sample &smp, Engines::Handle &hd, int fd, FILE *e, VcfAnswers *ans)
-        : o(opt), s(smp), h(hd), eng(hd.eng), out_fd(fd), err(e), vcf(opt.vcf), vcf_ans(ans), vcf_stream(opt.vcf && !opt.vcf_samples),
+    Run(const Options &opt, Sample &smp, Engines::Handle &hd, Out &dst, FILE *e, VcfAnswers *ans)
+        : o(opt), s(smp), h(hd), eng(hd.eng), out(dst), err(e), vcf(opt.vcf), vcf_ans(ans), vcf_stream(opt.vcf && !opt.vcf_samples),
           vcf_rec_of_region(smp.regions.size(), -1) {
         for (size_t k = 0; k < s.vcf_region.size(); ++k) if (s.vcf_region[k] >= 0) vcf_rec_of_region[(size_t)s.vcf_region[k]] = (int64_t)k;
         for (const auto &kv : s.rg_lib) { rg_ids.push_back(kv.first.c_str()); rg_libs.push_back(kv.second); }
@@ -562,12 +602,12 @@ struct Run {
         for (int64_t g = 0; g < res.n_regions; ++g) total_slots += res.regions[g].n_slots;
         const bool many_small = res.n_regions > 1 && total_slots <= (int64_t(1) << 22);  // a site list: all regions in one formatting pass
         if (argv_chain || many_small) {
-            if (brc_write_text(eng, -1, 0, -1, libs, out_fd) < 0) return fail("format");
+            if (out.text(eng, -1, 0, -1, libs) < 0) return fail("format");
         } else {
             const int64_t WIN = 1 << 21;   // stream big regions in 2M-site windows (each formatted by several threads)
             for (int64_t g = 0; g < res.n_regions; ++g)
                 for (int64_t first = 0; first < res.regions[g].n_slots; first += WIN)
-                    if (brc_write_text(eng, g, first, WIN, libs, out_fd) < 0) return fail("format");
+                    if (out.text(eng, g, first, WIN, libs) < 0) return fail("format");
         }
         t_format += now() - f0;
         return true;
@@ -595,7 +635,7 @@ struct Run {
         return write_out(out);
     }
     bool write_out(const std::string &text) {
-        if (write_all(out_fd, text)) return true;
+        if (out.write(text)) return true;
         std::fprintf(err, "writing the VCF: %s\n", std::strerror(errno));
         return false;
     }
@@ -612,16 +652,16 @@ bool decode_report(Sample &s, const RegionFetcher &fetcher, FILE *err) {
     return decode_error;
 }
 
-// One sample's region loop: text to out_fd, messages to err.  With --vcf the answers go to `vcf_ans`, and a single-sample run
-// streams the VCF to out_fd as its batches complete.  Returns the exit status of the run on this input alone (0 or 1), or -1
+// One sample's region loop: text to out, messages to err.  With --vcf the answers go to `vcf_ans`, and a single-sample run
+// streams the VCF to out as its batches complete.  Returns the exit status of the run on this input alone (0 or 1), or -1
 // when no engine could be created.
-int run_sample(const Options &o, Engines &engines, Sample &s, int out_fd, FILE *err, double t_main0, VcfAnswers *vcf_ans) {
+int run_sample(const Options &o, Engines &engines, Sample &s, Out &out, FILE *err, double t_main0, VcfAnswers *vcf_ans) {
     std::fputs(s.log.held.c_str(), err);
     if (s.status != 0) return 1;
     s.warner.err = err;
     RegionFetcher fetcher(s.bam);
     if (o.decode_only) {
-        DecodeSummary summary{out_fd};
+        DecodeSummary summary{out.fd};
         region_loop(s, fetcher, summary);
         return decode_report(s, fetcher, err) ? 1 : 0;
     }
@@ -630,7 +670,7 @@ int run_sample(const Options &o, Engines &engines, Sample &s, int out_fd, FILE *
     // nothing left from an earlier sample: no pushed reads (a sample that failed mid-way) and no queued deletion
     // (switching the carry empties the queue); the argv loop's queue is then carried across this sample's flushes
     brc_reset(h->eng); brc_set_queue_carry(h->eng, 0); brc_set_queue_carry(h->eng, 1);
-    Run run(o, s, *h, out_fd, err, vcf_ans);
+    Run run(o, s, *h, out, err, vcf_ans);
     if (run.vcf_stream && !run.write_out(vcf_header(*o.vcf))) return 1;
     const double t_loop0 = now();
     if (!region_loop(s, fetcher, run)) return 1;
@@ -751,11 +791,20 @@ int run_list(const Options &o, Engines &engines, const std::vector<ListSample> &
             continue;
         }
         const int out_fd = e.out.empty() ? STDOUT_FILENO : fd[0], err_fd = e.err.empty() ? -1 : fd.back();
+        Out out;                                                 // (--vcf-samples: the samples write no STDOUT)
+        out.fd = out_fd;
+        if (!e.out.empty() && !out.open(o, out_fd, why)) {
+            for (int f : fd) ::close(f);
+            if (ahead.valid()) ahead.get();
+            failed("sample %zu (%s) failed: %s\n", why);
+            if (next_ahead) ahead = open_ahead(k + 1, true);
+            continue;
+        }
         int saved_fd2 = -1;
         if (err_fd >= 0) { std::fflush(stderr); saved_fd2 = ::dup(2); ::dup2(err_fd, 2); }
         std::unique_ptr<Sample> cur = ahead.valid() ? ahead.get() : open_sample(o, e.in, now(), stderr, pool.get(), true);
         if (next_ahead) ahead = open_ahead(k + 1, !cur->uses_windows());
-        const int rc = run_sample(o, engines, *cur, out_fd, stderr, t_main0, vcf_ans ? &(*vcf_ans)[k] : nullptr);
+        const int rc = run_sample(o, engines, *cur, out, stderr, t_main0, vcf_ans ? &(*vcf_ans)[k] : nullptr);
         cur.reset();                                                     // htslib's closing lines still go to this ERR
         if (err_fd >= 0) {
             if (std::fflush(stderr) != 0) why = e.err + ": " + std::strerror(errno);
@@ -765,6 +814,7 @@ int run_list(const Options &o, Engines &engines, const std::vector<ListSample> &
             ::close(saved_fd2);
             if (::close(err_fd) != 0 && why.empty()) why = e.err + ": " + std::strerror(errno);
         }
+        if (!out.close() && why.empty()) why = e.out + ": " + std::strerror(errno);
         if (out_fd != STDOUT_FILENO && ::close(out_fd) != 0 && why.empty()) why = e.out + ": " + std::strerror(errno);
         const std::string see = e.err.empty() ? "the lines above" : e.err;
         if (rc < 0) {
@@ -810,13 +860,17 @@ int run_vcf_samples(const Options &o, Engines &engines, const std::vector<ListSa
     if (n_failed < 0) return leave(engines, none, 1);
     int status = n_failed ? 1 : 0;
     if (!o.decode_only) {
+        Out dst; std::string why;
+        if (!dst.open(o, STDOUT_FILENO, why)) { std::fprintf(stderr, "%s\n", why.c_str()); return leave(engines, none, 1); }
         std::string out = vcf_header(*o.vcf);
         bool ok = true;
         for (size_t ri = 0; ri < o.vcf->rec.size() && ok; ++ri) {
             vcf_line(*o.vcf, ri, ans.data(), out);
-            if (out.size() >= (size_t(1) << 22)) { ok = write_all(STDOUT_FILENO, out); out.clear(); }
+            if (out.size() >= (size_t(1) << 22)) { ok = dst.write(out); out.clear(); }
         }
-        if (!ok || !write_all(STDOUT_FILENO, out)) { std::fprintf(stderr, "writing the VCF: %s\n", std::strerror(errno)); status = 1; }
+        ok = ok && dst.write(out);
+        if (!dst.close()) ok = false;
+        if (!ok) { std::fprintf(stderr, "writing the VCF: %s\n", std::strerror(errno)); status = 1; }
     }
     if (o.timing) std::fprintf(stderr, "[brc timing] vcf-samples: %zu samples (%d failed) in %.3fs since main()\n", list.size(), n_failed, now() - t_main0);
     return leave(engines, none, status);
@@ -835,7 +889,7 @@ int main(int argc, char **argv) {
                           {"per-library", 0, 0, 'p'}, {"max-warnings", 1, 0, 'w'}, {"insertion-centric", 0, 0, 'i'}, {"shard", 1, 0, 1000},
                           {"min-alt-count", 1, 0, 1001}, {"min-alt-fraction", 1, 0, 1002}, {"bam-list", 1, 0, 1003},
                           {"vcf", 1, 0, 1004}, {"vcf-sample", 1, 0, 1005}, {"vcf-samples", 1, 0, 1006},
-                          {"vcf-complex", 0, 0, 1007}, {"alt-min", 1, 0, 1008}, {"alt-max", 1, 0, 1009}, {0, 0, 0, 0}};
+                          {"vcf-complex", 0, 0, 1007}, {"alt-min", 1, 0, 1008}, {"alt-max", 1, 0, 1009}, {"bgzf", 0, 0, 1010}, {0, 0, 0, 0}};
     long min_alt_count = 0; double min_alt_fraction = -1.0;       // site filter (brc_set_site_filter); off unless one is given
     bool help = false, version = false;
     for (int c; (c = getopt_long(argc, argv, "hvq:b:d:l:f:D:pw:i", lo, nullptr)) != -1;) {
@@ -865,6 +919,7 @@ int main(int argc, char **argv) {
         case 1007: o.vcf_complex = true; break;
         case 1008: if (!parse_bound("--alt-min", optarg, o.bounds.lo_set, o.bounds.lo)) return 1; break;
         case 1009: if (!parse_bound("--alt-max", optarg, o.bounds.hi_set, o.bounds.hi)) return 1; break;
+        case 1010: o.bgzf = true; break;
         default: usage(); return 1;
         }
     }
@@ -912,11 +967,12 @@ int main(int argc, char **argv) {
     o.decode_only = std::getenv("BRC_CLI_DECODE_ONLY") != nullptr;   // test hook: exercise BGZF/BAI/region fetch without a GPU
     o.device_decode = std::getenv("BRC_CLI_DEVICE_DECODE") != nullptr && !o.decode_only;
     o.timing = std::getenv("BRC_CLI_TIMING") != nullptr;
+    o.device = std::getenv("BRC_DEVICE") ? std::atoi(std::getenv("BRC_DEVICE")) : 0;
 
     Engines engines;
     brc_config &cfg = engines.cfg;
     cfg.min_mapq = o.min_mapq; cfg.min_bq = o.min_bq; cfg.max_cnt = o.max_cnt; cfg.per_lib = o.per_lib; cfg.insertion_centric = o.ic;
-    cfg.n_libs = 0; cfg.device = std::getenv("BRC_DEVICE") ? std::atoi(std::getenv("BRC_DEVICE")) : 0;
+    cfg.n_libs = 0; cfg.device = o.device;
     if (!bam_list.empty()) {
         o.region_args.assign(argv + optind, argv + argc);          // every positional argument is a region of every sample
         return run_cohort(o, engines, bam_list, t_main0);
@@ -930,7 +986,13 @@ int main(int argc, char **argv) {
     std::unique_ptr<Sample> s = open_sample(o, bam_path, t_main0, stderr, pool.get(), true);
     std::vector<VcfAnswers> vcf_ans;
     if (o.vcf) vcf_ans.emplace_back(vcf);
-    const int rc = run_sample(o, engines, *s, STDOUT_FILENO, stderr, t_main0, vcf_ans.data());
+    Out out; std::string why;
+    if (!out.open(o, STDOUT_FILENO, why)) { std::fprintf(stderr, "%s\n", why.c_str()); return leave(engines, s, 1); }
+    int rc = run_sample(o, engines, *s, out, stderr, t_main0, vcf_ans.data());
+    if (!out.close()) {                   // a failure a write already reported is not reported twice
+        if (!out.failed) std::fprintf(stderr, "writing the output: %s\n", std::strerror(errno));
+        rc = 1;
+    }
     return leave(engines, s, rc < 0 ? 1 : rc);
 }
 

@@ -94,6 +94,7 @@ const char *brc_strerror(int s) {
     case BRC_E_NO_REFERENCE: return "reference window missing or too small";
     case BRC_E_BAD_LIBRARY: return "library id out of range";
     case BRC_E_OVERFLOW: return "internal pool overflow";
+    case BRC_E_IO: return "write to the output failed";
     default: return "unknown status";
     }
 }

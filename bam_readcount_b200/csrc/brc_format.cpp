@@ -12,6 +12,7 @@
 // threads over disjoint site ranges — the deletion shift only needs the site to the left, which each
 // thread re-derives for its first site.
 #include <algorithm>
+#include <cerrno>
 #include <cstdio>
 #include <cstring>
 #include <deque>
@@ -330,6 +331,26 @@ extern "C" int64_t brc_write_text(brc_engine *e, int64_t region_index, int64_t f
             const ssize_t w = ::write(fd, p.data() + done, p.size() - done);
             if (w < 0) { release_parts(e); return brc::set_error(e, BRC_E_INVALID, "write_text: write() failed"); }
             done += (size_t)w;
+        }
+        total += (int64_t)p.size();
+    }
+    release_parts(e);
+    return total;
+}
+
+// Same text into a BGZF writer: each formatted part is copied once, into the writer's page-locked staging.
+extern "C" int64_t brc_write_text_bgzf(brc_engine *e, int64_t region_index, int64_t first, int64_t count, const char *const *lib_names,
+                                       brc_bgzf_writer *w) {
+    if (!e || !w || region_index >= (int64_t)e->regions.size() || first < 0) return BRC_E_INVALID;
+    if (int rc = brc::check_view(e, "write_text_bgzf", kTextKinds)) return rc;
+    if (region_index < 0) ensure_formatted(e, -1, -1, -1, lib_names);
+    else ensure_formatted(e, region_index, first, count < 0 ? (int64_t)0x7fffffff : count, lib_names);
+    int64_t total = 0;
+    for (auto &p : e->fmt_parts) {
+        if (int rc = brc_bgzf_write(w, p.data(), p.size())) {
+            const std::string why = rc == BRC_E_IO ? std::strerror(errno) : brc_strerror(rc);
+            release_parts(e);
+            return brc::set_error(e, rc, "write_text_bgzf: " + why);
         }
         total += (int64_t)p.size();
     }

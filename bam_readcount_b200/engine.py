@@ -171,6 +171,7 @@ EXPORTS = [
     "brc_get_reference_codes", "brc_get_read_descriptors", "brc_get_quotient_rows",
     "brc_set_site_filter", "brc_set_site_filter_bounds", "brc_get_selected_results", "brc_set_allele_queries", "brc_get_allele_answers", "brc_last_results_kind",
     "brc_set_complex_queries", "brc_get_complex_answers",
+    "brc_set_device", "brc_bgzf_open", "brc_bgzf_write", "brc_bgzf_close", "brc_bgzf_stats", "brc_write_text_bgzf",
 ]
 
 _lib = None
@@ -242,9 +243,54 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
                                             C.c_char_p, C.c_int64]
     lib.brc_get_complex_answers.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_int64),
                                             C.POINTER(C.c_int64)]
+    lib.brc_set_device.argtypes = [C.c_int]
+    lib.brc_bgzf_open.argtypes = [C.c_int, C.POINTER(C.c_void_p)]
+    lib.brc_bgzf_write.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
+    lib.brc_bgzf_close.argtypes = [C.c_void_p]
+    lib.brc_bgzf_stats.argtypes = [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_double)]
+    lib.brc_write_text_bgzf.argtypes = [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p]
+    lib.brc_write_text_bgzf.restype = C.c_int64
     if path is None:
         _lib = lib
     return lib
+
+
+class BgzfWriter:
+    """BGZF output compressed on the device (brc_bgzf_open / _write / _close) onto an open file descriptor, which stays open.
+    Raises BrcError(BRC_E_NO_DEVICE) without a usable device."""
+
+    def __init__(self, fd: int):
+        self.lib = load_library()
+        self.h = C.c_void_p()
+        rc = self.lib.brc_bgzf_open(fd, C.byref(self.h))
+        if rc != 0:
+            raise BrcError(rc, self.lib.brc_strerror(rc).decode())
+
+    def write(self, data) -> None:
+        mv = memoryview(data).cast("B")
+        buf = (C.c_char * len(mv)).from_buffer_copy(mv) if len(mv) else None
+        rc = self.lib.brc_bgzf_write(self.h, buf, len(mv))
+        if rc != 0:
+            raise BrcError(rc, self.lib.brc_strerror(rc).decode())
+
+    def stats(self) -> dict:
+        i, o, ms = C.c_int64(), C.c_int64(), C.c_double()
+        self.lib.brc_bgzf_stats(self.h, C.byref(i), C.byref(o), C.byref(ms))
+        return {"bytes_in": i.value, "bytes_out": o.value, "kernel_ms": ms.value}
+
+    def close(self) -> None:
+        if not self.h:
+            return
+        h, self.h = self.h, C.c_void_p()
+        rc = self.lib.brc_bgzf_close(h)
+        if rc != 0:
+            raise BrcError(rc, self.lib.brc_strerror(rc).decode())
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
 
 
 def _np_view(ptr, n, dtype):

@@ -62,7 +62,8 @@ typedef enum {
     BRC_E_UNSORTED = -5,      /* reads of a region not sorted by position (htslib: "Pileup aborts", V:htslib-1.10/sam.c:4502-4511) */
     BRC_E_NO_REFERENCE = -6,  /* reference window does not cover the region (the reference binary would SIGSEGV, SURVEY.md A.6) */
     BRC_E_BAD_LIBRARY = -7,   /* library id >= n_libs */
-    BRC_E_OVERFLOW = -8       /* internal pool overflow that retry could not resolve */
+    BRC_E_OVERFLOW = -8,      /* internal pool overflow that retry could not resolve */
+    BRC_E_IO = -9             /* write() to an output failed (errno holds its reason when a brc_bgzf_* call returns it) */
 } brc_status;
 
 #define BRC_TAG_ABSENT INT32_MIN  /* NM:i / SM:i tag not present on the read */
@@ -461,6 +462,29 @@ BRC_API int64_t brc_last_h2d_bytes(const brc_engine *e);
  * 3 = site selection + compaction (0 when no filter was set), 4 = allele queries (0 when none were set), 5 = the complex-record
  * kernel, without the upload of its queries (0 when none were set) */
 BRC_API float brc_last_stage_ms(const brc_engine *e, int stage);
+
+/* ---- BGZF output, compressed on the device (DESIGN.md §13) ----------------------------------
+ * A writer turns the bytes given to brc_bgzf_write into a BGZF file on `fd` as htslib writes one: members of 65280 input bytes
+ * (the last one shorter), each the smallest of a dynamic-Huffman, fixed-Huffman or stored DEFLATE stream, then the 28-byte
+ * empty EOF member.  The bytes written depend only on the byte stream, not on how it was split into calls.  No engine handle:
+ * the writer uses the device current at brc_bgzf_open (brc_set_device chooses it) on its own stream; each call makes that device
+ * current and restores the caller's.  It stages the stream in page-locked memory and compresses a chunk of members on the
+ * device while the caller produces the next one; members reach `fd` in order.
+ * A failed write() (EPIPE, ENOSPC, ...) or CUDA failure is returned by the next call and by brc_bgzf_close.  Not thread-safe. */
+typedef struct brc_bgzf_writer brc_bgzf_writer;
+/* makes `device` current on the calling thread (cudaSetDevice), so that a host built without the CUDA runtime opens its writer
+ * on the device its engines use (brc_config.device); BRC_E_NO_DEVICE when that is not a usable device */
+BRC_API int brc_set_device(int device);
+BRC_API int brc_bgzf_open(int fd, brc_bgzf_writer **out);           /* BRC_E_NO_DEVICE without a usable device */
+BRC_API int brc_bgzf_write(brc_bgzf_writer *w, const void *buf, size_t n);   /* BRC_E_IO: errno is set to the write's */
+/* flush, the EOF member, free (fd stays open); the first failure seen, if any (BRC_E_IO: errno is set to the write's) */
+BRC_API int brc_bgzf_close(brc_bgzf_writer *w);
+/* bytes taken, compressed bytes written, and GPU milliseconds of the chunks' kernels (CUDA events), so far */
+BRC_API int brc_bgzf_stats(const brc_bgzf_writer *w, int64_t *bytes_in, int64_t *bytes_out, double *kernel_ms);
+/* brc_write_text's text handed to a BGZF writer instead of a file descriptor (the formatted parts go straight into its staging).
+ * Returns the bytes of text, or a negative status (the writer's, when it failed). */
+BRC_API int64_t brc_write_text_bgzf(brc_engine *e, int64_t region_index, int64_t first, int64_t count, const char *const *lib_names,
+                                    brc_bgzf_writer *w);
 
 #ifdef __cplusplus
 }
