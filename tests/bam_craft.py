@@ -23,6 +23,7 @@ from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 
+import cases
 from bam_readcount_b200.batch import LIB_NONE, TAG_ABSENT, ReadBatch
 
 OPS = "MIDNSHP=X"
@@ -386,11 +387,11 @@ def write_corpus(d: str, samtools: str) -> List[dict]:
             subprocess.check_call([samtools, "view", "-C", "-T", os.path.join(d, "c.fa"), "-o", cram, bam])
             subprocess.check_call([samtools, "index", cram])
             out.append(dict(out[-1], name=name + "_cram", bam=cram))
-    out.append(long_cigar_bam(d, samtools))
+    out.append(long_cigar_bam(d))
     return out
 
 
-def long_cigar_bam(d: str, samtools: str) -> dict:
+def long_cigar_bam(d: str) -> dict:
     """A read of 65537 CIGAR ops among ordinary reads, written as SAM text and converted by samtools, which stores its CIGAR in
     CG:B:I (the only way BAM can hold more than 65535 ops)."""
     from bam_readcount_b200 import synth
@@ -409,10 +410,7 @@ def long_cigar_bam(d: str, samtools: str) -> dict:
     sam = os.path.join(d, "long.sam")
     with open(sam, "w") as fh:
         fh.write(f"@HD\tVN:1.6\tSO:coordinate\n@SQ\tSN:c1\tLN:{L}\n" + HEADER_RG + "\n".join(rows) + "\n")
-    bam = os.path.join(d, "long.bam")
-    subprocess.check_call([samtools, "view", "-b", "-o", bam, sam])
-    subprocess.check_call([samtools, "index", bam])
-    return dict(name="long", bam=bam, fasta=os.path.join(d, "long.fa"), regions=["c1:40-400", "c1:65480-65620"], vs_reference=True)
+    return dict(name="long", bam=cases.sam_to_bam(sam), fasta=os.path.join(d, "long.fa"), regions=["c1:40-400", "c1:65480-65620"], vs_reference=True)
 
 
 # ------------------------------------------------------------------------------------------------

@@ -7,18 +7,27 @@ them, ``site_list`` (True: -l loop, False: argv regions), flags, lib_names.
 The harness every parity test goes through: ``run_oracle`` / ``run_oracle_cached``, ``run_engine`` (one brc_compute over the
 case's regions) and ``run_engine_per_region`` (one per region, deletion queue carried), ``assert_same`` and ``first_diff`` to
 compare them, ``device_batch`` / ``run_device`` for the device-resident path, ``assert_anchor`` for the reference binary's
-SHA-256, and ``cli`` / ``samtools`` / ``inflate_check`` for the executables the tests run.
+SHA-256.
+
+The fixtures of the tests that run executables: ``cli`` / ``samtools`` / ``check_program`` build or find them;
+``write_fasta``, ``write_testbam_fasta``, ``write_bam``, ``sam_to_bam`` and ``synthetic_bam`` write their inputs;
+``load_golden_text`` / ``golden_texts`` read the committed outputs.
 """
 from __future__ import annotations
 
+import atexit
 import contextlib
 import dataclasses
+import functools
 import gzip
 import hashlib
 import json
 import os
+import re
+import shutil
 import subprocess
 import sys
+import tempfile
 from typing import NamedTuple, Optional
 
 import numpy as np
@@ -28,9 +37,11 @@ if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
 from bam_readcount_b200 import synth  # noqa: E402
-from bam_readcount_b200.batch import BatchBuilder, ReadBatch  # noqa: E402
+from bam_readcount_b200.batch import BatchBuilder, ReadBatch, TAG_ABSENT  # noqa: E402
 
 GOLDEN = os.path.join(ROOT, "tests", "golden")
+CRAM_DATA = os.path.join(ROOT, "oracle", "_ref", "test-data")      # the reference's test-data, CRAM fixture included
+DECODE_ONLY = dict(os.environ, BRC_CLI_DECODE_ONLY="1")            # brc-readcount prints per-region record summaries, no device
 
 FLAG_SETS = {
     "default": dict(),
@@ -86,6 +97,43 @@ def testbam_case(bad_rg=False):
     return dict(name="test_bam_bad_rg" if bad_rg else "test_bam", contigs=[("21", int(z["chrom_len"]), ref, win_beg)],
                 tid_map={20: 0}, batch=batch, regions=[(0, 10402985, 10402985), (0, 10405200, 10405200)], site_list=True,
                 lib_names=[s for s in str(z["lib_names"]).split("\t") if s])
+
+
+@functools.lru_cache(maxsize=None)
+def testbam_chr21() -> bytes:
+    """Contig 21 of test.bam as its ref.fa holds it: N everywhere except the window the fixture's reads touch."""
+    z = np.load(os.path.join(GOLDEN, "test_bam.npz"))
+    wb = int(z["ref_win_beg"])
+    seq = np.full(int(z["chrom_len"]), ord("N"), dtype=np.uint8)
+    seq[wb:wb + z["ref_win"].shape[0]] = z["ref_win"]
+    return seq.tobytes()
+
+
+def crafted_case(reads, regions, n_libs=1, L=300, seed=3):
+    """A case from hand-placed reads: (pos, cigar, mismatch positions, library), optionally followed by mapq and flag (default
+    60 and 0; SM is the mapq).  Every read copies the reference except at its mismatch positions."""
+    rng = np.random.default_rng(seed)
+    ref = bytes(rng.choice(list(b"ACGT"), L).astype(np.uint8))
+    other = {ord("A"): "C", ord("C"): "G", ord("G"): "T", ord("T"): "A"}
+    bb = BatchBuilder()
+    for k, (pos, cigar, mism, lib, *rest) in enumerate(reads):
+        mapq, flag = rest or (60, 0)
+        seq, p = [], pos
+        for n, op in re.findall(r"(\d+)([MID])", cigar):
+            n = int(n)
+            if op == "M":
+                seq += [other[ref[q]] if q in mism else chr(ref[q]) for q in range(p, p + n)]
+                p += n
+            elif op == "D":
+                p += n
+            else:
+                seq += ["A"] * n
+        bb.add_sam(tid=0, pos=pos, flag=flag, mapq=mapq, lib=lib, cigar=cigar, seq="".join(seq), qual="I" * len(seq),
+                   nm=len(mism), sm=mapq, qname=f"r{k}")
+    b = bb.build()
+    order = np.argsort(b.pos, kind="stable")
+    return dict(name="crafted", contigs=[("chr1", L, ref, 0)], batch=b.select(order), regions=list(regions), site_list=False,
+                lib_names=[f"lib{i}" for i in range(n_libs)])
 
 
 def case_tid(case, ci):
@@ -215,7 +263,9 @@ def run_engine_per_region(case, flags, site_list=None, *, dump=False) -> list:
 
 
 def first_diff(got: str, want: str) -> str:
-    """The first line where two texts differ (keeps pytest from diffing megabytes of text)."""
+    """The first line where two texts differ, '' when they are equal (keeps pytest from diffing megabytes of text)."""
+    if got == want:
+        return ""
     la, lb = got.splitlines(), want.splitlines()
     for i, (x, y) in enumerate(zip(la, lb)):
         if x != y:
@@ -316,12 +366,82 @@ def samtools() -> str:
     return REF_SAMTOOLS
 
 
-def inflate_check(workdir: str) -> str:
-    """Compiles tests/inflate_check.cpp (the device DEFLATE core against zlib, on the CPU) into workdir; the executable's path."""
-    exe = os.path.join(workdir, "inflate_check")
+def have_htslib() -> bool:
+    """brc-readcount can be built with htslib, and so read CRAM: tools/build_htslib.sh has left its library."""
+    return os.path.exists(os.path.join(ROOT, "bam_readcount_b200", "third_party", "htslib", "libhts.a"))
+
+
+@functools.lru_cache(maxsize=None)
+def _check_dir() -> str:
+    d = tempfile.mkdtemp(prefix="brc_checks_")
+    atexit.register(shutil.rmtree, d, True)
+    return d
+
+
+@functools.lru_cache(maxsize=None)
+def check_program(name: str, *extra_flags: str) -> str:
+    """Compiles tests/<name>.cpp, a CPU check program over headers in csrc/, once per test session; the executable's path.
+    extra_flags follow the source on the g++ line (libraries to link, -pthread)."""
+    exe = os.path.join(_check_dir(), name)
     subprocess.check_call(["g++", "-O2", "-std=c++17", "-I", os.path.join(ROOT, "bam_readcount_b200", "csrc"), "-o", exe,
-                           os.path.join(ROOT, "tests", "inflate_check.cpp"), "-lz"])
+                           os.path.join(ROOT, "tests", name + ".cpp"), *extra_flags])
     return exe
+
+
+def write_fasta(path: str, contigs) -> str:
+    """A FASTA of the (name, sequence bytes) contigs in 60 columns, and its .fai; the FASTA's path."""
+    with open(path, "wb") as fa, open(path + ".fai", "w") as fai:
+        off = 0
+        for name, seq in contigs:
+            head = f">{name}\n".encode()
+            body = b"".join(seq[i:i + 60] + b"\n" for i in range(0, len(seq), 60))
+            fa.write(head + body)
+            fai.write(f"{name}\t{len(seq)}\t{off + len(head)}\t60\t61\n")
+            off += len(head) + len(body)
+    return path
+
+
+def write_testbam_fasta(path: str) -> str:
+    """The ref.fa of test.bam's contig 21 (testbam_chr21) at path, and its .fai; the path."""
+    synth.write_fasta(path, "21", np.frombuffer(testbam_chr21(), dtype=np.uint8))
+    return path
+
+
+def sam_to_bam(sam: str, keep_sam: bool = True) -> str:
+    """samtools view -b of a .sam file into the .bam beside it, indexed; the BAM's path.  Skips the test without samtools."""
+    exe, bam = samtools(), sam[:-len(".sam")] + ".bam"
+    subprocess.check_call([exe, "view", "-b", "-o", bam, sam])
+    subprocess.check_call([exe, "index", bam])
+    if not keep_sam:
+        os.remove(sam)
+    return bam
+
+
+def write_bam(d: str, stem: str, batch, contigs, *, keep_sam: bool = True, **sam_kw) -> str:
+    """The batch as d/<stem>.sam (synth.write_sam with the contigs [(name, length)] and sam_kw), then as an indexed
+    d/<stem>.bam; the BAM's path."""
+    sam = os.path.join(d, stem + ".sam")
+    synth.write_sam(sam, batch, contigs, **sam_kw)
+    return sam_to_bam(sam, keep_sam)
+
+
+CONTIGS = {"chrA": (24000, 11), "chrB": (16000, 12), "chrC": (12000, 13)}       # name -> (length, reference seed)
+
+
+def synthetic_bam(d, name, order, n_libs, seed, depth=8, no_nm=0) -> str:
+    """A coordinate-sorted BAM d/<name>.bam whose @SQ lines are `order` (a subset of CONTIGS, in any order), with n_libs
+    libraries (0: no @RG at all) and `no_nm` reads without an NM tag (they draw warnings)."""
+    parts = []
+    for tid, c in enumerate(order):
+        ref = synth.synth_reference(CONTIGS[c][0], CONTIGS[c][1])
+        parts.append(synth.synth_reads(ref, depth, seed=seed + 101 * tid, n_libs=max(n_libs, 1), tid=tid))
+    b = ReadBatch.concat(parts)
+    if no_nm:
+        nm = np.array(b.nm, copy=True)
+        nm[np.random.default_rng(seed).choice(b.n_reads, no_nm, replace=False)] = TAG_ABSENT
+        b = dataclasses.replace(b, nm=nm)
+    return write_bam(d, name, b, [(c, CONTIGS[c][0]) for c in order], keep_sam=False, n_libs=max(n_libs, 1),
+                     read_group=n_libs > 0)
 
 
 def load_golden_text(name: str) -> str:
@@ -331,3 +451,9 @@ def load_golden_text(name: str) -> str:
             return fh.read().decode("latin-1")
     with open(p, "rb") as fh:
         return fh.read().decode("latin-1")
+
+
+def golden_texts():
+    """[(name, text)] of every committed output text: the expected_* files and the *.txt.gz files, by name."""
+    names = sorted({f[:-3] if f.endswith(".gz") else f for f in os.listdir(GOLDEN) if f.endswith(".txt.gz") or f.startswith("expected_")})
+    return [(n, load_golden_text(n)) for n in names]

@@ -5,7 +5,7 @@ import re
 
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from cases import ROOT
 
 
 def _declared():

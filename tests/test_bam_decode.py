@@ -22,9 +22,7 @@ import pytest
 import bam_craft
 import cases
 from bam_readcount_b200 import bamio
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-GOLDEN = os.path.join(ROOT, "tests", "golden")
+from cases import GOLDEN
 FLAGS = {"default": {}, "p": dict(per_lib=True), "i": dict(insertion_centric=True), "q20b20": dict(min_mapq=20, min_bq=20)}
 ARRAYS = ("pos", "flag", "mapq", "lib", "l_qseq", "nm", "sm", "cigar_off", "cigar", "seq_off", "seq", "qual_off", "qual")
 NAMES = ["cg", "dtag", "nmtype", "rg", "rg_nolib", "trunc", "long"]
@@ -125,10 +123,10 @@ RECUTS = [("level", 0), ("level", 1), ("level", 9), ("strategy", zlib.Z_FILTERED
           ("strategy", zlib.Z_RLE), ("strategy", zlib.Z_FIXED), ("cut", 97), ("empty",), ("full",)]
 
 
-def test_deflate_core_on_the_recut_corpus(corpus, tmp_path):
+def test_deflate_core_on_the_recut_corpus(corpus):
     """The DEFLATE core of the device kernel (one lane, on the CPU) against zlib on every member of every recut file, and its
     refusal of each member cut in half."""
-    exe = cases.inflate_check(str(tmp_path))
+    exe = cases.check_program("inflate_check", "-lz")
     files = [_recut(corpus[n], how) for n in ("cg", "long") for how in RECUTS]
     nblk, bad = map(int, subprocess.check_output([exe] + files).split())
     assert bad == 0 and nblk > 100
@@ -153,10 +151,10 @@ def test_deflate_corpus_covers_every_construct(crafted):
     assert sum(1 for e in crafted["deflate_info"][2:] if beg < e < end) >= 2
 
 
-def test_deflate_core_on_the_crafted_members(crafted, tmp_path):
+def test_deflate_core_on_the_crafted_members(crafted):
     """The DEFLATE core (one lane, on the CPU) against zlib on every crafted member, and its refusal of each member cut in half;
     bamio and the restatement read the same records from both crafted files."""
-    exe = cases.inflate_check(str(tmp_path))
+    exe = cases.check_program("inflate_check", "-lz")
     nblk, bad = map(int, subprocess.check_output([exe, crafted["deflate"]]).split())
     assert bad == 0 and nblk >= 8
     for path in (crafted["deflate"], crafted["frame"]):
@@ -313,7 +311,7 @@ def test_cli_cram_reads_the_first_rg_whatever_its_type(corpus, name):
     """The RG files as CRAM, read through htslib: brc-readcount -p prints the reference's stdout and stderr on the same CRAM
     (an H-typed first RG names its read group; a non-string one leaves the read without a library)."""
     from bam_readcount_b200 import build
-    if not os.path.exists(os.path.join(ROOT, "bam_readcount_b200", "third_party", "htslib", "libhts.a")):
+    if not cases.have_htslib():
         pytest.skip("host built without htslib (tools/build_htslib.sh)")
     exe = build.build_cli()
     f = corpus[name]

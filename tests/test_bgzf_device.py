@@ -12,13 +12,11 @@ import pytest
 
 import cases
 from bam_readcount_b200 import bamio
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-GOLDEN = os.path.join(ROOT, "tests", "golden")
+from cases import GOLDEN
 
 def test_deflate_core_matches_zlib_on_every_block(tmp_path):
     """The exact DEFLATE code the kernel runs (host+device source), block by block against zlib: dynamic, fixed and stored blocks."""
-    exe = cases.inflate_check(str(tmp_path))
+    exe = cases.check_program("inflate_check", "-lz")
     files = [os.path.join(GOLDEN, "test.bam"), os.path.join(GOLDEN, "test_bad_rg.bam")]
     from oracle.oracle import REF_SAMTOOLS
     if os.path.exists(REF_SAMTOOLS):

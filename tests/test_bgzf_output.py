@@ -15,20 +15,16 @@ import pytest
 
 import cases
 import vcf_cases
+from cases import GOLDEN
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-GOLDEN = os.path.join(ROOT, "tests", "golden")
 BLOCK = 0xff00
 HEADER = b"\x1f\x8b\x08\x04\x00\x00\x00\x00\x00\xff\x06\x00BC\x02\x00"
 EOF = HEADER + b"\x1b\x00\x03\x00\x00\x00\x00\x00\x00\x00\x00\x00"
 
 
 @pytest.fixture(scope="module")
-def dc(tmp_path_factory):
-    exe = str(tmp_path_factory.mktemp("dc") / "deflate_check")
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-I", os.path.join(ROOT, "bam_readcount_b200", "csrc"), "-o", exe,
-                           os.path.join(ROOT, "tests", "deflate_check.cpp")])
-    return exe
+def dc():
+    return cases.check_program("deflate_check")
 
 
 def members(data: bytes):
@@ -184,7 +180,7 @@ def _texts():
     return {n: cases.load_golden_text(n).encode("latin-1") for n in names}
 
 
-def _crafted():
+def _crafted_inputs():
     rng = random.Random(11)
     far = bytes(rng.getrandbits(8) for _ in range(300))
     return {
@@ -212,7 +208,7 @@ def test_writer_on_the_device_set_before_it_opens(tmp_path):
 
 @pytest.mark.gpu
 def test_writer_round_trip_and_member_layout(tmp_path):
-    inputs = dict(_crafted())
+    inputs = dict(_crafted_inputs())
     inputs.update(_texts())
     vcf = vcf_cases.vcf_text(vcf_cases.fixture_records()).encode()
     inputs["vcf fixture"] = vcf
@@ -235,7 +231,7 @@ def test_writer_round_trip_and_member_layout(tmp_path):
 @pytest.mark.gpu
 def test_writer_output_does_not_depend_on_the_write_calls(tmp_path):
     rng = random.Random(4)
-    data = b"".join(list(_texts().values())[:3]) + _crafted()["random"]
+    data = b"".join(list(_texts().values())[:3]) + _crafted_inputs()["random"]
     big = data * ((40 << 20) // len(data) + 1)          # about 40 MB: the writer's 16.7 MB chunks, and a part of one more
     whole = compress([big], tmp_path)
     assert gzip.decompress(whole) == big
@@ -273,8 +269,7 @@ def _plain_and_bgzf(argv, env=None, rc=0):
 
 @pytest.mark.gpu
 def test_cli_bgzf_integration_lines_and_site_filter(tmp_path):
-    from test_cli import _write_ref
-    ref = _write_ref(str(tmp_path))
+    ref = cases.write_testbam_fasta(str(tmp_path / "ref.fa"))
     sl = os.path.join(GOLDEN, "site_list")
     regions = ["21:10402985-10402985", "21:10405200-10405200"]
     runs = [["-l", sl], ["-p", "-l", sl], ["-i", "-l", sl], ["-i", "-p", "-l", sl]]
@@ -290,8 +285,7 @@ def test_cli_bgzf_integration_lines_and_site_filter(tmp_path):
 
 @pytest.mark.gpu
 def test_cli_bgzf_vcf_plain_bgzip_complex_and_samples(tmp_path):
-    fa = str(tmp_path / "ref.fa")
-    vcf_cases.write_fasta21(fa)
+    fa = cases.write_testbam_fasta(str(tmp_path / "ref.fa"))
     text = vcf_cases.vcf_text(vcf_cases.fixture_records())
     plain_vcf, gz_vcf = str(tmp_path / "a.vcf"), str(tmp_path / "a.vcf.gz")
     open(plain_vcf, "w").write(text)
@@ -311,9 +305,8 @@ def test_cli_bgzf_vcf_plain_bgzip_complex_and_samples(tmp_path):
 
 @pytest.mark.gpu
 def test_cli_bgzf_bam_list_out_files(tmp_path):
-    from test_cli import _write_ref
     exe = cases.cli()
-    ref = _write_ref(str(tmp_path))
+    ref = cases.write_testbam_fasta(str(tmp_path / "ref.fa"))
     bams = [os.path.join(GOLDEN, b) for b in ("test.bam", "test_bad_rg.bam", "test.bam")]
     regions = ["21:10402985-10402990", "21:10405200-10405210"]
     outs = {}

@@ -9,12 +9,8 @@ import numpy as np
 import pytest
 
 import cases
+from cases import CRAM_DATA, GOLDEN, ROOT
 from cases import cli as _cli
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-GOLDEN = os.path.join(ROOT, "tests", "golden")
-
-
 
 
 def test_cli_help_and_version_exit_code_1():
@@ -24,17 +20,6 @@ def test_cli_help_and_version_exit_code_1():
         assert p.returncode == 1          # R:src/exe/bam-readcount/bamreadcount.cpp:467-475
     p = subprocess.run([exe], capture_output=True)
     assert p.returncode == 1 and b"Usage: bam-readcount" in p.stdout
-
-
-def _write_ref(tmp):
-    """ref.fa of contig 21: N everywhere except the window the fixture reads touch (stored in test_bam.npz)."""
-    z = np.load(os.path.join(GOLDEN, "test_bam.npz"))
-    L, wb = int(z["chrom_len"]), int(z["ref_win_beg"])
-    seq = np.full(L, ord("N"), dtype=np.uint8)
-    seq[wb:wb + z["ref_win"].shape[0]] = z["ref_win"]
-    from bam_readcount_b200 import synth
-    synth.write_fasta(os.path.join(tmp, "ref.fa"), "21", seq)
-    return os.path.join(tmp, "ref.fa")
 
 
 @pytest.mark.gpu
@@ -48,7 +33,7 @@ def _write_ref(tmp):
 ])
 def test_cli_reproduces_reference_goldens(tmp_path, args, bam, golden):
     exe = _cli()
-    ref = _write_ref(str(tmp_path))
+    ref = cases.write_testbam_fasta(str(tmp_path / "ref.fa"))
     argv = [exe, "-f", ref]
     regions = []
     for a in args:
@@ -70,16 +55,13 @@ def test_cli_reproduces_reference_goldens(tmp_path, args, bam, golden):
 def test_cli_synthetic_bam_matches_oracle(tmp_path):
     """A coordinate-sorted synthetic BAM (written with the samtools the oracle build leaves in oracle/_ref) through the
     CLI, whole-contig region and a site list, against the CPU oracle."""
-    REF_SAMTOOLS = cases.samtools()
     from bam_readcount_b200 import synth
     exe = _cli()
     case = cases.synthetic_case(L=40000, depth=30, seed=31, regions=((0, 1001, 38000),), site_list=False)
     name, L, seq, _ = case["contigs"][0]
     d = str(tmp_path)
     synth.write_fasta(os.path.join(d, "ref.fa"), name, np.frombuffer(seq, dtype=np.uint8))
-    synth.write_sam(os.path.join(d, "s.sam"), case["batch"], [(name, L)])
-    subprocess.check_call([REF_SAMTOOLS, "view", "-b", "-o", os.path.join(d, "s.bam"), os.path.join(d, "s.sam")])
-    subprocess.check_call([REF_SAMTOOLS, "index", os.path.join(d, "s.bam")])
+    cases.write_bam(d, "s", case["batch"], [(name, L)])
     for fl, argv in ((dict(min_mapq=20, min_bq=20), ["-q", "20", "-b", "20"]), (dict(per_lib=True, insertion_centric=True), ["-p", "-i"])):
         want, _, _ = cases.run_oracle(case, fl, site_list=False)
         p = subprocess.run([exe, "-w", "0", "-f", os.path.join(d, "ref.fa")] + argv + [os.path.join(d, "s.bam"), "chr1:1001-38000"], capture_output=True)
@@ -91,16 +73,13 @@ def test_cli_synthetic_bam_matches_oracle(tmp_path):
 def test_cli_windowed_long_region_equals_unsplit(tmp_path):
     """brc-readcount cuts long regions into windows (bounded memory); the concatenation must equal the unsplit output,
     deletions across window edges included."""
-    REF_SAMTOOLS = cases.samtools()
     from bam_readcount_b200 import synth
     exe = _cli()
     case = cases.synthetic_case(L=30000, depth=30, seed=41, regions=((0, 1, 30000),), site_list=False)
     name, L, seq, _ = case["contigs"][0]
     d = str(tmp_path)
     synth.write_fasta(os.path.join(d, "ref.fa"), name, np.frombuffer(seq, dtype=np.uint8))
-    synth.write_sam(os.path.join(d, "s.sam"), case["batch"], [(name, L)])
-    subprocess.check_call([REF_SAMTOOLS, "view", "-b", "-o", os.path.join(d, "s.bam"), os.path.join(d, "s.sam")])
-    subprocess.check_call([REF_SAMTOOLS, "index", os.path.join(d, "s.bam")])
+    cases.write_bam(d, "s", case["batch"], [(name, L)])
     outs = []
     for win in ("100000000", "3777"):
         p = subprocess.run([exe, "-w", "0", "-p", "-f", os.path.join(d, "ref.fa"), os.path.join(d, "s.bam"), "chr1:1-30000"],
@@ -143,21 +122,16 @@ def _site_list_regions(L, rng):
 
 
 def _make_bam(case, d):
-    from oracle.oracle import REF_SAMTOOLS
     from bam_readcount_b200 import synth
     name, L, seq, _ = case["contigs"][0]
     synth.write_fasta(os.path.join(d, "ref.fa"), name, np.frombuffer(seq, dtype=np.uint8))
-    synth.write_sam(os.path.join(d, "s.sam"), case["batch"], [(name, L)], n_libs=len(case["lib_names"]))
-    subprocess.check_call([REF_SAMTOOLS, "view", "-b", "-o", os.path.join(d, "s.bam"), os.path.join(d, "s.sam")])
-    subprocess.check_call([REF_SAMTOOLS, "index", os.path.join(d, "s.bam")])
-    return os.path.join(d, "s.bam"), os.path.join(d, "ref.fa")
+    return cases.write_bam(d, "s", case["batch"], [(name, L)], n_libs=len(case["lib_names"])), os.path.join(d, "ref.fa")
 
 
 def test_cli_site_list_fetch_merging_yields_samfetch_records_in_one_pass(tmp_path):
     """CPU (SURVEY.md §8 f-3): consecutive site-list lines share one forward pass over the BAM instead of one index seek
     each; every region must still receive exactly the records samfetch yields (checked against the Python decoder), and the
     fetch must seek and decode about as little as one pass over the file."""
-    REF_SAMTOOLS = cases.samtools()
     exe = _cli()
     case = cases.synthetic_case(L=60000, depth=30, seed=77, regions=((0, 1, 60000),), site_list=True)
     bam, _ = _make_bam(case, str(tmp_path))
@@ -187,7 +161,6 @@ def test_cli_site_list_fetch_merging_yields_samfetch_records_in_one_pass(tmp_pat
 def test_cli_dense_site_list_matches_oracle(tmp_path):
     """A few hundred site-list lines (dense, overlapping, nested, repeated, out of order) through the merged fetch, the
     engine and the emitter, against the CPU oracle run region by region like the reference's -l loop."""
-    REF_SAMTOOLS = cases.samtools()
     exe = _cli()
     regs = _site_list_regions(60000, np.random.default_rng(5))
     case = cases.synthetic_case(L=60000, depth=30, seed=77, regions=tuple((0, s, e) for s, e in regs), site_list=True)
@@ -204,24 +177,19 @@ def test_cli_dense_site_list_matches_oracle(tmp_path):
 def test_cli_fetch_merging_two_contigs_unsorted_and_past_the_end(tmp_path):
     """CPU: the merged fetch across contig changes, lines that go backwards, duplicates, a line past the contig's last read
     and an unknown contig — record sets identical to the Python decoder's samfetch."""
-    REF_SAMTOOLS = cases.samtools()
     import dataclasses
-    from bam_readcount_b200 import synth
     from bam_readcount_b200.batch import ReadBatch
     exe = _cli()
     a = cases.synthetic_case(L=30000, depth=20, seed=3, regions=((0, 1, 30000),), site_list=True)["batch"]
     b = cases.synthetic_case(L=20000, depth=25, seed=4, regions=((0, 1, 20000),), site_list=True)["batch"]
     b = dataclasses.replace(b, tid=np.ones_like(b.tid))
     both = ReadBatch.concat([a, b])
-    d = str(tmp_path)
-    synth.write_sam(os.path.join(d, "s.sam"), both, [("chrA", 30000), ("chrB", 20000)])
-    subprocess.check_call([REF_SAMTOOLS, "view", "-b", "-o", os.path.join(d, "s.bam"), os.path.join(d, "s.sam")])
-    subprocess.check_call([REF_SAMTOOLS, "index", os.path.join(d, "s.bam")])
+    bam = cases.write_bam(str(tmp_path), "s", both, [("chrA", 30000), ("chrB", 20000)])
     lines = [("chrA", 100, 100), ("chrA", 101, 130), ("chrB", 5000, 5000), ("chrB", 5001, 5001), ("chrA", 120, 125), ("chrA", 120, 125),
              ("chrB", 19990, 25000), ("chrA", 29999, 30000), ("chrZ", 5, 6), ("chrB", 1, 1), ("chrB", 2, 2), ("chrB", 3, 400)]
     sl = tmp_path / "sites"
     sl.write_text("".join(f"{c}\t{s}\t{e}\n" for c, s, e in lines))
-    p = subprocess.run([exe, "-l", str(sl), os.path.join(d, "s.bam")], capture_output=True, env=dict(os.environ, BRC_CLI_DECODE_ONLY="1"))
+    p = subprocess.run([exe, "-l", str(sl), bam], capture_output=True, env=dict(os.environ, BRC_CLI_DECODE_ONLY="1"))
     assert p.returncode == 0, p.stderr.decode()
     assert b"chrZ not found in bam file" in p.stderr
     got = [tuple(int(x) for x in ln.split("\t")) for ln in p.stdout.decode().strip().splitlines()]
@@ -249,8 +217,7 @@ def test_patched_reference_needs_a_device():
     if torch.cuda.is_available():
         pytest.skip("GPU present")
     exe = _patched_reference()
-    data = os.path.join(ROOT, "oracle", "_ref", "test-data")
-    p = subprocess.run([exe, "-w", "1", "-f", "ref.fa", "-l", "site_list", "test.bam"], cwd=data, capture_output=True)
+    p = subprocess.run([exe, "-w", "1", "-f", "ref.fa", "-l", "site_list", "test.bam"], cwd=CRAM_DATA, capture_output=True)
     assert p.returncode == 1 and b"no usable CUDA device" in p.stderr and p.stdout == b""      # no CPU fallback behind the boundary
 
 
@@ -267,7 +234,6 @@ def test_reference_main_through_the_c_abi_reproduces_goldens(args, bam, golden):
     """R:integration-test/bam-readcount_test.py:29-116 — the six command lines, run by the reference's own main()
     linked against libbrc_engine.so."""
     exe = _patched_reference()
-    data = os.path.join(ROOT, "oracle", "_ref", "test-data")
     argv = [exe, "-f", "ref.fa"]
     regions = []
     for a in args:
@@ -277,7 +243,7 @@ def test_reference_main_through_the_c_abi_reproduces_goldens(args, bam, golden):
             argv.append(a)
     argv.append(bam)
     argv += regions
-    p = subprocess.run(argv, cwd=data, capture_output=True)
+    p = subprocess.run(argv, cwd=CRAM_DATA, capture_output=True)
     assert p.returncode == 0, p.stderr.decode()[-2000:]
     assert p.stdout.decode("latin-1") == cases.load_golden_text(golden)
 
@@ -286,9 +252,8 @@ def test_reference_main_through_the_c_abi_reproduces_goldens(args, bam, golden):
 def test_reference_main_through_the_c_abi_on_the_cram():
     """BASELINE config 2b on the CRAM itself: htslib (the reference's reader) decodes twolib.sorted.cram, the engine computes."""
     exe = _patched_reference()
-    data = os.path.join(ROOT, "oracle", "_ref", "test-data")
     for extra, golden in ((["-p"], "ref_cram_twolib_perlib.txt"), ([], "ref_cram_twolib_alllib.txt")):
-        p = subprocess.run([exe, "-w", "0"] + extra + ["-f", "rand1k.fa", "-l", "twolib_site_list.txt", "twolib.sorted.cram"], cwd=data, capture_output=True)
+        p = subprocess.run([exe, "-w", "0"] + extra + ["-f", "rand1k.fa", "-l", "twolib_site_list.txt", "twolib.sorted.cram"], cwd=CRAM_DATA, capture_output=True)
         assert p.returncode == 0, p.stderr.decode()[-2000:]
         assert p.stdout.decode("latin-1") == cases.load_golden_text(golden)
 
@@ -308,7 +273,7 @@ def test_cli_warning_lines_match_the_reference_binary(tmp_path, args, bam):
     if not have_reference_binary():
         pytest.skip("oracle/_ref not built")
     exe = _cli()
-    ref = _write_ref(str(tmp_path))
+    ref = cases.write_testbam_fasta(str(tmp_path / "ref.fa"))
     out = {}
     for name, binary in (("ours", exe), ("ref", REF_BIN)):
         argv = [binary, "-f", ref]
@@ -336,7 +301,7 @@ def test_cli_region_forms_match_the_reference_binary(tmp_path):
     if not have_reference_binary():
         pytest.skip("oracle/_ref not built")
     exe = _cli()
-    ref = _write_ref(str(tmp_path))
+    ref = cases.write_testbam_fasta(str(tmp_path / "ref.fa"))
     bam = os.path.join(GOLDEN, "test.bam")
     for regions in (["21:10405200"], ["21:10402985-10402985", "21:10405200"], ["21:10,402,985-10,402,990"], ["21:10402985-"],
                     ["21:10402985-10402985", "21"], ["21:-5"], ["21:10402985-10402986", "21:10402987-10402990"]):
@@ -362,13 +327,12 @@ def test_cli_reports_truncated_bam(tmp_path):
 
 
 def _cram_fixture():
-    d = os.path.join(ROOT, "oracle", "_ref", "test-data")
-    if not os.path.exists(os.path.join(d, "twolib.sorted.cram")):
+    if not os.path.exists(os.path.join(CRAM_DATA, "twolib.sorted.cram")):
         pytest.skip("oracle/_ref/test-data not present")
     exe = _cli()
-    if b"BRC_WITH_HTSLIB" not in open(exe, "rb").read() and not os.path.exists(os.path.join(ROOT, "bam_readcount_b200", "third_party", "htslib", "libhts.a")):
+    if b"BRC_WITH_HTSLIB" not in open(exe, "rb").read() and not cases.have_htslib():
         pytest.skip("host built without htslib (tools/build_htslib.sh)")
-    return exe, d
+    return exe, CRAM_DATA
 
 
 def test_cli_decodes_cram_through_htslib():
@@ -526,9 +490,7 @@ def test_cli_parallel_window_decode_two_contigs_unmapped_and_edges(tmp_path):
     """CPU: the parallel window decode on a two-contig BAM with placed-but-unmapped records, a fetch that starts inside a read,
     a fetch past the last read, a site-list line long enough to be cut into windows, and a contig without reads behind it:
     per-region (count, position sum, quality sum) identical to the Python decoder's samfetch, uncut and cut into windows."""
-    REF_SAMTOOLS = cases.samtools()
     import dataclasses
-    from bam_readcount_b200 import synth
     from bam_readcount_b200.batch import ReadBatch
     exe = _cli()
     a = cases.synthetic_case(L=600000, depth=4, seed=31, regions=((0, 1, 600000),), site_list=False)["batch"]
@@ -538,17 +500,14 @@ def test_cli_parallel_window_decode_two_contigs_unmapped_and_edges(tmp_path):
     a = dataclasses.replace(a, flag=fa)
     b = dataclasses.replace(b, tid=np.ones_like(b.tid))
     both = ReadBatch.concat([a, b])
-    d = str(tmp_path)
-    synth.write_sam(os.path.join(d, "s.sam"), both, [("chrA", 600000), ("chrB", 400000), ("chrC", 300000)])
-    subprocess.check_call([REF_SAMTOOLS, "view", "-b", "-o", os.path.join(d, "s.bam"), os.path.join(d, "s.sam")])
-    subprocess.check_call([REF_SAMTOOLS, "index", os.path.join(d, "s.bam")])
+    bam = cases.write_bam(str(tmp_path), "s", both, [("chrA", 600000), ("chrB", 400000), ("chrC", 300000)])
     lines = [("chrA", 1, 600000), ("chrA", 100077, 500000), ("chrB", 50, 399000), ("chrA", 300000, 300001), ("chrB", 120000, 400000),
              ("chrC", 1, 300000), ("chrA", 590000, 600000)]
     sl = tmp_path / "sites"
     sl.write_text("".join(f"{c}\t{s}\t{e}\n" for c, s, e in lines))
     outs = []
     for extra in ({}, {"BRC_CLI_DECODE_THREADS": "5", "BRC_CLI_WINDOW": "270000"}):
-        p = subprocess.run([exe, "-l", str(sl), os.path.join(d, "s.bam")], capture_output=True, env=dict(os.environ, BRC_CLI_DECODE_ONLY="1", BRC_CLI_TIMING="1", **extra))
+        p = subprocess.run([exe, "-l", str(sl), bam], capture_output=True, env=dict(os.environ, BRC_CLI_DECODE_ONLY="1", BRC_CLI_TIMING="1", **extra))
         assert p.returncode == 0, p.stderr.decode()[-1500:]
         outs.append((p.stdout.decode(), p.stderr.decode()))
         assert "(+ 0 records in 0 windows" not in outs[-1][1]

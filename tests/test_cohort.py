@@ -11,57 +11,12 @@ import numpy as np
 import pytest
 
 import cases
+from cases import CONTIGS, CRAM_DATA, DECODE_ONLY, GOLDEN, synthetic_bam, write_fasta
 from cases import cli as _cli
-from cases import samtools as _samtools
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-GOLDEN = os.path.join(ROOT, "tests", "golden")
-CRAM_DATA = os.path.join(ROOT, "oracle", "_ref", "test-data")
-CONTIGS = {"chrA": (24000, 11), "chrB": (16000, 12), "chrC": (12000, 13)}       # name -> (length, reference seed)
 
 
-
-
-def _have_htslib(exe):
-    return os.path.exists(os.path.join(ROOT, "bam_readcount_b200", "third_party", "htslib", "libhts.a")) and \
-        os.path.exists(os.path.join(CRAM_DATA, "twolib.sorted.cram"))
-
-
-def _write_fasta(path, contigs):
-    """Multi-contig FASTA (60 columns) and its .fai."""
-    with open(path, "wb") as fa, open(path + ".fai", "w") as fai:
-        off = 0
-        for name, seq in contigs:
-            head = f">{name}\n".encode()
-            fa.write(head)
-            off += len(head)
-            body = b"".join(seq[i:i + 60] + b"\n" for i in range(0, len(seq), 60))
-            fa.write(body)
-            fai.write(f"{name}\t{len(seq)}\t{off}\t60\t61\n")
-            off += len(body)
-
-
-def _synthetic_bam(d, name, order, n_libs, seed, depth=8, no_nm=0):
-    """A coordinate-sorted BAM whose @SQ lines are `order` (a subset of CONTIGS, in any order), with n_libs libraries
-    (0: no @RG at all) and `no_nm` reads without an NM tag (they draw warnings)."""
-    import dataclasses
-    from bam_readcount_b200 import synth
-    from bam_readcount_b200.batch import ReadBatch, TAG_ABSENT
-    parts = []
-    for tid, c in enumerate(order):
-        ref = synth.synth_reference(CONTIGS[c][0], CONTIGS[c][1])
-        parts.append(synth.synth_reads(ref, depth, seed=seed + 101 * tid, n_libs=max(n_libs, 1), tid=tid))
-    b = ReadBatch.concat(parts)
-    if no_nm:
-        nm = np.array(b.nm, copy=True)
-        nm[np.random.default_rng(seed).choice(b.n_reads, no_nm, replace=False)] = TAG_ABSENT
-        b = dataclasses.replace(b, nm=nm)
-    sam, bam = os.path.join(d, name + ".sam"), os.path.join(d, name + ".bam")
-    synth.write_sam(sam, b, [(c, CONTIGS[c][0]) for c in order], n_libs=max(n_libs, 1), read_group=n_libs > 0)
-    subprocess.check_call([_samtools(), "view", "-b", "-o", bam, sam])
-    subprocess.check_call([_samtools(), "index", bam])
-    os.remove(sam)
-    return bam
+def _have_cram():
+    return cases.have_htslib() and os.path.exists(os.path.join(CRAM_DATA, "twolib.sorted.cram"))
 
 
 @pytest.fixture(scope="module")
@@ -72,10 +27,10 @@ def cohort(tmp_path_factory):
     from bam_readcount_b200 import synth
     d = str(tmp_path_factory.mktemp("cohort"))
     s = {
-        "syn5a": _synthetic_bam(d, "syn5a", ["chrA", "chrB", "chrC"], 5, seed=21, no_nm=60),
-        "syn2": _synthetic_bam(d, "syn2", ["chrB", "chrA"], 2, seed=22),
-        "syn5b": _synthetic_bam(d, "syn5b", ["chrC", "chrA", "chrB"], 5, seed=23),
-        "syn0": _synthetic_bam(d, "syn0", ["chrA", "chrC"], 0, seed=24, no_nm=10),
+        "syn5a": synthetic_bam(d, "syn5a", ["chrA", "chrB", "chrC"], 5, seed=21, no_nm=60),
+        "syn2": synthetic_bam(d, "syn2", ["chrB", "chrA"], 2, seed=22),
+        "syn5b": synthetic_bam(d, "syn5b", ["chrC", "chrA", "chrB"], 5, seed=23),
+        "syn0": synthetic_bam(d, "syn0", ["chrA", "chrC"], 0, seed=24, no_nm=10),
         "test": os.path.join(GOLDEN, "test.bam"),
         "bad_rg": os.path.join(GOLDEN, "test_bad_rg.bam"),
     }
@@ -92,14 +47,9 @@ def cohort(tmp_path_factory):
         shutil.copy(cram, s["cram_old_idx"])
         shutil.copy(cram + ".crai", s["cram_old_idx"] + ".crai")
         os.utime(s["cram_old_idx"] + ".crai", (1e9, 1e9))
-    z = np.load(os.path.join(GOLDEN, "test_bam.npz"))
-    chr21 = np.full(int(z["chrom_len"]), ord("N"), dtype=np.uint8)
-    wb = int(z["ref_win_beg"])
-    chr21[wb:wb + z["ref_win"].shape[0]] = z["ref_win"]
     rand1k = b"".join(open(os.path.join(GOLDEN, "rand1k.fa"), "rb").read().split(b"\n")[1:])
-    fa = os.path.join(d, "all.fa")
-    _write_fasta(fa, [("21", chr21.tobytes()), ("rand1k", rand1k)] +
-                 [(c, synth.synth_reference(L, sd).tobytes()) for c, (L, sd) in CONTIGS.items()])
+    fa = write_fasta(os.path.join(d, "all.fa"), [("21", cases.testbam_chr21()), ("rand1k", rand1k)] +
+                     [(c, synth.synth_reference(L, sd).tobytes()) for c, (L, sd) in CONTIGS.items()])
     rng = np.random.default_rng(4)
     lines = open(os.path.join(GOLDEN, "site_list")).read() + open(os.path.join(GOLDEN, "twolib_site_list.txt")).read()
     for c, (L, _) in CONTIGS.items():
@@ -144,9 +94,6 @@ def _check_cohort_equals_single_runs(exe, d, tag, args, inputs, regions, env):
 
 
 # ---------------------------------------------------------------------------------------------------------------- CPU
-DECODE_ONLY = dict(os.environ, BRC_CLI_DECODE_ONLY="1")
-
-
 def test_cohort_decode_summaries_equal_single_runs(cohort):
     exe = _cli()
     s = cohort["samples"]
@@ -209,7 +156,7 @@ def test_cohort_cram_messages_of_htslib_go_to_the_sample_err(cohort, tmp_path):
     ERR, in the same place among the host's lines as in the sample's own run; BAM samples opened ahead of their turn around
     them keep their ERR clean of them."""
     exe = _cli()
-    if not _have_htslib(exe):
+    if not _have_cram():
         pytest.skip("host built without htslib, or no CRAM fixture")
     s = cohort["samples"]
     cram = os.path.join(CRAM_DATA, "twolib.sorted.cram")
@@ -245,7 +192,7 @@ def test_cohort_window_jobs_pass_from_sample_to_sample(tmp_path):
     for k, seed in enumerate((5, 6)):
         d = tmp_path / f"s{k}"
         d.mkdir()
-        bams.append(synth_cb.write_sample_bam(synth_cb.Spec(seed=seed, contig_len=1280 * 320), 0, 0, 320, str(d), _samtools())["bam"])
+        bams.append(synth_cb.write_sample_bam(synth_cb.Spec(seed=seed, contig_len=1280 * 320), 0, 0, 320, str(d), cases.samtools())["bam"])
     env = dict(DECODE_ONLY, BRC_CLI_WINDOW="300000")
     regions = ["chr1:1-400000", "chr1:1001-2000"]
     got, _ = _check_cohort_equals_single_runs(exe, str(tmp_path), "win", [], [bams[0], bams[1], bams[0]], regions, env)
@@ -281,7 +228,7 @@ def _gpu_inputs(cohort, exe):
     """The cohort in an order that switches library counts (5, 2, 5, 0 ...) and @SQ orders from one sample to the next."""
     s = cohort["samples"]
     inputs = [s["syn5a"], s["syn2"], s["syn5b"], s["test"], s["syn0"], s["bad_rg"], s["cut"]]
-    if _have_htslib(exe):
+    if _have_cram():
         inputs.insert(4, os.path.join(CRAM_DATA, "twolib.sorted.cram"))
         inputs.append(s["cram_noidx"])
     return inputs
@@ -294,7 +241,7 @@ def test_cohort_site_list_equals_single_runs(cohort, flags):
     args = FLAG_SETS[flags] + ["-f", cohort["fasta"], "-l", cohort["sites"]]
     inputs = _gpu_inputs(cohort, exe)
     got, want = _check_cohort_equals_single_runs(exe, cohort["dir"], f"l_{flags}", args, inputs, [], dict(os.environ))
-    assert [w[0] for w in want].count(1) == (2 if _have_htslib(exe) else 1)     # only the cut BAM and the CRAM without index fail
+    assert [w[0] for w in want].count(1) == (2 if _have_cram() else 1)     # only the cut BAM and the CRAM without index fail
     golden = {"default": "expected_all_lib", "p": "expected_per_lib", "i": "expected_insertion_centric_all_lib",
               "ip": "expected_insertion_centric_per_lib", "w2": "expected_all_lib"}.get(flags)
     if golden:
@@ -346,17 +293,14 @@ def test_cohort_deletion_queue_does_not_cross_samples(tmp_path):
     from bam_readcount_b200 import synth
     d = str(tmp_path)
     ref = synth.synth_reference(3000, 5)
-    _write_fasta(os.path.join(d, "ref.fa"), [("chrA", ref.tobytes())])
+    write_fasta(os.path.join(d, "ref.fa"), [("chrA", ref.tobytes())])
     seq = lambda p, n: ref[p:p + n].tobytes().decode()               # noqa: E731
     def sam(name, reads):
         with open(os.path.join(d, name + ".sam"), "w") as fh:
             fh.write("@HD\tVN:1.6\tSO:coordinate\n@SQ\tSN:chrA\tLN:3000\n")
             for k, (pos, cigar, s) in enumerate(sorted(reads)):
                 fh.write(f"r{k}\t0\tchrA\t{pos + 1}\t60\t{cigar}\t*\t0\t0\t{s}\t{'I' * len(s)}\tNM:i:0\n")
-        bam = os.path.join(d, name + ".bam")
-        subprocess.check_call([_samtools(), "view", "-b", "-o", bam, os.path.join(d, name + ".sam")])
-        subprocess.check_call([_samtools(), "index", bam])
-        return bam
+        return cases.sam_to_bam(os.path.join(d, name + ".sam"))
     # A: 1-based 1001-1050 matched, 1051-1055 deleted, then 50 more; plus plain reads across the same stretch
     a = sam("a", [(1000, "50M5D50M", seq(1000, 50) + seq(1055, 50))] + [(980 + 7 * k, "100M", seq(980 + 7 * k, 100)) for k in range(6)])
     b = sam("b", [(990 + 5 * k, "100M", seq(990 + 5 * k, 100)) for k in range(8)])

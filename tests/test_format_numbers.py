@@ -1,13 +1,10 @@
 """CPU: the emitter's printf-free "%.2f" (round-half-even on the exact binary value) against libc on 40M+ floats."""
-import os
 import subprocess
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+import cases
 
 
-def test_put_f2_matches_printf(tmp_path):
-    exe = str(tmp_path / "fmt_check")
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-o", exe, os.path.join(ROOT, "tests", "fmt_check.cpp")])
-    p = subprocess.run([exe], capture_output=True, text=True)
+def test_put_f2_matches_printf():
+    p = subprocess.run([cases.check_program("fmt_check")], capture_output=True, text=True)
     assert p.returncode == 0, p.stdout[-2000:]
     assert "0 mismatches" in p.stdout

@@ -27,8 +27,7 @@ import pytest
 import inflight_cases as ic
 from bam_readcount_b200 import stream as st
 from bam_readcount_b200 import synth_cb as sc
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from cases import ROOT
 
 C4_FLAG_SETS = {
     "ic": (dict(insertion_centric=True), []),                 # C4's own flags

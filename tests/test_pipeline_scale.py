@@ -32,9 +32,8 @@ import pytest
 
 import cases
 import pipeline_cases as pc
-from cases import first_diff, region_geometry
+from cases import ROOT, first_diff, region_geometry
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "bam_readcount_b200", "csrc")
 
 
@@ -244,7 +243,7 @@ def starved_child():
             os.environ.pop("BRC_PIPE_CHUNKS", None)
         w = got.warnings
         out[name] = dict(dump=got.dump == want.dump, text=got.text == want.text, warn=[w[0], w[1], w[3]] == list(want.warnings),
-                         launches=got.launches if n_chunks else 0, diff="" if got.dump == want.dump else first_diff(got.dump, want.dump))
+                         launches=got.launches if n_chunks else 0, diff=first_diff(got.dump, want.dump))
     print("STARVED " + json.dumps(out))
 
 

@@ -13,7 +13,7 @@ import sys
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from cases import ROOT
 pytestmark = pytest.mark.gpu
 
 FASTDIV_MAX, QTAB_MID, QTAB_W = 2048, 2048, 4096

@@ -14,11 +14,8 @@ from bam_readcount_b200 import bamio
 
 
 @pytest.fixture(scope="module")
-def seq_check(tmp_path_factory):
-    exe = str(tmp_path_factory.mktemp("seq_check") / "seq_check")
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-I", os.path.join(cases.ROOT, "bam_readcount_b200", "csrc"), "-o", exe,
-                           os.path.join(cases.ROOT, "tests", "seq_check.cpp")])
-    return exe
+def seq_check():
+    return cases.check_program("seq_check")
 
 
 def test_tables_equal_oracle(seq_check):

@@ -6,7 +6,6 @@ CPU: select_lines on the committed goldens and on hand-written lines, CLI option
 GPU: the engine and the C++ host, filtered, against select_lines of the reference goldens, the oracle and the unfiltered run.
 """
 import os
-import re
 import subprocess
 
 import numpy as np
@@ -14,29 +13,16 @@ import pytest
 
 import cases
 import golden_jobs
+from cases import GOLDEN, crafted_case, first_diff
 from cases import cli as _cli
-from cases import first_diff
 from site_filter_rule import THRESHOLDS, is_alt, line_entries, line_passes, select_lines
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-GOLDEN = os.path.join(ROOT, "tests", "golden")
-
-
-def _same(got: str, want: str) -> str:
-    """'' when equal, else the first differing line."""
-    return "" if got == want else first_diff(got, want)
 
 
 # ---------------------------------------------------------------------------------------------------------------------------
 # CPU
 # ---------------------------------------------------------------------------------------------------------------------------
-def _golden_texts():
-    names = sorted({f[:-3] if f.endswith(".gz") else f for f in os.listdir(GOLDEN) if f.endswith(".txt.gz") or f.startswith("expected_")})
-    return [(n, cases.load_golden_text(n)) for n in names]
-
-
 def test_select_lines_on_goldens_is_a_subsequence_dropping_only_lines_without_a_qualifying_allele():
-    texts = _golden_texts()
+    texts = cases.golden_texts()
     assert len(texts) >= 30
     for name, text in texts:
         lines = text.splitlines()
@@ -134,7 +120,7 @@ def test_engine_filtered_text_equals_selected_golden(job):
     case = getter()
     want_all = cases.load_golden_text(golden)
     for mc, mf in THRESHOLDS:
-        d = _same(_text(case, flags, site_list, (mc, mf)), select_lines(want_all, mc, mf))
+        d = first_diff(_text(case, flags, site_list, (mc, mf)), select_lines(want_all, mc, mf))
         assert not d, (mc, mf, d)
 
 
@@ -164,7 +150,7 @@ def test_synthetic_whole_region_and_filter_off_is_unchanged():
     for flags in (dict(), dict(per_lib=True, insertion_centric=True), dict(min_mapq=20, min_bq=20)):
         want, _, _ = cases.run_oracle(case, flags, site_list=False)
         for mc, mf in THRESHOLDS:
-            d = _same(_text(case, flags, False, (mc, mf)), select_lines(want, mc, mf))
+            d = first_diff(_text(case, flags, False, (mc, mf)), select_lines(want, mc, mf))
             assert not d, (flags, mc, mf, d)
     fresh = cases.run_engine(case, dict(), False, dump=False)
     import ctypes as C
@@ -201,7 +187,7 @@ def test_synthetic_whole_region_and_filter_off_is_unchanged():
         assert e.results_kind() == RESULTS_SELECTED
         res = step()
         assert res is not None and e.results_kind() == RESULTS_DENSE and e.launch_count() == fresh.launches
-        d = _same(e.format_text(-1), fresh.text)
+        d = first_diff(e.format_text(-1), fresh.text)
         assert not d, d
         with pytest.raises(BrcError):
             e.selected()
@@ -212,16 +198,6 @@ def test_synthetic_whole_region_and_filter_off_is_unchanged():
         assert e.results_kind() == RESULTS_DENSE
     finally:
         e.close()
-
-
-def _write_ref(tmp):
-    z = np.load(os.path.join(GOLDEN, "test_bam.npz"))
-    L, wb = int(z["chrom_len"]), int(z["ref_win_beg"])
-    seq = np.full(L, ord("N"), dtype=np.uint8)
-    seq[wb:wb + z["ref_win"].shape[0]] = z["ref_win"]
-    from bam_readcount_b200 import synth
-    synth.write_fasta(os.path.join(tmp, "ref.fa"), "21", seq)
-    return os.path.join(tmp, "ref.fa")
 
 
 def _cli_pair(exe, argv, env=None, filt=(("--min-alt-count", "2"), ("--min-alt-fraction", "0.05"))):
@@ -243,7 +219,7 @@ def _check_cli(exe, argv, env=None):
     text = full.stdout.decode("latin-1")
     for fl, mc, mf in filts:
         p = outs[fl]
-        d = _same(p.stdout.decode("latin-1"), select_lines(text, mc, mf))
+        d = first_diff(p.stdout.decode("latin-1"), select_lines(text, mc, mf))
         assert not d, (argv, fl, d)
         assert p.stderr == full.stderr                 # warning lines and counts do not depend on the filter
     return text
@@ -253,7 +229,7 @@ def _check_cli(exe, argv, env=None):
 def test_cli_filtered_output_on_the_reference_fixture(tmp_path):
     """Site list, argv regions that overlap and that abut (deletions carried from one argv region into the next), -d."""
     exe = _cli()
-    ref = _write_ref(str(tmp_path))
+    ref = cases.write_testbam_fasta(str(tmp_path / "ref.fa"))
     bam = os.path.join(GOLDEN, "test.bam")
     sl = os.path.join(GOLDEN, "site_list")
     _check_cli(exe, ["-w", "0", "-f", ref, "-l", sl, bam])
@@ -268,20 +244,17 @@ def test_cli_filtered_output_on_the_reference_fixture(tmp_path):
 def test_cli_filtered_output_on_a_synthetic_bam(tmp_path):
     """A few tens of kb of synthetic BAM: one argv region cut into 3777-site windows (deletions across window edges), the
     device BGZF decode path, overlapping argv regions on it and a site list."""
-    samtools = cases.samtools()
     from bam_readcount_b200 import synth
     exe = _cli()
     case = cases.synthetic_case(L=40000, depth=30, seed=47, regions=((0, 1, 40000),), site_list=False)
     name, L, seq, _ = case["contigs"][0]
     d = str(tmp_path)
     synth.write_fasta(os.path.join(d, "ref.fa"), name, np.frombuffer(seq, dtype=np.uint8))
-    synth.write_sam(os.path.join(d, "s.sam"), case["batch"], [(name, L)], n_libs=len(case["lib_names"]))
-    subprocess.check_call([samtools, "view", "-b", "-o", os.path.join(d, "s.bam"), os.path.join(d, "s.sam")])
-    subprocess.check_call([samtools, "index", os.path.join(d, "s.bam")])
+    cases.write_bam(d, "s", case["batch"], [(name, L)], n_libs=len(case["lib_names"]))
     base = ["-w", "0", "-f", os.path.join(d, "ref.fa"), os.path.join(d, "s.bam")]
     want, _, _ = cases.run_oracle(case, dict(per_lib=True), site_list=False)
     t = _check_cli(exe, ["-p"] + base + ["chr1:1-40000"], env={"BRC_CLI_WINDOW": "3777"})
-    diff = _same(t, want)
+    diff = first_diff(t, want)
     assert not diff, diff
     _check_cli(exe, ["-i"] + base + ["chr1:1-40000"], env={"BRC_CLI_DEVICE_DECODE": "1"})
     _check_cli(exe, base + ["chr1:1001-9000", "chr1:8000-15000", "chr1:15001-20000", "chr1:100-300"])
@@ -291,45 +264,18 @@ def test_cli_filtered_output_on_a_synthetic_bam(tmp_path):
 
 
 # ---- crafted inputs for the deletion queue ------------------------------------------------------------------------------
-def _crafted(reads, regions, n_libs=1, L=300, seed=3):
-    """A case from hand-placed reads: (pos, cigar, mismatch positions, library).  Every read copies the reference except at
-    its mismatch positions."""
-    from bam_readcount_b200.batch import BatchBuilder
-    rng = np.random.default_rng(seed)
-    ref = bytes(rng.choice(list(b"ACGT"), L).astype(np.uint8))
-    other = {ord("A"): "C", ord("C"): "G", ord("G"): "T", ord("T"): "A"}
-    bb = BatchBuilder()
-    for k, (pos, cigar, mism, lib) in enumerate(reads):
-        seq, p = [], pos
-        for n, op in re.findall(r"(\d+)([MID])", cigar):
-            n = int(n)
-            if op == "M":
-                seq += [other[ref[q]] if q in mism else chr(ref[q]) for q in range(p, p + n)]
-                p += n
-            elif op == "D":
-                p += n
-            else:
-                seq += ["A"] * n
-        bb.add_sam(tid=0, pos=pos, flag=0, mapq=60, lib=lib, cigar=cigar, seq="".join(seq), qual="I" * len(seq),
-                   nm=len(mism), sm=60, qname=f"r{k}")
-    b = bb.build()
-    order = np.argsort(b.pos, kind="stable")
-    return dict(name="crafted", contigs=[("chr1", L, ref, 0)], batch=b.select(order), regions=list(regions), site_list=False,
-                lib_names=[f"lib{i}" for i in range(n_libs)])
-
-
 @pytest.mark.gpu
 def test_last_site_of_an_argv_region_keeps_the_deletion_from_its_left_neighbour():
     """The last site of an argv region is formed as a line even when it fails the rule; its left neighbour must be replayed, or
     the line loses the deletion queued there (and that deletion's share of the depth) and can pass a fraction it fails."""
     reads = [(40, "60M", {79} if k < 6 else set(), 0) for k in range(30)] + [(40, "39M1D20M", set(), 0)]
-    case = _crafted(reads, [(0, 51, 80)])
+    case = crafted_case(reads, [(0, 51, 80)])
     want, _, _ = cases.run_oracle(case, dict(), site_list=False)
     last = want.splitlines()[-1].split("\t")
     assert last[1] == "80" and any(f.startswith("-") for f in last[4:])          # the last line prints the deletion
     fractions = sorted({6 / 32, 6 / 31, 6 / 30, 0.19, 0.194, 0.195, 0.198, 0.2, 0.21} | {round(x, 3) for x in np.linspace(0.15, 0.25, 21)})
     for f in fractions:
-        diff = _same(_text(case, dict(), False, (1, f)), select_lines(want, 1, f))
+        diff = first_diff(_text(case, dict(), False, (1, f)), select_lines(want, 1, f))
         assert not diff, (f, diff)
 
 
@@ -340,11 +286,11 @@ def test_per_library_queue_handed_to_an_overlapping_argv_region_is_the_unfiltere
     inside the first region, as the unfiltered pass does, and not print a second time in the second region."""
     reads = [(30, "80M", set(), 0) for _ in range(10)]
     reads += [(30, "40M", {60} if k < 3 else set(), 1) for k in range(5)] + [(30, "31M1D8M", set(), 1)]
-    case = _crafted(reads, [(0, 41, 90), (0, 55, 65)], n_libs=2)
+    case = crafted_case(reads, [(0, 41, 90), (0, 55, 65)], n_libs=2)
     flags = dict(per_lib=True)
     want, _, _ = cases.run_oracle(case, flags, site_list=False)
     for mc, mf in THRESHOLDS + [(2, 0.0), (3, 0.0)]:
-        diff = _same(_text(case, flags, False, (mc, mf)), select_lines(want, mc, mf))
+        diff = first_diff(_text(case, flags, False, (mc, mf)), select_lines(want, mc, mf))
         assert not diff, (mc, mf, diff)
     lines62 = [ln for ln in want.splitlines() if ln.split("\t")[1] == "62"]
     assert len(lines62) == 2 and all(sum(f.startswith("-") for f in ln.split("\t")) == 1 for ln in lines62)
@@ -358,13 +304,13 @@ def test_per_library_deletion_carried_through_a_region_that_drops_it():
     copy of that deletion once, not twice."""
     reads = [(30, "100M", {60} if k < 3 else set(), 0) for k in range(20)]
     reads += [(30, "50M", set(), 1) for _ in range(5)] + [(30, "30M1D19M", set(), 1)]
-    case = _crafted(reads, [(0, 41, 60), (0, 71, 120), (0, 41, 61)], n_libs=2)
+    case = crafted_case(reads, [(0, 41, 60), (0, 71, 120), (0, 41, 61)], n_libs=2)
     flags = dict(per_lib=True)
     want, _, _ = cases.run_oracle(case, flags, site_list=False)
     line61 = [ln for ln in want.splitlines() if ln.split("\t")[1] == "61"]
     assert len(line61) == 1 and sum(f.startswith("-") for f in line61[0].split("\t")) == 1
     for mc, mf in THRESHOLDS + [(2, 0.0), (3, 0.0)]:
-        diff = _same(_text(case, flags, False, (mc, mf)), select_lines(want, mc, mf))
+        diff = first_diff(_text(case, flags, False, (mc, mf)), select_lines(want, mc, mf))
         assert not diff, (mc, mf, diff)
 
 
@@ -391,5 +337,5 @@ def test_device_only_reference_is_judged_by_the_printed_reference_column():
     assert all(ln.split("\t")[2] == "N" for ln in full.splitlines()[:50])
     kept = select_lines(full, 20, 0.5)
     assert len(kept.splitlines()) > 1000
-    diff = _same(filtered, kept)
+    diff = first_diff(filtered, kept)
     assert not diff, diff

@@ -20,16 +20,9 @@ import pytest
 import cases
 import golden_jobs
 from alt_bounds_rule import FIELDS, FPFILTER_SETS, entries, line_passes_bounds, one_sided_sets, select_lines_bounds
+from cases import GOLDEN, crafted_case, first_diff
 from cases import cli as _cli
-from cases import first_diff
 from site_filter_rule import is_alt, select_lines
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-GOLDEN = os.path.join(ROOT, "tests", "golden")
-
-
-def _same(got: str, want: str) -> str:
-    return "" if got == want else first_diff(got, want)
 
 
 def _printed(bounds):
@@ -96,13 +89,8 @@ def test_rule_indel_basequality_library_blocks_and_deletions():
     assert not line_passes_bounds(_line("A", 6, *_base_entries(ref_count=6)), 1, 0.0, {})  # the reference base never counts
 
 
-def _golden_texts():
-    names = sorted({f[:-3] if f.endswith(".gz") else f for f in os.listdir(GOLDEN) if f.endswith(".txt.gz") or f.startswith("expected_")})
-    return [(n, cases.load_golden_text(n)) for n in names]
-
-
 def test_rule_on_goldens_is_a_subsequence_and_a_direct_restatement():
-    texts = _golden_texts()
+    texts = cases.golden_texts()
     assert len(texts) >= 30
     for name, text in texts:
         lines = text.splitlines()
@@ -127,10 +115,8 @@ def test_rule_on_goldens_is_a_subsequence_and_a_direct_restatement():
         assert select_lines_bounds(text, 1, 0.0, {n: (0, None) for n in FIELDS}) == select_lines(text, 1)
 
 
-def test_hundredths_routine_matches_printf(tmp_path):
-    exe = str(tmp_path / "hundredths_check")
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-pthread", "-o", exe, os.path.join(ROOT, "tests", "hundredths_check.cpp")])
-    p = subprocess.run([exe], capture_output=True, text=True)
+def test_hundredths_routine_matches_printf():
+    p = subprocess.run([cases.check_program("hundredths_check", "-pthread")], capture_output=True, text=True)
     assert p.returncode == 0 and " 0 mismatches" in p.stdout, p.stdout[-2000:]
 
 
@@ -232,43 +218,16 @@ def test_engine_bounded_text_equals_the_rule_on_the_oracle_text(job):
     assert len(sets) >= 2 * 12 + 4
     filters = [None] + [(1, 0.0, b) for b in sets] + [(2, 0.05, b) for b in FPFILTER_SETS]
     runs = _runs(case, flags, site_list, filters)
-    assert not _same(runs[0][0], want_all), _same(runs[0][0], want_all)
+    assert not first_diff(runs[0][0], want_all), first_diff(runs[0][0], want_all)
     exact = site_list or name.startswith("syn-")
     for filt, (text, sel, _) in zip(filters[1:], runs[1:]):
         want = select_lines_bounds(want_all, *filt)
-        d = _same(text, want)
+        d = first_diff(text, want)
         assert not d, (filt, d)
         if exact:
             assert [p + 1 for p in sel.positions(1)] == [int(ln.split("\t")[1]) for ln in want.splitlines()], filt
     n_min0 = filters.index((1, 0.0, {n: (0, None) for n in FIELDS}))
     assert runs[n_min0][0] == select_lines(want_all, 1)
-
-
-def _crafted(reads, regions, n_libs=1, L=300, seed=3):
-    """Hand-placed reads (pos, cigar, mismatch positions, library, mapq, flag); every read copies the reference except at its
-    mismatch positions."""
-    from bam_readcount_b200.batch import BatchBuilder
-    rng = np.random.default_rng(seed)
-    ref = bytes(rng.choice(list(b"ACGT"), L).astype(np.uint8))
-    other = {ord("A"): "C", ord("C"): "G", ord("G"): "T", ord("T"): "A"}
-    bb = BatchBuilder()
-    for k, (pos, cigar, mism, lib, mapq, flag) in enumerate(reads):
-        seq, p = [], pos
-        for n, op in re.findall(r"(\d+)([MID])", cigar):
-            n = int(n)
-            if op == "M":
-                seq += [other[ref[q]] if q in mism else chr(ref[q]) for q in range(p, p + n)]
-                p += n
-            elif op == "D":
-                p += n
-            else:
-                seq += ["A"] * n
-        bb.add_sam(tid=0, pos=pos, flag=flag, mapq=mapq, lib=lib, cigar=cigar, seq="".join(seq), qual="I" * len(seq),
-                   nm=len(mism), sm=mapq, qname=f"r{k}")
-    b = bb.build()
-    order = np.argsort(b.pos, kind="stable")
-    return dict(name="crafted", contigs=[("chr1", L, ref, 0)], batch=b.select(order), regions=list(regions), site_list=False,
-                lib_names=[f"lib{i}" for i in range(n_libs)])
 
 
 @pytest.mark.gpu
@@ -278,7 +237,7 @@ def test_rounding_at_the_threshold_and_on_binary_ties():
     reads = [(80, "60M", set(), 0, 60, 0) for _ in range(10)]
     reads += [(90, "40M", {100}, 0, 1 if k == 0 else 0, 16 * (k & 1)) for k in range(8)]
     reads += [(110, "40M", {120}, 0, 1 if k < 3 else 0, 0) for k in range(8)]
-    case = _crafted(reads, [(0, 81, 140)])
+    case = crafted_case(reads, [(0, 81, 140)])
     want, _, _ = cases.run_oracle(case, dict(), site_list=False)
     mq = {int(ln.split("\t")[1]): [v[1] for a, v in entries(ln.split("\t")[4:]) if is_alt(a, ln.split("\t")[2]) and v[0] > 0]
           for ln in want.splitlines()}
@@ -301,7 +260,7 @@ def test_argv_regions_deletion_from_an_earlier_region_judged_by_its_stats(carry)
     the deletion the only qualifying entry, or disqualify it, on the lines the host forms from the queue."""
     reads = [(30, "100M", {50} if k < 3 else set(), 0, 60, 0) for k in range(20)]
     reads += [(30, "50M", set(), 1, 60, 0) for _ in range(5)] + [(30, "30M1D19M", set(), 1, 30, 16)]
-    case = _crafted(reads, [(0, 41, 60), (0, 71, 120), (0, 41, 61)], n_libs=2)
+    case = crafted_case(reads, [(0, 41, 60), (0, 71, 120), (0, 41, 61)], n_libs=2)
     flags = dict(per_lib=True)
     want, _, _ = cases.run_oracle(case, flags, site_list=False)
     sets = [{"num_minus_strand": (100, None)}, {"num_minus_strand": (None, 0)}, {"avg_mapping_quality": (None, 3000)},
@@ -311,7 +270,7 @@ def test_argv_regions_deletion_from_an_earlier_region_judged_by_its_stats(carry)
     assert kept[0] == kept[2] and [ln.split("\t")[1] for ln in kept[1].splitlines()] == ["51", "51"]
     runs = _runs(case, flags, False, [(1, 0.0, b) for b in sets] + [(2, 0.0, b) for b in sets], carry=carry)
     for filt, (text, _, _) in zip([(1, 0.0, b) for b in sets] + [(2, 0.0, b) for b in sets], runs):
-        d = _same(text, select_lines_bounds(want, *filt))
+        d = first_diff(text, select_lines_bounds(want, *filt))
         assert not d, (filt, d)
 
 
@@ -325,7 +284,7 @@ def test_pipelined_path_with_bounds(n_chunks, monkeypatch):
         otext = cases.run_oracle_cached(case, cases.FLAG_SETS[fname], False).text
         filters = [(1, 0.0, b) for b in FPFILTER_SETS + one_sided_sets(otext)[::5]]
         for filt, (text, _, _) in zip(filters, _runs(case, cases.FLAG_SETS[fname], False, filters)):
-            d = _same(text, select_lines_bounds(otext, *filt))
+            d = first_diff(text, select_lines_bounds(otext, *filt))
             assert not d, (fname, n_chunks, filt, d)
 
 
@@ -336,7 +295,7 @@ def test_pool_overflow_fallback_with_bounds():
     want = cases.run_oracle(case, dict(), site_list=True).text
     filters = [(1, 0.0, b) for b in FPFILTER_SETS + one_sided_sets(want)[:4]]
     for filt, (text, _, _) in zip(filters, _runs(case, dict(), True, filters)):
-        d = _same(text, select_lines_bounds(want, *filt))
+        d = first_diff(text, select_lines_bounds(want, *filt))
         assert not d, (filt, d)
 
 
@@ -391,7 +350,7 @@ def test_absent_or_always_true_bounds_change_nothing():
                 e.compute()
                 results.append((how, e.format_text(-1), e.launch_count()))
             for how, text, launches in results:
-                assert text == plain.text, (flags, how, _same(text, plain.text))
+                assert text == plain.text, (flags, how, first_diff(text, plain.text))
                 assert launches == plain.launches, (flags, how)
             b = CEntryBounds()
             for bad in ("nofilter", "mask", "neg", "order"):
@@ -407,16 +366,6 @@ def test_absent_or_always_true_bounds_change_nothing():
                 assert rc != 0, bad
             with pytest.raises(BrcError):
                 e.set_site_filter(2, 0.05, bounds={"avg_basequality": ("20", "19.99")})
-
-
-def _write_ref(tmp):
-    z = np.load(os.path.join(GOLDEN, "test_bam.npz"))
-    L, wb = int(z["chrom_len"]), int(z["ref_win_beg"])
-    seq = np.full(L, ord("N"), dtype=np.uint8)
-    seq[wb:wb + z["ref_win"].shape[0]] = z["ref_win"]
-    from bam_readcount_b200 import synth
-    synth.write_fasta(os.path.join(tmp, "ref.fa"), "21", seq)
-    return os.path.join(tmp, "ref.fa")
 
 
 def _cli_args(bounds):
@@ -437,7 +386,7 @@ def _check_cli(exe, argv):
         for extra, mc in (([], 1), (["--min-alt-count", "2"], 2))[:1 if i else 2]:
             p = subprocess.run([exe] + extra + _cli_args(b) + argv, capture_output=True)
             assert p.returncode == 0, p.stderr.decode()[-2000:]
-            d = _same(p.stdout.decode("latin-1"), select_lines_bounds(text, mc, 0.0, b))
+            d = first_diff(p.stdout.decode("latin-1"), select_lines_bounds(text, mc, 0.0, b))
             assert not d, (argv, b, extra, d)
             assert p.stderr == full.stderr
     return text
@@ -446,19 +395,16 @@ def _check_cli(exe, argv):
 @pytest.mark.gpu
 def test_cli_bounds_on_the_reference_fixture_and_a_synthetic_bam(tmp_path):
     exe = _cli()
-    ref = _write_ref(str(tmp_path))
+    ref = cases.write_testbam_fasta(str(tmp_path / "ref.fa"))
     bam = os.path.join(GOLDEN, "test.bam")
     _check_cli(exe, ["-w", "0", "-f", ref, "-l", os.path.join(GOLDEN, "site_list"), bam])
     _check_cli(exe, ["-w", "0", "-p", "-f", ref, bam, "21:10402700-10403100", "21:10402950-10403300", "21:10403301-10403600"])
-    samtools = cases.samtools()
     from bam_readcount_b200 import synth
     case = cases.synthetic_case(L=30000, depth=30, seed=53, regions=((0, 1, 30000),), site_list=False)
     name, L, seq, _ = case["contigs"][0]
     d = str(tmp_path)
     synth.write_fasta(os.path.join(d, "s.fa"), name, np.frombuffer(seq, dtype=np.uint8))
-    synth.write_sam(os.path.join(d, "s.sam"), case["batch"], [(name, L)], n_libs=len(case["lib_names"]))
-    subprocess.check_call([samtools, "view", "-b", "-o", os.path.join(d, "s.bam"), os.path.join(d, "s.sam")])
-    subprocess.check_call([samtools, "index", os.path.join(d, "s.bam")])
+    cases.write_bam(d, "s", case["batch"], [(name, L)], n_libs=len(case["lib_names"]))
     base = ["-w", "0", "-f", os.path.join(d, "s.fa"), os.path.join(d, "s.bam")]
     text = _check_cli(exe, base + ["chr1:1-30000"])
     assert any("\t+" in ln for ln in text.splitlines()) and any("\t-" in ln for ln in text.splitlines())

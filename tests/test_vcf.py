@@ -218,7 +218,7 @@ CLI_FLAGS = {"default": [], "ic": ["-i"], "q20b20": ["-q", "20", "-b", "20"], "w
 @pytest.mark.parametrize("shape", ["one", "multi", "sites_only", "bgzf", "device_decode"])
 def test_cli_vcf_fixture(tmp_path, flags, shape):
     exe = cases.cli()
-    fa = vcf_cases.write_fasta21(str(tmp_path / "ref.fa"))
+    fa = cases.write_testbam_fasta(str(tmp_path / "ref.fa"))
     recs = vcf_cases.fixture_records()
     sample, extra = None, []
     if shape == "multi":
@@ -237,18 +237,15 @@ def test_cli_vcf_fixture(tmp_path, flags, shape):
 
 def test_cli_vcf_synthetic_indels(tmp_path):
     """A synthetic BAM with indels; records from its own text, so most alleles are present."""
-    REF_SAMTOOLS = cases.samtools()
     from bam_readcount_b200 import synth
     exe = cases.cli()
     L = 20000
     ref = synth.synth_reference(L, 31)
     batch = synth.synth_reads(ref, 30, seed=31, n_libs=2)
     d = str(tmp_path)
-    sam, bam, fa = os.path.join(d, "s.sam"), os.path.join(d, "s.bam"), os.path.join(d, "s.fa")
+    fa = os.path.join(d, "s.fa")
     synth.write_fasta(fa, "chr1", ref)
-    synth.write_sam(sam, batch, [("chr1", L)], n_libs=2, read_group=True)
-    subprocess.check_call([REF_SAMTOOLS, "view", "-b", "-o", bam, sam])
-    subprocess.check_call([REF_SAMTOOLS, "index", bam])
+    bam = cases.write_bam(d, "s", batch, [("chr1", L)], n_libs=2, read_group=True)
     sites = os.path.join(d, "all")
     open(sites, "w").write("".join(f"chr1\t{p}\t{p}\n" for p in range(200, L - 200)))
     lines = subprocess.run([exe, "-f", fa, "-l", sites, bam], capture_output=True, check=True).stdout.decode().splitlines()

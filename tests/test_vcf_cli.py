@@ -9,9 +9,9 @@ import pytest
 import cases
 import vcf_cases
 import vcf_rule
+from cases import DECODE_ONLY
 
 BAM = os.path.join(cases.GOLDEN, "test.bam")
-DECODE_ONLY = dict(os.environ, BRC_CLI_DECODE_ONLY="1")
 
 
 def _line(chrom, pos, ref, depth, entries):

@@ -269,7 +269,7 @@ def test_cli_fixture(tmp_path, flags, shape):
     if shape == "device_decode" and flags == "d5":
         pytest.skip("the device-decoded span path needs a -d above the region's read count")
     exe = cases.cli()
-    fa = vcf_cases.write_fasta21(str(tmp_path / "ref.fa"))
+    fa = cases.write_testbam_fasta(str(tmp_path / "ref.fa"))
     bam = os.path.join(cases.GOLDEN, "test.bam")
     argv, fl = CLI_FLAGS[flags]
     text = vcf_cases.vcf_text(vcf_cases.fixture_records(), sites_only=shape == "sites_only", pad=shape == "one")
@@ -326,7 +326,7 @@ def test_cli_crafted(tmp_path):
 
 def test_cli_vcf_samples_columns_equal_single_runs(tmp_path):
     exe = cases.cli()
-    fa = vcf_cases.write_fasta21(str(tmp_path / "ref.fa"))
+    fa = cases.write_testbam_fasta(str(tmp_path / "ref.fa"))
     bam = os.path.join(cases.GOLDEN, "test.bam")
     text = vcf_cases.vcf_text(vcf_cases.fixture_records(), samples=("S1", "S2"))
     path = tmp_path / "in.vcf"

@@ -13,18 +13,18 @@ import complex_rule
 import vcf_cases
 from bam_readcount_b200 import bamio
 from bam_readcount_b200.engine import admitted
+from cases import DECODE_ONLY
 
 BAM = os.path.join(cases.GOLDEN, "test.bam")
-DECODE_ONLY = dict(os.environ, BRC_CLI_DECODE_ONLY="1")
 
 
-def _crafted(tmp_path):
+def _crafted_batch(tmp_path):
     bam, _ = complex_cases.write_crafted(str(tmp_path))
     return bamio.read_bam(bam)[1]
 
 
 def test_rule_on_crafted_reads(tmp_path):
-    batch = _crafted(tmp_path)
+    batch = _crafted_batch(tmp_path)
     rows = complex_cases.crafted_reads()
     P = complex_cases.P
     reads = complex_rule.Reads(batch)
@@ -67,20 +67,13 @@ def test_rule_classifies_and_derives():
     assert complex_rule.complex_values(4, [(1, 1, 0), (2, 0, 2)], ["TT", None]) == "4:1,2,.:1,0,.:0,2,.:0.5,."
 
 
-def _check_exe(tmp_path):
-    exe = os.path.join(str(tmp_path), "complex_check")
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-I", os.path.join(cases.ROOT, "bam_readcount_b200", "csrc"), "-o", exe,
-                           os.path.join(cases.ROOT, "tests", "complex_check.cpp")])
-    return exe
-
-
 def test_device_resolver_equals_rule(tmp_path):
     """The kernel's flank walk, compiled for the CPU, gives the rule's flank query positions (or 'does not span') for every read
     of test.bam, the crafted BAM and a synthetic BAM over spans of lengths 1-20 placed all along each read."""
     from bam_readcount_b200 import synth
-    exe = _check_exe(tmp_path)
+    exe = cases.check_program("complex_check")
     ref = synth.synth_reference(4000, 5)
-    batches = [cases.testbam_case()["batch"], _crafted(tmp_path), synth.synth_reads(ref, 20, seed=5)]
+    batches = [cases.testbam_case()["batch"], _crafted_batch(tmp_path), synth.synth_reads(ref, 20, seed=5)]
     rng = np.random.default_rng(3)
     lines, want = [], []
     for b in batches:

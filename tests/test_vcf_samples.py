@@ -2,7 +2,6 @@
 Sample NAME's column must hold exactly what `--vcf FILE --vcf-sample NAME INPUT` writes there, and its ERR (or, without one,
 the process's STDERR) that run's STDERR.  CPU tests use the decode-only hook (BRC_CLI_DECODE_ONLY: per-region record
 summaries on STDOUT and no VCF); GPU tests compare the VCF with the fold of the single-sample runs."""
-import dataclasses
 import os
 import shutil
 import subprocess
@@ -12,48 +11,9 @@ import pytest
 
 import cases
 import vcf_cases
+from cases import CONTIGS, CRAM_DATA, DECODE_ONLY, synthetic_bam
 
-CRAM = os.path.join(cases.ROOT, "oracle", "_ref", "test-data", "twolib.sorted.cram")
-CONTIGS = {"chrA": (24000, 11), "chrB": (16000, 12), "chrC": (12000, 13)}       # name -> (length, reference seed)
-DECODE_ONLY = dict(os.environ, BRC_CLI_DECODE_ONLY="1")
-
-
-def _have_htslib():
-    return os.path.exists(os.path.join(cases.ROOT, "bam_readcount_b200", "third_party", "htslib", "libhts.a")) and os.path.exists(CRAM)
-
-
-def _write_fasta(path, contigs):
-    """Multi-contig FASTA (60 columns) and its .fai."""
-    with open(path, "wb") as fa, open(path + ".fai", "w") as fai:
-        off = 0
-        for name, seq in contigs:
-            head = f">{name}\n".encode()
-            body = b"".join(seq[i:i + 60] + b"\n" for i in range(0, len(seq), 60))
-            fa.write(head + body)
-            fai.write(f"{name}\t{len(seq)}\t{off + len(head)}\t60\t61\n")
-            off += len(head) + len(body)
-
-
-def _synthetic_bam(d, name, order, n_libs, seed, depth=8, no_nm=0):
-    """A coordinate-sorted BAM whose @SQ lines are `order` (a subset of CONTIGS, in any order), with n_libs libraries
-    (0: no @RG at all) and `no_nm` reads without an NM tag (they draw warnings)."""
-    from bam_readcount_b200 import synth
-    from bam_readcount_b200.batch import ReadBatch, TAG_ABSENT
-    parts = []
-    for tid, c in enumerate(order):
-        ref = synth.synth_reference(CONTIGS[c][0], CONTIGS[c][1])
-        parts.append(synth.synth_reads(ref, depth, seed=seed + 101 * tid, n_libs=max(n_libs, 1), tid=tid))
-    b = ReadBatch.concat(parts)
-    if no_nm:
-        nm = np.array(b.nm, copy=True)
-        nm[np.random.default_rng(seed).choice(b.n_reads, no_nm, replace=False)] = TAG_ABSENT
-        b = dataclasses.replace(b, nm=nm)
-    sam, bam = os.path.join(d, name + ".sam"), os.path.join(d, name + ".bam")
-    synth.write_sam(sam, b, [(c, CONTIGS[c][0]) for c in order], n_libs=max(n_libs, 1), read_group=n_libs > 0)
-    subprocess.check_call([cases.samtools(), "view", "-b", "-o", bam, sam])
-    subprocess.check_call([cases.samtools(), "index", bam])
-    os.remove(sam)
-    return bam
+CRAM = os.path.join(CRAM_DATA, "twolib.sorted.cram")
 
 
 def _records(seqs):
@@ -82,9 +42,9 @@ def cohort(tmp_path_factory):
     from bam_readcount_b200 import synth
     d = str(tmp_path_factory.mktemp("vcf_samples"))
     s = {
-        "syn5": _synthetic_bam(d, "syn5", ["chrA", "chrB", "chrC"], 5, seed=21, no_nm=60),
-        "syn2": _synthetic_bam(d, "syn2", ["chrB", "chrA"], 2, seed=22),
-        "syn0": _synthetic_bam(d, "syn0", ["chrA", "chrC"], 0, seed=24, no_nm=10),
+        "syn5": synthetic_bam(d, "syn5", ["chrA", "chrB", "chrC"], 5, seed=21, no_nm=60),
+        "syn2": synthetic_bam(d, "syn2", ["chrB", "chrA"], 2, seed=22),
+        "syn0": synthetic_bam(d, "syn0", ["chrA", "chrC"], 0, seed=24, no_nm=10),
         "test": os.path.join(cases.GOLDEN, "test.bam"),
     }
     s["cut"] = os.path.join(d, "cut.bam")
@@ -93,14 +53,10 @@ def cohort(tmp_path_factory):
     shutil.copy(s["test"] + ".bai", s["cut"] + ".bai")
     s["noidx"] = os.path.join(d, "noidx.bam")
     shutil.copy(s["test"], s["noidx"])
-    wb, win, L21 = vcf_cases.testbam_ref()
-    chr21 = bytearray(b"N" * L21)
-    chr21[wb:wb + len(win)] = win.encode("latin-1")
     rand1k = b"".join(open(os.path.join(cases.GOLDEN, "rand1k.fa"), "rb").read().split(b"\n")[1:])
-    seqs = {"21": bytes(chr21), "rand1k": rand1k}
+    seqs = {"21": cases.testbam_chr21(), "rand1k": rand1k}
     seqs.update({c: synth.synth_reference(L, sd).tobytes() for c, (L, sd) in CONTIGS.items()})
-    fa = os.path.join(d, "all.fa")
-    _write_fasta(fa, list(seqs.items()))
+    fa = cases.write_fasta(os.path.join(d, "all.fa"), list(seqs.items()))
     recs = _records({c: v.decode("latin-1").upper() for c, v in seqs.items()})
     return dict(dir=d, samples=s, fasta=fa, records=recs)
 
@@ -375,7 +331,7 @@ def test_vcf_samples_failed_sample_between_good_ones(cohort, tmp_path):
 
 @pytest.mark.gpu
 def test_vcf_samples_cram(cohort, tmp_path):
-    if not _have_htslib():
+    if not (cases.have_htslib() and os.path.exists(CRAM)):
         pytest.skip("host built without htslib, or no CRAM fixture")
     exe = cases.cli()
     s = cohort["samples"]

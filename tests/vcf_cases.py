@@ -1,29 +1,18 @@
 """Inputs of the --vcf tests: VCF text over the reference's test.bam fixture, its sample-column variants, and a BGZF writer."""
 from __future__ import annotations
 
-import os
-
-import numpy as np
-
 import bam_craft
-
-GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+import cases
 
 HEAD = "##fileformat=VCFv4.2\n##contig=<ID=21>\n##FORMAT=<ID=GT,Number=1,Type=String,Description=\"Genotype\">\n"
-
-
-def testbam_ref():
-    """(window start, window bytes, contig length) of contig 21 as test_bam.npz stores it."""
-    z = np.load(os.path.join(GOLDEN, "test_bam.npz"))
-    return int(z["ref_win_beg"]), z["ref_win"].tobytes().decode("latin-1"), int(z["chrom_len"])
 
 
 def fixture_records():
     """Records around the fixture's two covered sites: SNVs (all four bases, multi-allelic), insertions, deletions of several
     lengths, MNPs, '*', '<DEL>', lower case, a REF with an IUPAC letter, an N reference, a contig the BAM lacks and
     uncovered positions.  Each is (CHROM, POS, REF, ALT)."""
-    wb, win, _ = testbam_ref()
-    ref = lambda p, n=1: win[p - 1 - wb:p - 1 - wb + n].upper()        # 1-based
+    chr21 = cases.testbam_chr21()
+    ref = lambda p, n=1: chr21[p - 1:p - 1 + n].decode("latin-1").upper()        # 1-based
     out = []
     for site in (10402985, 10405200):
         for p in range(site - 6, site + 7):
@@ -62,11 +51,4 @@ def write_bgzf(path: str, data: bytes):
         fh.write(bam_craft.bgzf_member(b""))
 
 
-def write_fasta21(path: str):
-    """ref.fa of contig 21: N everywhere except the window the fixture's reads touch."""
-    from bam_readcount_b200 import synth
-    wb, win, L = testbam_ref()
-    seq = np.full(L, ord("N"), dtype=np.uint8)
-    seq[wb:wb + len(win)] = np.frombuffer(win.encode("latin-1"), dtype=np.uint8)
-    synth.write_fasta(path, "21", seq)
-    return path
+write_fasta21 = cases.write_testbam_fasta        # the name tests/golden/make_vcf_golden.py writes the fixture's ref.fa with
